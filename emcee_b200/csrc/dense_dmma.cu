@@ -20,15 +20,16 @@
 //     {8j+2t, 8j+2t+1}: the DMMA A fragments under a permutation of the contraction
 //     index that is folded into the packing of L, so rows move as 16-byte vectors),
 //     releases the slot (the producer refills it while the tile is on the tensor
-//     pipe), runs mma.sync.m8n8k4.f64 against the packed factor in shared memory,
-//     reduces |y|^2 over the 4 lanes of a row, applies the Metropolis test and
+//     pipe), runs mma.sync.m16n8k8.f64 with the packed factor in shared memory as
+//     the 16-row A operand and q as B (two 8x8 factor blocks per instruction),
+//     reduces |y|^2 over the 8 lanes of a walker, applies the Metropolis test and
 //     writes accepted rows straight from those registers.  A consumer does almost
 //     nothing but DMMAs.
 //   * tiles (8 walkers) are dealt SM-major, so every sub-partition gets the same count.
 //   * one cooperative launch runs MANY half-steps (all splits of all steps up to the
 //     next host-visible event): between half-steps the CTAs meet at a grid barrier on
 //     a global counter instead of paying a kernel boundary (launch gap, re-staging of
-//     the 70 KB factor, pipeline refill from cold).
+//     the 74 KB factor, pipeline refill from cold).
 #include <math.h>
 
 #include "engine.cuh"
@@ -40,15 +41,22 @@ namespace {
 
 constexpr int DMMA_CONSUMERS = 8;
 constexpr int DMMA_THREADS = 64 * DMMA_CONSUMERS;  // consumers are warps 0..7, producers 8..15
-constexpr int NI = 2;  // column tiles in flight per consumer (2*NI independent accumulator chains)
+constexpr int NI = 2;  // 16-column tiles of y in flight per consumer (NI independent accumulator chains)
 
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
+// C[16x8] += A[16x8] B[8x8]: lane (g,t) holds a = {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]},
+// b = {B[t][g], B[t+4][g]}, c = {C[g][2t], C[g][2t+1], C[g+8][2t], C[g+8][2t+1]}
+__device__ __forceinline__ void dmma1688(double (&c)[4], double2 a01, double2 a23, double b0, double b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a01.x), "d"(a01.y), "d"(a23.x), "d"(a23.y), "d"(b0), "d"(b1));
 }
 
-__host__ __device__ constexpr int packed_blocks(int KB) { return KB * (KB + 1); }  // 2 * KB(KB+1)/2
+// y = L^T x is computed 16 columns at a time: column pair m (8x8 column blocks 2m and 2m+1) needs the row
+// blocks j >= 2m, one m16n8k8 each (for odd KB the last pair has one block, padded with zeros)
+__host__ __device__ constexpr int col_pairs(int KB) { return (KB + 1) / 2; }
+__host__ __device__ constexpr int factor_dmmas(int KB) { return col_pairs(KB) * (KB - col_pairs(KB) + 1); }
+__host__ __device__ constexpr size_t factor_doubles(int KB) { return (size_t)factor_dmmas(KB) * 128; }
 // landing slot of one pair: [s|c][8 rows][D + 8] doubles; the +8 (64 B) row skew
 // makes the 16-byte fragment accesses of 8 consecutive lanes hit 32 distinct banks
 __host__ __device__ constexpr int row_stride(int KB) { return 8 * KB + 8; }
@@ -63,7 +71,7 @@ struct TileMeta {
 
 template <int KB>
 struct SmemLayout {
-  static constexpr size_t L_doubles = (size_t)packed_blocks(KB) * 32;
+  static constexpr size_t L_doubles = factor_doubles(KB);
   static constexpr size_t mu_doubles = 8 * KB;
   static constexpr size_t slot_doubles = 2 * 8 * row_stride(KB);
   static constexpr size_t off_mu = L_doubles;
@@ -76,22 +84,23 @@ struct SmemLayout {
   static constexpr size_t total_bytes = off_abort_bytes + 16;
 };
 
-// The tensor-pipe block of the stand-alone log-prob kernel: the same statements, in the same order, as
-// the block inlined in the half-step kernel's consumer (kept inline there: its register allocation is
-// tuned to the last register), so both produce bit-identical values for the same row: this lane's partial sum over its two columns of
-// |L^T (q - mu)|^2 for the 8 rows of the warp's tile; q holds the lane's A fragments.
+// The tensor-pipe block, shared by the half-step kernel's consumer and the stand-alone log-prob kernel so
+// both produce bit-identical values for the same row: |L^T (q - mu)|^2 of walker g of the warp's 8-walker
+// tile (every lane (g, t) returns its walker's value); q holds the lane's B fragments, row g, columns
+// {8j+2t, 8j+2t+1}.  C holds y[16 columns][8 walkers]: lane (g,t) accumulates walkers 2t and 2t+1.
 template <int KB, bool HAS_MEAN>
 __device__ __forceinline__ double tile_sumsq(const double (&q)[2 * KB], const double* sL, const double* sMu, int lane,
-                                             int t) {
-  double rs = 0.0;
-  const double* bptr = sL + 2 * lane;  // one 16-byte load feeds the two k-halves of a block pair
+                                             int g, int t) {
+  constexpr int NP = col_pairs(KB);
+  double rs0 = 0.0, rs1 = 0.0;  // walkers 2t, 2t+1
+  const double* aptr = sL + 2 * lane;  // two 16-byte loads per DMMA: {a0, a1} and, 64 doubles on, {a2, a3}
 #pragma unroll
-  for (int nb0 = 0; nb0 < KB; nb0 += NI) {
-    double c[NI][2][2];
+  for (int m0 = 0; m0 < NP; m0 += NI) {
+    double c[NI][4];
 #pragma unroll
-    for (int n = 0; n < NI; ++n) c[n][0][0] = c[n][0][1] = c[n][1][0] = c[n][1][1] = 0.0;
+    for (int n = 0; n < NI; ++n) c[n][0] = c[n][1] = c[n][2] = c[n][3] = 0.0;
 #pragma unroll
-    for (int j = nb0; j < KB; ++j) {
+    for (int j = 2 * m0; j < KB; ++j) {
       double x0 = q[2 * j + 0], x1 = q[2 * j + 1];
       if (HAS_MEAN) {
         const double2 m2 = *reinterpret_cast<const double2*>(sMu + 8 * j + 2 * t);
@@ -100,22 +109,30 @@ __device__ __forceinline__ double tile_sumsq(const double (&q)[2 * KB], const do
       }
 #pragma unroll
       for (int n = 0; n < NI; ++n) {
-        if (nb0 + n < KB && j >= nb0 + n) {
-          const double2 b2 = *reinterpret_cast<const double2*>(bptr);
-          dmma884(c[n][0][0], c[n][0][1], x0, b2.x);
-          dmma884(c[n][1][0], c[n][1][1], x1, b2.y);
-          bptr += 64;
+        if (m0 + n < NP && j >= 2 * (m0 + n)) {
+          const double2 a01 = *reinterpret_cast<const double2*>(aptr);
+          const double2 a23 = *reinterpret_cast<const double2*>(aptr + 64);
+          dmma1688(c[n], a01, a23, x0, x1);
+          aptr += 128;
         }
       }
     }
 #pragma unroll
     for (int n = 0; n < NI; ++n) {
-      const double y0 = c[n][0][0] + c[n][1][0], y1 = c[n][0][1] + c[n][1][1];
-      rs = fma(y0, y0, rs);
-      rs = fma(y1, y1, rs);
+      rs0 = fma(c[n][0], c[n][0], rs0);
+      rs0 = fma(c[n][2], c[n][2], rs0);
+      rs1 = fma(c[n][1], c[n][1], rs1);
+      rs1 = fma(c[n][3], c[n][3], rs1);
     }
   }
-  return rs;
+  // sum over the 8 lanes (g) that hold the same two walkers, then fetch walker g's sum from lane g / 2
+#pragma unroll
+  for (int o = 4; o < 32; o <<= 1) {
+    rs0 += __shfl_xor_sync(0xffffffffu, rs0, o);
+    rs1 += __shfl_xor_sync(0xffffffffu, rs1, o);
+  }
+  const double e = __shfl_sync(0xffffffffu, rs0, g >> 1), o = __shfl_sync(0xffffffffu, rs1, g >> 1);
+  return (g & 1) ? o : e;
 }
 
 // grid-wide barrier between consecutive half-steps of one persistent launch: the
@@ -421,41 +438,8 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       if (lane == 0) mbar_arrive(barFree + pair);  // slot and meta may be refilled while this tile computes
       if (tlk) tlk[3] = clock64() - t_entry;
 
-      // ---- y = L^T (q - mu) block by block on the tensor pipe; rs = sum_n y_n^2
-      double rs = 0.0;
-      const double* bptr = sL + 2 * lane;  // one 16-byte load feeds the two k-halves of a block pair
-#pragma unroll
-      for (int nb0 = 0; nb0 < KB; nb0 += NI) {
-        double c[NI][2][2];
-#pragma unroll
-        for (int n = 0; n < NI; ++n) c[n][0][0] = c[n][0][1] = c[n][1][0] = c[n][1][1] = 0.0;
-#pragma unroll
-        for (int j = nb0; j < KB; ++j) {
-          double x0 = q[2 * j + 0], x1 = q[2 * j + 1];
-          if (HAS_MEAN) {
-            const double2 m2 = *reinterpret_cast<const double2*>(sMu + 8 * j + 2 * t);
-            x0 -= m2.x;
-            x1 -= m2.y;
-          }
-#pragma unroll
-          for (int n = 0; n < NI; ++n) {
-            if (nb0 + n < KB && j >= nb0 + n) {
-              const double2 b2 = *reinterpret_cast<const double2*>(bptr);
-              dmma884(c[n][0][0], c[n][0][1], x0, b2.x);
-              dmma884(c[n][1][0], c[n][1][1], x1, b2.y);
-              bptr += 64;
-            }
-          }
-        }
-#pragma unroll
-        for (int n = 0; n < NI; ++n) {
-          const double y0 = c[n][0][0] + c[n][1][0], y1 = c[n][0][1] + c[n][1][1];
-          rs = fma(y0, y0, rs);
-          rs = fma(y1, y1, rs);
-        }
-      }
-      rs += __shfl_xor_sync(0xffffffffu, rs, 1);
-      rs += __shfl_xor_sync(0xffffffffu, rs, 2);
+      // ---- y = L^T (q - mu) on the tensor pipe; rs = sum_n y_n^2
+      const double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, g, t);
       const double lp_new = -0.5 * rs;
       if (tlk) tlk[4] = clock64() - t_entry;
 
@@ -543,7 +527,7 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
   constexpr int D = 8 * KB;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double* sL = reinterpret_cast<double*>(smem_raw);
-  double* sMu = sL + (size_t)packed_blocks(KB) * 32;
+  double* sMu = sL + factor_doubles(KB);
   uint64_t* barL = reinterpret_cast<uint64_t*>(sMu + D);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -555,7 +539,7 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
     for (int k = tid; k < D; k += blockDim.x) sMu[k] = m.params[k];
   __syncthreads();
   if (tid == 0) {
-    constexpr unsigned bytes = (unsigned)((size_t)packed_blocks(KB) * 32 * sizeof(double));
+    constexpr unsigned bytes = (unsigned)(factor_doubles(KB) * sizeof(double));
     mbar_arrive_expect_tx(barL, bytes);
     bulk_g2s(sL, m.chol, bytes, barL);
   }
@@ -582,9 +566,7 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
       mbar_wait(barL, 0);
       waited = true;
     }
-    double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, t);
-    rs += __shfl_xor_sync(0xffffffffu, rs, 1);
-    rs += __shfl_xor_sync(0xffffffffu, rs, 2);
+    const double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, g, t);
     const double lp = -0.5 * rs;
     if (valid && t == 0) {
       out[r] = lp;
@@ -596,7 +578,7 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
 template <int KB>
 cudaError_t launch_lp_t(const ModelDev& m, const double* x, int64_t rows, double* out, int* status, int sm_count,
                         cudaStream_t st) {
-  const size_t smem = ((size_t)packed_blocks(KB) * 32 + 8 * KB) * sizeof(double) + sizeof(uint64_t);
+  const size_t smem = (factor_doubles(KB) + 8 * KB) * sizeof(double) + sizeof(uint64_t);
   const bool has_mean = m.s0 != 0.0;
   auto kern = has_mean ? logprob_dense_dmma_kernel<KB, true> : logprob_dense_dmma_kernel<KB, false>;
   if (smem > 48 * 1024) {
@@ -659,24 +641,28 @@ cudaError_t launch_t(const HalfStepArgs& a, const HalfDesc& d0, const HalfDesc* 
 // any ndim that is a multiple of 8 up to 128 (the proposal tile lives in D/4 registers per lane)
 bool dense_dmma_supported(int D) { return D >= 8 && D <= 128 && D % 8 == 0; }
 
-size_t dense_dmma_factor_doubles(int D) { return (size_t)packed_blocks(D / 8) * 32; }
+size_t dense_dmma_factor_doubles(int D) { return factor_doubles(D / 8); }
 
-// L: row-major lower-triangular factor (A = L L^T).  Packed in the order the
-// kernel consumes it: for each group of NI 8-column tiles, for each 8-row group
-// j, for each tile nb of the group with j >= nb, the two 4x8 fragments (half = 0, 1)
-// interleaved per lane: lane (g, t) holds L[8j + 2t + half][8nb + g], half = 0, 1 side by side.
+// L: row-major lower-triangular factor (A = L L^T).  Packed in the order the kernel consumes it: for each
+// group of NI column pairs, for each 8-row group j, for each pair m of the group with j >= 2m, the A fragment
+// of L[8j .. 8j+8][16m .. 16m+16]^T (zero beyond column D) as two planes of 32 lanes x 16 bytes: lane (g, t)
+// holds {L[8j+2t][16m+g], L[8j+2t][16m+8+g]} in the first and {L[8j+2t+1][16m+g], L[8j+2t+1][16m+8+g]} in the
+// second (k = t, t+4 of the fragment are columns 2t, 2t+1 of the row group, as in q).
 void dense_dmma_pack_factor(const double* L, int D, double* packed) {
-  const int KB = D / 8;
+  const int KB = D / 8, NP = col_pairs(KB);
   size_t idx = 0;
-  for (int nb0 = 0; nb0 < KB; nb0 += NI)
-    for (int j = nb0; j < KB; ++j)
+  for (int m0 = 0; m0 < NP; m0 += NI)
+    for (int j = 2 * m0; j < KB; ++j)
       for (int n = 0; n < NI; ++n) {
-        const int nb = nb0 + n;
-        if (nb >= KB || j < nb) continue;
-        for (int lane = 0; lane < 32; ++lane)
-          for (int half = 0; half < 2; ++half) {  // the two k-halves of a lane sit side by side (one LDS.128)
-            const int g = lane >> 2, t = lane & 3;
-            packed[idx++] = L[(size_t)(8 * j + 2 * t + half) * D + (8 * nb + g)];
+        const int m = m0 + n;
+        if (m >= NP || j < 2 * m) continue;
+        for (int half = 0; half < 2; ++half)
+          for (int lane = 0; lane < 32; ++lane) {
+            const int g = lane >> 2, t = lane & 3, row = 8 * j + 2 * t + half;
+            for (int hi = 0; hi < 2; ++hi) {
+              const int col = 16 * m + 8 * hi + g;
+              packed[idx++] = (col < D && col <= row) ? L[(size_t)row * D + col] : 0.0;
+            }
           }
       }
 }

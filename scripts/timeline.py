@@ -15,11 +15,13 @@ eng.step(sched, 20, want_accepted=False)
 eng.set_option("dmma_timeline", 1)
 eng.step(sched, 3, want_accepted=False)
 tl = eng.debug_timeline()  # [SM, consumer, tile, event]
+nsm, ncons = tl.shape[0], tl.shape[1]
 ntile = (tl[..., 5] > 0).sum(-1)
+print("SMs %d, consumers per SM %d" % (nsm, ncons))
 print("tiles per consumer (SM0):", ntile[0], " total per SM min/max:", ntile.sum(1).min(), ntile.sum(1).max())
-for sm in (0, 73, 147):
+for sm in sorted({0, nsm // 2, nsm - 1}):
     print("SM", sm)
-    for c in range(8):
+    for c in range(ncons):
         rows = []
         for k in range(int(ntile[sm, c])):
             e = tl[sm, c, k]
@@ -33,6 +35,10 @@ epi = (tl[..., 5] - tl[..., 4])[valid]
 end = tl[..., 5].max(axis=(1, 2))
 print("mean wait %.0f  qload %.0f  mma %.0f  epilogue %.0f  | kernel end per SM: mean %.0f max %.0f" % (
     wait.mean(), qld.mean(), mma.mean(), epi.mean(), end.mean(), end.max()))
+# share of each consumer's time from its first wait to its last tile's end spent in each segment
+busy = (tl[..., 5].max(-1) - tl[..., 0, 1])[ntile > 0]
+print("per consumer, share of first-wait..last-end: wait %.2f  qload %.2f  mma %.2f  epilogue %.2f" % tuple(
+    x.sum() / busy.sum() for x in (wait, qld, mma, epi)))
 first = tl[:, :, 0, 2]
 print("first proposal ready at: mean %.0f min %.0f max %.0f cycles" % (first.mean(), first.min(), first.max()))
 for k in range(4):
