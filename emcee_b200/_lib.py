@@ -95,6 +95,7 @@ _SIGNATURES = {
     "eb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "eb_debug_timeline": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.c_size_t, C.POINTER(C.c_size_t)]),
     "eb_last_kernel_name": (C.c_char_p, [C.c_void_p]),
+    "eb_last_kernel_variant": (C.c_char_p, [C.c_void_p]),
     "eb_microbench": (C.c_int, [C.c_int, C.c_int, _dp]),
     "eb_host_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p)]),
     "eb_host_free": (C.c_int, [C.c_void_p]),
@@ -369,6 +370,11 @@ class Engine(object):
 
     def last_kernel_name(self):
         return lib().eb_last_kernel_name(self._h).decode()
+
+    def last_kernel_variant(self):
+        """The cell of that kernel the last half-step launch ran (``eb_last_kernel_variant``),
+        e.g. ``"tma_rows R=8 epl=8 own_reg=1 warps=16"``."""
+        return lib().eb_last_kernel_variant(self._h).decode()
 
     def set_option(self, name, value):
         self._check(lib().eb_set_option(self._h, name.encode(), int(value)))

@@ -74,6 +74,8 @@ struct eb_ctx {
   double last_ms = 0.0;
   uint64_t last_launches = 0;
   const char* last_kernel = "none";
+  char last_variant[96] = "none";  // eb_last_kernel_variant: the parameters the last half-step launch chose
+  int dmma_nhalf_max = 0;          // most half-steps one dense_dmma launch ran in the current stepping call
   bool allow_dmma = true;
   int allow_tma = 2;  // TMA row-gather kernel for the HBM-bound models: 0 off, 1 short rows only, 2 long rows too
   bool tma_own_reg = true;  // tma_rows, stretch rows <= 512 B: own rows through registers instead of the TMA unit
@@ -738,13 +740,17 @@ int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, const int32
     }
     c->chain_ok = false;
     bool used_tma = false;
+    TmaVariant tv{};
     if (c->allow_tma && !c->debug)
-      CK(c, launch_half_step_tma(mv.kind, a, c->sm_count, c->allow_tma >= 2, c->tma_own_reg, c->st, &used_tma));
+      CK(c, launch_half_step_tma(mv.kind, a, c->sm_count, c->allow_tma >= 2, c->tma_own_reg, c->st, &used_tma, &tv));
     if (used_tma) {
       c->last_kernel = "tma_rows";
+      snprintf(c->last_variant, sizeof(c->last_variant), "tma_rows R=%d epl=%d own_reg=%d warps=%d", tv.R, tv.epl,
+               tv.own_reg, tv.warps);
     } else {
       CK(c, launch_half_step_generic(mv.kind, a, c->st));
       c->last_kernel = "generic";
+      snprintf(c->last_variant, sizeof(c->last_variant), "generic G=%d", lanes_per_walker(c->D));
     }
     ++launches;
     c->tap_count = a.a_count;
@@ -809,6 +815,7 @@ int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
     ++launches;
   }
   c->last_kernel = "walk";
+  snprintf(c->last_variant, sizeof(c->last_variant), "walk");
   return EB_OK;
 }
 
@@ -850,6 +857,7 @@ int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step,
   CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st));
   launches += 2;
   c->last_kernel = "gaussian";
+  snprintf(c->last_variant, sizeof(c->last_variant), "gaussian");
   return EB_OK;
 }
 
@@ -886,6 +894,8 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
                           &grid, c->st));
   c->gbar_count += (unsigned long long)(grp.nhalf - 1) * (unsigned long long)grid;
   c->last_kernel = "dense_dmma";
+  c->dmma_nhalf_max = std::max(c->dmma_nhalf_max, grp.nhalf);
+  snprintf(c->last_variant, sizeof(c->last_variant), "dense_dmma nhalf_max=%d grid=%d", c->dmma_nhalf_max, grid);
   c->chain_ok = grid > 0;
   ++launches;
   grp = DmmaGroup{};
@@ -911,6 +921,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
     }
   }
   c->chain_ok = false;
+  c->dmma_nhalf_max = 0;
   CK(c, cudaEventRecord(c->ev0, c->st));
   if (comm_begin(c->comm, c->st, c->status_dev, launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   c->fused_last = false;
@@ -1391,6 +1402,8 @@ int eb_last_step_timing(const eb_ctx* c, double* ms, uint64_t* launches) {
 }
 
 const char* eb_last_kernel_name(const eb_ctx* c) { return c ? c->last_kernel : "none"; }
+
+const char* eb_last_kernel_variant(const eb_ctx* c) { return c ? c->last_variant : "none"; }
 
 int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
   if (!c || !name) return EB_ERR_INVALID;

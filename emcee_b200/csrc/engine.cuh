@@ -95,11 +95,19 @@ cudaError_t launch_locality_tables(const int32_t* order, const StepInfo* info_de
                                    int64_t N, uint64_t seed, uint64_t step0, int64_t rows_per_rank, int rank,
                                    int front_cap, int32_t* aperm, cudaStream_t st);
 cudaError_t launch_half_step_generic(int move_kind, const HalfStepArgs& a, cudaStream_t st);
+// the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)
+struct TmaVariant {
+  int R;        // walkers per tile (G = 32 / R lanes per walker)
+  int epl;      // 8: register path, 0: strided path
+  int own_reg;  // stretch register path with the own row in registers
+  int warps;    // warps per CTA
+};
 // TMA row-gather variant for the HBM-bound models (tma_rows.cu); *used == false: not applicable, use the generic one
 // (long_rows: also take rows so long that only one walker per tile fits; own_reg: stretch rows of <= 512 bytes keep
-// the own row in registers -- plain loads / stores -- and stage only the partner rows)
+// the own row in registers -- plain loads / stores -- and stage only the partner rows).  *variant (nullable) gets
+// the cell when *used.
 cudaError_t launch_half_step_tma(int move_kind, const HalfStepArgs& a, int sm_count, bool long_rows, bool own_reg,
-                                 cudaStream_t st, bool* used);
+                                 cudaStream_t st, bool* used, TmaVariant* variant = nullptr);
 cudaError_t launch_logprob_generic(const ModelDev& m, const double* x, int64_t rows, int D, double* out,
                                    int* status, cudaStream_t st);
 // specialised: stretch + dense Gaussian on FP64 tensor cores (DMMA).  Returns

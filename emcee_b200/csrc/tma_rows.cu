@@ -433,7 +433,7 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
 
 template <int MOVE, int MODEL>
 cudaError_t launch_tma_t(const HalfStepArgs& a, int sm_count, bool long_rows, bool own_rows_in_registers, cudaStream_t st,
-                         bool* used) {
+                         bool* used, TmaVariant* variant) {
   constexpr int NR = RowsPerWalker<MOVE>::value;
   *used = false;
   const int D = a.D;
@@ -467,6 +467,7 @@ cudaError_t launch_tma_t(const HalfStepArgs& a, int sm_count, bool long_rows, bo
   const bool own_reg = MOVE == EB_MOVE_STRETCH && epl8 && D <= 64 && own_rows_in_registers;
   const int nr_smem = NR - (own_reg ? 1 : 0);
   const size_t smem = (size_t)nwarps * warp_bytes(R) / NR * nr_smem + (size_t)nwarps * 2 * sizeof(uint64_t);
+  if (variant) *variant = TmaVariant{R, epl8 ? 8 : 0, own_reg ? 1 : 0, nwarps};
   const int64_t count = (int64_t)a.i_hi - a.i_lo;
   if (count <= 0) {
     *used = true;
@@ -488,14 +489,15 @@ cudaError_t launch_tma_t(const HalfStepArgs& a, int sm_count, bool long_rows, bo
 }
 
 template <int MOVE>
-cudaError_t launch_tma_m(const HalfStepArgs& a, int sm_count, bool long_rows, bool own_reg, cudaStream_t st, bool* used) {
+cudaError_t launch_tma_m(const HalfStepArgs& a, int sm_count, bool long_rows, bool own_reg, cudaStream_t st, bool* used,
+                         TmaVariant* variant) {
   switch (a.model.kind) {
     case EB_MODEL_GAUSS_ISO:
-      return launch_tma_t<MOVE, EB_MODEL_GAUSS_ISO>(a, sm_count, long_rows, own_reg, st, used);
+      return launch_tma_t<MOVE, EB_MODEL_GAUSS_ISO>(a, sm_count, long_rows, own_reg, st, used, variant);
     case EB_MODEL_ROSENBROCK:
-      return launch_tma_t<MOVE, EB_MODEL_ROSENBROCK>(a, sm_count, long_rows, own_reg, st, used);
+      return launch_tma_t<MOVE, EB_MODEL_ROSENBROCK>(a, sm_count, long_rows, own_reg, st, used, variant);
     case EB_MODEL_RING:
-      return launch_tma_t<MOVE, EB_MODEL_RING>(a, sm_count, long_rows, own_reg, st, used);
+      return launch_tma_t<MOVE, EB_MODEL_RING>(a, sm_count, long_rows, own_reg, st, used, variant);
   }
   *used = false;  // dense Gaussian outside the DMMA envelope: CUDA-core generic kernel
   return cudaSuccess;
@@ -506,14 +508,14 @@ cudaError_t launch_tma_m(const HalfStepArgs& a, int sm_count, bool long_rows, bo
 // Tries the TMA row-gather kernel; *used tells whether it took the half-step (otherwise the
 // caller falls back to half_step_generic_kernel).
 cudaError_t launch_half_step_tma(int move_kind, const HalfStepArgs& a, int sm_count, bool long_rows, bool own_reg,
-                                 cudaStream_t st, bool* used) {
+                                 cudaStream_t st, bool* used, TmaVariant* variant) {
   switch (move_kind) {
     case EB_MOVE_STRETCH:
-      return launch_tma_m<EB_MOVE_STRETCH>(a, sm_count, long_rows, own_reg, st, used);
+      return launch_tma_m<EB_MOVE_STRETCH>(a, sm_count, long_rows, own_reg, st, used, variant);
     case EB_MOVE_DE:
-      return launch_tma_m<EB_MOVE_DE>(a, sm_count, long_rows, own_reg, st, used);
+      return launch_tma_m<EB_MOVE_DE>(a, sm_count, long_rows, own_reg, st, used, variant);
     case EB_MOVE_SNOOKER:
-      return launch_tma_m<EB_MOVE_SNOOKER>(a, sm_count, long_rows, own_reg, st, used);
+      return launch_tma_m<EB_MOVE_SNOOKER>(a, sm_count, long_rows, own_reg, st, used, variant);
   }
   *used = false;
   return cudaErrorInvalidValue;

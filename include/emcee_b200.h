@@ -228,6 +228,11 @@ int eb_set_option(eb_ctx* ctx, const char* name, int64_t value);
 /* name of the kernel variant the last eb_step used for its half-steps
  * ("generic", "dense_dmma", ...). */
 const char* eb_last_kernel_name(const eb_ctx* ctx);
+/* the cell of that kernel the last half-step launch ran, with the parameters its launcher chose:
+ * "tma_rows R=<walkers per tile> epl=<8 register path | 0 strided> own_reg=<0|1> warps=<per CTA>",
+ * "dense_dmma nhalf_max=<most half-steps of one launch in the call> grid=<CTAs>", "generic G=<lanes per
+ * walker>", "walk", "gaussian" or "none". */
+const char* eb_last_kernel_variant(const eb_ctx* ctx);
 
 /* device micro-benchmarks that anchor the FP64 roofline: what = 0 DFMA, 1 DMMA m8n8k4, 2 DMMA m16n8k8,
  * 3 DMMA m16n8k16 (result in TFLOP/s), 4 HBM copy (GB/s).  Current device. */

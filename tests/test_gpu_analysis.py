@@ -77,7 +77,12 @@ def test_moments_at_scale_vs_oracle():
     assert s._engine.last_kernel_name() == "dense_dmma"
 
 
-@pytest.mark.parametrize("shape", [(64, 5), (300, 17), (4096, 128), (2048, 256)])
+@pytest.mark.parametrize(
+    "shape",
+    [(64, 5), (300, 17), (4096, 128), (2048, 256),
+     # above 128 columns the moment sums take several passes (MOM_MAXB); odd row counts leave partial CTAs
+     (301, 129), (517, 255), (1041, 520), (2053, 1023), (2049, 1024)],
+)
 def test_walkers_gram_matches_host(shape):
     rng = np.random.default_rng(5)
     N, D = shape

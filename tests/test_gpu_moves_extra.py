@@ -42,6 +42,14 @@ def test_walk_whole_complement_odd_sizes_three_splits():
     _run_pair("ring", 1003, 7, [(rb.Walk(nsplits=3), 1.0)], moves.WalkMove(nsplits=3), 6)
 
 
+@pytest.mark.parametrize("name,D", [("gauss_iso", 136), ("ring", 260)])
+def test_walk_whole_complement_above_128_dims(name, D):
+    """The moment sums of the complement take several passes above 128 columns (analysis.cu MOM_MAXB), and
+    cov_chol factors a matrix larger than 128 x 128."""
+    s, _ = _run_pair(name, 4 * D + 3, D, [(rb.Walk(), 1.0)], moves.WalkMove(), 4)
+    assert s._engine.last_kernel_variant() == "walk"
+
+
 def test_walk_helper_subsets():
     _run_pair("rosenbrock", 512, 16, [(rb.Walk(s=40), 1.0)], moves.WalkMove(s=40), 6)
     # rank-deficient covariances (s <= ndim): the walk stays in the helpers' span
