@@ -69,6 +69,7 @@ _SIGNATURES = {
     "eb_destroy": (C.c_int, [C.c_void_p]),
     "eb_last_error": (C.c_char_p, [C.c_void_p]),
     "eb_model_set": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_size_t]),
+    "eb_model_set_bounds": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_set_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_get_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_owned_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
@@ -224,6 +225,16 @@ class Engine(object):
     def set_model(self, kind, params):
         params = _f64(np.asarray(params, dtype=np.float64).ravel())
         self._check(lib().eb_model_set(self._h, MODEL_KINDS[kind], _as_dp(params), params.size))
+
+    def set_bounds(self, lower=None, upper=None):
+        """The prior's support ``lower <= x <= upper`` (``eb_model_set_bounds``): outside it the
+        log-probability is ``-inf``.  ``None, None`` clears it; ``set_model`` clears it too."""
+        if lower is None and upper is None:
+            self._check(lib().eb_model_set_bounds(self._h, None, None))
+            return
+        lo = _f64(np.asarray(lower, dtype=np.float64).ravel(), (self.ndim,))
+        hi = _f64(np.asarray(upper, dtype=np.float64).ravel(), (self.ndim,))
+        self._check(lib().eb_model_set_bounds(self._h, _as_dp(lo), _as_dp(hi)))
 
     def set_state(self, coords, log_prob=None):
         coords = _f64(coords, (self.nwalkers, self.ndim))

@@ -33,6 +33,7 @@ struct eb_ctx {
   ModelDev model{};
   double* model_params = nullptr;
   double* model_chol = nullptr;
+  double* model_box = nullptr;  // [lo[D] | hi[D]] of eb_model_set_bounds, or null
   bool have_model = false, have_state = false;
 
   int32_t* order = nullptr;  // [table_cap, N]
@@ -249,6 +250,7 @@ int eb_destroy(eb_ctx* c) {
   cudaFreeHost(c->status_host);
   cudaFree(c->model_params);
   cudaFree(c->model_chol);
+  cudaFree(c->model_box);
   cudaFree(c->order);
   cudaFree(c->info_dev);
   cudaFreeHost(c->info_host);
@@ -337,8 +339,10 @@ int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
   CK(c, cudaStreamSynchronize(c->st));
   cudaFree(c->model_params);
   cudaFree(c->model_chol);
+  cudaFree(c->model_box);  // a new model starts unbounded
   c->model_params = nullptr;
   c->model_chol = nullptr;
+  c->model_box = nullptr;
   if (!host.empty()) {
     CK(c, cudaMalloc(&c->model_params, host.size() * sizeof(double)));
     CK(c, cudaMemcpy(c->model_params, host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice));
@@ -357,6 +361,36 @@ int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
   }
   c->model = m;
   c->have_model = true;
+  return EB_OK;
+}
+
+int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_model_set_bounds: no model set");
+  if ((lower == nullptr) != (upper == nullptr))
+    FAIL(c, EB_ERR_INVALID, "eb_model_set_bounds: pass both bounds, or NULL for both to clear them");
+  const size_t D = (size_t)c->D;
+  if (lower) {
+    for (size_t k = 0; k < D; ++k) {
+      if (isnan(lower[k]) || isnan(upper[k])) FAIL(c, EB_ERR_INVALID, "bounds must not be NaN (parameter %zu)", k);
+      if (!(lower[k] < upper[k]))
+        FAIL(c, EB_ERR_INVALID, "lower bound must be below the upper bound (parameter %zu: %g >= %g)", k, lower[k],
+             upper[k]);
+    }
+  }
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st));
+  c->chain_ok = false;
+  cudaFree(c->model_box);
+  c->model_box = nullptr;
+  c->model.lo = c->model.hi = nullptr;
+  if (lower) {
+    CK(c, cudaMalloc(&c->model_box, 2 * D * sizeof(double)));
+    CK(c, cudaMemcpy(c->model_box, lower, D * sizeof(double), cudaMemcpyHostToDevice));
+    CK(c, cudaMemcpy(c->model_box + D, upper, D * sizeof(double), cudaMemcpyHostToDevice));
+    c->model.lo = c->model_box;
+    c->model.hi = c->model_box + D;
+  }
   return EB_OK;
 }
 

@@ -81,7 +81,10 @@ struct SmemLayout {
   static constexpr size_t off_bars_bytes = off_meta * sizeof(double) + meta_bytes;
   static constexpr int nbars = 1 + 3 * DMMA_CONSUMERS;
   static constexpr size_t off_abort_bytes = off_bars_bytes + nbars * sizeof(uint64_t);
-  static constexpr size_t total_bytes = off_abort_bytes + 16;
+  // bounded models: [pair][record][8 rows] "the proposal lies in the prior's support", written with the proposal
+  // (kept out of TileMeta: the unbounded kernels keep their layout and their register allocation)
+  static constexpr size_t off_inbox_bytes = off_abort_bytes + 16;
+  static constexpr size_t total_bytes = off_inbox_bytes + sizeof(int32_t) * 2 * 8 * DMMA_CONSUMERS;
 };
 
 // The tensor-pipe block, shared by the half-step kernel's consumer and the stand-alone log-prob kernel so
@@ -172,7 +175,9 @@ __device__ __forceinline__ bool peer_wait(const unsigned* my_flags, int rank, in
   return __all_sync(0xffffffffu, ok);
 }
 
-template <int KB, bool HAS_MEAN>
+// BOUNDED (the model has a prior support, ModelDev::lo / hi) is a template flag here, unlike in the other kernels:
+// a run-time branch raised the spills of the register-capped D = 128 instantiations (ptxas: 184 -> 208 bytes)
+template <int KB, bool HAS_MEAN, bool BOUNDED>
 __global__ void __launch_bounds__(DMMA_THREADS, 1)
     half_step_dense_dmma_kernel(const HalfStepArgs a, const HalfDesc d0, const HalfDesc* __restrict__ descs,
                                 const int nhalf, unsigned long long* gbar, const unsigned long long gbar_base) {
@@ -192,6 +197,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   // producer of pair 0).  Tiles whose partners are all local start before it; remote fetches and every
   // store of an accepted row wait for it.
   volatile int* sPeers = sAbort + 1;
+  int32_t* sInbox = reinterpret_cast<int32_t*>(smem_raw + SL::off_inbox_bytes);
   uint64_t* barL = bars;                                  // packed factor landed
   uint64_t* barFull = bars + 1;                           // [pair] TMA: rows of a tile landed
   uint64_t* barReady = bars + 1 + DMMA_CONSUMERS;         // [pair] producer: proposal written
@@ -370,15 +376,35 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         long long* tlq = (tlp && h == nhalf - 1 && (tile - tile0) / tstride < TL_TILES && lane == 0)
                              ? tlp + ((tile - tile0) / tstride) * TL_EVENTS : nullptr;
         if (tlq) tlq[7] = clock64() - t_entry_p;
+        if constexpr (BOUNDED) {
+          // the same pass tests the prior's support: lane (g, t) checks its columns, the 4 lanes of row g AND
+          bool in = true;
 #pragma unroll
-        for (int j = 0; j < KB; ++j) {
-          const double2 s2 = *reinterpret_cast<const double2*>(myS + 8 * j);
-          const double2 c2 = *reinterpret_cast<const double2*>(myC + 8 * j);
-          // stretch.py:33  q = c - (c - s) * zz, each op rounded once (no FMA contraction)
-          double2 q2;
-          q2.x = __dsub_rn(c2.x, __dmul_rn(__dsub_rn(c2.x, s2.x), zz));
-          q2.y = __dsub_rn(c2.y, __dmul_rn(__dsub_rn(c2.y, s2.y), zz));
-          *reinterpret_cast<double2*>(myC + 8 * j) = q2;
+          for (int j = 0; j < KB; ++j) {
+            const double2 s2 = *reinterpret_cast<const double2*>(myS + 8 * j);
+            const double2 c2 = *reinterpret_cast<const double2*>(myC + 8 * j);
+            double2 q2;  // stretch.py:33, as below
+            q2.x = __dsub_rn(c2.x, __dmul_rn(__dsub_rn(c2.x, s2.x), zz));
+            q2.y = __dsub_rn(c2.y, __dmul_rn(__dsub_rn(c2.y, s2.y), zz));
+            *reinterpret_cast<double2*>(myC + 8 * j) = q2;
+            const double2 l2 = __ldg(reinterpret_cast<const double2*>(a.model.lo + 8 * j + 2 * t));
+            const double2 h2 = __ldg(reinterpret_cast<const double2*>(a.model.hi + 8 * j + 2 * t));
+            in &= (l2.x <= q2.x) & (q2.x <= h2.x) & (l2.y <= q2.y) & (q2.y <= h2.y);
+          }
+          in &= __shfl_xor_sync(0xffffffffu, in, 1);
+          in &= __shfl_xor_sync(0xffffffffu, in, 2);
+          if (t == 0) sInbox[(2 * pair + (k & 1u)) * 8 + g] = in ? 1 : 0;  // next to this tile's TileMeta
+        } else {
+#pragma unroll
+          for (int j = 0; j < KB; ++j) {
+            const double2 s2 = *reinterpret_cast<const double2*>(myS + 8 * j);
+            const double2 c2 = *reinterpret_cast<const double2*>(myC + 8 * j);
+            // stretch.py:33  q = c - (c - s) * zz, each op rounded once (no FMA contraction)
+            double2 q2;
+            q2.x = __dsub_rn(c2.x, __dmul_rn(__dsub_rn(c2.x, s2.x), zz));
+            q2.y = __dsub_rn(c2.y, __dmul_rn(__dsub_rn(c2.y, s2.y), zz));
+            *reinterpret_cast<double2*>(myC + 8 * j) = q2;
+          }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(barReady + pair);
@@ -440,7 +466,9 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
 
       // ---- y = L^T (q - mu) on the tensor pipe; rs = sum_n y_n^2
       const double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, g, t);
-      const double lp_new = -0.5 * rs;
+      // outside the prior's support: -inf.  The predicate is read only now, so nothing extra is live across the
+      // DMMA block; the record stays valid until this warp releases the NEXT tile's slot (two records in flight)
+      const double lp_new = (BOUNDED && sInbox[(2 * pair + (k & 1u)) * 8 + g] == 0) ? -INFINITY : -0.5 * rs;
       if (tlk) tlk[4] = clock64() - t_entry;
 
       // ---- guards (ensemble.py:476-479, 550-551): a non-finite lp is the only way
@@ -551,7 +579,7 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
     if (!valid) r = rows - 1;
     const double* src = x + (size_t)r * D + 2 * t;
     double q[2 * KB];
-    bool any_inf = false, any_nan = false;
+    bool any_inf = false, any_nan = false, in = true;
 #pragma unroll
     for (int j = 0; j < KB; ++j) {
       const double2 v = __ldcg(reinterpret_cast<const double2*>(src + 8 * j));
@@ -559,7 +587,14 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
       q[2 * j + 1] = v.y;
       any_inf |= isinf(v.x) | isinf(v.y);
       any_nan |= isnan(v.x) | isnan(v.y);
+      if (m.lo != nullptr) {  // the prior's support, the same test as the half-step kernel's producer
+        const double2 l2 = __ldg(reinterpret_cast<const double2*>(m.lo + 8 * j + 2 * t));
+        const double2 h2 = __ldg(reinterpret_cast<const double2*>(m.hi + 8 * j + 2 * t));
+        in &= (l2.x <= v.x) & (v.x <= h2.x) & (l2.y <= v.y) & (v.y <= h2.y);
+      }
     }
+    in &= __shfl_xor_sync(0xffffffffu, in, 1);
+    in &= __shfl_xor_sync(0xffffffffu, in, 2);
     if (valid && any_inf) atomicOr(status, FLAG_INF_PARAM);  // ensemble.py:476-477
     if (valid && any_nan) atomicOr(status, FLAG_NAN_PARAM);  // ensemble.py:478-479
     if (!waited) {
@@ -567,7 +602,7 @@ __global__ void __launch_bounds__(256) logprob_dense_dmma_kernel(const ModelDev 
       waited = true;
     }
     const double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, g, t);
-    const double lp = -0.5 * rs;
+    const double lp = in ? -0.5 * rs : -INFINITY;
     if (valid && t == 0) {
       out[r] = lp;
       if (isnan(lp)) atomicOr(status, FLAG_NAN_LOGPROB);  // ensemble.py:550-551
@@ -598,15 +633,18 @@ cudaError_t launch_t(const HalfStepArgs& a, const HalfDesc& d0, const HalfDesc* 
                      cudaStream_t st) {
   const size_t smem = SmemLayout<KB>::total_bytes;
   const bool has_mean = a.model.s0 != 0.0;  // set by eb_model_set when mu != 0
-  auto kern = has_mean ? half_step_dense_dmma_kernel<KB, true> : half_step_dense_dmma_kernel<KB, false>;
+  const bool bounded = a.model.lo != nullptr;  // set by eb_model_set_bounds
+  auto kern = bounded ? (has_mean ? half_step_dense_dmma_kernel<KB, true, true> : half_step_dense_dmma_kernel<KB, false, true>)
+                      : (has_mean ? half_step_dense_dmma_kernel<KB, true, false> : half_step_dense_dmma_kernel<KB, false, false>);
   // the opt-in to > 48 KB of dynamic shared memory is per device: remember where it has been done
-  static bool configured[2][64] = {};
+  static bool configured[4][64] = {};
+  const int variant = (has_mean ? 1 : 0) + (bounded ? 2 : 0);
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !configured[has_mean][dev]) {
+  if (dev < 0 || dev >= 64 || !configured[variant][dev]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[has_mean][dev] = true;
+    if (dev >= 0 && dev < 64) configured[variant][dev] = true;
   }
   *grid_out = 0;
   if (max_count <= 0 || nhalf <= 0) return cudaSuccess;

@@ -28,6 +28,10 @@ struct ModelDev {
   const double* params;  // device: gauss_dense mu[D], A[D*D]; else unused
   const double* chol;    // device: gauss_dense packed factor for the DMMA kernel (or null)
   double s0, s1;         // rosenbrock a,b ; ring R,sigma
+  // device: the prior's support lo[D] <= x <= hi[D] (eb_model_set_bounds); null when unbounded.  Outside it the
+  // log-probability is -inf; every kernel tests the box on a warp-uniform branch on lo != nullptr
+  const double* lo;
+  const double* hi;
 };
 
 // per-step split description handed to split_table_kernel

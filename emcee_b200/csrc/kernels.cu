@@ -325,7 +325,8 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
   __syncwarp(mask);
 
   // red_blue.py:93 -> ensemble.py:458-553
-  const double lp_new = model_logprob<MODEL>(q, xc, D, g, G, mask, a.model);
+  double lp_new = model_logprob<MODEL>(q, xc, D, g, G, mask, a.model);
+  if (a.model.lo != nullptr && !row_in_box(q, D, g, G, mask, a.model)) lp_new = -INFINITY;
   if (isnan(lp_new) && g == 0) atomicOr(a.status, FLAG_NAN_LOGPROB);
 
   // red_blue.py:96-101
@@ -433,7 +434,8 @@ __global__ void __launch_bounds__(256) logprob_generic_kernel(const ModelDev m, 
     if (!isfinite(v)) flag_nonfinite(v, status);  // ensemble.py:476-479
   }
   __syncwarp(mask);
-  const double lp = model_logprob<MODEL>(q, xc, D, g, G, mask, m);
+  double lp = model_logprob<MODEL>(q, xc, D, g, G, mask, m);
+  if (m.lo != nullptr && !row_in_box(q, D, g, G, mask, m)) lp = -INFINITY;
   if (g == 0) {
     out[r] = lp;
     if (isnan(lp)) atomicOr(status, FLAG_NAN_LOGPROB);  // ensemble.py:550-551

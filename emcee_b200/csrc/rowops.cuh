@@ -53,6 +53,15 @@ __device__ __forceinline__ double model_logprob(const double* __restrict__ x, do
   }
 }
 
+// the prior's support (m.lo != nullptr): true on every lane of the group when lo[e] <= x[e] <= hi[e] for all e of
+// the staged row (a NaN coordinate is outside); callers then select -inf for a row outside the box
+__device__ __forceinline__ bool row_in_box(const double* __restrict__ x, int D, int g, int G, unsigned mask,
+                                           const ModelDev& m) {
+  bool in = true;
+  for (int e = g; e < D; e += G) in &= (__ldg(m.lo + e) <= x[e]) & (x[e] <= __ldg(m.hi + e));
+  return __all_sync(mask, in);
+}
+
 __device__ __forceinline__ void flag_nonfinite(double v, int* status) {
   if (isinf(v)) atomicOr(status, FLAG_INF_PARAM);
   if (isnan(v)) atomicOr(status, FLAG_NAN_PARAM);

@@ -299,6 +299,18 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
         for (int k = 0; k < 4; ++k)  // the proposal replaces the own row: source of the bulk store
           *reinterpret_cast<double2*>(s + 2 * (g + G * k)) = make_double2(q[2 * k], q[2 * k + 1]);
       }
+      // the prior's support: this lane's four chunks against lo / hi at the same indices, then AND over the group
+      bool out_of_box = false;
+      if (a.model.lo != nullptr) {
+        bool in = true;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const double2 l2 = __ldg(reinterpret_cast<const double2*>(a.model.lo + 2 * (g + G * k)));
+          const double2 h2 = __ldg(reinterpret_cast<const double2*>(a.model.hi + 2 * (g + G * k)));
+          in &= (l2.x <= q[2 * k]) & (q[2 * k] <= h2.x) & (l2.y <= q[2 * k + 1]) & (q[2 * k + 1] <= h2.y);
+        }
+        out_of_box = !__all_sync(mask, in);
+      }
       // red_blue.py:93 -> ensemble.py:458-553: the registered models on registers (lane-sequential partial sums,
       // then the xor-shuffle reduction over the walker's lanes: the order depends only on ndim)
       double acc = 0.0;
@@ -331,6 +343,7 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
         }
         lp_new = -group_sum(acc, G, mask);
       }
+      if (out_of_box) lp_new = -INFINITY;
     } else {
       if (MOVE == EB_MOVE_STRETCH) {
         const double* c = buf + ((size_t)1 * R + grp) * RS;
@@ -388,6 +401,7 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
 
       // red_blue.py:93 -> ensemble.py:458-553
       lp_new = model_logprob<MODEL>(s, nullptr, D, g, G, mask, a.model);
+      if (a.model.lo != nullptr && !row_in_box(s, D, g, G, mask, a.model)) lp_new = -INFINITY;  // the prior's support
     }
     if (isnan(lp_new) && g == 0) atomicOr(a.status, FLAG_NAN_LOGPROB);
     // red_blue.py:96-101

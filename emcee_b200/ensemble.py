@@ -118,7 +118,7 @@ class EnsembleSampler(object):
         self._device = int(device)
         self._engine = _lib.Engine(self.nwalkers, self.ndim, _seed_from_numpy() if seed is None else seed,
                                    device=device)
-        self._engine.set_model(log_prob_fn.kind, log_prob_fn.device_params(self.ndim))
+        self._load_model()
         self._random = DeviceRandom(self._engine)
         self._pinned = None
         if pinned_results:
@@ -141,6 +141,15 @@ class EnsembleSampler(object):
                 self._previous_state = self.get_last_sample()
             else:
                 self._previous_state = None
+
+    def _load_model(self):
+        # the registered model, then its prior support (models.Bounded): a box is part of the model,
+        # so a rebuilt engine (__setstate__) gets it back too
+        m = self.log_prob_fn
+        self._engine.set_model(m.kind, m.device_params(self.ndim))
+        box = m.bounds(self.ndim)
+        if box is not None:
+            self._engine.set_bounds(*box)
 
     # ------------------------------------------------------------------ state
     @property
@@ -189,7 +198,7 @@ class EnsembleSampler(object):
         pinned = d.pop("_saved_pinned")
         self.__dict__.update(d)
         self._engine = _lib.Engine(self.nwalkers, self.ndim, seed, device=self._device)
-        self._engine.set_model(self.log_prob_fn.kind, self.log_prob_fn.device_params(self.ndim))
+        self._load_model()
         self._engine.set_rng(seed, step)
         self._random = DeviceRandom(self._engine)
         self._pinned = None

@@ -11,7 +11,7 @@ callable, so no code path can silently evaluate a model on the host.
 
 import numpy as np
 
-__all__ = ["DeviceModel", "GaussianIso", "GaussianDense", "Rosenbrock", "Ring"]
+__all__ = ["DeviceModel", "GaussianIso", "GaussianDense", "Rosenbrock", "Ring", "Bounded"]
 
 
 class DeviceModel(object):
@@ -20,6 +20,11 @@ class DeviceModel(object):
     def device_params(self, ndim):
         """flat float64 parameter vector for ``eb_model_set``"""
         raise NotImplementedError
+
+    def bounds(self, ndim):
+        """``(lower, upper)`` of the prior's support for ``eb_model_set_bounds``, or None
+        (unbounded)"""
+        return None
 
     def __call__(self, *a, **k):
         raise TypeError(
@@ -81,3 +86,54 @@ class Ring(DeviceModel):
 
     def device_params(self, ndim):
         return np.array([self.radius, self.sigma])
+
+
+class Bounded(DeviceModel):
+    """``model`` restricted to the closed box ``lower <= x <= upper``: the log-probability
+    is the model's value inside the box and exactly ``-inf`` outside, which is what the
+    usual emcee prior ::
+
+        def log_prior(theta):
+            if not ((lower <= theta) & (theta <= upper)).all():
+                return -np.inf
+            return 0.0
+
+    adds to a log-likelihood.  The bounds are the prior's support, not a
+    reparametrisation: walkers move in the same coordinates, proposals outside the
+    box are rejected (``red_blue.py:96-101`` with ``lp = -inf``), and walkers that
+    start outside have ``log_prob = -inf`` until they accept a proposal inside.
+
+    ``lower`` / ``upper`` are scalars (broadcast to every parameter) or vectors of
+    length ``ndim``; ``-inf`` / ``+inf`` give one-sided bounds.  NaN bounds and
+    ``lower >= upper`` are refused with ValueError.  Every kernel that evaluates
+    the model applies the box, and inside it the values are bit-identical to the
+    unbounded model."""
+
+    def __init__(self, model, lower, upper):
+        if not isinstance(model, DeviceModel) or isinstance(model, Bounded):
+            raise TypeError("Bounded wraps one of the registered device models (not another Bounded)")
+        self.model = model
+        self.kind = model.kind
+        lo = np.array(lower, dtype=np.float64)
+        hi = np.array(upper, dtype=np.float64)
+        for name, v in (("lower", lo), ("upper", hi)):
+            if v.ndim > 1:
+                raise ValueError("%s must be a scalar or a vector of length ndim" % name)
+            if np.isnan(v).any():
+                raise ValueError("%s bound must not be NaN" % name)
+        if lo.ndim == 1 and hi.ndim == 1 and lo.shape != hi.shape:
+            raise ValueError("lower and upper have different lengths (%d, %d)" % (lo.size, hi.size))
+        if not (lo < hi).all():
+            raise ValueError("every lower bound must be below its upper bound")
+        self.lower, self.upper = lo, hi
+
+    def device_params(self, ndim):
+        return self.model.device_params(ndim)
+
+    def bounds(self, ndim):
+        out = []
+        for name, v in (("lower", self.lower), ("upper", self.upper)):
+            if v.ndim == 1 and v.shape != (ndim,):
+                raise ValueError("%s bound has length %d but ndim = %d" % (name, v.size, ndim))
+            out.append(np.ascontiguousarray(np.broadcast_to(v, (ndim,)), dtype=np.float64))
+        return out[0], out[1]

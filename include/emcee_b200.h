@@ -103,6 +103,14 @@ const char* eb_last_error(const eb_ctx* ctx);
 /* ---- model ------------------------------------------------------------- */
 /* replaces passing log_prob_fn/args/kwargs (ensemble.py:79-98,169-171). */
 int eb_model_set(eb_ctx* ctx, int kind, const double* params, size_t nparams);
+/* the prior's support, a closed box: lower[ndim], upper[ndim] (host, read during
+ * the call).  The log-probability of x becomes the model's value when
+ * lower[k] <= x[k] <= upper[k] for every k and exactly -inf otherwise, on every
+ * kernel (the `if not in box: return -np.inf` of a log_prior).  -inf / +inf
+ * bounds give one-sided boxes; NaN bounds and lower[k] >= upper[k] are refused
+ * (EB_ERR_INVALID).  NULL, NULL clears the box.  Needs a model (EB_ERR_STATE);
+ * eb_model_set clears the box. */
+int eb_model_set_bounds(eb_ctx* ctx, const double* lower, const double* upper);
 
 /* ---- state (state.py:10-45) ------------------------------------------- */
 /* State(initial_state, copy=True) + the initial compute_log_prob
