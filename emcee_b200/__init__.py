@@ -6,9 +6,9 @@ that the hot path covers."""
 __version__ = "0.1.0"
 
 from . import autocorr, models, moves
-from .backend import Backend
+from .backend import Backend, DeviceBackend
 from .ensemble import EnsembleSampler, walkers_independent
 from .model import Model
 from .state import State
 
-__all__ = ["EnsembleSampler", "walkers_independent", "State", "Model", "Backend", "moves", "models", "autocorr", "__version__"]
+__all__ = ["EnsembleSampler", "walkers_independent", "State", "Model", "Backend", "DeviceBackend", "moves", "models", "autocorr", "__version__"]

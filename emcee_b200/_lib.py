@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-__all__ = ["lib", "Engine", "EngineError", "device_count", "LIB_PATH", "EbMove"]
+__all__ = ["lib", "Engine", "Chain", "EngineError", "device_count", "LIB_PATH", "EbMove"]
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 # EMCEE_B200_LIB: developer override (A/B of two builds); the product always loads the in-tree library
@@ -23,6 +23,7 @@ EB_ERR_CUDA = -2
 EB_ERR_COMM = -3
 EB_ERR_STATE = -4
 EB_ERR_UNSUPPORTED = -5
+EB_ERR_NOMEM = -6
 EB_ERR_NAN_LOGPROB = -10
 EB_ERR_INF_PARAM = -11
 EB_ERR_NAN_PARAM = -12
@@ -82,6 +83,19 @@ _SIGNATURES = {
         C.c_int,
         [C.c_void_p, C.POINTER(EbMove), C.c_size_t, C.c_uint64, C.c_uint64, _dp, _dp, _dp],
     ),
+    "eb_step_store_chain": (
+        C.c_int,
+        [C.c_void_p, C.POINTER(EbMove), C.c_size_t, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64],
+    ),
+    "eb_chain_create": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_void_p)]),
+    "eb_chain_destroy": (C.c_int, [C.c_void_p]),
+    "eb_chain_last_error": (C.c_char_p, [C.c_void_p]),
+    "eb_chain_grow": (C.c_int, [C.c_void_p, C.c_uint64]),
+    "eb_chain_capacity": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_chain_write": (C.c_int, [C.c_void_p, C.c_uint64, _dp, _dp, C.POINTER(C.c_uint8)]),
+    "eb_chain_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, _dp, _dp]),
+    "eb_chain_accepted": (C.c_int, [C.c_void_p, _dp]),
+    "eb_chain_autocorr": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, _dp]),
     "eb_get_naccepted": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "eb_reset_counters": (C.c_int, [C.c_void_p]),
     "eb_move_picks": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_size_t]),
@@ -183,6 +197,97 @@ def _f64(a, shape=None):
     return a
 
 
+def _raise(rc, msg):
+    if rc in (EB_ERR_INVALID, EB_ERR_NAN_LOGPROB, EB_ERR_INF_PARAM, EB_ERR_NAN_PARAM, EB_ERR_NAN_INITIAL):
+        raise ValueError(msg)
+    if rc == EB_ERR_UNSUPPORTED:
+        raise NotImplementedError(msg)
+    if rc == EB_ERR_FEW_WALKERS:
+        raise RuntimeError(msg)
+    if rc == EB_ERR_NOMEM:
+        raise MemoryError(msg)
+    raise EngineError("%s (eb_status %d)" % (msg, rc))
+
+
+class Chain(object):
+    """Thin owner of one ``eb_chain``: a stored chain ``[slots, nwalkers, ndim]`` in device memory
+    (``emcee_b200.DeviceBackend`` builds on it).  Errors map as in :class:`Engine`, and a device
+    allocation that fails or cannot fit raises ``MemoryError``."""
+
+    def __init__(self, nwalkers, ndim, device=0):
+        self._h = C.c_void_p()
+        self.nwalkers, self.ndim, self.device = int(nwalkers), int(ndim), int(device)
+        rc = lib().eb_chain_create(self.device, self.nwalkers, self.ndim, C.byref(self._h))
+        if rc != EB_OK:
+            msg = lib().eb_chain_last_error(None).decode()
+            self._h = C.c_void_p()
+            raise (ValueError if rc == EB_ERR_INVALID else EngineError)(msg)
+
+    def _check(self, rc):
+        if rc != EB_OK:
+            _raise(rc, lib().eb_chain_last_error(self._h).decode())
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            lib().eb_chain_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def grow(self, nslots):
+        """Capacity of at least ``nslots`` stored steps (one new segment for the missing ones)."""
+        self._check(lib().eb_chain_grow(self._h, int(nslots)))
+
+    def capacity(self):
+        """``(slots, device bytes)``."""
+        n, b = C.c_uint64(), C.c_uint64()
+        self._check(lib().eb_chain_capacity(self._h, C.byref(n), C.byref(b)))
+        return int(n.value), int(b.value)
+
+    def write(self, slot, coords, log_prob, accepted=None):
+        coords = _f64(coords, (self.nwalkers, self.ndim))
+        log_prob = _f64(log_prob, (self.nwalkers,))
+        acc = None
+        if accepted is not None:
+            acc = np.ascontiguousarray(accepted, dtype=np.uint8)
+            assert acc.shape == (self.nwalkers,)
+        self._check(
+            lib().eb_chain_write(
+                self._h, int(slot), _as_dp(coords), _as_dp(log_prob),
+                None if acc is None else acc.ctypes.data_as(C.POINTER(C.c_uint8)),
+            )
+        )
+
+    def read(self, first, stride, count, coords=True, log_prob=True):
+        """``(coords[count, nwalkers, ndim] or None, log_prob[count, nwalkers] or None)`` of the slots
+        ``first + k * stride``."""
+        x = np.empty((count, self.nwalkers, self.ndim)) if coords else None
+        lp = np.empty((count, self.nwalkers)) if log_prob else None
+        self._check(
+            lib().eb_chain_read(
+                self._h, int(first), int(stride), int(count),
+                None if x is None else _as_dp(x), None if lp is None else _as_dp(lp),
+            )
+        )
+        return x, lp
+
+    def accepted(self):
+        out = np.empty(self.nwalkers)
+        self._check(lib().eb_chain_accepted(self._h, _as_dp(out)))
+        return out
+
+    def autocorr_function(self, first, stride, count):
+        """Walker-averaged normalised autocorrelation function ``[count, ndim]`` of the stored slice
+        (``eb_chain_autocorr``; the same numbers as :meth:`Engine.autocorr_function` of its host copy)."""
+        out = np.empty((self.ndim, int(count)), dtype=np.float64)
+        self._check(lib().eb_chain_autocorr(self._h, int(first), int(stride), int(count), _as_dp(out)))
+        return np.ascontiguousarray(out.T)
+
+
 class Engine(object):
     """Thin owner of one ``eb_ctx``.  Maps error codes onto the exception types
     the reference raises for the same conditions (``ensemble.py:314-323,
@@ -199,16 +304,8 @@ class Engine(object):
 
     # -- plumbing -------------------------------------------------------------
     def _check(self, rc):
-        if rc == EB_OK:
-            return
-        msg = lib().eb_last_error(self._h).decode()
-        if rc in (EB_ERR_INVALID, EB_ERR_NAN_LOGPROB, EB_ERR_INF_PARAM, EB_ERR_NAN_PARAM, EB_ERR_NAN_INITIAL):
-            raise ValueError(msg)
-        if rc == EB_ERR_UNSUPPORTED:
-            raise NotImplementedError(msg)
-        if rc == EB_ERR_FEW_WALKERS:
-            raise RuntimeError(msg)
-        raise EngineError("%s (eb_status %d)" % (msg, rc))
+        if rc != EB_OK:
+            _raise(rc, lib().eb_last_error(self._h).decode())
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
@@ -365,6 +462,12 @@ class Engine(object):
                 _as_dp(chain), _as_dp(log_prob), _as_dp(accepted),
             )
         )
+
+    def step_store_chain(self, moves, nsteps, thin_by, chain, slot0):
+        """Like :meth:`step_store`, into slots ``slot0, slot0 + 1, ...`` of the device
+        :class:`Chain` ``chain``."""
+        arr = self.pack_moves(moves)
+        self._check(lib().eb_step_store_chain(self._h, arr, len(arr), int(nsteps), int(thin_by), chain._h, int(slot0)))
 
     def naccepted(self):
         out = np.zeros(self.nwalkers, dtype=np.uint64)

@@ -11,7 +11,7 @@ import logging
 
 import numpy as np
 
-__all__ = ["function_1d", "integrated_time", "AutocorrError"]
+__all__ = ["function_1d", "integrated_time", "integrated_time_from_acf", "AutocorrError"]
 
 logger = logging.getLogger(__name__)
 
@@ -59,11 +59,18 @@ def integrated_time(x, c=5, tol=50, quiet=False, has_walkers=True, engine=None):
         x = x[:, None, :] if not has_walkers else x[:, :, None]
     if x.ndim != 3:
         raise ValueError("invalid dimensions")
-    n_t, n_w, n_d = x.shape
     if engine is not None:
         rho = engine.autocorr_function(x)  # [n_t, n_d], walker-averaged on the device
     else:
         rho = np.mean(_acf(x), axis=1)  # [n_t, n_d], walker-averaged
+    return integrated_time_from_acf(rho, c=c, tol=tol, quiet=quiet)
+
+
+def integrated_time_from_acf(rho, c=5, tol=50, quiet=False):
+    """Sokal's automatic window on the walker-averaged autocorrelation function
+    ``rho[n_step, n_param]`` (``autocorr.py:107-123``): ``tau[n_param]``, with the
+    :class:`AutocorrError` / warning of :func:`integrated_time`."""
+    n_t, n_d = rho.shape
     taus = 2.0 * np.cumsum(rho, axis=0) - 1.0
     lags = np.arange(n_t)[:, None]
     inside = lags < c * taus  # Sokal: smallest M with M >= c * tau(M)

@@ -1,7 +1,8 @@
-"""In-memory chain store with the reference's ``Backend`` protocol
+"""Chain stores with the reference's ``Backend`` protocol
 (``src/emcee/backends/backend.py:12-237``): ``reset / grow / save_step /
 get_chain / get_log_prob / get_last_sample / shape / iteration / accepted /
-random_state``.  Blobs do not exist on the device path.
+random_state``.  ``Backend`` keeps the chain in host memory, ``DeviceBackend``
+in the GPU's.  Blobs do not exist on the device path.
 
 The engine's ``eb_step_store`` writes stored steps straight into the
 ``chain`` / ``log_prob`` arrays of this class (pinned double-buffered D2H), so
@@ -11,7 +12,7 @@ import numpy as np
 
 from .state import State
 
-__all__ = ["Backend"]
+__all__ = ["Backend", "DeviceBackend", "slice_plan"]
 
 
 class Backend(object):
@@ -113,3 +114,188 @@ class Backend(object):
 
     def __exit__(self, *exc):
         pass
+
+
+def slice_plan(iteration, discard=0, thin=1):
+    """``(first, stride, count)`` of the stored steps ``get_value`` returns: the indices of
+    ``range(iteration)[discard + thin - 1 : iteration : thin]`` (``backend.py:53``)."""
+    thin = int(thin)
+    if thin < 1:
+        raise ValueError("thin must be >= 1")
+    r = range(int(iteration))[int(discard) + thin - 1 : int(iteration) : thin]
+    return r.start, r.step, len(r)
+
+
+class DeviceBackend(object):
+    """The ``Backend`` protocol with the chain kept in the GPU's memory (``eb_chain``).
+
+    ``EnsembleSampler`` stores into it on the device: a stored step is one
+    copy inside HBM instead of a transfer to the host, ``get_autocorr_time``
+    reads the chain where it is, and only the slice a reader asks for
+    (``get_chain`` / ``get_log_prob`` / ``get_last_sample`` / ``accepted``)
+    crosses PCIe.  Capacity is bounded by device memory, not host RAM: a
+    ``grow`` that cannot fit raises ``MemoryError``.
+
+    Nothing is allocated before ``reset`` (the sampler calls it), so the
+    object can be built without a GPU.  ``close()`` frees the device memory;
+    pickling downloads the contents, and loading uploads them again.
+    Blobs and chains other than float64 are not supported."""
+
+    def __init__(self, dtype=None, device=0):
+        self.initialized = False
+        self.dtype = np.float64 if dtype is None else dtype
+        if np.dtype(self.dtype) != np.float64:
+            raise NotImplementedError("the device path stores float64 chains only")
+        self.device = int(device)
+        self._chain = None
+        self._closed = False
+
+    @property
+    def _ch(self):
+        if self._closed:
+            raise ValueError("this DeviceBackend was closed")
+        return self._chain
+
+    def reset(self, nwalkers, ndim):
+        from . import _lib
+
+        if self._closed:
+            raise ValueError("this DeviceBackend was closed")
+        self._free()
+        self.nwalkers, self.ndim = int(nwalkers), int(ndim)
+        self.iteration = 0
+        self.random_state = None
+        self._chain = _lib.Chain(self.nwalkers, self.ndim, self.device)
+        self.initialized = True
+
+    def _free(self):
+        if self._chain is not None:
+            self._chain.close()
+            self._chain = None
+
+    def close(self):
+        """Free the device memory; any later use raises ``ValueError``."""
+        self._free()
+        self._closed = True
+        self.initialized = False
+
+    @property
+    def nbytes(self):
+        """Device bytes the chain holds."""
+        return 0 if self._chain is None else self._chain.capacity()[1]
+
+    def has_blobs(self):
+        return False
+
+    @property
+    def shape(self):
+        if self._ch is None:
+            raise AttributeError("shape: the backend has not been reset")
+        return self.nwalkers, self.ndim
+
+    @property
+    def accepted(self):
+        """Per-walker accepted proposals of the stored steps (float64, ``backend.py:31``), downloaded."""
+        return self._ch.accepted()
+
+    # -- growth / writes ------------------------------------------------------
+    def grow(self, ngrow, blobs):
+        """Room for ``ngrow`` more stored steps (``backend.py:164-185``): one new device segment for
+        exactly the missing slots; stored steps are never copied."""
+        if blobs is not None:
+            raise NotImplementedError("blobs are not supported on the device path")
+        self._ch.grow(self.iteration + int(ngrow))
+
+    def save_step(self, state, accepted):
+        """Append one step (``backend.py:214-231``), uploaded to the device."""
+        ch = self._ch
+        if state.coords.shape != self.shape:
+            raise ValueError("invalid coordinate dimensions; expected {0}".format(self.shape))
+        if state.log_prob.shape != (self.nwalkers,):
+            raise ValueError("invalid log probability size; expected {0}".format(self.nwalkers))
+        if accepted.shape != (self.nwalkers,):
+            raise ValueError("invalid acceptance size; expected {0}".format(self.nwalkers))
+        if state.blobs is not None:
+            raise NotImplementedError("blobs are not supported on the device path")
+        ch.write(self.iteration, state.coords, state.log_prob, accepted)
+        self.random_state = state.random_state
+        self.iteration += 1
+
+    # -- reads ---------------------------------------------------------------
+    def _plan(self, discard, thin):
+        ch = self._ch
+        if (not self.initialized) or self.iteration <= 0:
+            raise AttributeError(
+                "you must run the sampler with 'store == True' before accessing the results"
+            )
+        return ch, slice_plan(self.iteration, discard, thin)
+
+    def get_value(self, name, flat=False, thin=1, discard=0):
+        ch, (first, stride, count) = self._plan(discard, thin)
+        if name == "blobs":
+            return None
+        if name not in ("chain", "log_prob"):
+            raise AttributeError(name)
+        want_chain = name == "chain"
+        x, lp = ch.read(first, stride, count, coords=want_chain, log_prob=not want_chain)
+        v = x if want_chain else lp
+        if flat:
+            return v.reshape((v.shape[0] * v.shape[1],) + v.shape[2:])
+        return v
+
+    def get_chain(self, **kwargs):
+        """``[nsteps, nwalkers, ndim]`` (or flattened over walkers), downloaded."""
+        return self.get_value("chain", **kwargs)
+
+    def get_log_prob(self, **kwargs):
+        return self.get_value("log_prob", **kwargs)
+
+    def get_blobs(self, **kwargs):
+        return self.get_value("blobs", **kwargs)
+
+    def get_last_sample(self):
+        ch, _ = self._plan(0, 1)
+        x, lp = ch.read(self.iteration - 1, 1, 1)
+        return State(x[0], log_prob=lp[0], blobs=None, random_state=self.random_state)
+
+    def get_autocorr_time(self, discard=0, thin=1, **kwargs):
+        """Integrated autocorrelation time per parameter, in steps (``backend.py:130-150``): the
+        FFTs read the stored slice in device memory (``eb_chain_autocorr``)."""
+        from . import autocorr
+
+        ch, (first, stride, count) = self._plan(discard, thin)
+        rho = ch.autocorr_function(first, stride, count)
+        return thin * autocorr.integrated_time_from_acf(rho, **kwargs)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        pass
+
+    # -- pickling: the contents travel through the host ---------------------------
+    def __getstate__(self):
+        d = dict(dtype=self.dtype, device=self.device, closed=self._closed, initialized=self.initialized)
+        if self.initialized:
+            d.update(nwalkers=self.nwalkers, ndim=self.ndim, iteration=self.iteration,
+                     random_state=self.random_state, accepted=self.accepted)
+            x, lp = self._chain.read(0, 1, self.iteration) if self.iteration else (None, None)
+            d.update(chain=x, log_prob=lp)
+        return d
+
+    def __setstate__(self, d):
+        self.__init__(d["dtype"], d["device"])
+        if d["initialized"]:
+            self.reset(d["nwalkers"], d["ndim"])
+            it = d["iteration"]
+            self.grow(it, None)
+            acc = d["accepted"]
+            if not np.all((acc == np.floor(acc)) & (acc >= 0) & (acc <= it)):
+                raise ValueError("accept counts must be integers in [0, iteration]")
+            # the chain only adds accept masks: slot k adds (count > k), which sums to count over the slots
+            for k in range(it):
+                self._chain.write(k, d["chain"][k], d["log_prob"][k], acc > k)
+            self.iteration = it
+            self.random_state = d["random_state"]
+        if d["closed"]:
+            self.close()

@@ -9,10 +9,32 @@
 #include <string>
 #include <vector>
 
+#include "chain_map.h"
 #include "comm.h"
 #include "engine.cuh"
 
 using namespace eb;
+
+// a stored chain in device memory (eb_chain_*): segments of [n, N, D] coords and [n, N] log-probs, one per grow
+struct ChainSeg {
+  double* x = nullptr;
+  double* lp = nullptr;
+};
+
+struct eb_chain {
+  int device = 0;
+  int sm_count = 0;
+  int64_t N = 0;
+  int D = 0;
+  size_t xs = 0, ls = 0;  // slot pitches in doubles: N * D and N rounded up to even (16-byte aligned slots)
+  size_t max_pitch = 0;   // cudaMemcpy2D limit; larger strides are copied row by row
+  cudaStream_t st = nullptr;
+  std::vector<ChainSeg> segs;
+  std::vector<uint64_t> start{0};  // segment s holds slots [start[s], start[s + 1])
+  double* accepted = nullptr;      // [N] float64 (backend.py:31)
+  uint8_t* mask = nullptr;         // [N] eb_chain_write's accept mask
+  std::string err;
+};
 
 struct eb_ctx {
   int device = 0;
@@ -1262,6 +1284,306 @@ int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nstep
   return r1;
 }
 
+}  // extern "C"
+
+namespace {
+
+// rows of `width` bytes at pitches dpitch / spitch: one 2D copy, or one copy per row past the 2D pitch limit
+cudaError_t copy_rows(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height,
+                      cudaMemcpyKind kind, size_t max_pitch, cudaStream_t st) {
+  if (height == 1 || (dpitch <= max_pitch && spitch <= max_pitch))
+    return cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, kind, st);
+  for (size_t r = 0; r < height; ++r) {
+    cudaError_t e = cudaMemcpyAsync((char*)dst + r * dpitch, (const char*)src + r * spitch, width, kind, st);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+int chain_check_slice(eb_chain* ch, const char* who, uint64_t first, uint64_t stride, uint64_t count) {
+  if (!for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+                          [](size_t, uint64_t, uint64_t, uint64_t) {}))
+    FAIL(ch, EB_ERR_INVALID, "%s: slots %llu + k * %llu, k < %llu, out of range (capacity %llu slots, stride >= 1)",
+         who, (unsigned long long)first, (unsigned long long)stride, (unsigned long long)count,
+         (unsigned long long)ch->start.back());
+  return EB_OK;
+}
+
+// the device part of autocorr.integrated_time over walker slabs of ~1 GiB: fill(xin, w0, wn) enqueues
+// chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd] for every t on stream st
+template <class Obj, class Fill>
+int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, size_t nd, double* acf, Fill&& fill) {
+  if (n_t > ((size_t)1 << 26) || nw * nd > ((size_t)1 << 31))
+    FAIL(c, EB_ERR_UNSUPPORTED, "%s: chain too long (n_step <= 2^26)", who);
+  const int M = acf_fft_length(n_t);
+  // slab of walkers sized to ~1 GiB of scratch (at least one walker)
+  const size_t per_walker = acf_bytes_per_series(n_t) * nd;
+  size_t wb = ((size_t)1 << 30) / per_walker;
+  wb = std::max<size_t>(1, std::min(wb, nw));
+  const size_t S = wb * nd;
+  double *xin = nullptr, *mean = nullptr, *f = nullptr;
+  double2 *z = nullptr, *tw = nullptr;
+  auto release = [&]() {
+    cudaFree(xin);
+    cudaFree(mean);
+    cudaFree(f);
+    cudaFree(z);
+    cudaFree(tw);
+  };
+#define AC(call)                                                                             \
+  do {                                                                                       \
+    cudaError_t _e = (call);                                                                 \
+    if (_e != cudaSuccess) {                                                                 \
+      cudaGetLastError();                                                                    \
+      release();                                                                             \
+      FAIL(c, EB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
+    }                                                                                        \
+  } while (0)
+  AC(cudaMalloc(&xin, n_t * S * sizeof(double)));
+  AC(cudaMalloc(&mean, S * sizeof(double)));
+  AC(cudaMalloc(&f, nd * n_t * sizeof(double)));
+  AC(cudaMalloc(&z, S * (size_t)M * sizeof(double2)));
+  AC(cudaMalloc(&tw, (size_t)std::max(1, M / 2) * sizeof(double2)));
+  AC(cudaMemsetAsync(f, 0, nd * n_t * sizeof(double), st));
+  AC(launch_acf_twiddles(tw, M, st));
+  for (size_t w0 = 0; w0 < nw; w0 += wb) {
+    const size_t wn = std::min(wb, nw - w0);
+    AC(fill(xin, w0, wn));
+    AC(launch_acf_slab(xin, (int)n_t, (int)wn, (int)nd, M, tw, z, mean, f, st));
+  }
+  AC(launch_acf_scale(f, nd * n_t, 1.0 / (double)nw, st));  // autocorr.py:106  f /= n_w
+  AC(cudaMemcpyAsync(acf, f, nd * n_t * sizeof(double), cudaMemcpyDeviceToHost, st));
+  AC(cudaStreamSynchronize(st));
+#undef AC
+  release();
+  return EB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
+                        eb_chain* ch, uint64_t slot0) {
+  if (!c) return EB_ERR_INVALID;
+  if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
+  if (!ch) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: null chain");
+  if (ch->device != c->device || ch->N != c->N || ch->D != c->D)
+    FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: the chain is [%lld, %d] on device %d, the engine [%lld, %d] on device %d",
+         (long long)ch->N, ch->D, ch->device, (long long)c->N, c->D, c->device);
+  if (c->comm.nranks > 1)
+    FAIL(c, EB_ERR_UNSUPPORTED,
+         "eb_step_store_chain: a stored step holds every walker, and sharded ensembles replicate the other ranks' "
+         "rows before each stored step only for host chains (eb_step_store); device chains are not sharded");
+  const uint64_t nstore = nsteps / thin_by;
+  if (nstore > 0 && (slot0 >= ch->start.back() || nstore > ch->start.back() - slot0))
+    FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: slots [%llu, %llu) out of range (capacity %llu slots)",
+         (unsigned long long)slot0, (unsigned long long)(slot0 + nstore), (unsigned long long)ch->start.back());
+  int rc = step_preflight(c);
+  if (rc) return rc;
+  Schedule s;
+  rc = build_schedule(c, moves, nmoves, s);
+  if (rc) return rc;
+  const size_t nx = (size_t)c->N * c->D;
+  uint64_t slot = slot0;
+  size_t seg = 0;
+  // no host synchronisation per stored step: the store kernel is enqueued behind the step on the engine's
+  // stream, and run_steps synchronises once at its end
+  return run_steps(c, s, nsteps, thin_by, [&](uint64_t k) -> int {
+    if ((k + 1) % thin_by != 0) return EB_OK;  // ensemble.py:416
+    while (slot >= ch->start[seg + 1]) ++seg;
+    const uint64_t off = slot - ch->start[seg];
+    c->chain_ok = false;
+    CK(c, launch_chain_store(c->coords, c->logp, c->accepted, ch->segs[seg].x + off * ch->xs,
+                             ch->segs[seg].lp + off * ch->ls, ch->accepted, nx, (size_t)c->N, c->N, c->sm_count, c->st));
+    ++slot;
+    return EB_OK;
+  });
+}
+
+const char* eb_chain_last_error(const eb_chain* ch) { return ch ? ch->err.c_str() : g_create_err.c_str(); }
+
+int eb_chain_create(int device, int64_t nwalkers, int64_t ndim, eb_chain** out) {
+  if (!out) return EB_ERR_INVALID;
+  *out = nullptr;
+  if (nwalkers < 2 || ndim < 1 || nwalkers > (int64_t)0x7fffffff || ndim > 16384) {
+    g_create_err = "eb_chain_create: need 2 <= nwalkers < 2^31 and 1 <= ndim <= 16384";
+    return EB_ERR_INVALID;
+  }
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    g_create_err = std::string("eb_chain_create: no CUDA device (") + cudaGetErrorString(e) +
+                   "); this engine has no CPU fallback";
+    return EB_ERR_CUDA;
+  }
+  if (device < 0 || device >= ndev) {
+    g_create_err = "eb_chain_create: device index out of range";
+    return EB_ERR_INVALID;
+  }
+  eb_chain* ch = new eb_chain();
+  ch->device = device;
+  ch->N = nwalkers;
+  ch->D = (int)ndim;
+  ch->xs = ((size_t)nwalkers * (size_t)ndim + 1) & ~(size_t)1;
+  ch->ls = ((size_t)nwalkers + 1) & ~(size_t)1;
+  auto fail = [&](const char* what, cudaError_t err) {
+    g_create_err = std::string("eb_chain_create: ") + what + ": " + cudaGetErrorString(err);
+    cudaGetLastError();
+    eb_chain_destroy(ch);
+    return EB_ERR_CUDA;
+  };
+#define CC(call)                                   \
+  do {                                             \
+    cudaError_t _e = (call);                       \
+    if (_e != cudaSuccess) return fail(#call, _e); \
+  } while (0)
+  CC(cudaSetDevice(device));
+  int v = 0;
+  CC(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device));
+  ch->sm_count = v;
+  CC(cudaDeviceGetAttribute(&v, cudaDevAttrMaxPitch, device));
+  ch->max_pitch = (size_t)v;
+  CC(cudaStreamCreateWithFlags(&ch->st, cudaStreamNonBlocking));
+  CC(cudaMalloc(&ch->accepted, (size_t)nwalkers * sizeof(double)));
+  CC(cudaMalloc(&ch->mask, (size_t)nwalkers));
+  CC(cudaMemsetAsync(ch->accepted, 0, (size_t)nwalkers * sizeof(double), ch->st));
+  CC(cudaStreamSynchronize(ch->st));
+#undef CC
+  *out = ch;
+  return EB_OK;
+}
+
+int eb_chain_destroy(eb_chain* ch) {
+  if (!ch) return EB_OK;
+  cudaSetDevice(ch->device);
+  if (ch->st) cudaStreamSynchronize(ch->st);
+  for (ChainSeg& s : ch->segs) {
+    cudaFree(s.x);
+    cudaFree(s.lp);
+  }
+  cudaFree(ch->accepted);
+  cudaFree(ch->mask);
+  if (ch->st) cudaStreamDestroy(ch->st);
+  cudaGetLastError();
+  delete ch;
+  return EB_OK;
+}
+
+int eb_chain_grow(eb_chain* ch, uint64_t nslots) {
+  if (!ch) return EB_ERR_INVALID;
+  const uint64_t have = ch->start.back();
+  if (nslots <= have) return EB_OK;
+  CK(ch, cudaSetDevice(ch->device));
+  const uint64_t add = nslots - have;
+  const size_t per_slot = (ch->xs + ch->ls) * sizeof(double);
+  size_t free_b = 0, total_b = 0;
+  CK(ch, cudaMemGetInfo(&free_b, &total_b));
+  if (add > total_b / per_slot)  // decided before any allocation
+    FAIL(ch, EB_ERR_NOMEM,
+         "eb_chain_grow: %llu more slots need %.0f bytes, more than the device's %zu bytes in total (%zu free)",
+         (unsigned long long)add, (double)add * (double)per_slot, total_b, free_b);
+  ChainSeg seg;
+  cudaError_t e = cudaMalloc(&seg.x, add * ch->xs * sizeof(double));
+  if (e == cudaSuccess) e = cudaMalloc(&seg.lp, add * ch->ls * sizeof(double));
+  if (e != cudaSuccess) {  // the chain stays as it was
+    cudaGetLastError();
+    cudaFree(seg.x);
+    cudaMemGetInfo(&free_b, &total_b);
+    FAIL(ch, EB_ERR_NOMEM, "eb_chain_grow: %llu more slots need %zu bytes, %zu bytes free (%s)",
+         (unsigned long long)add, (size_t)add * per_slot, free_b, cudaGetErrorString(e));
+  }
+  ch->segs.push_back(seg);
+  ch->start.push_back(nslots);
+  return EB_OK;
+}
+
+int eb_chain_capacity(const eb_chain* ch, uint64_t* nslots, uint64_t* bytes) {
+  if (!ch) return EB_ERR_INVALID;
+  if (nslots) *nslots = ch->start.back();
+  if (bytes)
+    *bytes = ch->start.back() * (ch->xs + ch->ls) * sizeof(double) + (uint64_t)ch->N * (sizeof(double) + 1);
+  return EB_OK;
+}
+
+int eb_chain_write(eb_chain* ch, uint64_t slot, const double* coords, const double* log_prob,
+                   const uint8_t* accepted) {
+  if (!ch) return EB_ERR_INVALID;
+  if (!coords || !log_prob) FAIL(ch, EB_ERR_INVALID, "eb_chain_write: null buffer");
+  int rc = chain_check_slice(ch, "eb_chain_write", slot, 1, 1);
+  if (rc) return rc;
+  CK(ch, cudaSetDevice(ch->device));
+  const size_t s = (size_t)(std::upper_bound(ch->start.begin(), ch->start.end(), slot) - ch->start.begin()) - 1;
+  const uint64_t off = slot - ch->start[s];
+  const size_t N = (size_t)ch->N;
+  CK(ch, cudaMemcpyAsync(ch->segs[s].x + off * ch->xs, coords, N * ch->D * sizeof(double), cudaMemcpyHostToDevice,
+                         ch->st));
+  CK(ch, cudaMemcpyAsync(ch->segs[s].lp + off * ch->ls, log_prob, N * sizeof(double), cudaMemcpyHostToDevice, ch->st));
+  if (accepted) {
+    CK(ch, cudaMemcpyAsync(ch->mask, accepted, N, cudaMemcpyHostToDevice, ch->st));
+    CK(ch, launch_chain_store(nullptr, nullptr, ch->mask, nullptr, nullptr, ch->accepted, 0, 0, ch->N, ch->sm_count,
+                              ch->st));
+  }
+  CK(ch, cudaStreamSynchronize(ch->st));
+  return EB_OK;
+}
+
+int eb_chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* coords, double* log_prob) {
+  if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_slice(ch, "eb_chain_read", first, stride, count);
+  if (rc) return rc;
+  CK(ch, cudaSetDevice(ch->device));
+  const size_t N = (size_t)ch->N, nx = N * ch->D;
+  cudaError_t e = cudaSuccess;
+  for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+                     [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
+                       if (coords && e == cudaSuccess)
+                         e = copy_rows(coords + k0 * nx, nx * sizeof(double), ch->segs[s].x + off * ch->xs,
+                                       stride * ch->xs * sizeof(double), nx * sizeof(double), n,
+                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st);
+                       if (log_prob && e == cudaSuccess)
+                         e = copy_rows(log_prob + k0 * N, N * sizeof(double), ch->segs[s].lp + off * ch->ls,
+                                       stride * ch->ls * sizeof(double), N * sizeof(double), n,
+                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st);
+                     });
+  CK(ch, e);
+  CK(ch, cudaStreamSynchronize(ch->st));
+  return EB_OK;
+}
+
+int eb_chain_accepted(eb_chain* ch, double* accepted) {
+  if (!ch || !accepted) return EB_ERR_INVALID;
+  CK(ch, cudaSetDevice(ch->device));
+  CK(ch, cudaMemcpyAsync(accepted, ch->accepted, (size_t)ch->N * sizeof(double), cudaMemcpyDeviceToHost, ch->st));
+  CK(ch, cudaStreamSynchronize(ch->st));
+  return EB_OK;
+}
+
+int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* acf) {
+  if (!ch) return EB_ERR_INVALID;
+  if (!acf || count == 0) FAIL(ch, EB_ERR_INVALID, "eb_chain_autocorr: empty chain or null buffer");
+  int rc = chain_check_slice(ch, "eb_chain_autocorr", first, stride, count);
+  if (rc) return rc;
+  CK(ch, cudaSetDevice(ch->device));
+  const size_t nw = (size_t)ch->N, nd = (size_t)ch->D;
+  // the slab is filled from the stored slots in place (one strided copy per run of steps inside a segment), so
+  // the FFT kernels see the numbers eb_autocorr gets from the host copy of the same slice
+  return acf_slabs(ch, "eb_chain_autocorr", ch->st, (size_t)count, nw, nd, acf,
+                   [&](double* xin, size_t w0, size_t wn) {
+                     cudaError_t e = cudaSuccess;
+                     for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+                                        [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
+                                          if (e == cudaSuccess)
+                                            e = copy_rows(xin + k0 * wn * nd, wn * nd * sizeof(double),
+                                                          ch->segs[s].x + off * ch->xs + w0 * nd,
+                                                          stride * ch->xs * sizeof(double), wn * nd * sizeof(double),
+                                                          n, cudaMemcpyDeviceToDevice, ch->max_pitch, ch->st);
+                                        });
+                     return e;
+                   });
+}
+
 int eb_get_naccepted(eb_ctx* c, uint64_t* naccepted) {
   if (!c || !naccepted) return EB_ERR_INVALID;
   CK(c, cudaSetDevice(c->device));
@@ -1378,54 +1700,13 @@ int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, 
 int eb_autocorr(eb_ctx* c, const double* chain, size_t n_t, size_t nw, size_t nd, double* acf) {
   if (!c) return EB_ERR_INVALID;
   if (!chain || !acf || n_t == 0 || nw == 0 || nd == 0) FAIL(c, EB_ERR_INVALID, "eb_autocorr: empty chain or null buffer");
-  if (n_t > ((size_t)1 << 26) || nw * nd > ((size_t)1 << 31))
-    FAIL(c, EB_ERR_UNSUPPORTED, "eb_autocorr: chain too long (n_step <= 2^26)");
   CK(c, cudaSetDevice(c->device));
-  const int M = acf_fft_length(n_t);
-  // slab of walkers sized to ~1 GiB of scratch (at least one walker)
-  const size_t per_walker = acf_bytes_per_series(n_t) * nd;
-  size_t wb = ((size_t)1 << 30) / per_walker;
-  wb = std::max<size_t>(1, std::min(wb, nw));
-  const size_t S = wb * nd;
-  double *xin = nullptr, *mean = nullptr, *f = nullptr;
-  double2 *z = nullptr, *tw = nullptr;
-  auto release = [&]() {
-    cudaFree(xin);
-    cudaFree(mean);
-    cudaFree(f);
-    cudaFree(z);
-    cudaFree(tw);
-  };
-#define AC(call)                                                                             \
-  do {                                                                                       \
-    cudaError_t _e = (call);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      cudaGetLastError();                                                                    \
-      release();                                                                             \
-      FAIL(c, EB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
-    }                                                                                        \
-  } while (0)
-  AC(cudaMalloc(&xin, n_t * S * sizeof(double)));
-  AC(cudaMalloc(&mean, S * sizeof(double)));
-  AC(cudaMalloc(&f, nd * n_t * sizeof(double)));
-  AC(cudaMalloc(&z, S * (size_t)M * sizeof(double2)));
-  AC(cudaMalloc(&tw, (size_t)std::max(1, M / 2) * sizeof(double2)));
   c->chain_ok = false;
-  AC(cudaMemsetAsync(f, 0, nd * n_t * sizeof(double), c->st));
-  AC(launch_acf_twiddles(tw, M, c->st));
-  for (size_t w0 = 0; w0 < nw; w0 += wb) {
-    const size_t wn = std::min(wb, nw - w0);
+  return acf_slabs(c, "eb_autocorr", c->st, n_t, nw, nd, acf, [&](double* xin, size_t w0, size_t wn) {
     // chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd]: one strided copy (rows of the slab are contiguous in a step)
-    AC(cudaMemcpy2DAsync(xin, wn * nd * sizeof(double), chain + w0 * nd, nw * nd * sizeof(double),
-                         wn * nd * sizeof(double), n_t, cudaMemcpyHostToDevice, c->st));
-    AC(launch_acf_slab(xin, (int)n_t, (int)wn, (int)nd, M, tw, z, mean, f, c->st));
-  }
-  AC(launch_acf_scale(f, nd * n_t, 1.0 / (double)nw, c->st));  // autocorr.py:106  f /= n_w
-  AC(cudaMemcpyAsync(acf, f, nd * n_t * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  AC(cudaStreamSynchronize(c->st));
-#undef AC
-  release();
-  return EB_OK;
+    return cudaMemcpy2DAsync(xin, wn * nd * sizeof(double), chain + w0 * nd, nw * nd * sizeof(double),
+                             wn * nd * sizeof(double), n_t, cudaMemcpyHostToDevice, c->st);
+  });
 }
 
 int eb_last_step_timing(const eb_ctx* c, double* ms, uint64_t* launches) {

@@ -170,6 +170,12 @@ cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, c
                             double* mean, double* f, cudaStream_t st);
 cudaError_t launch_acf_scale(double* f, size_t n, double scale, cudaStream_t st);
 
+// ---- device chain storage (chain.cu) ----------------------------------------------------------
+// one stored step: cx[nx] = x[nx], clp[nl] = lp[nl], accepted[N] += acc[N] (acc nullable; nx = nl = 0: only the
+// accept counts).  x, lp, cx, clp 16-byte aligned.
+cudaError_t launch_chain_store(const double* x, const double* lp, const uint8_t* acc, double* cx, double* clp,
+                               double* accepted, size_t nx, size_t nl, int64_t N, int sm_count, cudaStream_t st);
+
 inline int lanes_per_walker(int D) {
   int g = 4;
   while (g < 32 && g * 4 < D) g <<= 1;

@@ -14,7 +14,7 @@ from collections.abc import Iterable
 import numpy as np
 
 from . import _lib
-from .backend import Backend
+from .backend import Backend, DeviceBackend
 from .model import Model
 from .models import DeviceModel
 from .moves import StretchMove
@@ -22,6 +22,12 @@ from .rng import DeviceRandom
 from .state import State
 
 __all__ = ["EnsembleSampler", "walkers_independent"]
+
+
+_NO_SHARDED_DEVICE_CHAIN = (
+    "a DeviceBackend cannot store a sharded ensemble: a stored step holds every walker, and the replication "
+    "of the other ranks' rows before each stored step is built for host chains only; use Backend()"
+)
 
 
 def _seed_from_numpy():
@@ -127,6 +133,11 @@ class EnsembleSampler(object):
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
+        if isinstance(self.backend, DeviceBackend) and self.backend.device != self._device:
+            raise ValueError(
+                "the backend keeps its chain on device {0}, the sampler runs on device {1}".format(
+                    self.backend.device, self._device)
+            )
         if not self.backend.initialized:  # ensemble.py:137-141
             self._previous_state = None
             self.reset()
@@ -217,6 +228,8 @@ class EnsembleSampler(object):
         returned arrays are not refreshed."""
         from . import dist
 
+        if isinstance(self.backend, DeviceBackend):
+            raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
         dist.attach(self._engine, rdv, mode)
         self._rdv = rdv
         self._gather_results = bool(gather_results)
@@ -296,6 +309,9 @@ class EnsembleSampler(object):
                 pbar = None
         if iterations is None and store:
             raise ValueError("'store' must be False when 'iterations' is None")
+        device_store = isinstance(self.backend, DeviceBackend)
+        if device_store and self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
 
         # ``State(initial_state, copy=True)`` in the reference (ensemble.py:312): here the
         # upload to the device IS the copy -- the caller's arrays are only read, and
@@ -335,7 +351,7 @@ class EnsembleSampler(object):
             if store:
                 self.backend.grow(iterations, None)
 
-        native_store = store and type(self.backend) is Backend
+        native_store = store and (type(self.backend) is Backend or device_store)
         sched = self._schedule()
         eng = self._engine
 
@@ -356,7 +372,10 @@ class EnsembleSampler(object):
                 if store:
                     b = self.backend
                     k0, k1 = b.iteration, b.iteration + iterations
-                    eng.step_store(sched, total, checkpoint_step, b.chain[k0:k1], b.log_prob[k0:k1], b.accepted)
+                    if device_store:
+                        eng.step_store_chain(sched, total, checkpoint_step, b._ch, k0)
+                    else:
+                        eng.step_store(sched, total, checkpoint_step, b.chain[k0:k1], b.log_prob[k0:k1], b.accepted)
                     self._after_steps()
                     b.iteration = k1
                     b.random_state = self.random_state
@@ -380,7 +399,10 @@ class EnsembleSampler(object):
             if last_is_checkpoint and native_store:
                 b = self.backend
                 k = b.iteration
-                eng.step_store(sched, yield_step, yield_step, b.chain[k : k + 1], b.log_prob[k : k + 1], b.accepted)
+                if device_store:
+                    eng.step_store_chain(sched, yield_step, yield_step, b._ch, k)
+                else:
+                    eng.step_store(sched, yield_step, yield_step, b.chain[k : k + 1], b.log_prob[k : k + 1], b.accepted)
                 self._after_steps()
                 b.iteration = k + 1
                 b.random_state = self.random_state
@@ -458,9 +480,12 @@ class EnsembleSampler(object):
 
     def get_autocorr_time(self, discard=0, thin=1, **kwargs):
         """Integrated autocorrelation time of the stored chain (``ensemble.py:619-623``
-        -> ``backends/backend.py:130-150``), the FFTs on the GPU (``eb_autocorr``)."""
+        -> ``backends/backend.py:130-150``), the FFTs on the GPU (``eb_autocorr``; a
+        ``DeviceBackend`` is read in place by ``eb_chain_autocorr``)."""
         from . import autocorr
 
+        if isinstance(self.backend, DeviceBackend):
+            return self.backend.get_autocorr_time(discard=discard, thin=thin, **kwargs)
         x = self.get_chain(discard=discard, thin=thin)
         return thin * autocorr.integrated_time(x, engine=self._engine, **kwargs)
 

@@ -35,6 +35,7 @@ typedef enum eb_status {
   EB_ERR_COMM = -3,         /* NCCL / peer-memory failure      -> RuntimeError */
   EB_ERR_STATE = -4,        /* call order (no model, no state) -> RuntimeError */
   EB_ERR_UNSUPPORTED = -5,  /*                                 -> NotImplementedError */
+  EB_ERR_NOMEM = -6,        /* device allocation failed or would not fit -> MemoryError */
   /* device-detected conditions the reference raises as exceptions */
   EB_ERR_NAN_LOGPROB = -10, /* ensemble.py:550-551 "Probability function returned NaN" */
   EB_ERR_INF_PARAM = -11,   /* ensemble.py:476-477 "At least one parameter value was infinite" */
@@ -165,6 +166,54 @@ int eb_step(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
  * incremented per accepted proposal of the stored steps' windows. */
 int eb_step_store(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
                   uint64_t thin_by, double* chain, double* log_prob, double* accepted);
+
+/* ---- device chain storage (backends/backend.py:12-237 kept in HBM) ----- */
+/* A stored chain on one device: coords[slots, nwalkers, ndim], log_prob[slots,
+ * nwalkers] and accepted[nwalkers] (float64, backend.py:31), with its own
+ * stream and error string.  It belongs to no engine: any engine of the same
+ * shape on the same device may store into it (a second sampler on an already
+ * initialised backend appends, ensemble.py:137-162).  Storage is a list of
+ * segments, one per eb_chain_grow; growing never copies stored steps. */
+typedef struct eb_chain eb_chain;
+/* Backend.reset (backend.py:20-36): an empty chain, accepted = 0. */
+int eb_chain_create(int device, int64_t nwalkers, int64_t ndim, eb_chain** out);
+int eb_chain_destroy(eb_chain* ch);
+/* message of the last failing call on ch (ch == NULL: last eb_chain_create
+ * failure of this thread). */
+const char* eb_chain_last_error(const eb_chain* ch);
+/* Backend.grow (backend.py:164-185): capacity becomes nslots by one new segment
+ * for exactly the missing slots (no-op when it already holds nslots).  More than
+ * the device's total memory is refused before any allocation, a failed
+ * allocation leaves the chain as it was: both EB_ERR_NOMEM, naming the requested
+ * and the free bytes. */
+int eb_chain_grow(eb_chain* ch, uint64_t nslots);
+/* slots allocated, and the device bytes the chain holds. */
+int eb_chain_capacity(const eb_chain* ch, uint64_t* nslots, uint64_t* bytes);
+/* eb_step_store into a device chain (ensemble.py:416-417 -> backend.py:214-231):
+ * every thin_by-th step's coords / log_prob go to slots slot0, slot0 + 1, ...
+ * (nsteps / thin_by of them) and its accept mask is added to the chain's
+ * accepted, each by one kernel behind the step on the engine's stream; the call
+ * synchronises once, at its end.  The chain must match the engine's shape and
+ * device; sharded engines are refused (EB_ERR_UNSUPPORTED). */
+int eb_step_store_chain(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
+                        uint64_t thin_by, eb_chain* ch, uint64_t slot0);
+/* Backend.save_step (backend.py:214-231): host coords[nwalkers*ndim] /
+ * log_prob[nwalkers] into slot `slot`, accepted (nullable, nwalkers bytes of 0/1)
+ * added to the chain's counts. */
+int eb_chain_write(eb_chain* ch, uint64_t slot, const double* coords, const double* log_prob,
+                   const uint8_t* accepted);
+/* Backend.get_value (backend.py:42-58): the slots first + k * stride, k < count,
+ * into host coords[count, nwalkers, ndim] / log_prob[count, nwalkers] (either
+ * may be NULL); stride >= 1. */
+int eb_chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count,
+                  double* coords, double* log_prob);
+/* Backend.accepted (backend.py:31,229): accepted[nwalkers] to the host. */
+int eb_chain_accepted(eb_chain* ch, double* accepted);
+/* eb_autocorr of the stored slice first + k * stride, k < count, read where it
+ * is stored: acf[ndim, count], bit-identical to eb_autocorr of the same slice
+ * copied to the host. */
+int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* acf);
+
 /* per-walker number of accepted proposals since creation / eb_reset_counters
  * (numerator of acceptance_fraction, ensemble.py:555-558). */
 int eb_get_naccepted(eb_ctx* ctx, uint64_t* naccepted);
@@ -203,8 +252,9 @@ int eb_autocorr(eb_ctx* ctx, const double* chain, size_t n_step, size_t n_walker
 
 /* ---- measurement / test taps ------------------------------------------- */
 /* device time (ms, CUDA events on the engine's stream) of the last eb_step /
- * eb_step_store call, first launch to last, and the number of kernels it
- * launched. */
+ * eb_step_store / eb_step_store_chain call, first launch to last, and the
+ * number of kernels it launched for the steps (the store kernels of
+ * eb_step_store_chain are not counted, so both store calls report the same). */
 int eb_last_step_timing(const eb_ctx* ctx, double* ms, uint64_t* launches);
 /* draws of the LAST half-step executed (known-answer tests): for each active
  * rank i of that split, partner walker ids (up to 3 per walker: stretch uses
