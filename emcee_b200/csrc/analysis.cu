@@ -181,8 +181,8 @@ __global__ void moments_reduce_kernel(const double* __restrict__ partial, int np
 // power spectrum (order-agnostic), decimation-in-time inverse (bit-reversed in, natural out).
 // Butterflies of span h < ACF_BLOCK / 2 stay inside aligned blocks of ACF_BLOCK points and run in
 // shared memory (one CTA per block: all small-span forward stages, the power spectrum and all
-// small-span inverse stages in one pass); larger spans are one global-memory pass each.
-constexpr int ACF_BLOCK = 8192;  // 128 KB of double2 in shared memory
+// small-span inverse stages in one pass); larger spans are one global-memory pass each.  Every grid is 1-D
+// (acf_grid.h): a slab may hold millions of series, and grid y stops at 65 535.
 
 __device__ __forceinline__ double2 cmul(double2 a, double2 b) {
   return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
@@ -206,12 +206,15 @@ __global__ void acf_mean_kernel(const double* __restrict__ xin, int n_t, int S, 
   mean[s] = acc / (double)n_t;
 }
 
-// z[s][t] = (xin[t][s] - mean[s], 0) for t < n_t, 0 beyond: 32 x 32 tiles through shared memory
+// z[s][t] = (xin[t][s] - mean[s], 0) for t < n_t, 0 beyond: 32 x 32 tiles through shared memory, CTA
+// k = series tile * tiles_t + t tile
 __global__ void __launch_bounds__(256) acf_load_kernel(const double* __restrict__ xin, const double* __restrict__ mean,
-                                                       int n_t, int S, int M, double2* __restrict__ z) {
+                                                       int n_t, int S, int M, unsigned tiles_t,
+                                                       double2* __restrict__ z) {
   __shared__ double tile[32][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const int t0 = blockIdx.x * 32, s0 = blockIdx.y * 32;
+  const unsigned st = blockIdx.x / tiles_t;
+  const int t0 = (int)(blockIdx.x - st * tiles_t) * 32, s0 = (int)st * 32;
   for (int y = ty; y < 32; y += 8) {
     const int t = t0 + y, s = s0 + tx;
     tile[y][tx] = (t < n_t && s < S) ? xin[(size_t)t * S + s] - mean[s] : 0.0;
@@ -247,11 +250,12 @@ __global__ void fft_global_stage_kernel(double2* __restrict__ z, const double2* 
   }
 }
 
-// grid (M / B, S): the stages of span < B of one aligned block of B points, in shared memory
+// the stages of span < B of one aligned block of B points, in shared memory: CTA k holds z[k B, (k + 1) B), block
+// k mod (M / B) of series k / (M / B)
 __global__ void __launch_bounds__(512) fft_local_kernel(double2* __restrict__ z, const double2* __restrict__ tw, int M,
                                                         int B) {
   extern __shared__ double2 sz[];
-  double2* base = z + (size_t)blockIdx.y * M + (size_t)blockIdx.x * B;
+  double2* base = z + (size_t)blockIdx.x * B;
   for (int i = threadIdx.x; i < B; i += blockDim.x) sz[i] = base[i];
   for (int h = B / 2; h >= 1; h >>= 1) {  // forward, decimation in frequency
     __syncthreads();
@@ -286,11 +290,12 @@ __global__ void __launch_bounds__(512) fft_local_kernel(double2* __restrict__ z,
   for (int i = threadIdx.x; i < B; i += blockDim.x) base[i] = sz[i];
 }
 
-// f[d][lag] += sum over the slab's walkers (ascending) of acf[(w, d)][lag] / acf[(w, d)][0]   (autocorr.py:45,105)
+// f[d][lag] += sum over the slab's walkers (ascending) of acf[(w, d)][lag] / acf[(w, d)][0]   (autocorr.py:45,105);
+// CTA k = d * lag_tiles + lag tile
 __global__ void acf_accumulate_kernel(const double2* __restrict__ z, int wb, int nd, int n_t, int M,
-                                      double* __restrict__ f) {
-  const int lag = blockIdx.x * blockDim.x + threadIdx.x;
-  const int d = blockIdx.y;
+                                      unsigned lag_tiles, double* __restrict__ f) {
+  const int d = (int)(blockIdx.x / lag_tiles);
+  const int lag = (int)(blockIdx.x - (unsigned)d * lag_tiles) * blockDim.x + threadIdx.x;
   if (lag >= n_t) return;
   double acc = 0.0;
   for (int w = 0; w < wb; ++w) {
@@ -358,15 +363,6 @@ cudaError_t launch_moments(const double* X, int64_t nrows, int D, const double* 
 
 
 // ---- autocorrelation -------------------------------------------------------------------------
-int acf_fft_length(size_t n_t) {
-  size_t n = 1;
-  while (n < n_t) n <<= 1;  // autocorr.py:12-17 next_pow_two
-  return (int)(2 * n);
-}
-
-// bytes of device scratch per series of the slab: complex work array + its row of the chain slab
-size_t acf_bytes_per_series(size_t n_t) { return (size_t)acf_fft_length(n_t) * sizeof(double2) + n_t * sizeof(double); }
-
 cudaError_t launch_acf_twiddles(double2* tw, int M, cudaStream_t st) {
   acf_twiddle_kernel<<<(M / 2 + 255) / 256, 256, 0, st>>>(tw, M);
   return cudaGetLastError();
@@ -377,18 +373,19 @@ cudaError_t launch_acf_twiddles(double2* tw, int M, cudaStream_t st) {
 cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, const double2* tw, double2* z,
                             double* mean, double* f, cudaStream_t st) {
   const int S = wb * nd;
-  acf_mean_kernel<<<(S + 127) / 128, 128, 0, st>>>(xin, n_t, S, mean);
-  acf_load_kernel<<<dim3((M + 31) / 32, (S + 31) / 32), 256, 0, st>>>(xin, mean, n_t, S, M, z);
-  const int B = M < ACF_BLOCK ? M : ACF_BLOCK;
-  const size_t butterflies = (size_t)S * (M / 2);
-  const unsigned gblocks = (unsigned)((butterflies + 255) / 256);
-  for (int h = M / 2; h >= B; h >>= 1) fft_global_stage_kernel<<<gblocks, 256, 0, st>>>(z, tw, S, M, h, 0);
+  const AcfGrid g = acf_grid(n_t, wb, nd, M);
+  const int B = g.B;
+  acf_mean_kernel<<<(unsigned)g.mean_blocks, 128, 0, st>>>(xin, n_t, S, mean);
+  acf_load_kernel<<<(unsigned)g.load_blocks, 256, 0, st>>>(xin, mean, n_t, S, M, (unsigned)g.load_tiles_t, z);
+  for (int h = M / 2; h >= B; h >>= 1)
+    fft_global_stage_kernel<<<(unsigned)g.global_blocks, 256, 0, st>>>(z, tw, S, M, h, 0);
   const size_t smem = (size_t)B * sizeof(double2);
   cudaError_t e = cudaFuncSetAttribute(fft_local_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  fft_local_kernel<<<dim3(M / B, S), B >= 1024 ? 512 : 128, smem, st>>>(z, tw, M, B);
-  for (int h = B; h <= M / 2; h <<= 1) fft_global_stage_kernel<<<gblocks, 256, 0, st>>>(z, tw, S, M, h, 1);
-  acf_accumulate_kernel<<<dim3((n_t + 255) / 256, nd), 256, 0, st>>>(z, wb, nd, n_t, M, f);
+  fft_local_kernel<<<(unsigned)g.local_blocks, g.local_threads, smem, st>>>(z, tw, M, B);
+  for (int h = B; h <= M / 2; h <<= 1)
+    fft_global_stage_kernel<<<(unsigned)g.global_blocks, 256, 0, st>>>(z, tw, S, M, h, 1);
+  acf_accumulate_kernel<<<(unsigned)g.accumulate_blocks, 256, 0, st>>>(z, wb, nd, n_t, M, (unsigned)g.lag_tiles, f);
   return cudaGetLastError();
 }
 

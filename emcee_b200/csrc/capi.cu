@@ -1316,10 +1316,7 @@ int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, s
   if (n_t > ((size_t)1 << 26) || nw * nd > ((size_t)1 << 31))
     FAIL(c, EB_ERR_UNSUPPORTED, "%s: chain too long (n_step <= 2^26)", who);
   const int M = acf_fft_length(n_t);
-  // slab of walkers sized to ~1 GiB of scratch (at least one walker)
-  const size_t per_walker = acf_bytes_per_series(n_t) * nd;
-  size_t wb = ((size_t)1 << 30) / per_walker;
-  wb = std::max<size_t>(1, std::min(wb, nw));
+  const size_t wb = acf_slab_walkers(n_t, nw, nd);  // slab of walkers sized to ~1 GiB of scratch
   const size_t S = wb * nd;
   double *xin = nullptr, *mean = nullptr, *f = nullptr;
   double2 *z = nullptr, *tw = nullptr;

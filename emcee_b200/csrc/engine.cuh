@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../include/emcee_b200.h"
+#include "acf_grid.h"
 #include "philox.cuh"
 
 namespace eb {
@@ -162,9 +163,8 @@ cudaError_t launch_moments(const double* X, int64_t nrows, int D, const double* 
                            int sm_count, cudaStream_t st, const int32_t* rowidx = nullptr, int skip_start = 0,
                            int skip_count = 0);
 
-// walker-averaged normalised autocorrelation function (autocorr.py:21-46,101-107), slab by slab
-int acf_fft_length(size_t n_t);
-size_t acf_bytes_per_series(size_t n_t);
+// walker-averaged normalised autocorrelation function (autocorr.py:21-46,101-107), slab by slab (geometry:
+// acf_grid.h)
 cudaError_t launch_acf_twiddles(double2* tw, int M, cudaStream_t st);
 cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, const double2* tw, double2* z,
                             double* mean, double* f, cudaStream_t st);

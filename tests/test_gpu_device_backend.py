@@ -225,8 +225,8 @@ def test_autocorr_matches_host_route():
 
 def test_autocorr_wider_than_one_slab_two_segments():
     # 8192 walkers x 8 parameters x 640 steps: ~300 KB of FFT scratch per walker, so a ~1 GiB slab holds
-    # 3573 walkers and the ensemble takes three slabs; two run_mcmc calls make two segments.  (The slab's
-    # series count stays below the 65 536 the FFT kernels' grid takes, which shorter chains would exceed.)
+    # 3573 walkers and the ensemble takes three slabs; two run_mcmc calls make two segments.  (Slabs of more
+    # than 65 535 series are covered by test_gpu_autocorr_exact.py.)
     N, D = 8192, 8
     target, p0 = T.make_config("gauss_iso", N, D)
     make = _sampler_factory(N, D, models.GaussianIso(), None, 0x62)
