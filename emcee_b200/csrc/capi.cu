@@ -664,7 +664,13 @@ int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) 
       const int64_t nc_min = c->N - (c->N + m.nsplits - 1) / std::max(m.nsplits, 1);
       if (m.p0 != floor(m.p0) || m.p0 < 2 || (m.nsplits >= 2 && m.p0 > (double)nc_min))
         FAIL(c, EB_ERR_INVALID, "eb_step: WalkMove needs 2 <= s <= size of the smallest complement (got %g)", m.p0);
-      if ((int64_t)m.p0 != nc_min && !walk_subset_supported(c->D, (int)m.p0))
+      // launch_step_walk picks the kernel per split: a split whose own complement is larger than s runs the
+      // helper-subset kernel, even when s equals the smallest complement (nwalkers not divisible by nsplits).
+      // Complements grow with the split index, so the first and the last split cover every size.
+      const int P = std::max(m.nsplits, 1);
+      const int64_t nc_max = c->N - c->N / P;
+      const bool subset = (int64_t)m.p0 != nc_min || (int64_t)m.p0 != nc_max;
+      if (subset && !walk_subset_supported(c->D, (int)m.p0))
         FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove with a helper subset is limited to ndim <= 64 and s <= 4096");
     }
     if (m.kind == EB_MOVE_WALK && c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove is limited to ndim <= 1024");
