@@ -25,11 +25,12 @@ DE         24, 32, 64, 128   R=8 / 4 / 2 / 1 (G=4 / 8 / 16 / 32)   de24-iso, de3
 DE         256               R=1 (G=32) EPL=8, 13 warps            de256-ring
 snooker    16, 32, 64        R=8 / 4 / 2 (G=4 / 8 / 16) EPL=0      sn16-iso, sn32-ring, sn64-rosen
 snooker    96, 200           R=1 (G=32), 16 and 13 warps           sn96-iso, sn200-ring
+snooker    256               R=1 (G=32) EPL=8, 10 warps            sn256-iso
 any        odd D             generic kernel                        s37-iso-generic
 =========  ================  ====================================  ==========================================
 
 The Rosenbrock register path (its cross-lane ``x[e+1]`` shuffle) and the ring / iso register path run at each of
-G = 2, 4, 8 and 16 (stretch D = 16, 32, 64, 128) and G = 32 (stretch D = 256, DE D = 256).  The ``-aK`` rows have
+G = 2, 4, 8 and 16 (stretch D = 16, 32, 64, 128) and G = 32 (stretch, DE and snooker D = 256).  The ``-aK`` rows have
 an active count of K mod R: partial tiles on the register and OWN_REG paths.  Batch crossings (a warp with more
 than G tiles, so the per-lane walker metadata of a new batch is tabulated mid-loop) are in test_batch_crossing at
 G = 16 and G = 32, sized from the device's SM count.  test_options_bit_identical runs one shape per path under
@@ -100,6 +101,7 @@ CELLS = [
     ("sn64-rosen", "rosenbrock", 413, 64, SN, _tma(2, 0, 0)),
     ("sn96-iso", "gauss_iso", 517, 96, SN, _tma(1, 0, 0)),
     ("sn200-ring", "ring", 806, 200, SN, _tma(1, 0, 0, 13)),
+    ("sn256-iso", "gauss_iso", 1030, 256, SN, _tma(1, 8, 0, 10)),
     ("s37-iso-generic", "gauss_iso", 301, 37, ST, "generic G=16"),
 ]
 
