@@ -108,6 +108,7 @@ struct eb_ctx {
   int pdl = 1;           // dense_dmma launches chain as programmatic dependents (1: one GPU only, 2: sharded too)
   int local_first = 0;  // sharded dense_dmma: local-partner tiles first, peer barrier behind them (0 never, 1 auto, 2 always)
   bool chain_ok = false; // the last operation enqueued on the stream is a dense_dmma kernel of this run
+  HalfDesc dmma_first{}, dmma_last{};  // first and last half-step of the last dense_dmma launch (while chain_ok)
   // multi-GPU: log_prob / accept mask / counters (and, P2P, coords) of rows owned by OTHER ranks are stale
   // on this rank until the next collective read (eb_get_state, eb_get_naccepted, ...) replicates them
   bool replicas_dirty = false;
@@ -951,6 +952,13 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
   // (sharded ensembles: measured slower with the dependent launch -- the early CTAs only add pollers on the
   // peer flags -- so it is opt-in there: option "pdl" = 2)
   const bool pdl = c->chain_ok && grp.nhalf == 1 && (c->comm.nranks > 1 ? c->pdl >= 2 : c->pdl >= 1);
+  // The predecessor ran only earlier splits of the same step, the last one being split - 1: they write only
+  // their own active walkers, so this split's rows may be requested before the predecessor has finished.
+  // Not across a step boundary (a randomised split can write any row), not sharded (peer GPUs write rows too).
+  const HalfDesc& d0 = c->descs_host[grp.first];
+  a.dmma_early_own = pdl && c->comm.nranks == 1 && d0.split > 0 && c->dmma_first.step == d0.step &&
+                     c->dmma_first.order_step == d0.order_step && c->dmma_last.step == d0.step &&
+                     c->dmma_last.split == d0.split - 1;
   int grid = 0;
   CK(c, launch_dense_dmma(a, c->descs_host[grp.first], c->descs_dev + grp.first, grp.nhalf, bound, c->gbar, c->gbar_count, c->sm_count, pdl,
                           &grid, c->st));
@@ -959,6 +967,8 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
   c->dmma_nhalf_max = std::max(c->dmma_nhalf_max, grp.nhalf);
   snprintf(c->last_variant, sizeof(c->last_variant), "dense_dmma nhalf_max=%d grid=%d", c->dmma_nhalf_max, grid);
   c->chain_ok = grid > 0;
+  c->dmma_first = c->descs_host[grp.first];
+  c->dmma_last = c->descs_host[grp.first + grp.nhalf - 1];
   ++launches;
   grp = DmmaGroup{};
   return EB_OK;

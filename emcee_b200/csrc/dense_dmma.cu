@@ -176,8 +176,10 @@ __device__ __forceinline__ bool peer_wait(const unsigned* my_flags, int rank, in
 }
 
 // BOUNDED (the model has a prior support, ModelDev::lo / hi) is a template flag here, unlike in the other kernels:
-// a run-time branch raised the spills of the register-capped D = 128 instantiations (ptxas: 184 -> 208 bytes)
-template <int KB, bool HAS_MEAN, bool BOUNDED>
+// a run-time branch raised the spills of the register-capped D = 128 instantiations (ptxas: 184 -> 208 bytes).
+// TIMELINE (option "dmma_timeline") selects the instrumented instantiation: in the others the cycle stamps and
+// their per-tile branches do not exist, so they cost no registers.
+template <int KB, bool HAS_MEAN, bool BOUNDED, bool TIMELINE>
 __global__ void __launch_bounds__(DMMA_THREADS, 1)
     half_step_dense_dmma_kernel(const HalfStepArgs a, const HalfDesc d0, const HalfDesc* __restrict__ descs,
                                 const int nhalf, unsigned long long* gbar, const unsigned long long gbar_base) {
@@ -228,8 +230,9 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
     bulk_g2s(sL, a.model.chol, bytes, barL);
   }
 
-  const int64_t tstride = (int64_t)gridDim.x * DMMA_CONSUMERS;
-  const int64_t tile0 = (int64_t)blockIdx.x + (int64_t)gridDim.x * pair;  // SM-major deal
+  // tile indices fit 32 bits: a half-step has at most 2^31 / 8 tiles (HalfDesc::a_count is an int32)
+  const int tstride = (int)gridDim.x * DMMA_CONSUMERS;
+  const int tile0 = (int)blockIdx.x + (int)gridDim.x * pair;  // SM-major deal
   double* slot = sSlots + (size_t)pair * SL::slot_doubles;
   double* myS = slot + (size_t)g * RS + 2 * t;  // this lane's 16-byte chunks of row g
   double* myC = myS + 8 * RS;                   // partner row, later the proposal
@@ -242,7 +245,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
     // optional stamps of the LAST half-step, events 6..8 of the tile's record (cycles since this warp entered
     // the kernel): 6 rows requested, 7 rows landed, 8 proposal published
     const long long t_entry_p = clock64();
-    long long* tlp = (a.timeline && lane == 0)
+    long long* tlp = (TIMELINE && lane == 0)
                          ? a.timeline + ((size_t)blockIdx.x * DMMA_CONSUMERS + pair) * TL_TILES * TL_EVENTS : nullptr;
     const double dm1 = (double)a.D - 1.0;
     const int row = lane & 7;
@@ -257,15 +260,15 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       const int32_t* order = a.order + (size_t)d.order_step * a.N;
       const int2 rg = a.range ? a.range[(size_t)d.order_step * MAX_SPLITS + d.split] : make_int2(0, d.a_count);
       const int i_lo = rg.x, i_hi = rg.y;
-      const int64_t ntiles = ((int64_t)i_hi - i_lo + 7) >> 3;
+      const int ntiles = (int)(((int64_t)i_hi - i_lo + 7) >> 3);
       const int64_t Nc = a.N - d.a_count;
       // draws + index lookups: independent of the walker state, so they run ahead of the grid barrier
       const int32_t* aperm = a.aperm ? a.aperm + (size_t)d.order_step * a.N + d.a_start : nullptr;
-      auto prep = [&](int64_t tile, bool with_lp) -> Prep {
+      auto prep = [&](int tile, bool with_lp) -> Prep {
         Prep p;
-        int64_t i = (int64_t)i_lo + tile * 8 + row;
+        int i = i_lo + tile * 8 + row;
         p.valid = i < i_hi;
-        if (!p.valid) i = (int64_t)i_hi - 1;
+        if (!p.valid) i = i_hi - 1;
         if (aperm) i = __ldg(aperm + i);  // sharded: tiles are built partner-local first (locality_table_kernel)
         const u32x4 A = draw_words(a.seed, d.step, (uint32_t)d.split, TAG_PROP_A, (uint32_t)i);
         const double tt = __dadd_rn(__dmul_rn(__dsub_rn(a.p0, 1.0), u53(A.x, A.y)), 1.0);  // stretch.py:30
@@ -300,20 +303,19 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         asm volatile("fence.proxy.async;" ::: "memory");  // peers' generic-proxy writes -> our TMA reads
         return true;
       };
-      // publish the meta record and launch the 16 row copies of one tile into the landing slot
-      auto issue = [&](Prep& p, int par, bool load_lp) -> bool {
-        if (__any_sync(0xffffffffu, p.remote) && !peers_ready()) return false;
-        if (lane == 0) mbar_arrive_expect_tx(barFull + pair, 16u * D * (unsigned)sizeof(double));
-        __syncwarp();
-        if (lane < 16) {
+      // bulk copies of slot rows [lo, hi) of one tile (0..7: the active walkers' own rows, 8..15: their
+      // partners'), counted on the pair's full barrier
+      auto request = [&](const Prep& p, int lo, int hi) {
+        if (lane >= lo && lane < hi) {
           const bool partner = lane >= 8;
-          const int64_t wr = partner ? (int64_t)p.wp : (int64_t)p.w;
+          const int32_t wr = partner ? p.wp : p.w;
           const double* base =
               (partner && a.peer_coords != nullptr) ? a.peer_coords[wr / a.rows_per_rank] : a.coords;
           bulk_g2s(slot + (size_t)(partner ? 8 : 0) * RS + (size_t)row * RS, base + (size_t)wr * D,
                    (unsigned)(D * sizeof(double)), barFull + pair);
         }
-        if (load_lp) p.lp_old = a.logp[p.w];  // behind the row copies: off the post-barrier critical path
+      };
+      auto publish = [&](const Prep& p, int par) {
         TileMeta* m = meta + par;
         if (lane < 8) {
           m->factor[row] = p.factor;
@@ -321,10 +323,32 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
           m->lp_old[row] = p.lp_old;
           m->w[row] = p.valid ? p.w : -1;
         }
+      };
+      // publish the meta record and launch the 16 row copies of one tile into the landing slot
+      auto issue = [&](Prep& p, int par, bool load_lp) -> bool {
+        if (__any_sync(0xffffffffu, p.remote) && !peers_ready()) return false;
+        if (lane == 0) mbar_arrive_expect_tx(barFull + pair, 16u * D * (unsigned)sizeof(double));
+        __syncwarp();
+        request(p, 0, 16);
+        if (load_lp) p.lp_old = a.logp[p.w];  // behind the row copies: off the post-barrier critical path
+        publish(p, par);
         return true;
       };
       Prep cur{}, nxt{};
-      if (tile0 < ntiles) cur = prep(tile0, false);  // (the old log-prob is state: it is read behind the barrier)
+      // a.dmma_early_own: the predecessor ran only earlier splits of the same step on this GPU, which write only
+      // the rows (and log-probs) of THEIR active walkers -- partners of this split.  This split's own rows and
+      // log-probs were final before that kernel started, so the first tile's own rows are requested here, under
+      // its tail; only the partner rows wait for it.
+      const bool early = h == 0 && a.dmma_early_own && tile0 < ntiles;
+      if (early) {
+        cur = prep(tile0, true);
+        if (lane == 0) mbar_arrive_expect_tx(barFull + pair, 16u * D * (unsigned)sizeof(double));
+        __syncwarp();
+        if (tlp) tlp[6] = clock64() - t_entry_p;
+        request(cur, 0, 8);
+      } else if (tile0 < ntiles) {
+        cur = prep(tile0, false);  // (the old log-prob is state: it is read behind the barrier)
+      }
       if (h == 0) {
         // everything above (barrier set-up, factor copy, first draws and index lookups) overlapped the tail of
         // the previous kernel when this one was launched as its programmatic dependent; the state that
@@ -340,12 +364,18 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         // 17 MB burst (132 SMs x 8 slots x 16 KB) during which nobody computes -- and, sharded, a burst on
         // the NVLink ports; with the stagger the second pair of each sub-partition asks only when the first
         // pair's rows are in, so one consumer per sub-partition starts after half the burst.
+        // (Early own rows: the stagger applies to the partner rows, the half of the burst that is left.)
         if (tile0 < ntiles) {
           // (best effort: a bounded peek at the neighbour's barrier, never a dependency)
           if (a.dmma_stagger && pair >= DMMA_CONSUMERS / 2)
             mbar_wait_for(barFull + pair - DMMA_CONSUMERS / 2, 0, multi ? 40000 : 12000);
-          if (tlp) tlp[6] = clock64() - t_entry_p;
-          if (!issue(cur, (int)(k & 1u), true)) return;
+          if (early) {
+            request(cur, 8, 16);
+            publish(cur, (int)(k & 1u));
+          } else {
+            if (tlp) tlp[6] = clock64() - t_entry_p;
+            if (!issue(cur, (int)(k & 1u), true)) return;
+          }
         }
         // pair 0 takes the barrier now if its first tile did not need it (the flags normally arrive while that
         // tile's rows are in flight); the other producers only wait for it inside issue(), when they need it
@@ -369,7 +399,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
           if (!issue(cur, (int)(k & 1u), true)) return;
         }
       }
-      for (int64_t tile = tile0; tile < ntiles; tile += tstride, ++k) {
+      for (int tile = tile0; tile < ntiles; tile += tstride, ++k) {
         // ---- rows of this tile have landed: form the proposal over the partner rows
         const double zz = __shfl_sync(0xffffffffu, cur.zz, g);
         if (!mbar_wait_abortable(barFull + pair, k & 1u, sAbort)) return;
@@ -427,7 +457,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   // optional per-tile timestamps of the LAST half-step (cycles since this warp entered the kernel):
   // 1 wait start, 2 proposal ready, 3 proposal in registers, 4 DMMA block done, 5 tile done
   const long long t_entry = clock64();
-  long long* tl = a.timeline ? a.timeline + ((size_t)blockIdx.x * DMMA_CONSUMERS + pair) * TL_TILES * TL_EVENTS : nullptr;
+  long long* tl = TIMELINE ? a.timeline + ((size_t)blockIdx.x * DMMA_CONSUMERS + pair) * TL_TILES * TL_EVENTS : nullptr;
   pdl_wait();  // nothing of this warp's global traffic may overtake the previous kernel
   pdl_launch_dependents();
   // On an abort a consumer stops working but keeps walking the same sequence of named barriers as its
@@ -436,10 +466,10 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   for (int h = 0; h < nhalf; ++h) {
     const HalfDesc d = (h == 0) ? d0 : descs[h];
     const int2 rg = a.range ? a.range[(size_t)d.order_step * MAX_SPLITS + d.split] : make_int2(0, d.a_count);
-    const int64_t ntiles = ((int64_t)rg.y - rg.x + 7) >> 3;
+    const int ntiles = (int)(((int64_t)rg.y - rg.x + 7) >> 3);
     unsigned kk = 0;
     bool peers_passed = false;
-    for (int64_t tile = tile0; alive && tile < ntiles; tile += tstride, ++k, ++kk) {
+    for (int tile = tile0; alive && tile < ntiles; tile += tstride, ++k, ++kk) {
       const TileMeta* m = meta + (k & 1u);
       long long* tlk = (tl && h == nhalf - 1 && kk < TL_TILES && lane == 0) ? tl + kk * TL_EVENTS : nullptr;
       if (tlk) {
@@ -458,16 +488,17 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         q[2 * j + 0] = q2.x;
         q[2 * j + 1] = q2.y;
       }
-      const int32_t w = m->w[g];
-      const double factor = m->factor[g], log_u = m->log_u[g], lp_old = m->lp_old[g];
       __syncwarp();
-      if (lane == 0) mbar_arrive(barFree + pair);  // slot and meta may be refilled while this tile computes
+      if (lane == 0) mbar_arrive(barFree + pair);  // the slot may be refilled while this tile computes
       if (tlk) tlk[3] = clock64() - t_entry;
 
       // ---- y = L^T (q - mu) on the tensor pipe; rs = sum_n y_n^2
       const double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, g, t);
-      // outside the prior's support: -inf.  The predicate is read only now, so nothing extra is live across the
-      // DMMA block; the record stays valid until this warp releases the NEXT tile's slot (two records in flight)
+      // The tile's meta record and box predicate are read only now, so nothing but q is live across the DMMA
+      // block (ptxas spilled at the 128-register cap while they were); the record stays valid until this warp
+      // releases the NEXT tile's slot (two records in flight).  Outside the prior's support: -inf.
+      const int32_t w = m->w[g];
+      const double factor = m->factor[g], log_u = m->log_u[g], lp_old = m->lp_old[g];
       const double lp_new = (BOUNDED && sInbox[(2 * pair + (k & 1u)) * 8 + g] == 0) ? -INFINITY : -0.5 * rs;
       if (tlk) tlk[4] = clock64() - t_entry;
 
@@ -634,11 +665,17 @@ cudaError_t launch_t(const HalfStepArgs& a, const HalfDesc& d0, const HalfDesc* 
   const size_t smem = SmemLayout<KB>::total_bytes;
   const bool has_mean = a.model.s0 != 0.0;  // set by eb_model_set when mu != 0
   const bool bounded = a.model.lo != nullptr;  // set by eb_model_set_bounds
-  auto kern = bounded ? (has_mean ? half_step_dense_dmma_kernel<KB, true, true> : half_step_dense_dmma_kernel<KB, false, true>)
-                      : (has_mean ? half_step_dense_dmma_kernel<KB, true, false> : half_step_dense_dmma_kernel<KB, false, false>);
+  const bool timeline = a.timeline != nullptr;  // option "dmma_timeline": the instrumented instantiation
+  using Kern = decltype(&half_step_dense_dmma_kernel<KB, false, false, false>);
+  static const Kern kerns[8] = {
+      half_step_dense_dmma_kernel<KB, false, false, false>, half_step_dense_dmma_kernel<KB, true, false, false>,
+      half_step_dense_dmma_kernel<KB, false, true, false>,  half_step_dense_dmma_kernel<KB, true, true, false>,
+      half_step_dense_dmma_kernel<KB, false, false, true>,  half_step_dense_dmma_kernel<KB, true, false, true>,
+      half_step_dense_dmma_kernel<KB, false, true, true>,   half_step_dense_dmma_kernel<KB, true, true, true>};
+  const int variant = (has_mean ? 1 : 0) + (bounded ? 2 : 0) + (timeline ? 4 : 0);
+  const Kern kern = kerns[variant];
   // the opt-in to > 48 KB of dynamic shared memory is per device: remember where it has been done
-  static bool configured[4][64] = {};
-  const int variant = (has_mean ? 1 : 0) + (bounded ? 2 : 0);
+  static bool configured[8][64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !configured[variant][dev]) {

@@ -59,6 +59,9 @@ struct HalfStepArgs {
   int p2p_rank, p2p_nranks;
   unsigned p2p_wait, p2p_signal;
   int dmma_stagger;  // dense_dmma: pairs 4..7 request their first tile only when pairs 0..3's rows have landed
+  // dense_dmma, one half-step per launch on one GPU: the launch is the programmatic dependent of a launch that
+  // ran only earlier splits of the same step, so its own rows and log-probs may be read before griddepcontrol.wait
+  int dmma_early_own;
   int64_t N;
   int D;
   int split;

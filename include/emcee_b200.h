@@ -264,7 +264,8 @@ int eb_last_step_timing(const eb_ctx* ctx, double* ms, uint64_t* launches);
 int eb_debug_taps(eb_ctx* ctx, int64_t* partners, double* scalar, double* u_accept,
                   int64_t* active, int64_t* nactive);
 /* per-tile cycle stamps of the dense_dmma consumers during the LAST half-step
- * launched (option "dmma_timeline"): [SM][8 consumers][8 tiles][6 events]. */
+ * launched (option "dmma_timeline"): [SM][8 consumers][8 tiles][10 events]
+ * (0..5 consumer, 6..8 producer). */
 int eb_debug_timeline(eb_ctx* ctx, int64_t* out, size_t capacity, size_t* written);
 /* engine options: "debug_taps" (0/1: record the draws of each half-step for
  * eb_debug_taps; forces the generic kernel), "dense_dmma" (0/1: allow the
@@ -278,7 +279,7 @@ int eb_debug_timeline(eb_ctx* ctx, int64_t* out, size_t capacity, size_t* writte
  * partner is local and take the peer barrier behind them; 0 never (default: the measured effect changes sign with the
  * number of GPUs), 1 when a consumer warp has at most two tiles per half-step, 2 always), "moments_every" (n >= 0: see
  * eb_moments; setting it resets the accumulators), "dmma_timeline" (0/1: record consumer cycle stamps
- * for eb_debug_timeline), "l2_flush"
+ * for eb_debug_timeline; 1 runs a separately compiled, instrumented kernel), "l2_flush"
  * (0/1: benchmark hygiene -- write a 256 MiB buffer before every step and time
  * each step with its own CUDA-event pair, so eb_last_step_timing excludes the
  * flush). */
