@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-__all__ = ["lib", "Engine", "Chain", "EngineError", "device_count", "LIB_PATH", "EbMove"]
+__all__ = ["lib", "Engine", "Chain", "EngineError", "device_count", "LIB_PATH", "EbMove", "DeviceRows"]
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 # EMCEE_B200_LIB: developer override (A/B of two builds); the product always loads the in-tree library
@@ -24,6 +24,7 @@ EB_ERR_COMM = -3
 EB_ERR_STATE = -4
 EB_ERR_UNSUPPORTED = -5
 EB_ERR_NOMEM = -6
+EB_ERR_CALLBACK = -7
 EB_ERR_NAN_LOGPROB = -10
 EB_ERR_INF_PARAM = -11
 EB_ERR_NAN_PARAM = -12
@@ -34,6 +35,9 @@ EB_COMM_ID_BYTES = 128
 EB_IPC_BLOB_BYTES = 256
 EB_COMM_ALLGATHER = 0
 EB_COMM_P2P = 1
+EB_CALLBACK_HOST = 0
+EB_CALLBACK_DEVICE = 1
+EB_STREAM_UNKNOWN = 2**64 - 1  # eb_callback_result: the producer named no stream -> wait for the whole device
 
 MODEL_KINDS = {"gauss_iso": 0, "gauss_dense": 1, "rosenbrock": 2, "ring": 3}
 MOVE_KINDS = {"stretch": 0, "de": 1, "snooker": 2, "walk": 3, "gaussian": 4}
@@ -63,6 +67,8 @@ class EngineError(RuntimeError):
 
 
 _dp = C.POINTER(C.c_double)
+# eb_logprob_fn: (user, x, m, ndim, lp, stream) -> 0 | non-zero
+LOGPROB_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, _dp, C.c_int64, C.c_int64, _dp, C.c_void_p)
 _SIGNATURES = {
     "eb_abi_version": (C.c_int, []),
     "eb_device_count": (C.c_int, []),
@@ -71,6 +77,8 @@ _SIGNATURES = {
     "eb_last_error": (C.c_char_p, [C.c_void_p]),
     "eb_model_set": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_size_t]),
     "eb_model_set_bounds": (C.c_int, [C.c_void_p, _dp, _dp]),
+    "eb_model_set_callback": (C.c_int, [C.c_void_p, LOGPROB_FN, C.c_void_p, C.c_int]),
+    "eb_callback_result": (C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_set_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_get_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_owned_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
@@ -209,6 +217,95 @@ def _raise(rc, msg):
     raise EngineError("%s (eb_status %d)" % (msg, rc))
 
 
+class DeviceRows(object):
+    """The ``[m, ndim]`` float64 rows a device-mode callback receives: an immutable object with the
+    CUDA Array Interface (v3) whose ``stream`` is the engine's stream; the rows are complete when the
+    function is called, so a consumer that ignores ``stream`` reads them correctly too.  The memory is a scratch copy of the proposals that belongs to the engine: the function may
+    overwrite it (so the interface's read-only flag is False, which torch requires), and it is valid
+    only during the call; afterwards the interface raises ``RuntimeError``."""
+
+    __slots__ = ("_cai",)
+
+    def __init__(self, ptr, m, ndim, stream):
+        self._cai = {"shape": (int(m), int(ndim)), "typestr": "<f8", "data": (int(ptr or 0), False),
+                     "strides": None, "version": 3, "stream": int(stream) if stream else None}
+
+    @property
+    def __cuda_array_interface__(self):
+        if self._cai is None:
+            raise RuntimeError("the rows of a log-probability callback are only valid during the call")
+        return dict(self._cai)
+
+    @property
+    def shape(self):
+        return self.__cuda_array_interface__["shape"]
+
+    def _release(self):
+        self._cai = None
+
+
+def _host_result(out, m):
+    """``out`` as a float64 ``[m]`` array, or the shape / dtype error."""
+    a = np.asarray(out)
+    if a.shape != (m,):
+        raise ValueError("the log-probability function returned shape %s for %d rows; expected (%d,)" % (a.shape, m, m))
+    if a.dtype != np.float64:
+        raise TypeError("the log-probability function must return float64 values, got %s" % a.dtype)
+    return a
+
+
+def _device_result(h, lp, out, m):
+    """Copy a callback's result -- a CUDA-array-interface object or a host array -- into the engine's lp."""
+    cai = getattr(out, "__cuda_array_interface__", None)
+    if cai is None:
+        a = np.ascontiguousarray(_host_result(out, m))
+        ptr, stride, stream = a.ctypes.data, 8, 0
+    else:
+        shape = tuple(cai["shape"])
+        if shape != (m,):
+            raise ValueError("the log-probability function returned shape %s for %d rows; expected (%d,)" % (shape, m, m))
+        if np.dtype(cai["typestr"]) != np.float64:
+            raise TypeError("the log-probability function must return float64 values, got %s" % cai["typestr"])
+        if cai.get("mask") is not None:
+            raise ValueError("masked CUDA arrays are not supported as log-probabilities")
+        strides = cai.get("strides")
+        # a "stream" entry is the producer's word on ordering (None: none needed); without one (interface v2,
+        # which torch exports) the result may still be in flight on any stream, so the engine waits for all
+        stream = (cai["stream"] or 0) if "stream" in cai else EB_STREAM_UNKNOWN
+        ptr, stride = cai["data"][0], 8 if strides is None else strides[0]
+    rc = lib().eb_callback_result(h, lp, C.c_void_p(ptr), int(stride), int(m), int(stream))
+    if rc != EB_OK:
+        _raise(rc, lib().eb_last_error(h).decode())
+
+
+def make_trampoline(h, evaluate, where, failure):
+    """The C callback of one engine: calls ``evaluate`` (host mode: a fresh ``x[m, ndim]`` ndarray the
+    function owns; device mode: :class:`DeviceRows`) and writes its result into the engine's ``lp``.
+    Any exception is stored as ``failure[0]`` and the engine is told to stop (``EB_ERR_CALLBACK``)."""
+
+    def host(user, x, m, ndim, lp, stream):
+        try:
+            rows = np.ctypeslib.as_array(x, shape=(m, ndim)).copy()
+            np.ctypeslib.as_array(lp, shape=(m,))[:] = _host_result(evaluate(rows), m)
+            return 0
+        except BaseException as e:  # noqa: B902 -- re-raised unchanged when the ABI call returns
+            failure[0] = e
+            return 1
+
+    def device(user, x, m, ndim, lp, stream):
+        rows = DeviceRows(C.cast(x, C.c_void_p).value, m, ndim, stream)
+        try:
+            _device_result(h, lp, evaluate(rows), m)
+            return 0
+        except BaseException as e:  # noqa: B902
+            failure[0] = e
+            return 1
+        finally:
+            rows._release()
+
+    return LOGPROB_FN(host if where == EB_CALLBACK_HOST else device)
+
+
 class Chain(object):
     """Thin owner of one ``eb_chain``: a stored chain ``[slots, nwalkers, ndim]`` in device memory
     (``emcee_b200.DeviceBackend`` builds on it).  Errors map as in :class:`Engine`, and a device
@@ -295,6 +392,8 @@ class Engine(object):
 
     def __init__(self, nwalkers, ndim, seed, device=0):
         self._h = C.c_void_p()
+        self._cb = None  # the registered C callback (kept alive while the engine may call it)
+        self._cb_failure = [None]
         self.nwalkers, self.ndim = int(nwalkers), int(ndim)
         rc = lib().eb_create(int(device), self.nwalkers, self.ndim, int(seed) & (2**64 - 1), C.byref(self._h))
         if rc != EB_OK:
@@ -304,6 +403,10 @@ class Engine(object):
 
     # -- plumbing -------------------------------------------------------------
     def _check(self, rc):
+        if rc == EB_ERR_CALLBACK:
+            exc, self._cb_failure[0] = self._cb_failure[0], None
+            if exc is not None:
+                raise exc  # the caller's own exception, with its traceback
         if rc != EB_OK:
             _raise(rc, lib().eb_last_error(self._h).decode())
 
@@ -332,6 +435,15 @@ class Engine(object):
         lo = _f64(np.asarray(lower, dtype=np.float64).ravel(), (self.ndim,))
         hi = _f64(np.asarray(upper, dtype=np.float64).ravel(), (self.ndim,))
         self._check(lib().eb_model_set_bounds(self._h, _as_dp(lo), _as_dp(hi)))
+
+    def set_callback(self, evaluate, where):
+        """Make ``evaluate`` the model (``eb_model_set_callback``): called once per half-step with the
+        split's proposals, ``where`` = ``"host"`` (a fresh ``[m, ndim]`` ndarray) or ``"device"``
+        (:class:`DeviceRows`).  Its exceptions propagate unchanged from the call that ran it."""
+        mode = {"host": EB_CALLBACK_HOST, "device": EB_CALLBACK_DEVICE}[where]
+        cb = make_trampoline(self._h, evaluate, mode, self._cb_failure)
+        self._check(lib().eb_model_set_callback(self._h, cb, None, mode))
+        self._cb = cb
 
     def set_state(self, coords, log_prob=None):
         coords = _f64(coords, (self.nwalkers, self.ndim))

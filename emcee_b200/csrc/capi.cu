@@ -131,10 +131,30 @@ struct eb_ctx {
 
   Comm comm;  // multi-GPU (comm.h)
 
+  // log-probability callback (eb_model_set_callback; model.kind == MODEL_EXTERNAL)
+  eb_logprob_fn cb_fn = nullptr;
+  void* cb_user = nullptr;
+  int cb_where = EB_CALLBACK_HOST;
+  bool in_callback = false;        // every other call on the context is refused while fn runs
+  double* cb_x = nullptr;          // host mode: pinned [cb_rows, D] proposals
+  double* cb_lp = nullptr;         // host mode: pinned [cb_rows] results
+  double* cb_xdev = nullptr;       // device mode: [cb_rows, D] copy of the rows, the function's to overwrite
+  size_t cb_rows = 0;
+  double* ext_f = nullptr;         // device [N] Hastings factors of the propose phase
+  double* ext_lp = nullptr;        // device [N] the callback's log-probabilities
+
   std::string err;
 };
 
 static thread_local std::string g_create_err;
+
+#define NOT_IN_CALLBACK(ctx)                                                      \
+  do {                                                                            \
+    if ((ctx)->in_callback) {                                                     \
+      (ctx)->err = "engine is inside a log-probability callback";                 \
+      return EB_ERR_STATE;                                                        \
+    }                                                                             \
+  } while (0)
 
 #define FAIL(ctx, code, ...)                      \
   do {                                            \
@@ -262,6 +282,7 @@ int eb_create(int device, int64_t nwalkers, int64_t ndim, uint64_t seed, eb_ctx*
 
 int eb_destroy(eb_ctx* c) {
   if (!c) return EB_OK;
+  NOT_IN_CALLBACK(c);
   cudaSetDevice(c->device);
   comm_destroy(c->comm);
   if (c->st) cudaStreamSynchronize(c->st);
@@ -300,6 +321,11 @@ int eb_destroy(eb_ctx* c) {
   cudaFree(c->tap_scalar);
   cudaFree(c->tap_u);
   cudaFree(c->tap_active);
+  cudaFreeHost(c->cb_x);
+  cudaFreeHost(c->cb_lp);
+  cudaFree(c->cb_xdev);
+  cudaFree(c->ext_f);
+  cudaFree(c->ext_lp);
   if (c->ev0) cudaEventDestroy(c->ev0);
   if (c->ev1) cudaEventDestroy(c->ev1);
   if (c->st) cudaStreamDestroy(c->st);
@@ -330,6 +356,7 @@ static bool cholesky_lower(const double* A, int D, std::vector<double>& L) {
 
 int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   const size_t D = (size_t)c->D;
   ModelDev m{};
@@ -384,12 +411,77 @@ int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
   }
   c->model = m;
   c->have_model = true;
+  c->cb_fn = nullptr;
+  c->cb_user = nullptr;
+  return EB_OK;
+}
+
+int eb_model_set_callback(eb_ctx* c, eb_logprob_fn fn, void* user, int where) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!fn) FAIL(c, EB_ERR_INVALID, "eb_model_set_callback: null function");
+  if (where != EB_CALLBACK_HOST && where != EB_CALLBACK_DEVICE)
+    FAIL(c, EB_ERR_INVALID, "eb_model_set_callback: where must be EB_CALLBACK_HOST or EB_CALLBACK_DEVICE (got %d)", where);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st));
+  cudaFree(c->model_params);
+  cudaFree(c->model_chol);
+  cudaFree(c->model_box);
+  c->model_params = nullptr;
+  c->model_chol = nullptr;
+  c->model_box = nullptr;
+  if (!c->ext_f) CK(c, cudaMalloc(&c->ext_f, (size_t)c->N * sizeof(double)));
+  if (!c->ext_lp) CK(c, cudaMalloc(&c->ext_lp, (size_t)c->N * sizeof(double)));
+  if (!c->qbuf) CK(c, cudaMalloc(&c->qbuf, (size_t)c->N * c->D * sizeof(double)));
+  c->model = ModelDev{};
+  c->model.kind = MODEL_EXTERNAL;
+  c->cb_fn = fn;
+  c->cb_user = user;
+  c->cb_where = where;
+  c->chain_ok = false;
+  c->have_model = true;
+  return EB_OK;
+}
+
+int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_bytes, int64_t m, uint64_t src_stream) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->in_callback || c->cb_where != EB_CALLBACK_DEVICE)
+    FAIL(c, EB_ERR_STATE, "eb_callback_result: only from inside a device-mode log-probability callback");
+  if (m < 0 || (m > 0 && (!lp || !src))) FAIL(c, EB_ERR_INVALID, "eb_callback_result: null buffer");
+  if (stride_bytes <= 0 || stride_bytes % (int64_t)sizeof(double) != 0)
+    FAIL(c, EB_ERR_INVALID, "eb_callback_result: the stride must be a positive multiple of 8 bytes (got %lld)",
+         (long long)stride_bytes);
+  if (m == 0) return EB_OK;
+  if (src_stream == EB_STREAM_UNKNOWN) {
+    // a producer that names no stream (CUDA Array Interface v2, e.g. torch): its last kernel may be on any
+    // stream of the device, so wait for all of them
+    CK(c, cudaDeviceSynchronize());
+  } else if (src_stream != 0) {
+    // the producer's work on its stream comes first (CUDA Array Interface v3 stream encoding)
+    cudaStream_t s = src_stream == 1 ? cudaStreamLegacy
+                     : src_stream == 2 ? cudaStreamPerThread
+                                       : reinterpret_cast<cudaStream_t>((uintptr_t)src_stream);
+    cudaEvent_t ev;
+    CK(c, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    cudaError_t e = cudaEventRecord(ev, s);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->st, ev, 0);
+    cudaEventDestroy(ev);
+    CK(c, e);
+  }
+  CK(c, cudaMemcpy2DAsync(lp, sizeof(double), src, (size_t)stride_bytes, sizeof(double), (size_t)m, cudaMemcpyDefault,
+                          c->st));
+  // the caller may free or reuse src as soon as this returns
+  CK(c, cudaStreamSynchronize(c->st));
   return EB_OK;
 }
 
 int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_model_set_bounds: no model set");
+  if (c->model.kind == MODEL_EXTERNAL)
+    FAIL(c, EB_ERR_UNSUPPORTED, "eb_model_set_bounds: a callback model has no box; apply the prior in the function");
   if ((lower == nullptr) != (upper == nullptr))
     FAIL(c, EB_ERR_INVALID, "eb_model_set_bounds: pass both bounds, or NULL for both to clear them");
   const size_t D = (size_t)c->D;
@@ -418,6 +510,63 @@ int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
 }
 
 // ---- log-prob ----------------------------------------------------------------
+// the rows handed to the function for `rows` rows: pinned staging (host mode) or a device copy (device mode)
+static int ensure_callback_staging(eb_ctx* c, size_t rows) {
+  const bool host = c->cb_where == EB_CALLBACK_HOST;
+  if (rows <= c->cb_rows && (host ? c->cb_x != nullptr : c->cb_xdev != nullptr)) return EB_OK;
+  rows = std::max(rows, c->cb_rows);
+  CK(c, cudaStreamSynchronize(c->st));
+  cudaFreeHost(c->cb_x);
+  cudaFreeHost(c->cb_lp);
+  cudaFree(c->cb_xdev);
+  c->cb_x = nullptr;
+  c->cb_lp = nullptr;
+  c->cb_xdev = nullptr;
+  c->cb_rows = 0;
+  if (host) {
+    CK(c, cudaMallocHost(&c->cb_x, rows * (size_t)c->D * sizeof(double)));
+    CK(c, cudaMallocHost(&c->cb_lp, rows * sizeof(double)));
+  } else {
+    CK(c, cudaMalloc(&c->cb_xdev, rows * (size_t)c->D * sizeof(double)));
+  }
+  c->cb_rows = rows;
+  return EB_OK;
+}
+
+// steps 2-7 of a callback half-step (include/emcee_b200.h): the device rows x[m, D] have been enqueued;
+// lp[m] (device) gets the callback's values.  scan_x: the rows were not written by a kernel that raises the
+// non-finite flags (WalkMove / GaussianMove proposals, the caller's coordinates)
+static int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x) {
+  const size_t D = (size_t)c->D;
+  if (scan_x) CK(c, launch_scan_nonfinite(x, (size_t)m * D, 0, c->status_dev, c->st));
+  int rc = fetch_status(c);  // synchronises; ensemble.py:476-479: the function never sees a non-finite row
+  if (rc) return rc;
+  rc = ensure_callback_staging(c, (size_t)m);
+  if (rc) return rc;
+  const bool host = c->cb_where == EB_CALLBACK_HOST;
+  // the function gets its own copy of the rows: writing to it cannot change the proposals the update reads
+  if (host) {
+    CK(c, cudaMemcpyAsync(c->cb_x, x, (size_t)m * D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    CK(c, cudaStreamSynchronize(c->st));
+  } else {
+    CK(c, cudaMemcpyAsync(c->cb_xdev, x, (size_t)m * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
+    // complete before fn runs: a consumer may ignore the stream it is given (torch does) and read x from any
+    // stream of its own
+    CK(c, cudaStreamSynchronize(c->st));
+  }
+  c->in_callback = true;
+  const int r = host ? c->cb_fn(c->cb_user, c->cb_x, m, (int64_t)D, c->cb_lp, nullptr)
+                     : c->cb_fn(c->cb_user, c->cb_xdev, m, (int64_t)D, lp, (void*)c->st);
+  c->in_callback = false;
+  if (r != 0) {
+    cudaStreamSynchronize(c->st);  // whatever the function enqueued before it failed
+    FAIL(c, EB_ERR_CALLBACK, "the log-probability callback failed (returned %d)", r);
+  }
+  if (host) CK(c, cudaMemcpyAsync(lp, c->cb_lp, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  CK(c, launch_scan_nonfinite(lp, (size_t)m, 1, c->status_dev, c->st));
+  return fetch_status(c);  // ensemble.py:550-551, before any update
+}
+
 // rows of x -> out with the kernel that matches the stepping path of the model
 static cudaError_t launch_logprob(eb_ctx* c, const double* x, int64_t rows, double* out) {
   if (c->allow_dmma && c->model.kind == EB_MODEL_GAUSS_DENSE && c->model.chol != nullptr)
@@ -441,6 +590,7 @@ static int ensure_scratch(eb_ctx* c, size_t rows) {
 
 int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_compute_log_prob: no model set");
   if (m == 0) return EB_OK;
   if (!coords || !out) FAIL(c, EB_ERR_INVALID, "eb_compute_log_prob: null buffer");
@@ -449,7 +599,12 @@ int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) 
   if (rc) return rc;
   CK(c, cudaMemcpyAsync(c->scratch_x, coords, m * (size_t)c->D * sizeof(double), cudaMemcpyHostToDevice,
                         c->st));
-  CK(c, launch_logprob(c, c->scratch_x, (int64_t)m, c->scratch_lp));
+  if (c->model.kind == MODEL_EXTERNAL) {
+    rc = run_callback(c, c->scratch_x, (int64_t)m, c->scratch_lp, true);
+    if (rc) return rc;
+  } else {
+    CK(c, launch_logprob(c, c->scratch_x, (int64_t)m, c->scratch_lp));
+  }
   CK(c, cudaMemcpyAsync(out, c->scratch_lp, m * sizeof(double), cudaMemcpyDeviceToHost, c->st));
   return fetch_status(c);
 }
@@ -481,6 +636,7 @@ static int sync_replicas(eb_ctx* c) {
 
 int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!coords) FAIL(c, EB_ERR_INVALID, "eb_set_state: coords is null");
   if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_set_state: no model set");
   CK(c, cudaSetDevice(c->device));
@@ -507,6 +663,9 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
                         cudaMemcpyHostToDevice, c->st));
   if (log_prob) {
     CK(c, cudaMemcpyAsync(c->logp + r0, log_prob + r0, rows * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  } else if (c->model.kind == MODEL_EXTERNAL) {
+    int rc = run_callback(c, c->coords, (int64_t)rows, c->logp, true);  // one GPU: rows == nwalkers
+    if (rc) return rc;
   } else {
     CK(c, launch_logprob(c, c->coords + (size_t)r0 * D, (int64_t)rows, c->logp + r0));
   }
@@ -526,6 +685,7 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
 
 int eb_get_state(eb_ctx* c, double* coords, double* log_prob) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->have_state) FAIL(c, EB_ERR_STATE, "eb_get_state: no state set");
   CK(c, cudaSetDevice(c->device));
   int rc = sync_replicas(c);  // multi-GPU: the GLOBAL state (collective)
@@ -551,6 +711,7 @@ int eb_owned_rows(const eb_ctx* c, int64_t* row0, int64_t* nrows) {
 
 int eb_get_state_rows(eb_ctx* c, int64_t row0, int64_t nrows, double* coords, double* log_prob) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->have_state) FAIL(c, EB_ERR_STATE, "eb_get_state_rows: no state set");
   if (row0 < 0 || nrows < 0 || row0 + nrows > c->N) FAIL(c, EB_ERR_INVALID, "eb_get_state_rows: rows out of range");
   int64_t r0, r1;
@@ -572,6 +733,7 @@ int eb_get_state_rows(eb_ctx* c, int64_t row0, int64_t nrows, double* coords, do
 
 int eb_set_rng(eb_ctx* c, uint64_t seed, uint64_t step) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   c->seed = seed;
   c->step = step;
   return EB_OK;
@@ -771,6 +933,27 @@ int check_walker_count(eb_ctx* c, const eb_move& mv) {
   return EB_OK;
 }
 
+// one half-step of a callback model (eb_model_set_callback): the propose phase of the fused kernel (STRETCH / DE /
+// SNOOKER) -- or the proposals a move's own kernels left in qbuf (MOVE_PRECOMPUTED) --, the callback, then the
+// accept phase.  The proposal rows are the fused kernel's by construction: the same code stages them.
+int callback_half_step(eb_ctx* c, int move_kind, HalfStepArgs a, uint64_t& launches) {
+  ExternalBufs ext{c->qbuf, nullptr, c->ext_lp};
+  if (move_kind != MOVE_PRECOMPUTED) {
+    ext.f = c->ext_f;
+    CK(c, launch_half_step_external(move_kind, a, ext, c->st));
+    ++launches;
+  }
+  int rc = run_callback(c, c->qbuf, (int64_t)a.i_hi - a.i_lo, c->ext_lp, move_kind == MOVE_PRECOMPUTED);
+  if (rc) return rc;
+  a.qbuf = c->qbuf;
+  CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st));
+  ++launches;
+  c->last_kernel = "callback";
+  snprintf(c->last_variant, sizeof(c->last_variant), "callback G=%d where=%s", lanes_per_walker(c->D),
+           c->cb_where == EB_CALLBACK_HOST ? "host" : "device");
+  return EB_OK;
+}
+
 // launch the P half-steps of one step with the generic kernels (one launch per split)
 int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t* order, size_t step_in_chunk,
                         uint64_t& launches) {
@@ -802,6 +985,12 @@ int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, const int32
       c->fused_last = false;
     }
     c->chain_ok = false;
+    if (c->model.kind == MODEL_EXTERNAL) {
+      rc = callback_half_step(c, mv.kind, a, launches);
+      if (rc) return rc;
+      c->tap_count = a.a_count;
+      continue;
+    }
     bool used_tma = false;
     TmaVariant tv{};
     if (c->allow_tma && !c->debug)
@@ -874,9 +1063,15 @@ int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
       CK(c, launch_walk_subset_propose(a, (int)s0, c->qbuf, c->st));
       ++launches;
     }
+    if (c->model.kind == MODEL_EXTERNAL) {
+      rc = callback_half_step(c, MOVE_PRECOMPUTED, a, launches);
+      if (rc) return rc;
+      continue;
+    }
     CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st));
     ++launches;
   }
+  if (c->model.kind == MODEL_EXTERNAL) return EB_OK;
   c->last_kernel = "walk";
   snprintf(c->last_variant, sizeof(c->last_variant), "walk");
   return EB_OK;
@@ -917,6 +1112,10 @@ int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step,
   a.i_hi = (int)c->N;
   a.range = nullptr;
   a.qbuf = c->qbuf;
+  if (c->model.kind == MODEL_EXTERNAL) {
+    ++launches;
+    return callback_half_step(c, MOVE_PRECOMPUTED, a, launches);
+  }
   CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st));
   launches += 2;
   c->last_kernel = "gaussian";
@@ -1219,6 +1418,7 @@ extern "C" {
 
 int eb_step(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint8_t* accepted_last) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   int rc = step_preflight(c);
   if (rc) return rc;
   Schedule s;
@@ -1240,6 +1440,7 @@ int eb_step(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uin
 int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
                   double* chain, double* log_prob, double* accepted) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
   if (!chain || !log_prob) FAIL(c, EB_ERR_INVALID, "eb_step_store: null output buffer");
   int rc = step_preflight(c);
@@ -1379,6 +1580,7 @@ extern "C" {
 int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
                         eb_chain* ch, uint64_t slot0) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
   if (!ch) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: null chain");
   if (ch->device != c->device || ch->N != c->N || ch->D != c->D)
@@ -1599,6 +1801,7 @@ int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t co
 
 int eb_get_naccepted(eb_ctx* c, uint64_t* naccepted) {
   if (!c || !naccepted) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   int rc = sync_replicas(c);  // multi-GPU: every rank's counters (collective)
   if (rc) return rc;
@@ -1615,6 +1818,7 @@ int eb_move_picks(const eb_ctx* c, uint64_t* picks, size_t nmoves) {
 
 int eb_reset_counters(eb_ctx* c) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   CK(c, cudaMemsetAsync(c->nacc, 0, (size_t)c->N * sizeof(unsigned long long), c->st));
   CK(c, cudaStreamSynchronize(c->st));
@@ -1623,6 +1827,7 @@ int eb_reset_counters(eb_ctx* c) {
 
 int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* naccepted_total) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->mom_acc) FAIL(c, EB_ERR_STATE, "eb_moments: enable with eb_set_option(\"moments_every\", n) before stepping");
   CK(c, cudaSetDevice(c->device));
   const size_t D = (size_t)c->D, n = D + D * D;
@@ -1663,6 +1868,7 @@ int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* 
 
 int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, int* flags) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!coords || !gram || rows == 0) FAIL(c, EB_ERR_INVALID, "eb_walkers_gram: null buffer");
   if (c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "eb_walkers_gram is limited to ndim <= 1024");
   CK(c, cudaSetDevice(c->device));
@@ -1712,6 +1918,7 @@ int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, 
 
 int eb_autocorr(eb_ctx* c, const double* chain, size_t n_t, size_t nw, size_t nd, double* acf) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!chain || !acf || n_t == 0 || nw == 0 || nd == 0) FAIL(c, EB_ERR_INVALID, "eb_autocorr: empty chain or null buffer");
   CK(c, cudaSetDevice(c->device));
   c->chain_ok = false;
@@ -1735,6 +1942,7 @@ const char* eb_last_kernel_variant(const eb_ctx* c) { return c ? c->last_variant
 
 int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
   if (!c || !name) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!strcmp(name, "debug_taps")) {
     CK(c, cudaSetDevice(c->device));
     if (value && !c->tap_scalar) {
@@ -1801,6 +2009,7 @@ int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
 
 int eb_debug_timeline(eb_ctx* c, int64_t* out, size_t capacity, size_t* written) {
   if (!c || !out) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->timeline) FAIL(c, EB_ERR_STATE, "eb_debug_timeline: enable with eb_set_option(\"dmma_timeline\", 1)");
   CK(c, cudaSetDevice(c->device));
   const size_t n = (size_t)c->sm_count * 8 * TL_TILES * TL_EVENTS;
@@ -1813,6 +2022,7 @@ int eb_debug_timeline(eb_ctx* c, int64_t* out, size_t capacity, size_t* written)
 int eb_debug_taps(eb_ctx* c, int64_t* partners, double* scalar, double* u_accept, int64_t* active,
                   int64_t* nactive) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   if (!c->debug || !c->tap_scalar) FAIL(c, EB_ERR_STATE, "eb_debug_taps: enable with eb_set_option(\"debug_taps\", 1)");
   CK(c, cudaSetDevice(c->device));
   const size_t N = (size_t)c->N;
@@ -1847,6 +2057,9 @@ int eb_comm_id(char id[EB_COMM_ID_BYTES]) { return comm_unique_id(id) ? EB_ERR_C
 
 int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nranks, int mode) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->have_model && c->model.kind == MODEL_EXTERNAL && nranks > 1)
+    FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path
@@ -1858,6 +2071,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
 
 int eb_comm_export(eb_ctx* c, char blob[EB_IPC_BLOB_BYTES]) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   if (comm_export(c->comm, blob)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   return EB_OK;
@@ -1865,6 +2079,7 @@ int eb_comm_export(eb_ctx* c, char blob[EB_IPC_BLOB_BYTES]) {
 
 int eb_comm_probe(eb_ctx* c, int peer, int what, double* gbs) {
   if (!c || !gbs) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   if (comm_probe(c->comm, peer, what, c->D, c->st, gbs)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   return EB_OK;
@@ -1872,6 +2087,7 @@ int eb_comm_probe(eb_ctx* c, int peer, int what, double* gbs) {
 
 int eb_comm_import(eb_ctx* c, const char* blobs) {
   if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   if (comm_import(c->comm, blobs)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   return EB_OK;

@@ -88,6 +88,19 @@ struct HalfStepArgs {
 // the Hastings factor is 0 (WalkMove walk.py:37, GaussianMove gaussian.py:104); order == nullptr: walker id = i
 constexpr int MOVE_PRECOMPUTED = 100;
 
+// internal model kind of half_step_generic_kernel: the log-probabilities come from outside the kernel (a host or
+// CUDA-array callback, eb_model_set_callback).  A half-step runs as two launches around the callback:
+//   propose  <STRETCH | DE | SNOOKER, MODEL_EXTERNAL>: the proposal code of the fused kernel, then row i of the
+//            staged proposal -> ExternalBufs::q[i - i_lo] and its Hastings factor -> f[i - i_lo]; nothing else
+//   accept   <MOVE_PRECOMPUTED, MODEL_EXTERNAL>: lp_new = lp[i - i_lo], factor = f[i - i_lo] (0 when f is null:
+//            WalkMove / GaussianMove), then the accept draw and update of the fused kernel
+constexpr int MODEL_EXTERNAL = 100;
+struct ExternalBufs {
+  double* q;         // propose: [a_count, D] proposals (the accept launch reads them back through HalfStepArgs::qbuf)
+  double* f;         // [a_count] Hastings factors, or null
+  const double* lp;  // accept: [a_count] log-probabilities of the proposals
+};
+
 struct Engine;  // defined in capi.cu
 
 // ---- kernel launchers (implemented in the .cu files) ----------------------
@@ -103,6 +116,11 @@ cudaError_t launch_locality_tables(const int32_t* order, const StepInfo* info_de
                                    int64_t N, uint64_t seed, uint64_t step0, int64_t rows_per_rank, int rank,
                                    int front_cap, int32_t* aperm, cudaStream_t st);
 cudaError_t launch_half_step_generic(int move_kind, const HalfStepArgs& a, cudaStream_t st);
+// the two launches of a half-step of a callback model (MODEL_EXTERNAL above): move_kind STRETCH / DE / SNOOKER
+// runs the propose phase, MOVE_PRECOMPUTED the accept phase
+cudaError_t launch_half_step_external(int move_kind, const HalfStepArgs& a, const ExternalBufs& ext, cudaStream_t st);
+// status |= FLAG_NAN_LOGPROB if any of x[n] is NaN (logprob != 0), else the non-finite parameter flags of x[n]
+cudaError_t launch_scan_nonfinite(const double* x, size_t n, int logprob, int* status, cudaStream_t st);
 // the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)
 struct TmaVariant {
   int R;        // walkers per tile (G = 32 / R lanes per walker)

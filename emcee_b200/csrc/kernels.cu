@@ -10,6 +10,8 @@
 //   accept + update .............................. moves/red_blue.py:96-104, moves/move.py:29-34
 #include <math.h>
 
+#include <algorithm>
+
 #include "engine.cuh"
 #include "rowops.cuh"
 
@@ -199,8 +201,10 @@ cudaError_t launch_locality_tables(const int32_t* order, const StepInfo* info_de
 // ===========================================================================
 // G lanes per active walker; the proposal row is staged in shared memory
 // (rows_per_group rows of D doubles per group).
+// MODEL_EXTERNAL (engine.cuh): the same kernel split in two launches around the log-probability callback; `ext` is
+// read only by those instantiations.
 template <int MOVE, int MODEL>
-__global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepArgs a, const int G) {
+__global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepArgs a, const int G, const ExternalBufs ext) {
   extern __shared__ double smem[];
   constexpr int NROWS = (MOVE == EB_MOVE_SNOOKER ? 4 : 1) + (MODEL == EB_MODEL_GAUSS_DENSE ? 1 : 0);
   const int D = a.D;
@@ -261,12 +265,14 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     tap_scalar = gamma;
   } else if (MOVE == MOVE_PRECOMPUTED) {
     // WalkMove / GaussianMove: the proposal was written by its own kernel (moves_extra.cu); factors = 0
+    // (accept phase of a callback model: written by the propose phase, factor from ext.f)
     const double* qrow = a.qbuf + (size_t)(i - i_lo) * D;
     for (int e = g; e < D; e += G) {
       const double v = qrow[e];
       q[e] = v;
       if (!isfinite(v)) flag_nonfinite(v, a.status);
     }
+    if (MODEL == MODEL_EXTERNAL && ext.f != nullptr) factor = ext.f[i - i_lo];
   } else {  // EB_MOVE_SNOOKER
     const u32x4 B = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_B, (uint32_t)i);
     int64_t cw[3];
@@ -324,10 +330,31 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
   }
   __syncwarp(mask);
 
+  if (MODEL == MODEL_EXTERNAL && MOVE != MOVE_PRECOMPUTED) {
+    // propose phase of a callback model: hand the staged row and its factor to the host, stop before the model
+    double* dst = ext.q + (size_t)(i - i_lo) * D;
+    for (int e = g; e < D; e += G) dst[e] = q[e];
+    if (g == 0) {
+      ext.f[i - i_lo] = factor;
+      if (a.tap_scalar != nullptr) {
+        a.tap_partners[i] = pw[0];
+        a.tap_partners[a.N + i] = pw[1];
+        a.tap_partners[2 * a.N + i] = pw[2];
+        a.tap_scalar[i] = tap_scalar;
+      }
+    }
+    return;
+  }
+
   // red_blue.py:93 -> ensemble.py:458-553
-  double lp_new = model_logprob<MODEL>(q, xc, D, g, G, mask, a.model);
-  if (a.model.lo != nullptr && !row_in_box(q, D, g, G, mask, a.model)) lp_new = -INFINITY;
-  if (isnan(lp_new) && g == 0) atomicOr(a.status, FLAG_NAN_LOGPROB);
+  double lp_new;
+  if (MODEL == MODEL_EXTERNAL) {
+    lp_new = ext.lp[i - i_lo];  // the callback's value; NaN was refused before this launch
+  } else {
+    lp_new = model_logprob<MODEL>(q, xc, D, g, G, mask, a.model);
+    if (a.model.lo != nullptr && !row_in_box(q, D, g, G, mask, a.model)) lp_new = -INFINITY;
+    if (isnan(lp_new) && g == 0) atomicOr(a.status, FLAG_NAN_LOGPROB);
+  }
 
   // red_blue.py:96-101
   const u32x4 U = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_ACCEPT, (uint32_t)i);
@@ -347,10 +374,12 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     }
     a.accepted[w] = acc ? 1 : 0;
     if (a.tap_scalar != nullptr) {
-      a.tap_partners[i] = pw[0];
-      a.tap_partners[a.N + i] = pw[1];
-      a.tap_partners[2 * a.N + i] = pw[2];
-      a.tap_scalar[i] = tap_scalar;
+      if (MODEL != MODEL_EXTERNAL) {  // a callback model's propose phase recorded them
+        a.tap_partners[i] = pw[0];
+        a.tap_partners[a.N + i] = pw[1];
+        a.tap_partners[2 * a.N + i] = pw[2];
+        a.tap_scalar[i] = tap_scalar;
+      }
       a.tap_u[i] = u_acc;
       a.tap_active[i] = w;
     }
@@ -358,7 +387,7 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
 }
 
 template <int MOVE, int MODEL>
-static cudaError_t launch_generic_t(const HalfStepArgs& a, cudaStream_t st) {
+static cudaError_t launch_generic_t(const HalfStepArgs& a, cudaStream_t st, const ExternalBufs& ext = ExternalBufs{}) {
   const int G = lanes_per_walker(a.D);
   constexpr int NROWS = (MOVE == EB_MOVE_SNOOKER ? 4 : 1) + (MODEL == EB_MODEL_GAUSS_DENSE ? 1 : 0);
   int threads = 256;
@@ -377,7 +406,7 @@ static cudaError_t launch_generic_t(const HalfStepArgs& a, cudaStream_t st) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  kern<<<grid, threads, smem, st>>>(a, G);
+  kern<<<grid, threads, smem, st>>>(a, G, ext);
   return cudaGetLastError();
 }
 
@@ -408,6 +437,40 @@ cudaError_t launch_half_step_generic(int move_kind, const HalfStepArgs& a, cudaS
       return launch_generic_m<MOVE_PRECOMPUTED>(a, st);
   }
   return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_half_step_external(int move_kind, const HalfStepArgs& a, const ExternalBufs& ext, cudaStream_t st) {
+  switch (move_kind) {
+    case EB_MOVE_STRETCH:
+      return launch_generic_t<EB_MOVE_STRETCH, MODEL_EXTERNAL>(a, st, ext);
+    case EB_MOVE_DE:
+      return launch_generic_t<EB_MOVE_DE, MODEL_EXTERNAL>(a, st, ext);
+    case EB_MOVE_SNOOKER:
+      return launch_generic_t<EB_MOVE_SNOOKER, MODEL_EXTERNAL>(a, st, ext);
+    case MOVE_PRECOMPUTED:
+      return launch_generic_t<MOVE_PRECOMPUTED, MODEL_EXTERNAL>(a, st, ext);
+  }
+  return cudaErrorInvalidValue;
+}
+
+// non-finite scan of a callback's input rows (ensemble.py:476-479) or of its log-probabilities (:550-551)
+__global__ void __launch_bounds__(256) scan_nonfinite_kernel(const double* __restrict__ x, size_t n, int logprob,
+                                                             int* status) {
+  bool nan = false, inf = false;
+  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) {
+    const double v = x[k];
+    nan |= isnan(v);
+    inf |= isinf(v);
+  }
+  const int f = logprob ? (nan ? FLAG_NAN_LOGPROB : 0) : ((inf ? FLAG_INF_PARAM : 0) | (nan ? FLAG_NAN_PARAM : 0));
+  if (f) atomicOr(status, f);
+}
+
+cudaError_t launch_scan_nonfinite(const double* x, size_t n, int logprob, int* status, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  const unsigned grid = (unsigned)std::min<size_t>((n + 255) / 256, 1024);
+  scan_nonfinite_kernel<<<grid, 256, 0, st>>>(x, n, logprob, status);
+  return cudaGetLastError();
 }
 
 // ===========================================================================

@@ -2,12 +2,14 @@
 ``src/emcee/ensemble.py:32-623``).
 
 Same constructor / ``sample`` / ``run_mcmc`` / ``compute_log_prob`` surface and
-the same exceptions, but ``log_prob_fn`` is a registered device model
-(``emcee_b200.models``) and every step runs inside the CUDA library through the
-C ABI: the walker array stays in HBM between steps, ``run_mcmc`` is one call
-for all iterations, and stored steps stream back through pinned buffers.
-Features that need a host callback per walker (``pool``, ``args``/``kwargs``,
-blobs, named parameters) raise ``NotImplementedError``."""
+the same exceptions, but ``log_prob_fn`` is a registered device model or an
+explicitly wrapped user function (``emcee_b200.models``), and every step runs
+inside the CUDA library through the C ABI: the walker array stays in HBM
+between steps, ``run_mcmc`` is one call for all iterations (a user function is
+called back from inside it once per half-step), and stored steps stream back
+through pinned buffers.  ``pool`` / ``args`` / ``kwargs`` / ``vectorize``
+belong to ``models.HostFunction``; blobs and named parameters raise
+``NotImplementedError``."""
 
 from collections.abc import Iterable
 
@@ -16,7 +18,7 @@ import numpy as np
 from . import _lib
 from .backend import Backend, DeviceBackend
 from .model import Model
-from .models import DeviceModel
+from .models import CallbackFunction, DeviceModel
 from .moves import StretchMove
 from .rng import DeviceRandom
 from .state import State
@@ -76,15 +78,18 @@ class EnsembleSampler(object):
                           ("live_dangerously", live_dangerously), ("runtime_sortingfn", runtime_sortingfn)):
             if val is not None:
                 raise NotImplementedError("the deprecated '%s' argument is not supported; use 'moves'" % name)
-        if not isinstance(log_prob_fn, DeviceModel):
+        if not isinstance(log_prob_fn, (DeviceModel, CallbackFunction)):
             raise TypeError(
-                "log_prob_fn must be a registered device model (emcee_b200.models.*): the "
-                "walker update runs on the GPU and cannot call back into Python"
+                "log_prob_fn must be a registered device model (emcee_b200.models.GaussianIso, ...) or a "
+                "wrapped user function: models.HostFunction(fn, vectorize=...) for a numpy function, "
+                "models.CudaArrayFunction(fn) for one on CUDA arrays"
             )
         if pool is not None:
-            raise NotImplementedError("pool: log-probabilities are evaluated on the GPU, not through map()")
+            raise NotImplementedError("pool: pass it to models.HostFunction(fn, pool=pool)")
         if args or kwargs:
-            raise NotImplementedError("args/kwargs: put the parameters into the device model")
+            raise NotImplementedError(
+                "args/kwargs: put the parameters into the device model, or pass them to "
+                "models.HostFunction / models.CudaArrayFunction")
         if parameter_names is not None:
             raise NotImplementedError("parameter_names need a host callable")
         if blobs_dtype is not None:
@@ -155,8 +160,12 @@ class EnsembleSampler(object):
 
     def _load_model(self):
         # the registered model, then its prior support (models.Bounded): a box is part of the model,
-        # so a rebuilt engine (__setstate__) gets it back too
+        # so a rebuilt engine (__setstate__) gets it back too; a user function is registered as the
+        # engine's callback
         m = self.log_prob_fn
+        if isinstance(m, CallbackFunction):
+            self._engine.set_callback(m.evaluate, m.where)
+            return
         self._engine.set_model(m.kind, m.device_params(self.ndim))
         box = m.bounds(self.ndim)
         if box is not None:
@@ -230,6 +239,8 @@ class EnsembleSampler(object):
 
         if isinstance(self.backend, DeviceBackend):
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
+        if isinstance(self.log_prob_fn, CallbackFunction):
+            raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         dist.attach(self._engine, rdv, mode)
         self._rdv = rdv
         self._gather_results = bool(gather_results)
@@ -261,6 +272,16 @@ class EnsembleSampler(object):
     # ------------------------------------------------------------- the driver
     def _schedule(self):
         return [(m.descriptor(), w) for m, w in zip(self._moves, self._raw_weights)]
+
+    def _stored_before_failure(self, step0, thin_by, k0):
+        """A bulk run stopped by an exception: the backend keeps the stored steps that completed
+        (the engine drained them before returning), and the random state of the last of them."""
+        b = self.backend
+        seed, step = self._engine.get_rng()
+        stored = (step - step0) // thin_by
+        b.iteration = k0 + stored
+        if stored:
+            b.random_state = (self.random_state[0], seed, step0 + stored * thin_by)
 
     def _after_steps(self):
         """Advance the host mirrors of stateful moves by what the engine just ran (``GaussianMove``
@@ -372,16 +393,26 @@ class EnsembleSampler(object):
                 if store:
                     b = self.backend
                     k0, k1 = b.iteration, b.iteration + iterations
-                    if device_store:
-                        eng.step_store_chain(sched, total, checkpoint_step, b._ch, k0)
-                    else:
-                        eng.step_store(sched, total, checkpoint_step, b.chain[k0:k1], b.log_prob[k0:k1], b.accepted)
+                    step0 = eng.get_rng()[1]
+                    try:
+                        if device_store:
+                            eng.step_store_chain(sched, total, checkpoint_step, b._ch, k0)
+                        else:
+                            eng.step_store(sched, total, checkpoint_step, b.chain[k0:k1], b.log_prob[k0:k1],
+                                           b.accepted)
+                    except BaseException:
+                        # a user function's exception, or a NaN it returned, stops the run inside a step
+                        self._after_steps()
+                        self._stored_before_failure(step0, checkpoint_step, k0)
+                        raise
                     self._after_steps()
                     b.iteration = k1
                     b.random_state = self.random_state
                 else:
-                    eng.step(sched, total, want_accepted=False)
-                    self._after_steps()
+                    try:
+                        eng.step(sched, total, want_accepted=False)
+                    finally:
+                        self._after_steps()
             refresh()
             if pbar is not None:
                 pbar.update(iterations)
@@ -399,17 +430,22 @@ class EnsembleSampler(object):
             if last_is_checkpoint and native_store:
                 b = self.backend
                 k = b.iteration
-                if device_store:
-                    eng.step_store_chain(sched, yield_step, yield_step, b._ch, k)
-                else:
-                    eng.step_store(sched, yield_step, yield_step, b.chain[k : k + 1], b.log_prob[k : k + 1], b.accepted)
-                self._after_steps()
+                try:  # a window that stops early stores nothing: its one stored step is its last
+                    if device_store:
+                        eng.step_store_chain(sched, yield_step, yield_step, b._ch, k)
+                    else:
+                        eng.step_store(sched, yield_step, yield_step, b.chain[k : k + 1], b.log_prob[k : k + 1],
+                                       b.accepted)
+                finally:
+                    self._after_steps()
                 b.iteration = k + 1
                 b.random_state = self.random_state
                 refresh()
             else:
-                accepted = eng.step(sched, yield_step, want_accepted=last_is_checkpoint)
-                self._after_steps()
+                try:
+                    accepted = eng.step(sched, yield_step, want_accepted=last_is_checkpoint)
+                finally:
+                    self._after_steps()
                 refresh()
                 if last_is_checkpoint:
                     self.backend.save_step(state, accepted)
@@ -453,8 +489,8 @@ class EnsembleSampler(object):
         return walkers_independent(coords)
 
     def compute_log_prob(self, coords):
-        """``(log_prob, None)`` for ``coords[..., ndim]`` evaluated on the device
-        (``ensemble.py:458-553``); raises ``ValueError`` for non-finite
+        """``(log_prob, None)`` for ``coords[..., ndim]`` evaluated on the device, or by the user
+        function in one call (``ensemble.py:458-553``); raises ``ValueError`` for non-finite
         parameters or a NaN log-probability like the reference."""
         return self._engine.compute_log_prob(np.asarray(coords, dtype=np.float64)), None
 

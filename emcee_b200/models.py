@@ -1,17 +1,28 @@
-"""Registered device-side log-probability models.
+"""Log-probability models: registered device models and user functions.
 
 The reference takes an arbitrary Python callable ``log_prob_fn``
 (``src/emcee/ensemble.py:79-83``) and evaluates it row by row or through
-``pool.map`` (``ensemble.py:486-496``).  A GPU engine cannot call back into
-Python per walker, so the drop-in takes a *registered model*: a small object
-naming one of the log-probabilities compiled into the CUDA library plus its
-parameters.  These classes only carry parameters -- they are deliberately not
-callable, so no code path can silently evaluate a model on the host.
+``pool.map`` (``ensemble.py:486-496``).  The drop-in takes one of two things:
+
+* a *registered model* (``GaussianIso``, ``GaussianDense``, ``Rosenbrock``,
+  ``Ring``, optionally ``Bounded``): a small object naming one of the
+  log-probabilities compiled into the CUDA library plus its parameters.  The
+  whole half-step -- proposal, log-probability, accept -- is one kernel.
+  These classes only carry parameters and are deliberately not callable.
+* a *user function*, wrapped explicitly in ``HostFunction`` (numpy on the
+  host) or ``CudaArrayFunction`` (any CUDA-array library).  The engine calls
+  it once per half-step with the whole ``[M, ndim]`` block of proposals of
+  one split, never once per walker; split assignment, proposals, the accept
+  decision and the update stay on the GPU.  The explicit wrapper keeps the
+  rule that nothing is evaluated on the host unless the caller asked for it.
 """
 
 import numpy as np
 
-__all__ = ["DeviceModel", "GaussianIso", "GaussianDense", "Rosenbrock", "Ring", "Bounded"]
+__all__ = [
+    "DeviceModel", "GaussianIso", "GaussianDense", "Rosenbrock", "Ring", "Bounded",
+    "CallbackFunction", "HostFunction", "CudaArrayFunction",
+]
 
 
 class DeviceModel(object):
@@ -111,7 +122,10 @@ class Bounded(DeviceModel):
 
     def __init__(self, model, lower, upper):
         if not isinstance(model, DeviceModel) or isinstance(model, Bounded):
-            raise TypeError("Bounded wraps one of the registered device models (not another Bounded)")
+            raise TypeError(
+                "Bounded wraps one of the registered device models (not another Bounded, nor a user function: "
+                "a HostFunction / CudaArrayFunction applies its prior itself)"
+            )
         self.model = model
         self.kind = model.kind
         lo = np.array(lower, dtype=np.float64)
@@ -137,3 +151,108 @@ class Bounded(DeviceModel):
                 raise ValueError("%s bound has length %d but ndim = %d" % (name, v.size, ndim))
             out.append(np.ascontiguousarray(np.broadcast_to(v, (ndim,)), dtype=np.float64))
         return out[0], out[1]
+
+
+def _scalar(fx):
+    """The reference's ``_scalar`` (``ensemble.py:703-713``): 1.0, np.float64(1.0), np.array([1.0]) and
+    np.array(1.0) are all the float 1.0; anything with more than one element is an error."""
+    if not np.isscalar(fx):
+        try:
+            fx = np.asarray(fx).item()
+        except (TypeError, ValueError) as e:
+            raise ValueError("log_prob_fn should return scalar") from e
+        return float(fx)
+    else:
+        return float(fx)
+
+
+def log_prob_values(results):
+    """The log-probability vector of a batch of results, by the reference's rules
+    (``ensemble.py:498-512``): each result is a scalar (``_scalar``), or a sequence whose first entry
+    is the log-probability and the rest blobs -- which the engine does not store, so they raise
+    ``NotImplementedError``."""
+    if isinstance(results, np.ndarray) and results.ndim == 1 and results.dtype == np.float64:
+        return results  # what the rules below give element by element, without the Python loop
+    try:
+        blob = [r[1:] for r in results if len(r) > 1]
+        if not len(blob):
+            raise IndexError
+        np.array([_scalar(r[0]) for r in results])
+    except (IndexError, TypeError):
+        return np.array([_scalar(r) for r in results], dtype=np.float64)
+    raise NotImplementedError(
+        "the log-probability function returned blobs (a sequence per walker); blobs are not supported "
+        "by this engine -- return the log-probability alone"
+    )
+
+
+class CallbackFunction(object):
+    """A user log-probability function the engine calls back once per half-step
+    (``HostFunction`` / ``CudaArrayFunction``)."""
+
+    where = None
+
+    def __init__(self, fn, args=None, kwargs=None):
+        if not callable(fn):
+            raise TypeError("fn must be callable, got {0!r}".format(fn))
+        self.fn = fn
+        self.args = list(args or [])
+        self.kwargs = dict(kwargs or {})
+
+    def _call(self, x):
+        return self.fn(x, *self.args, **self.kwargs)
+
+
+class HostFunction(CallbackFunction):
+    """A numpy log-probability function, with the reference sampler's arguments and semantics
+    (``ensemble.py:79-98, 486-496, 626-650``).
+
+    ``vectorize=True``: one call ``fn(x, *args, **kwargs)`` per half-step with ``x[M, ndim]``, returning
+    ``M`` values.  Otherwise one call per row through ``pool.map`` (``pool`` given) or the built-in
+    ``map``.  Each row's result goes through the reference's ``_scalar`` rule; blobs raise
+    ``NotImplementedError``.  ``x`` is a fresh array that the function owns.  Rows reach the function
+    only when every parameter is finite; a NaN result stops the run with ``ValueError`` at that
+    half-step.  Pickling drops ``pool``, as the sampler does (``ensemble.py:251-256``)."""
+
+    where = "host"
+
+    def __init__(self, fn, vectorize=False, pool=None, args=None, kwargs=None):
+        super().__init__(fn, args, kwargs)
+        self.vectorize = bool(vectorize)
+        self.pool = pool
+        if pool is not None and not callable(getattr(pool, "map", None)):
+            raise TypeError("pool must have a map() method")
+
+    def evaluate(self, x):
+        """``float64[M]`` for ``x[M, ndim]``."""
+        if self.vectorize:
+            results = self._call(x)
+        else:
+            map_func = self.pool.map if self.pool is not None else map
+            results = list(map_func(self._call, x))
+        return log_prob_values(results)
+
+    def __getstate__(self):
+        d = dict(self.__dict__)
+        d["pool"] = None
+        return d
+
+
+class CudaArrayFunction(CallbackFunction):
+    """A log-probability function on device arrays, for any library that speaks the CUDA Array
+    Interface (torch, CuPy, Numba, ...; this package imports none of them).
+
+    ``fn(x, *args, **kwargs)`` receives an immutable object with ``__cuda_array_interface__`` (v3):
+    shape ``(M, ndim)``, ``<f8``, and ``stream`` set to the engine's stream.  It points to a scratch
+    copy of the proposals in the engine's memory, complete when ``fn`` is called, which ``fn`` may
+    overwrite (the proposals the update reads are elsewhere); it is valid only during the call -- copy
+    it to keep it.  ``fn`` returns ``M`` float64 values: any CUDA-array-interface object of shape
+    ``(M,)``, strided or not, or a numpy array (copied).  A result whose interface has a ``stream``
+    entry (v3) is read after the work on that stream; one without (v2, which torch exports) after all
+    work on the device, so a result still being computed on any stream is never read early.  ``M`` is
+    the size of one split, ``nwalkers`` for ``GaussianMove`` and for the initial state."""
+
+    where = "device"
+
+    def evaluate(self, x):
+        return self._call(x)

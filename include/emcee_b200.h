@@ -36,6 +36,7 @@ typedef enum eb_status {
   EB_ERR_STATE = -4,        /* call order (no model, no state) -> RuntimeError */
   EB_ERR_UNSUPPORTED = -5,  /*                                 -> NotImplementedError */
   EB_ERR_NOMEM = -6,        /* device allocation failed or would not fit -> MemoryError */
+  EB_ERR_CALLBACK = -7,     /* the log-probability callback failed -> re-raise the caller's exception */
   /* device-detected conditions the reference raises as exceptions */
   EB_ERR_NAN_LOGPROB = -10, /* ensemble.py:550-551 "Probability function returned NaN" */
   EB_ERR_INF_PARAM = -11,   /* ensemble.py:476-477 "At least one parameter value was infinite" */
@@ -110,8 +111,46 @@ int eb_model_set(eb_ctx* ctx, int kind, const double* params, size_t nparams);
  * kernel (the `if not in box: return -np.inf` of a log_prior).  -inf / +inf
  * bounds give one-sided boxes; NaN bounds and lower[k] >= upper[k] are refused
  * (EB_ERR_INVALID).  NULL, NULL clears the box.  Needs a model (EB_ERR_STATE);
- * eb_model_set clears the box. */
+ * eb_model_set clears the box.  A callback model has no box (EB_ERR_UNSUPPORTED). */
 int eb_model_set_bounds(eb_ctx* ctx, const double* lower, const double* upper);
+
+/* a user log-probability function, called once per half-step on the [m, ndim]
+ * block of proposals of one split (red_blue.py:90-93 -> ensemble.py:458-553):
+ * rows in ascending walker order, m = the split's size (nwalkers for
+ * GaussianMove and for the initial state).  It writes lp[m] and returns 0, or
+ * returns non-zero to stop the calling ABI function with EB_ERR_CALLBACK. */
+#define EB_CALLBACK_HOST 0   /* x, lp are host pointers (pinned staging owned by the engine), stream = NULL */
+#define EB_CALLBACK_DEVICE 1 /* x, lp are device pointers, x complete when fn is called; stream = the engine's
+                                cudaStream_t (idle during the call) */
+/* In both modes x is the engine's copy of the proposals: the function may overwrite it, the update reads the
+ * proposals from elsewhere.  x and lp are valid only during the call. */
+typedef int (*eb_logprob_fn)(void* user, const double* x, int64_t m, int64_t ndim, double* lp, void* stream);
+/* replaces the model, like eb_model_set, by fn (`user` is passed back unchanged;
+ * both must stay valid while the model is set).  Each half-step then runs:
+ *   1. the proposal kernel(s) of the move;  2. a stream synchronisation;
+ *   3. a non-finite proposal stops the call with EB_ERR_INF_PARAM / EB_ERR_NAN_PARAM
+ *      before fn sees it (ensemble.py:476-479);
+ *   4. host mode: the proposals are copied to the host;  5. fn;
+ *   6. host mode: lp is copied back;
+ *   7. a NaN in lp stops the call with EB_ERR_NAN_LOGPROB before the update
+ *      (ensemble.py:550-551);
+ *   8. the accept + update kernel (red_blue.py:96-104).
+ * eb_set_state(coords, NULL) and eb_compute_log_prob call fn too, with the same
+ * guards.  When a call stops inside a step, the step counter is that step, the
+ * splits of it that ran before stay applied, and every completed step is fully
+ * stored.  Inside fn, every other call on the same context returns EB_ERR_STATE
+ * ("engine is inside a log-probability callback").  Sharded engines
+ * (eb_comm_init) are refused with EB_ERR_UNSUPPORTED, both ways round. */
+int eb_model_set_callback(eb_ctx* ctx, eb_logprob_fn fn, void* user, int where);
+/* EB_CALLBACK_DEVICE, from inside fn: copy m float64 values, stride_bytes apart
+ * (> 0, a multiple of 8), from src (device or host memory) into fn's lp, ordered
+ * after the work on src_stream (CUDA Array Interface v3 encoding: 0 = none,
+ * 1 = legacy default stream, 2 = per-thread default stream, else a
+ * cudaStream_t), or after all work on the device for EB_STREAM_UNKNOWN (a
+ * producer that names no stream, such as an interface v2 object).  The copy
+ * has completed when the call returns. */
+#define EB_STREAM_UNKNOWN UINT64_MAX
+int eb_callback_result(eb_ctx* ctx, double* lp, const void* src, int64_t stride_bytes, int64_t m, uint64_t src_stream);
 
 /* ---- state (state.py:10-45) ------------------------------------------- */
 /* State(initial_state, copy=True) + the initial compute_log_prob
@@ -254,7 +293,9 @@ int eb_autocorr(eb_ctx* ctx, const double* chain, size_t n_step, size_t n_walker
 /* device time (ms, CUDA events on the engine's stream) of the last eb_step /
  * eb_step_store / eb_step_store_chain call, first launch to last, and the
  * number of kernels it launched for the steps (the store kernels of
- * eb_step_store_chain are not counted, so both store calls report the same). */
+ * eb_step_store_chain are not counted, so both store calls report the same).
+ * With a callback model the span includes the time the stream waits for the
+ * callbacks (and their copies). */
 int eb_last_step_timing(const eb_ctx* ctx, double* ms, uint64_t* launches);
 /* draws of the LAST half-step executed (known-answer tests): for each active
  * rank i of that split, partner walker ids (up to 3 per walker: stretch uses
@@ -290,7 +331,8 @@ const char* eb_last_kernel_name(const eb_ctx* ctx);
 /* the cell of that kernel the last half-step launch ran, with the parameters its launcher chose:
  * "tma_rows R=<walkers per tile> epl=<8 register path | 0 strided> own_reg=<0|1> warps=<per CTA>",
  * "dense_dmma nhalf_max=<most half-steps of one launch in the call> grid=<CTAs>", "generic G=<lanes per
- * walker>", "walk", "gaussian" or "none". */
+ * walker>", "walk", "gaussian", "callback G=<lanes per walker> where=host|device" (eb_last_kernel_name
+ * "callback": any move with a callback model) or "none". */
 const char* eb_last_kernel_variant(const eb_ctx* ctx);
 
 /* device micro-benchmarks that anchor the FP64 roofline: what = 0 DFMA, 1 DMMA m8n8k4, 2 DMMA m16n8k8,
