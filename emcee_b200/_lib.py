@@ -79,8 +79,14 @@ _SIGNATURES = {
     "eb_model_set_bounds": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_model_set_callback": (C.c_int, [C.c_void_p, LOGPROB_FN, C.c_void_p, C.c_int]),
     "eb_callback_result": (C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
+    "eb_callback_blobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_set_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_get_state": (C.c_int, [C.c_void_p, _dp, _dp]),
+    "eb_set_state_blobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "eb_get_blobs": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "eb_compute_log_prob_blobs": (
+        C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)],
+    ),
     "eb_owned_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "eb_get_state_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _dp]),
     "eb_compute_log_prob": (C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp]),
@@ -90,6 +96,10 @@ _SIGNATURES = {
     "eb_step_store": (
         C.c_int,
         [C.c_void_p, C.POINTER(EbMove), C.c_size_t, C.c_uint64, C.c_uint64, _dp, _dp, _dp],
+    ),
+    "eb_step_store_blobs": (
+        C.c_int,
+        [C.c_void_p, C.POINTER(EbMove), C.c_size_t, C.c_uint64, C.c_uint64, _dp, _dp, _dp, C.c_void_p],
     ),
     "eb_step_store_chain": (
         C.c_int,
@@ -278,15 +288,125 @@ def _device_result(h, lp, out, m):
         _raise(rc, lib().eb_last_error(h).decode())
 
 
-def make_trampoline(h, evaluate, where, failure):
+def _squeeze(shape):
+    """The record shape with its size-1 axes dropped (``ensemble.py:541-545``)."""
+    return tuple(int(n) for n in shape if n != 1)
+
+
+FIXED_WIDTH = (
+    "device blobs are fixed-width records: numeric, bool, subarray or structured dtypes; object, string and "
+    "ragged blobs are not supported"
+)
+
+
+def _variable_width(dt):
+    if dt.hasobject:
+        return True
+    if dt.subdtype is not None:
+        return _variable_width(dt.subdtype[0])
+    if dt.fields:
+        return any(_variable_width(f[0]) for f in dt.fields.values())
+    return dt.kind in "US"  # the reference stores strings as objects (ensemble.py:530-532)
+
+
+def fixed_width_dtype(dtype, what="blobs_dtype"):
+    """``np.dtype(dtype)``, or ``NotImplementedError`` when its records are not plain bytes the engine may copy
+    (object pointers, strings)."""
+    dt = np.dtype(dtype)
+    if _variable_width(dt):
+        raise NotImplementedError("%s %s: %s" % (what, dt, FIXED_WIDTH))
+    return dt
+
+
+class BlobSink(object):
+    """The blob half of a callback that declares ``blobs_dtype``: checks the records the function returned and
+    hands them to the engine (``eb_callback_blobs``).  A layout is ``(dtype, shape)``: one walker's record is an
+    array of that dtype and shape, ``record_bytes = dtype.itemsize * prod(shape)``.
+
+    ``expect``: the live layout the records must have (None: any); ``last``: the layout of the records the last
+    call delivered, None when it delivered none."""
+
+    def __init__(self, blobs_dtype):
+        declared = fixed_width_dtype(blobs_dtype)
+        self.dtype = declared.base  # a subarray dtype's shape becomes trailing axes, as np.array(blob, dtype) does
+        self.expect = None
+        self.last = None
+
+    def layout(self, dtype, shape, m):
+        if len(shape) < 1 or shape[0] != m:
+            raise ValueError("the function returned blobs of shape %s for %d rows; expected (%d, ...)"
+                             % (tuple(shape), m, m))
+        if np.dtype(dtype) != self.dtype:
+            raise TypeError("the function must return blobs of dtype %s, got %s" % (self.dtype, np.dtype(dtype)))
+        lay = (self.dtype, _squeeze(shape[1:]))
+        if self.dtype.itemsize * int(np.prod(lay[1], dtype=np.int64)) == 0:
+            raise ValueError("the function returned empty blob records")
+        if self.expect is not None and lay != self.expect:
+            raise ValueError("the function returned blobs of dtype %s and shape %s; the state's blobs have dtype %s "
+                             "and shape %s" % (lay[0], lay[1], self.expect[0], self.expect[1]))
+        return lay
+
+    def deliver(self, h, blobs, m, device):
+        if blobs is None:
+            raise ValueError("the log-probability function was declared with blobs_dtype=%s but returned no blobs"
+                             % self.dtype)
+        cai = getattr(blobs, "__cuda_array_interface__", None) if device else None
+        if cai is None:
+            a = np.ascontiguousarray(blobs)
+            lay = self.layout(a.dtype, a.shape, m)
+            rec = a.itemsize * int(np.prod(lay[1], dtype=np.int64))
+            ptr, stride, stream = a.ctypes.data, rec, 0
+        else:
+            if cai.get("mask") is not None:
+                raise ValueError("masked CUDA arrays are not supported as blobs")
+            dt = np.dtype(cai["descr"]) if cai["typestr"].startswith("|V") and "descr" in cai else np.dtype(cai["typestr"])
+            shape = tuple(cai["shape"])
+            lay = self.layout(dt, shape, m)
+            rec = dt.itemsize * int(np.prod(lay[1], dtype=np.int64))
+            strides = cai.get("strides")
+            stride = rec
+            if strides is not None:
+                # a record must be one packed block: the axes after the first C-contiguous (size-1 axes aside)
+                inner = [(int(n), int(s)) for n, s in zip(shape[1:], strides[1:]) if n != 1]
+                want = dt.itemsize
+                for n, s in reversed(inner):
+                    if s != want:
+                        raise ValueError("blob records must be contiguous; only the first axis may be strided")
+                    want *= n
+                if m > 1:
+                    stride = int(strides[0])
+                    if stride < rec:
+                        raise ValueError("the blobs' first-axis stride (%d bytes) is shorter than a record (%d bytes)"
+                                         % (stride, rec))
+            stream = (cai["stream"] or 0) if "stream" in cai else EB_STREAM_UNKNOWN
+            ptr = cai["data"][0]
+        rc = lib().eb_callback_blobs(h, C.c_void_p(ptr), int(rec), int(stride), int(m), int(stream))
+        if rc != EB_OK:
+            _raise(rc, lib().eb_last_error(h).decode())
+        self.last = lay
+
+
+def _split_blobs(out):
+    """``(lp, blobs)`` of a blob function's result; a result that is not such a pair carries no blobs."""
+    if isinstance(out, tuple) and len(out) == 2:
+        return out
+    return out, None
+
+
+def make_trampoline(h, evaluate, where, failure, blobs=None):
     """The C callback of one engine: calls ``evaluate`` (host mode: a fresh ``x[m, ndim]`` ndarray the
     function owns; device mode: :class:`DeviceRows`) and writes its result into the engine's ``lp``.
-    Any exception is stored as ``failure[0]`` and the engine is told to stop (``EB_ERR_CALLBACK``)."""
+    With a :class:`BlobSink` ``blobs``, ``evaluate`` returns ``(lp, blobs)`` and the records go to the engine
+    too.  Any exception is stored as ``failure[0]`` and the engine is told to stop (``EB_ERR_CALLBACK``)."""
 
     def host(user, x, m, ndim, lp, stream):
         try:
             rows = np.ctypeslib.as_array(x, shape=(m, ndim)).copy()
-            np.ctypeslib.as_array(lp, shape=(m,))[:] = _host_result(evaluate(rows), m)
+            out = evaluate(rows)
+            if blobs is not None:
+                out, b = _split_blobs(out)
+                blobs.deliver(h, b, m, False)
+            np.ctypeslib.as_array(lp, shape=(m,))[:] = _host_result(out, m)
             return 0
         except BaseException as e:  # noqa: B902 -- re-raised unchanged when the ABI call returns
             failure[0] = e
@@ -295,7 +415,11 @@ def make_trampoline(h, evaluate, where, failure):
     def device(user, x, m, ndim, lp, stream):
         rows = DeviceRows(C.cast(x, C.c_void_p).value, m, ndim, stream)
         try:
-            _device_result(h, lp, evaluate(rows), m)
+            out = evaluate(rows)
+            if blobs is not None:
+                out, b = _split_blobs(out)
+                blobs.deliver(h, b, m, True)
+            _device_result(h, lp, out, m)
             return 0
         except BaseException as e:  # noqa: B902
             failure[0] = e
@@ -394,6 +518,8 @@ class Engine(object):
         self._h = C.c_void_p()
         self._cb = None  # the registered C callback (kept alive while the engine may call it)
         self._cb_failure = [None]
+        self._blob_sink = None  # BlobSink of a callback that declares blobs_dtype
+        self._blob_layout = None  # (dtype, shape) of the state's blob records, or None
         self.nwalkers, self.ndim = int(nwalkers), int(ndim)
         rc = lib().eb_create(int(device), self.nwalkers, self.ndim, int(seed) & (2**64 - 1), C.byref(self._h))
         if rc != EB_OK:
@@ -436,19 +562,61 @@ class Engine(object):
         hi = _f64(np.asarray(upper, dtype=np.float64).ravel(), (self.ndim,))
         self._check(lib().eb_model_set_bounds(self._h, _as_dp(lo), _as_dp(hi)))
 
-    def set_callback(self, evaluate, where):
+    def set_callback(self, evaluate, where, blobs_dtype=None):
         """Make ``evaluate`` the model (``eb_model_set_callback``): called once per half-step with the
         split's proposals, ``where`` = ``"host"`` (a fresh ``[m, ndim]`` ndarray) or ``"device"``
-        (:class:`DeviceRows`).  Its exceptions propagate unchanged from the call that ran it."""
+        (:class:`DeviceRows`).  Its exceptions propagate unchanged from the call that ran it.  With
+        ``blobs_dtype``, ``evaluate`` returns ``(lp, blobs)`` and the engine carries the blobs."""
         mode = {"host": EB_CALLBACK_HOST, "device": EB_CALLBACK_DEVICE}[where]
-        cb = make_trampoline(self._h, evaluate, mode, self._cb_failure)
+        sink = None if blobs_dtype is None else BlobSink(blobs_dtype)
+        cb = make_trampoline(self._h, evaluate, mode, self._cb_failure, sink)
         self._check(lib().eb_model_set_callback(self._h, cb, None, mode))
         self._cb = cb
+        self._blob_sink = sink
+        self._blob_layout = None
 
-    def set_state(self, coords, log_prob=None):
+    def _expect_blobs(self):
+        if self._blob_sink is not None:
+            self._blob_sink.expect = self._blob_layout
+            self._blob_sink.last = None
+
+    def set_state(self, coords, log_prob=None, blobs=None):
+        """Upload the state.  ``log_prob=None``: evaluated by the model, and a blob function's records become
+        the state's blobs.  Otherwise ``blobs`` (``[nwalkers, ...]``, or None) are the state's blobs: they must
+        have the dtype the function declared, and are checked before anything is uploaded -- the engine copies
+        them as raw bytes."""
         coords = _f64(coords, (self.nwalkers, self.ndim))
         lp = None if log_prob is None else _f64(log_prob, (self.nwalkers,))
+        if blobs is not None:
+            if self._blob_sink is None:
+                raise NotImplementedError("the state carries blobs, but the log-probability function declares none")
+            blobs = np.asarray(blobs)
+            fixed_width_dtype(blobs.dtype, "the state's blobs have dtype")
+            if blobs.dtype != self._blob_sink.dtype:
+                raise ValueError("the state's blobs have dtype %s; the function declares %s"
+                                 % (blobs.dtype, self._blob_sink.dtype))
+            blobs = np.ascontiguousarray(blobs)
+            if blobs.ndim < 1 or blobs.shape[0] != self.nwalkers:
+                raise ValueError("invalid blobs size; expected {0}".format(self.nwalkers))
+            if blobs.nbytes == 0:
+                raise ValueError("the state's blob records are empty")
+        self._blob_layout = None
+        self._expect_blobs()
         self._check(lib().eb_set_state(self._h, _as_dp(coords), None if lp is None else _as_dp(lp)))
+        if lp is None:
+            self._blob_layout = None if self._blob_sink is None else self._blob_sink.last
+        elif blobs is not None:
+            self._check(lib().eb_set_state_blobs(self._h, C.c_void_p(blobs.ctypes.data), blobs.nbytes // self.nwalkers))
+            self._blob_layout = (blobs.dtype, _squeeze(blobs.shape[1:]))
+
+    def get_blobs(self):
+        """The state's blobs ``[nwalkers, *shape]`` (a fresh array), or None when it has none."""
+        if self._blob_layout is None:
+            return None
+        dt, shape = self._blob_layout
+        out = np.empty((self.nwalkers,) + shape, dtype=dt)
+        self._check(lib().eb_get_blobs(self._h, C.c_void_p(out.ctypes.data)))
+        return out
 
     def get_state(self, coords=None, log_prob=None):
         """Device -> host copy of the live state, into fresh arrays or into the
@@ -514,6 +682,29 @@ class Engine(object):
         self._check(lib().eb_compute_log_prob(self._h, _as_dp(flat), flat.shape[0], _as_dp(out)))
         return out.reshape(coords.shape[:-1])
 
+    def compute_log_prob_blobs(self, coords):
+        """``(log_prob[...], blobs[..., *shape] or None)`` of a blob function for ``coords[..., ndim]``."""
+        coords = _f64(coords)
+        if coords.shape[-1] != self.ndim:
+            raise ValueError("incompatible input dimensions {0}".format(coords.shape))
+        flat = coords.reshape(-1, self.ndim)
+        m = flat.shape[0]
+        out = np.empty(m, dtype=np.float64)
+        ptr, nbytes = C.c_void_p(), C.c_size_t()
+        self._expect_blobs()
+        self._check(lib().eb_compute_log_prob_blobs(self._h, _as_dp(flat), m, _as_dp(out), C.byref(ptr),
+                                                    C.byref(nbytes)))
+        blobs = None
+        if ptr.value:
+            try:
+                dt, shape = self._blob_sink.last
+                raw = (C.c_char * (m * nbytes.value)).from_address(ptr.value)
+                blobs = np.frombuffer(raw, dtype=dt).reshape((m,) + shape).copy()
+            finally:
+                lib().eb_host_free(ptr)
+            blobs = blobs.reshape(coords.shape[:-1] + shape)
+        return out.reshape(coords.shape[:-1]), blobs
+
     # -- rng -----------------------------------------------------------------
     def set_rng(self, seed, step):
         self._check(lib().eb_set_rng(self._h, int(seed) & (2**64 - 1), int(step)))
@@ -555,6 +746,7 @@ class Engine(object):
 
     def step(self, moves, nsteps, want_accepted=True):
         arr = self.pack_moves(moves)
+        self._expect_blobs()
         acc = np.zeros(self.nwalkers, dtype=np.uint8) if want_accepted else None
         self._check(
             lib().eb_step(
@@ -564,14 +756,29 @@ class Engine(object):
         )
         return None if acc is None else acc.astype(bool)
 
-    def step_store(self, moves, nsteps, thin_by, chain, log_prob, accepted):
+    def step_store(self, moves, nsteps, thin_by, chain, log_prob, accepted, blobs=None):
+        """``blobs`` (``[nstore, nwalkers, ...]`` C-contiguous, the state's record layout, or None) gets the
+        blobs of the stored steps."""
         arr = self.pack_moves(moves)
         assert chain.flags.c_contiguous and log_prob.flags.c_contiguous and accepted.flags.c_contiguous
         assert chain.dtype == np.float64 and log_prob.dtype == np.float64 and accepted.dtype == np.float64
+        self._expect_blobs()
+        if blobs is None:
+            self._check(
+                lib().eb_step_store(
+                    self._h, arr, len(arr), int(nsteps), int(thin_by),
+                    _as_dp(chain), _as_dp(log_prob), _as_dp(accepted),
+                )
+            )
+            return
+        dt, shape = self._blob_layout
+        nstore = int(nsteps) // int(thin_by)
+        if not blobs.flags.c_contiguous or blobs.nbytes != nstore * self.nwalkers * dt.itemsize * int(np.prod(shape)):
+            raise ValueError("the blob store does not match the state's blob records")
         self._check(
-            lib().eb_step_store(
+            lib().eb_step_store_blobs(
                 self._h, arr, len(arr), int(nsteps), int(thin_by),
-                _as_dp(chain), _as_dp(log_prob), _as_dp(accepted),
+                _as_dp(chain), _as_dp(log_prob), _as_dp(accepted), C.c_void_p(blobs.ctypes.data),
             )
         )
 

@@ -1,12 +1,12 @@
 """Chain stores with the reference's ``Backend`` protocol
 (``src/emcee/backends/backend.py:12-237``): ``reset / grow / save_step /
 get_chain / get_log_prob / get_last_sample / shape / iteration / accepted /
-random_state``.  ``Backend`` keeps the chain in host memory, ``DeviceBackend``
-in the GPU's.  Blobs do not exist on the device path.
+random_state``.  ``Backend`` keeps the chain in host memory, with the reference's
+blob storage; ``DeviceBackend`` keeps it in the GPU's, without blobs.
 
-The engine's ``eb_step_store`` writes stored steps straight into the
-``chain`` / ``log_prob`` arrays of this class (pinned double-buffered D2H), so
-``store=True`` does not need a host round trip per step."""
+The engine's ``eb_step_store_blobs`` writes stored steps straight into the
+``chain`` / ``log_prob`` / ``blobs`` arrays of this class (pinned double-buffered
+D2H), so ``store=True`` does not need a host round trip per step."""
 
 import numpy as np
 
@@ -33,39 +33,69 @@ class Backend(object):
         self.initialized = True
 
     def has_blobs(self):
-        return False
+        return self.blobs is not None
 
     @property
     def shape(self):
         return self.nwalkers, self.ndim
 
     # -- growth / writes ------------------------------------------------------
+    def _check_blobs(self, blobs):
+        """``backend.py:157-162``."""
+        if self.has_blobs() and blobs is None:
+            raise ValueError("inconsistent use of blobs")
+        if self.iteration > 0 and blobs is not None and not self.has_blobs():
+            raise ValueError("inconsistent use of blobs")
+
     def grow(self, ngrow, blobs):
-        """Room for ``ngrow`` more stored steps (``backend.py:164-185``)."""
-        if blobs is not None:
-            raise NotImplementedError("blobs are not supported on the device path")
-        extra = int(ngrow) - (len(self.chain) - self.iteration)
-        if extra <= 0:
+        """Room for ``ngrow`` more stored steps (``backend.py:164-185``).  ``blobs`` (the state's,
+        ``[nwalkers, ...]``, or None) gives the record type of the blob store,
+        ``(blobs.dtype, blobs.shape[1:])``; every grow must bring the same one."""
+        self._check_blobs(blobs)
+        extra = max(int(ngrow) - (len(self.chain) - self.iteration), 0)
+        if extra:
+            total = len(self.chain) + extra
+            chain = np.empty((total, self.nwalkers, self.ndim), dtype=self.dtype)
+            chain[: len(self.chain)] = self.chain
+            log_prob = np.empty((total, self.nwalkers), dtype=self.dtype)
+            log_prob[: len(self.log_prob)] = self.log_prob
+            self.chain, self.log_prob = chain, log_prob
+        if blobs is None:
             return
-        total = len(self.chain) + extra
-        chain = np.empty((total, self.nwalkers, self.ndim), dtype=self.dtype)
-        chain[: len(self.chain)] = self.chain
-        log_prob = np.empty((total, self.nwalkers), dtype=self.dtype)
-        log_prob[: len(self.log_prob)] = self.log_prob
-        self.chain, self.log_prob = chain, log_prob
+        blobs = np.asarray(blobs)
+        dt = np.dtype((blobs.dtype, blobs.shape[1:]))
+        if self.blobs is None:
+            self.blobs = np.empty((len(self.chain), self.nwalkers), dtype=dt)
+            return
+        # the reference concatenates (backend.py:180-185), which refuses another record shape; the engine
+        # writes raw records, so another dtype of the same size is refused too
+        if np.dtype((self.blobs.dtype, self.blobs.shape[2:])) != dt:
+            raise ValueError("inconsistent blobs: stored as {0}, got {1}".format(
+                np.dtype((self.blobs.dtype, self.blobs.shape[2:])), dt))
+        if len(self.blobs) < len(self.chain):
+            grown = np.empty((len(self.chain), self.nwalkers), dtype=dt)
+            grown[: len(self.blobs)] = self.blobs
+            self.blobs = grown
 
     def save_step(self, state, accepted):
-        """Append one step (``backend.py:214-231``)."""
+        """Append one step (``backend.py:187-231``)."""
+        self._check_blobs(state.blobs)
         if state.coords.shape != self.shape:
             raise ValueError("invalid coordinate dimensions; expected {0}".format(self.shape))
         if state.log_prob.shape != (self.nwalkers,):
             raise ValueError("invalid log probability size; expected {0}".format(self.nwalkers))
+        if state.blobs is not None and not self.has_blobs():
+            raise ValueError("unexpected blobs")
+        if state.blobs is None and self.has_blobs():
+            raise ValueError("expected blobs, but none were given")
+        if state.blobs is not None and len(state.blobs) != self.nwalkers:
+            raise ValueError("invalid blobs size; expected {0}".format(self.nwalkers))
         if accepted.shape != (self.nwalkers,):
             raise ValueError("invalid acceptance size; expected {0}".format(self.nwalkers))
-        if state.blobs is not None:
-            raise ValueError("unexpected blobs")
         self.chain[self.iteration] = state.coords
         self.log_prob[self.iteration] = state.log_prob
+        if state.blobs is not None:
+            self.blobs[self.iteration] = state.blobs
         self.accepted += accepted
         self.random_state = state.random_state
         self.iteration += 1
@@ -76,7 +106,7 @@ class Backend(object):
             raise AttributeError(
                 "you must run the sampler with 'store == True' before accessing the results"
             )
-        if name == "blobs":
+        if name == "blobs" and not self.has_blobs():
             return None
         v = getattr(self, name)[discard + thin - 1 : self.iteration : thin]  # backend.py:53
         if flat:
@@ -99,7 +129,8 @@ class Backend(object):
                 "you must run the sampler with 'store == True' before accessing the results"
             )
         k = self.iteration - 1
-        return State(self.chain[k], log_prob=self.log_prob[k], blobs=None, random_state=self.random_state)
+        blobs = self.blobs[k] if self.has_blobs() else None
+        return State(self.chain[k], log_prob=self.log_prob[k], blobs=blobs, random_state=self.random_state)
 
     def get_autocorr_time(self, discard=0, thin=1, **kwargs):
         """Integrated autocorrelation time per parameter, in steps

@@ -142,11 +142,35 @@ struct eb_ctx {
   size_t cb_rows = 0;
   double* ext_f = nullptr;         // device [N] Hastings factors of the propose phase
   double* ext_lp = nullptr;        // device [N] the callback's log-probabilities
+  int cb_phase = 0;                // CB_STEP / CB_SET_STATE / CB_COMPUTE: what the running callback evaluates
+  int64_t cb_m = 0;                // rows of the running callback
+
+  // blobs of a callback model (eb_callback_blobs): packed records of blob_bytes bytes, one per walker
+  size_t blob_bytes = 0;           // the live layout (0: none)
+  bool blobs_live = false;         // blob_live holds the records of the current state
+  uint8_t* blob_live = nullptr;    // device [N, blob_bytes]
+  uint8_t* blob_prop = nullptr;    // device [N, blob_bytes] the records of the running half-step's proposals
+  uint8_t* blob_host = nullptr;    // host mode: pinned [N, blob_bytes] staging of the function's records
+  size_t blob_cap = 0;             // bytes of each of the three buffers
+  int64_t cb_blob_rows = -1;       // records the running callback delivered (-1: none)
+  size_t cb_blob_bytes = 0;        // their size
+  uint8_t* cb_blob_dst = nullptr;  // host mode: where run_callback copies blob_host to, next to the lp copy-back
+  uint8_t* cmp_blobs = nullptr;    // CB_COMPUTE: pinned [m, record] records handed to the caller
+  uint8_t* stage_blob[2] = {nullptr, nullptr};  // eb_step_store_blobs: pinned [N, blob_bytes] staging
+  size_t stage_blob_cap = 0;
 
   std::string err;
 };
 
 static thread_local std::string g_create_err;
+
+// what a running log-probability callback evaluates: a half-step's proposals, the state of eb_set_state(coords,
+// NULL), or the rows of eb_compute_log_prob -- it decides where eb_callback_blobs puts the records
+enum { CB_STEP = 0, CB_SET_STATE = 1, CB_COMPUTE = 2 };
+
+static const char* const MSG_BLOBS_WITH_LOG_PROB =  // moves/move.py:38-42
+    "If you start sampling with a given log_prob, you also need to provide the current list of blobs at that "
+    "position.";
 
 #define NOT_IN_CALLBACK(ctx)                                                      \
   do {                                                                            \
@@ -326,6 +350,11 @@ int eb_destroy(eb_ctx* c) {
   cudaFree(c->cb_xdev);
   cudaFree(c->ext_f);
   cudaFree(c->ext_lp);
+  cudaFree(c->blob_live);
+  cudaFree(c->blob_prop);
+  cudaFreeHost(c->blob_host);
+  cudaFreeHost(c->cmp_blobs);
+  for (int k = 0; k < 2; ++k) cudaFreeHost(c->stage_blob[k]);
   if (c->ev0) cudaEventDestroy(c->ev0);
   if (c->ev1) cudaEventDestroy(c->ev1);
   if (c->st) cudaStreamDestroy(c->st);
@@ -413,6 +442,8 @@ int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
   c->have_model = true;
   c->cb_fn = nullptr;
   c->cb_user = nullptr;
+  c->blob_bytes = 0;
+  c->blobs_live = false;
   return EB_OK;
 }
 
@@ -441,18 +472,49 @@ int eb_model_set_callback(eb_ctx* c, eb_logprob_fn fn, void* user, int where) {
   c->cb_where = where;
   c->chain_ok = false;
   c->have_model = true;
+  c->blob_bytes = 0;
+  c->blobs_live = false;
   return EB_OK;
 }
 
-int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_bytes, int64_t m, uint64_t src_stream) {
-  if (!c) return EB_ERR_INVALID;
-  if (!c->in_callback || c->cb_where != EB_CALLBACK_DEVICE)
-    FAIL(c, EB_ERR_STATE, "eb_callback_result: only from inside a device-mode log-probability callback");
-  if (m < 0 || (m > 0 && (!lp || !src))) FAIL(c, EB_ERR_INVALID, "eb_callback_result: null buffer");
-  if (stride_bytes <= 0 || stride_bytes % (int64_t)sizeof(double) != 0)
-    FAIL(c, EB_ERR_INVALID, "eb_callback_result: the stride must be a positive multiple of 8 bytes (got %lld)",
-         (long long)stride_bytes);
-  if (m == 0) return EB_OK;
+// device buffers for records of `record_bytes` (live + one call's proposals, and the host-mode staging): the size
+// is checked against the free device memory before any allocation, as eb_chain_grow does
+static int ensure_blob_buffers(eb_ctx* c, size_t record_bytes) {
+  const size_t N = (size_t)c->N;
+  const bool host = c->cb_where == EB_CALLBACK_HOST;
+  if (record_bytes > ((size_t)1 << 40) / N)
+    FAIL(c, EB_ERR_NOMEM, "blob records of %zu bytes for %zu walkers do not fit in device memory", record_bytes, N);
+  const size_t need = N * record_bytes;
+  if (need <= c->blob_cap && (!host || c->blob_host)) return EB_OK;
+  CK(c, cudaStreamSynchronize(c->st));
+  size_t free_b = 0, total_b = 0;
+  CK(c, cudaMemGetInfo(&free_b, &total_b));
+  const size_t held = 2 * c->blob_cap;  // freed below before the new buffers are allocated
+  if (2 * need > free_b + held)
+    FAIL(c, EB_ERR_NOMEM, "blob buffers need %zu bytes of device memory, %zu are free", 2 * need, free_b + held);
+  cudaFree(c->blob_live);
+  cudaFree(c->blob_prop);
+  cudaFreeHost(c->blob_host);
+  c->blob_live = c->blob_prop = c->blob_host = nullptr;
+  c->blob_cap = 0;
+  c->blobs_live = false;
+  const size_t cap = need;
+  if (cudaMalloc(&c->blob_live, cap) != cudaSuccess || cudaMalloc(&c->blob_prop, cap) != cudaSuccess ||
+      (host && cudaMallocHost(&c->blob_host, cap) != cudaSuccess)) {
+    cudaGetLastError();
+    cudaFree(c->blob_live);
+    cudaFree(c->blob_prop);
+    c->blob_live = c->blob_prop = nullptr;
+    FAIL(c, EB_ERR_NOMEM, "allocating %zu bytes of blob buffers failed", 2 * cap);
+  }
+  c->blob_cap = cap;
+  return EB_OK;
+}
+
+// m records of `width` bytes, `spitch` apart in src (device or host memory), packed into dst (eb_callback_result,
+// eb_callback_blobs): ordered after the producer's work, complete when this returns
+static int copy_records(eb_ctx* c, void* dst, const void* src, size_t width, size_t spitch, size_t m,
+                        uint64_t src_stream) {
   if (src_stream == EB_STREAM_UNKNOWN) {
     // a producer that names no stream (CUDA Array Interface v2, e.g. torch): its last kernel may be on any
     // stream of the device, so wait for all of them
@@ -469,11 +531,87 @@ int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_by
     cudaEventDestroy(ev);
     CK(c, e);
   }
-  CK(c, cudaMemcpy2DAsync(lp, sizeof(double), src, (size_t)stride_bytes, sizeof(double), (size_t)m, cudaMemcpyDefault,
-                          c->st));
-  // the caller may free or reuse src as soon as this returns
-  CK(c, cudaStreamSynchronize(c->st));
+  if (spitch == width || m == 1)
+    CK(c, cudaMemcpyAsync(dst, src, width * m, cudaMemcpyDefault, c->st));
+  else
+    CK(c, cudaMemcpy2DAsync(dst, width, src, spitch, width, m, cudaMemcpyDefault, c->st));
+  CK(c, cudaStreamSynchronize(c->st));  // the caller may free or reuse src as soon as this returns
   return EB_OK;
+}
+
+int eb_callback_blobs(eb_ctx* c, const void* src, int64_t record_bytes, int64_t stride_bytes, int64_t m,
+                      uint64_t src_stream) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->in_callback) FAIL(c, EB_ERR_STATE, "eb_callback_blobs: only from inside a log-probability callback");
+  if (c->cb_blob_rows >= 0) FAIL(c, EB_ERR_INVALID, "eb_callback_blobs: this call's blobs were already delivered");
+  if (m != c->cb_m)
+    FAIL(c, EB_ERR_INVALID, "the function returned %lld blob records for %lld rows", (long long)m, (long long)c->cb_m);
+  if (record_bytes <= 0) FAIL(c, EB_ERR_INVALID, "eb_callback_blobs: records must have at least one byte");
+  if (m > 1 && stride_bytes < record_bytes)
+    FAIL(c, EB_ERR_INVALID, "eb_callback_blobs: the stride (%lld bytes) is shorter than a record (%lld bytes)",
+         (long long)stride_bytes, (long long)record_bytes);
+  if (m > 0 && !src) FAIL(c, EB_ERR_INVALID, "eb_callback_blobs: null records");
+  const size_t R = (size_t)record_bytes;
+  uint8_t* dst = nullptr;
+  bool to_host = c->cb_where == EB_CALLBACK_HOST;
+  switch (c->cb_phase) {
+    case CB_SET_STATE: {  // the initial evaluation fixes the live layout
+      int rc = ensure_blob_buffers(c, R);
+      if (rc) return rc;
+      dst = c->blob_live;
+      break;
+    }
+    case CB_STEP:
+      if (!c->blobs_live) FAIL(c, EB_ERR_INVALID, "%s", MSG_BLOBS_WITH_LOG_PROB);
+      if (R != c->blob_bytes)
+        FAIL(c, EB_ERR_INVALID, "the function returned blob records of %zu bytes; the state's records have %zu", R,
+             c->blob_bytes);
+      dst = c->blob_prop;
+      break;
+    default:  // CB_COMPUTE: straight to the caller's pinned buffer
+      if (c->blob_bytes && R != c->blob_bytes)
+        FAIL(c, EB_ERR_INVALID, "the function returned blob records of %zu bytes; the state's records have %zu", R,
+             c->blob_bytes);
+      cudaFreeHost(c->cmp_blobs);
+      c->cmp_blobs = nullptr;
+      if (cudaMallocHost(&c->cmp_blobs, std::max<size_t>(1, (size_t)m * R)) != cudaSuccess) {
+        cudaGetLastError();
+        c->cmp_blobs = nullptr;
+        FAIL(c, EB_ERR_NOMEM, "allocating %zu bytes of pinned host memory for blobs failed", (size_t)m * R);
+      }
+      dst = c->cmp_blobs;
+      to_host = false;  // copied below, whatever the mode
+  }
+  if (m > 0) {
+    if (to_host) {
+      // host mode: into the pinned staging; run_callback copies it to dst next to the lp copy-back
+      const uint8_t* s = static_cast<const uint8_t*>(src);
+      if ((size_t)stride_bytes == R)
+        memcpy(c->blob_host, s, (size_t)m * R);
+      else
+        for (int64_t r = 0; r < m; ++r) memcpy(c->blob_host + (size_t)r * R, s + (size_t)r * stride_bytes, R);
+      c->cb_blob_dst = dst;
+    } else {
+      int rc = copy_records(c, dst, src, R, (size_t)stride_bytes, (size_t)m, src_stream);
+      if (rc) return rc;
+      c->cb_blob_dst = nullptr;
+    }
+  }
+  c->cb_blob_rows = m;
+  c->cb_blob_bytes = R;
+  return EB_OK;
+}
+
+int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_bytes, int64_t m, uint64_t src_stream) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->in_callback || c->cb_where != EB_CALLBACK_DEVICE)
+    FAIL(c, EB_ERR_STATE, "eb_callback_result: only from inside a device-mode log-probability callback");
+  if (m < 0 || (m > 0 && (!lp || !src))) FAIL(c, EB_ERR_INVALID, "eb_callback_result: null buffer");
+  if (stride_bytes <= 0 || stride_bytes % (int64_t)sizeof(double) != 0)
+    FAIL(c, EB_ERR_INVALID, "eb_callback_result: the stride must be a positive multiple of 8 bytes (got %lld)",
+         (long long)stride_bytes);
+  if (m == 0) return EB_OK;
+  return copy_records(c, lp, src, sizeof(double), (size_t)stride_bytes, (size_t)m, src_stream);
 }
 
 int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
@@ -554,6 +692,9 @@ static int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool 
     // stream of its own
     CK(c, cudaStreamSynchronize(c->st));
   }
+  c->cb_m = m;
+  c->cb_blob_rows = -1;
+  c->cb_blob_dst = nullptr;
   c->in_callback = true;
   const int r = host ? c->cb_fn(c->cb_user, c->cb_x, m, (int64_t)D, c->cb_lp, nullptr)
                      : c->cb_fn(c->cb_user, c->cb_xdev, m, (int64_t)D, lp, (void*)c->st);
@@ -562,7 +703,13 @@ static int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool 
     cudaStreamSynchronize(c->st);  // whatever the function enqueued before it failed
     FAIL(c, EB_ERR_CALLBACK, "the log-probability callback failed (returned %d)", r);
   }
+  if (c->cb_phase == CB_STEP && c->blobs_live && c->cb_blob_rows < 0)
+    FAIL(c, EB_ERR_INVALID, "the log-probability function returned no blobs; the state has blob records of %zu bytes",
+         c->blob_bytes);
   if (host) CK(c, cudaMemcpyAsync(lp, c->cb_lp, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  // host-mode blob records ride with the lp copy-back: no synchronisation of their own
+  if (c->cb_blob_dst)
+    CK(c, cudaMemcpyAsync(c->cb_blob_dst, c->blob_host, (size_t)m * c->cb_blob_bytes, cudaMemcpyHostToDevice, c->st));
   CK(c, launch_scan_nonfinite(lp, (size_t)m, 1, c->status_dev, c->st));
   return fetch_status(c);  // ensemble.py:550-551, before any update
 }
@@ -600,6 +747,7 @@ int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) 
   CK(c, cudaMemcpyAsync(c->scratch_x, coords, m * (size_t)c->D * sizeof(double), cudaMemcpyHostToDevice,
                         c->st));
   if (c->model.kind == MODEL_EXTERNAL) {
+    c->cb_phase = CB_COMPUTE;
     rc = run_callback(c, c->scratch_x, (int64_t)m, c->scratch_lp, true);
     if (rc) return rc;
   } else {
@@ -607,6 +755,29 @@ int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) 
   }
   CK(c, cudaMemcpyAsync(out, c->scratch_lp, m * sizeof(double), cudaMemcpyDeviceToHost, c->st));
   return fetch_status(c);
+}
+
+int eb_compute_log_prob_blobs(eb_ctx* c, const double* coords, size_t m, double* out, void** blobs_out,
+                              size_t* record_bytes) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!blobs_out || !record_bytes) FAIL(c, EB_ERR_INVALID, "eb_compute_log_prob_blobs: null output");
+  *blobs_out = nullptr;
+  *record_bytes = 0;
+  if (c->have_model && c->model.kind != MODEL_EXTERNAL)
+    FAIL(c, EB_ERR_UNSUPPORTED, "eb_compute_log_prob_blobs: only log-probability callbacks return blobs");
+  cudaFreeHost(c->cmp_blobs);
+  c->cmp_blobs = nullptr;
+  c->cb_blob_rows = -1;
+  const int rc = eb_compute_log_prob(c, coords, m, out);
+  if (rc == EB_OK && c->cb_blob_rows >= 0 && c->cmp_blobs) {
+    *blobs_out = c->cmp_blobs;
+    *record_bytes = c->cb_blob_bytes;
+  } else {
+    cudaFreeHost(c->cmp_blobs);
+  }
+  c->cmp_blobs = nullptr;
+  return rc;
 }
 
 // ---- state -------------------------------------------------------------------
@@ -643,6 +814,8 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   const size_t D = (size_t)c->D;
   c->have_state = false;
   c->chain_ok = false;
+  c->blobs_live = false;  // a given log_prob comes without blobs (eb_set_state_blobs adds them)
+  c->blob_bytes = 0;
   if (log_prob) {
     for (int64_t w = 0; w < c->N; ++w)
       if (isnan(log_prob[w])) FAIL(c, EB_ERR_NAN_INITIAL, "The initial log_prob was NaN");  // ensemble.py:357-358
@@ -664,8 +837,13 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   if (log_prob) {
     CK(c, cudaMemcpyAsync(c->logp + r0, log_prob + r0, rows * sizeof(double), cudaMemcpyHostToDevice, c->st));
   } else if (c->model.kind == MODEL_EXTERNAL) {
+    c->cb_phase = CB_SET_STATE;
     int rc = run_callback(c, c->coords, (int64_t)rows, c->logp, true);  // one GPU: rows == nwalkers
     if (rc) return rc;
+    if (c->cb_blob_rows >= 0) {  // the records went to blob_live: they fix the live layout
+      c->blob_bytes = c->cb_blob_bytes;
+      c->blobs_live = true;
+    }
   } else {
     CK(c, launch_logprob(c, c->coords + (size_t)r0 * D, (int64_t)rows, c->logp + r0));
   }
@@ -696,6 +874,38 @@ int eb_get_state(eb_ctx* c, double* coords, double* log_prob) {
                           c->st));
   if (log_prob)
     CK(c, cudaMemcpyAsync(log_prob, c->logp, (size_t)c->N * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  CK(c, cudaStreamSynchronize(c->st));
+  return EB_OK;
+}
+
+int eb_set_state_blobs(eb_ctx* c, const void* blobs, size_t record_bytes) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->have_state) FAIL(c, EB_ERR_STATE, "eb_set_state_blobs: no state set");
+  if ((blobs == nullptr) != (record_bytes == 0))
+    FAIL(c, EB_ERR_INVALID, "eb_set_state_blobs: pass records and their size, or NULL, 0 to clear them");
+  c->blobs_live = false;
+  c->blob_bytes = 0;
+  if (!blobs) return EB_OK;
+  if (c->model.kind != MODEL_EXTERNAL)
+    FAIL(c, EB_ERR_UNSUPPORTED, "eb_set_state_blobs: only log-probability callbacks have blobs");
+  CK(c, cudaSetDevice(c->device));
+  int rc = ensure_blob_buffers(c, record_bytes);
+  if (rc) return rc;
+  CK(c, cudaMemcpyAsync(c->blob_live, blobs, (size_t)c->N * record_bytes, cudaMemcpyHostToDevice, c->st));
+  CK(c, cudaStreamSynchronize(c->st));
+  c->blob_bytes = record_bytes;
+  c->blobs_live = true;
+  return EB_OK;
+}
+
+int eb_get_blobs(eb_ctx* c, void* out) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->blobs_live) FAIL(c, EB_ERR_STATE, "eb_get_blobs: the state has no blobs");
+  if (!out) FAIL(c, EB_ERR_INVALID, "eb_get_blobs: null buffer");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaMemcpyAsync(out, c->blob_live, (size_t)c->N * c->blob_bytes, cudaMemcpyDeviceToHost, c->st));
   CK(c, cudaStreamSynchronize(c->st));
   return EB_OK;
 }
@@ -943,11 +1153,17 @@ int callback_half_step(eb_ctx* c, int move_kind, HalfStepArgs a, uint64_t& launc
     CK(c, launch_half_step_external(move_kind, a, ext, c->st));
     ++launches;
   }
+  c->cb_phase = CB_STEP;
   int rc = run_callback(c, c->qbuf, (int64_t)a.i_hi - a.i_lo, c->ext_lp, move_kind == MOVE_PRECOMPUTED);
   if (rc) return rc;
   a.qbuf = c->qbuf;
   CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st));
   ++launches;
+  if (c->blobs_live) {  // accepted walkers take their proposal's record (moves/move.py:36-43)
+    CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop, c->blob_live,
+                             c->blob_bytes, c->st));
+    ++launches;
+  }
   c->last_kernel = "callback";
   snprintf(c->last_variant, sizeof(c->last_variant), "callback G=%d where=%s", lanes_per_walker(c->D),
            c->cb_where == EB_CALLBACK_HOST ? "host" : "device");
@@ -1439,10 +1655,16 @@ int eb_step(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uin
 
 int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
                   double* chain, double* log_prob, double* accepted) {
+  return eb_step_store_blobs(c, moves, nmoves, nsteps, thin_by, chain, log_prob, accepted, nullptr);
+}
+
+int eb_step_store_blobs(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
+                        double* chain, double* log_prob, double* accepted, void* blobs) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
   if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
   if (!chain || !log_prob) FAIL(c, EB_ERR_INVALID, "eb_step_store: null output buffer");
+  if (blobs && !c->blobs_live) FAIL(c, EB_ERR_STATE, "eb_step_store_blobs: the state has no blobs");
   int rc = step_preflight(c);
   if (rc) return rc;
   Schedule s;
@@ -1457,6 +1679,17 @@ int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nstep
       CK(c, cudaEventCreateWithFlags(&c->stage_ev[k], cudaEventDisableTiming));
     }
   }
+  const size_t blob_row = blobs ? N * c->blob_bytes : 0;  // the blob records of a stored step, staged beside them
+  if (blob_row > c->stage_blob_cap) {
+    for (int k = 0; k < 2; ++k) {
+      cudaFreeHost(c->stage_blob[k]);
+      c->stage_blob[k] = nullptr;
+    }
+    c->stage_blob_cap = 0;
+    for (int k = 0; k < 2; ++k) CK(c, cudaMallocHost(&c->stage_blob[k], blob_row));
+    c->stage_blob_cap = blob_row;
+  }
+  uint8_t* blob_out = static_cast<uint8_t*>(blobs);
   // double-buffered pinned staging: the D2H of stored step k overlaps the
   // kernels of the following steps; the host drains slot k-1 while k is in flight
   uint64_t stored = 0;
@@ -1467,6 +1700,7 @@ int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nstep
     const size_t k = (size_t)pending[slot];
     memcpy(chain + k * N * D, c->stage[slot], N * D * sizeof(double));          // backend.py:224
     memcpy(log_prob + k * N, c->stage[slot] + N * D, N * sizeof(double));        // backend.py:225
+    if (blob_out) memcpy(blob_out + k * blob_row, c->stage_blob[slot], blob_row);  // backend.py:226-227
     if (accepted)
       for (size_t w = 0; w < N; ++w) accepted[w] += (double)c->stage_acc[slot][w];  // backend.py:229
     pending[slot] = -1;
@@ -1489,6 +1723,7 @@ int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nstep
     CK(c, cudaMemcpyAsync(c->stage[slot], c->coords, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     CK(c, cudaMemcpyAsync(c->stage[slot] + N * D, c->logp, N * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     CK(c, cudaMemcpyAsync(c->stage_acc[slot], c->accepted, N, cudaMemcpyDeviceToHost, c->st));
+    if (blob_out) CK(c, cudaMemcpyAsync(c->stage_blob[slot], c->blob_live, blob_row, cudaMemcpyDeviceToHost, c->st));
     CK(c, cudaEventRecord(c->stage_ev[slot], c->st));
     pending[slot] = (int64_t)stored;
     ++stored;

@@ -119,6 +119,10 @@ cudaError_t launch_half_step_generic(int move_kind, const HalfStepArgs& a, cudaS
 // the two launches of a half-step of a callback model (MODEL_EXTERNAL above): move_kind STRETCH / DE / SNOOKER
 // runs the propose phase, MOVE_PRECOMPUTED the accept phase
 cudaError_t launch_half_step_external(int move_kind, const HalfStepArgs& a, const ExternalBufs& ext, cudaStream_t st);
+// blobs of a callback model (blobs.cu): for each active rank i in [i_lo, i_hi), walker w = order ? order[a_start + i]
+// : i takes record i - i_lo of prop[rows, record_bytes] into live[w] when accepted[w] is set (packed records)
+cudaError_t launch_blob_select(const int32_t* order, int a_start, int i_lo, int i_hi, const uint8_t* accepted,
+                               const void* prop, void* live, size_t record_bytes, cudaStream_t st);
 // status |= FLAG_NAN_LOGPROB if any of x[n] is NaN (logprob != 0), else the non-finite parameter flags of x[n]
 cudaError_t launch_scan_nonfinite(const double* x, size_t n, int logprob, int* status, cudaStream_t st);
 // the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)

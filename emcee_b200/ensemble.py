@@ -8,8 +8,8 @@ inside the CUDA library through the C ABI: the walker array stays in HBM
 between steps, ``run_mcmc`` is one call for all iterations (a user function is
 called back from inside it once per half-step), and stored steps stream back
 through pinned buffers.  ``pool`` / ``args`` / ``kwargs`` / ``vectorize``
-belong to ``models.HostFunction``; blobs and named parameters raise
-``NotImplementedError``."""
+and ``blobs_dtype`` belong to ``models.HostFunction`` / ``models.CudaArrayFunction``;
+named parameters raise ``NotImplementedError``."""
 
 from collections.abc import Iterable
 
@@ -30,6 +30,7 @@ _NO_SHARDED_DEVICE_CHAIN = (
     "a DeviceBackend cannot store a sharded ensemble: a stored step holds every walker, and the replication "
     "of the other ranks' rows before each stored step is built for host chains only; use Backend()"
 )
+_NO_DEVICE_CHAIN_BLOBS = "a DeviceBackend does not store blobs; use Backend() with a function that returns blobs"
 
 
 def _seed_from_numpy():
@@ -93,7 +94,10 @@ class EnsembleSampler(object):
         if parameter_names is not None:
             raise NotImplementedError("parameter_names need a host callable")
         if blobs_dtype is not None:
-            raise NotImplementedError("blobs are not supported on the device path")
+            raise NotImplementedError(
+                "blobs_dtype: pass it to models.HostFunction / models.CudaArrayFunction(fn, blobs_dtype=...)")
+        if isinstance(backend, DeviceBackend) and getattr(log_prob_fn, "blobs_dtype", None) is not None:
+            raise NotImplementedError(_NO_DEVICE_CHAIN_BLOBS)
 
         # move schedule (ensemble.py:115-129)
         if moves is None:
@@ -120,7 +124,7 @@ class EnsembleSampler(object):
 
         self.pool = None
         self.vectorize = True  # the device path is always batched
-        self.blobs_dtype = None
+        self.blobs_dtype = getattr(log_prob_fn, "blobs_dtype", None)
         self.ndim = int(ndim)
         self.nwalkers = int(nwalkers)
         self.log_prob_fn = log_prob_fn
@@ -164,7 +168,7 @@ class EnsembleSampler(object):
         # engine's callback
         m = self.log_prob_fn
         if isinstance(m, CallbackFunction):
-            self._engine.set_callback(m.evaluate, m.where)
+            self._engine.set_callback(m.evaluate, m.where, self.blobs_dtype)
             return
         self._engine.set_model(m.kind, m.device_params(self.ndim))
         box = m.bounds(self.ndim)
@@ -274,8 +278,8 @@ class EnsembleSampler(object):
         return [(m.descriptor(), w) for m, w in zip(self._moves, self._raw_weights)]
 
     def _stored_before_failure(self, step0, thin_by, k0):
-        """A bulk run stopped by an exception: the backend keeps the stored steps that completed
-        (the engine drained them before returning), and the random state of the last of them."""
+        """A bulk run stopped by an exception: the backend keeps the stored steps that completed, blobs
+        included (the engine drained them before returning), and the random state of the last of them."""
         b = self.backend
         seed, step = self._engine.get_rng()
         stored = (step - step0) // thin_by
@@ -333,6 +337,9 @@ class EnsembleSampler(object):
         device_store = isinstance(self.backend, DeviceBackend)
         if device_store and self._rdv is not None:
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
+        has_blobs = self.blobs_dtype is not None
+        if device_store and has_blobs:
+            raise NotImplementedError(_NO_DEVICE_CHAIN_BLOBS)
 
         # ``State(initial_state, copy=True)`` in the reference (ensemble.py:312): here the
         # upload to the device IS the copy -- the caller's arrays are only read, and
@@ -342,8 +349,10 @@ class EnsembleSampler(object):
         state_shape = np.shape(state.coords)
         if state_shape != (self.nwalkers, self.ndim):
             raise ValueError("incompatible input dimensions {0}".format(state_shape))
-        if state.blobs is not None:
-            raise NotImplementedError("blobs are not supported on the device path")
+        if state.blobs is not None and not has_blobs:
+            raise NotImplementedError(
+                "the state carries blobs, but the log-probability function declares none "
+                "(models.HostFunction / models.CudaArrayFunction(fn, blobs_dtype=...))")
         if (not skip_initial_state_check) and (not self._walkers_independent(state.coords)):
             raise ValueError(
                 "Initial state has a large condition number. "
@@ -354,8 +363,12 @@ class EnsembleSampler(object):
 
         if state.log_prob is not None and np.shape(state.log_prob) != (self.nwalkers,):
             raise ValueError("incompatible input dimensions")
-        # upload; a missing log_prob is evaluated on the device (ensemble.py:350-358)
-        self._engine.set_state(state.coords, state.log_prob)
+        # upload; a missing log_prob is evaluated on the device (ensemble.py:350-358), and a blob function's
+        # records of that evaluation become the state's blobs
+        self._engine.set_state(state.coords, state.log_prob, state.blobs if state.log_prob is not None else None)
+        eng = self._engine
+        if has_blobs:
+            state.blobs = eng.get_blobs()
 
         if thin is not None:  # deprecated form: store every `thin`-th, yield every step
             thin = int(thin)
@@ -363,18 +376,18 @@ class EnsembleSampler(object):
                 raise ValueError("Invalid thinning argument")
             yield_step, checkpoint_step = 1, thin
             if store:
-                self.backend.grow(iterations // checkpoint_step, None)
+                self.backend.grow(iterations // checkpoint_step, state.blobs)
         else:
             thin_by = int(thin_by)
             if thin_by <= 0:
                 raise ValueError("Invalid thinning argument")
             yield_step = checkpoint_step = thin_by
             if store:
-                self.backend.grow(iterations, None)
+                self.backend.grow(iterations, state.blobs)
 
         native_store = store and (type(self.backend) is Backend or device_store)
+        store_blobs = native_store and state.blobs is not None  # the engine writes them into backend.blobs
         sched = self._schedule()
-        eng = self._engine
 
         def refresh():
             bufs = self._pinned if self._pinned is not None else (
@@ -384,6 +397,8 @@ class EnsembleSampler(object):
                 state.coords, state.log_prob = eng.get_state_rows(r0, n, *bufs)
             else:
                 state.coords, state.log_prob = eng.get_state(*bufs)
+            if has_blobs:
+                state.blobs = eng.get_blobs()
             state.random_state = self.random_state
 
         if _bulk and iterations is not None and (not store or (native_store and thin is None)):
@@ -399,7 +414,7 @@ class EnsembleSampler(object):
                             eng.step_store_chain(sched, total, checkpoint_step, b._ch, k0)
                         else:
                             eng.step_store(sched, total, checkpoint_step, b.chain[k0:k1], b.log_prob[k0:k1],
-                                           b.accepted)
+                                           b.accepted, b.blobs[k0:k1] if store_blobs else None)
                     except BaseException:
                         # a user function's exception, or a NaN it returned, stops the run inside a step
                         self._after_steps()
@@ -435,7 +450,7 @@ class EnsembleSampler(object):
                         eng.step_store_chain(sched, yield_step, yield_step, b._ch, k)
                     else:
                         eng.step_store(sched, yield_step, yield_step, b.chain[k : k + 1], b.log_prob[k : k + 1],
-                                       b.accepted)
+                                       b.accepted, b.blobs[k : k + 1] if store_blobs else None)
                 finally:
                     self._after_steps()
                 b.iteration = k + 1
@@ -489,10 +504,14 @@ class EnsembleSampler(object):
         return walkers_independent(coords)
 
     def compute_log_prob(self, coords):
-        """``(log_prob, None)`` for ``coords[..., ndim]`` evaluated on the device, or by the user
-        function in one call (``ensemble.py:458-553``); raises ``ValueError`` for non-finite
-        parameters or a NaN log-probability like the reference."""
-        return self._engine.compute_log_prob(np.asarray(coords, dtype=np.float64)), None
+        """``(log_prob, blobs)`` for ``coords[..., ndim]`` evaluated on the device, or by the user
+        function in one call (``ensemble.py:458-553``); ``blobs`` is None unless the function declares
+        ``blobs_dtype``.  Raises ``ValueError`` for non-finite parameters or a NaN log-probability like
+        the reference."""
+        coords = np.asarray(coords, dtype=np.float64)
+        if self.blobs_dtype is not None:
+            return self._engine.compute_log_prob_blobs(coords)
+        return self._engine.compute_log_prob(coords), None
 
     # ---------------------------------------------------------------- results
     @property

@@ -19,6 +19,9 @@ The reference takes an arbitrary Python callable ``log_prob_fn``
 
 import numpy as np
 
+from ._lib import FIXED_WIDTH as _FIXED_WIDTH
+from ._lib import fixed_width_dtype
+
 __all__ = [
     "DeviceModel", "GaussianIso", "GaussianDense", "Rosenbrock", "Ring", "Bounded",
     "CallbackFunction", "HostFunction", "CudaArrayFunction",
@@ -166,11 +169,44 @@ def _scalar(fx):
         return float(fx)
 
 
+def blobs_dtype_of(blobs_dtype):
+    """``np.dtype(blobs_dtype)``, or ``NotImplementedError`` for a dtype whose records are not fixed-width bytes."""
+    return None if blobs_dtype is None else fixed_width_dtype(blobs_dtype)
+
+
+def log_prob_and_blobs(results, blobs_dtype):
+    """``(log_prob[M], blobs[M, ...] or None)`` of a batch of results, by the reference's rules
+    (``ensemble.py:498-547``): a result is a scalar (``_scalar``), or a sequence whose first entry is the
+    log-probability and whose rest is the blob, ``blob = [r[1:] for r in results if len(r) > 1]``; the blobs
+    become ``np.array(blob, dtype=blobs_dtype)`` with the size-1 axes after the first squeezed
+    (``ensemble.py:541-545``).  Blobs that do not convert to the fixed-width dtype (strings, objects, ragged
+    rows) raise ``NotImplementedError``."""
+    try:
+        blob = [r[1:] for r in results if len(r) > 1]
+        if not len(blob):
+            raise IndexError
+        log_prob = np.array([_scalar(r[0]) for r in results], dtype=np.float64)
+    except (IndexError, TypeError):
+        return np.array([_scalar(r) for r in results], dtype=np.float64), None
+    if len(blob) != len(log_prob):
+        raise ValueError("%d of %d results carry blobs; every result must" % (len(blob), len(log_prob)))
+    try:
+        blob = np.array(blob, dtype=blobs_dtype)
+    except (TypeError, ValueError) as e:
+        raise NotImplementedError(_FIXED_WIDTH) from e
+    shape = blob.shape[1:]
+    if len(shape):
+        axes = np.arange(len(shape))[np.array(shape) == 1] + 1
+        if len(axes):
+            blob = np.squeeze(blob, tuple(axes))
+    return log_prob, blob
+
+
 def log_prob_values(results):
     """The log-probability vector of a batch of results, by the reference's rules
     (``ensemble.py:498-512``): each result is a scalar (``_scalar``), or a sequence whose first entry
-    is the log-probability and the rest blobs -- which the engine does not store, so they raise
-    ``NotImplementedError``."""
+    is the log-probability and the rest blobs -- which a function without ``blobs_dtype`` may not
+    return, so they raise ``NotImplementedError``."""
     if isinstance(results, np.ndarray) and results.ndim == 1 and results.dtype == np.float64:
         return results  # what the rules below give element by element, without the Python loop
     try:
@@ -181,23 +217,29 @@ def log_prob_values(results):
     except (IndexError, TypeError):
         return np.array([_scalar(r) for r in results], dtype=np.float64)
     raise NotImplementedError(
-        "the log-probability function returned blobs (a sequence per walker); blobs are not supported "
-        "by this engine -- return the log-probability alone"
+        "the log-probability function returned blobs (a sequence per walker); declare them with "
+        "blobs_dtype=... on the wrapper, or return the log-probability alone"
     )
 
 
 class CallbackFunction(object):
     """A user log-probability function the engine calls back once per half-step
-    (``HostFunction`` / ``CudaArrayFunction``)."""
+    (``HostFunction`` / ``CudaArrayFunction``).
+
+    ``blobs_dtype`` (default None: the function returns no blobs, and blobs raise ``NotImplementedError``)
+    declares that it returns blobs of that fixed-width dtype: the engine carries each walker's record with it
+    through the accept step on the GPU and stores it with the chain (``State.blobs``, ``get_blobs``,
+    ``compute_log_prob``), as the reference sampler's ``blobs_dtype`` does (``ensemble.py:92-95``)."""
 
     where = None
 
-    def __init__(self, fn, args=None, kwargs=None):
+    def __init__(self, fn, args=None, kwargs=None, blobs_dtype=None):
         if not callable(fn):
             raise TypeError("fn must be callable, got {0!r}".format(fn))
         self.fn = fn
         self.args = list(args or [])
         self.kwargs = dict(kwargs or {})
+        self.blobs_dtype = blobs_dtype_of(blobs_dtype)
 
     def _call(self, x):
         return self.fn(x, *self.args, **self.kwargs)
@@ -210,26 +252,30 @@ class HostFunction(CallbackFunction):
     ``vectorize=True``: one call ``fn(x, *args, **kwargs)`` per half-step with ``x[M, ndim]``, returning
     ``M`` values.  Otherwise one call per row through ``pool.map`` (``pool`` given) or the built-in
     ``map``.  Each row's result goes through the reference's ``_scalar`` rule; blobs raise
-    ``NotImplementedError``.  ``x`` is a fresh array that the function owns.  Rows reach the function
+    ``NotImplementedError`` unless ``blobs_dtype`` is given, and then follow the reference's blob rules
+    (``log_prob_and_blobs``): per-row ``(lp, blob...)`` tuples, ``(lp, array)`` and ``[M, 1 + k]`` arrays
+    all work.  ``x`` is a fresh array that the function owns.  Rows reach the function
     only when every parameter is finite; a NaN result stops the run with ``ValueError`` at that
     half-step.  Pickling drops ``pool``, as the sampler does (``ensemble.py:251-256``)."""
 
     where = "host"
 
-    def __init__(self, fn, vectorize=False, pool=None, args=None, kwargs=None):
-        super().__init__(fn, args, kwargs)
+    def __init__(self, fn, vectorize=False, pool=None, args=None, kwargs=None, blobs_dtype=None):
+        super().__init__(fn, args, kwargs, blobs_dtype)
         self.vectorize = bool(vectorize)
         self.pool = pool
         if pool is not None and not callable(getattr(pool, "map", None)):
             raise TypeError("pool must have a map() method")
 
     def evaluate(self, x):
-        """``float64[M]`` for ``x[M, ndim]``."""
+        """``float64[M]`` for ``x[M, ndim]``; ``(float64[M], blobs[M, ...] or None)`` with ``blobs_dtype``."""
         if self.vectorize:
             results = self._call(x)
         else:
             map_func = self.pool.map if self.pool is not None else map
             results = list(map_func(self._call, x))
+        if self.blobs_dtype is not None:
+            return log_prob_and_blobs(results, self.blobs_dtype)
         return log_prob_values(results)
 
     def __getstate__(self):
@@ -250,7 +296,11 @@ class CudaArrayFunction(CallbackFunction):
     ``(M,)``, strided or not, or a numpy array (copied).  A result whose interface has a ``stream``
     entry (v3) is read after the work on that stream; one without (v2, which torch exports) after all
     work on the device, so a result still being computed on any stream is never read early.  ``M`` is
-    the size of one split, ``nwalkers`` for ``GaussianMove`` and for the initial state."""
+    the size of one split, ``nwalkers`` for ``GaussianMove`` and for the initial state.
+
+    With ``blobs_dtype``, ``fn`` returns ``(lp, blobs)``: ``blobs`` is a CUDA-array-interface object (first
+    axis strided or not, each record contiguous) or a numpy array of shape ``(M, *shape)`` and dtype
+    ``blobs_dtype``, read under the same stream rules as ``lp``."""
 
     where = "device"
 

@@ -14,7 +14,8 @@ __all__ = ["State"]
 
 class State(object):
     """Snapshot of the ensemble: ``coords[nwalkers, ndim]``, ``log_prob[nwalkers]``,
-    ``blobs`` (always ``None`` on the device path) and ``random_state``.
+    ``blobs`` (``[nwalkers, ...]`` records of a user function declared with ``blobs_dtype``, else ``None``)
+    and ``random_state``.
 
     Iterating yields ``coords, log_prob, random_state`` (plus ``blobs`` when
     present), as the reference does for pre-3.0 callers (``state.py:47-75``)."""

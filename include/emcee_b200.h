@@ -151,6 +151,22 @@ int eb_model_set_callback(eb_ctx* ctx, eb_logprob_fn fn, void* user, int where);
  * has completed when the call returns. */
 #define EB_STREAM_UNKNOWN UINT64_MAX
 int eb_callback_result(eb_ctx* ctx, double* lp, const void* src, int64_t stride_bytes, int64_t m, uint64_t src_stream);
+/* Blobs (ensemble.py:498-547 splits them off the function's results; moves/move.py:36-43 carries them with each
+ * accepted walker; backends/backend.py:157-231 stores them).  From inside fn, either mode, at most once per call:
+ * m (= fn's m) records of record_bytes bytes, stride_bytes apart (>= record_bytes), from src (host or device
+ * memory), ordered on src_stream as eb_callback_result orders its copy.  The engine keeps fixed-width records
+ * packed, one per walker; what they hold is the caller's business.
+ *   - inside eb_set_state(coords, NULL): the records become the state's blobs and fix the live layout
+ *     (record_bytes); a function that delivers none leaves the state without blobs;
+ *   - inside a step: record_bytes must equal the live layout (EB_ERR_INVALID otherwise, before any update); each
+ *     walker that accepts its proposal takes the proposal's record, on the device, behind the accept launch;
+ *     a state without blobs (eb_set_state given log_prob, no eb_set_state_blobs) refuses them with the message of
+ *     moves/move.py:38-42, and a state with blobs refuses a call that delivers none;
+ *   - inside eb_compute_log_prob_blobs: record_bytes must equal the live layout if there is one.
+ * Host mode copies the records to pinned staging here; they reach the device beside lp (step 6), without a
+ * synchronisation of their own.  Device mode copies them before returning. */
+int eb_callback_blobs(eb_ctx* ctx, const void* src, int64_t record_bytes, int64_t stride_bytes, int64_t m,
+                      uint64_t src_stream);
 
 /* ---- state (state.py:10-45) ------------------------------------------- */
 /* State(initial_state, copy=True) + the initial compute_log_prob
@@ -173,12 +189,24 @@ int eb_owned_rows(const eb_ctx* ctx, int64_t* row0, int64_t* nrows);
  * on a sharded ensemble only the owned block (or any rows after a collective
  * read) is valid; other rows are refused with EB_ERR_STATE. */
 int eb_get_state_rows(eb_ctx* ctx, int64_t row0, int64_t nrows, double* coords, double* log_prob);
+/* State(coords, log_prob, blobs) of a callback model (state.py:10-45, ensemble.py:344-349): after an eb_set_state
+ * given log_prob, upload blobs[nwalkers * record_bytes] (host) as the state's blobs and fix the live layout.
+ * NULL, 0 clears them.  Device blob memory is checked before allocation (EB_ERR_NOMEM, as eb_chain_grow). */
+int eb_set_state_blobs(eb_ctx* ctx, const void* blobs, size_t record_bytes);
+/* the state's blobs (State.blobs, moves/move.py:36-43): out[nwalkers * record_bytes] (host); EB_ERR_STATE when the
+ * state has none. */
+int eb_get_blobs(eb_ctx* ctx, void* out);
 
 /* ---- log-probability (ensemble.py:458-553) ------------------------------ */
 /* EnsembleSampler.compute_log_prob(coords[m, ndim]) -> out[m], with the
  * isinf/isnan guards on the input (:476-479) and the NaN guard on the output
  * (:550-551). */
 int eb_compute_log_prob(eb_ctx* ctx, const double* coords, size_t m, double* out);
+/* compute_log_prob returning blobs (ensemble.py:458-553 `return log_prob, blob`) for a callback model: as
+ * eb_compute_log_prob, and *blobs_out receives page-locked host memory holding the m records the function
+ * delivered, *record_bytes their size (free it with eb_host_free); NULL and 0 when it delivered none. */
+int eb_compute_log_prob_blobs(eb_ctx* ctx, const double* coords, size_t m, double* out, void** blobs_out,
+                              size_t* record_bytes);
 
 /* ---- random state (ensemble.py:216-238) --------------------------------- */
 /* The engine's "random_state" is (seed, step): every draw is a pure function
@@ -205,6 +233,12 @@ int eb_step(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
  * incremented per accepted proposal of the stored steps' windows. */
 int eb_step_store(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
                   uint64_t thin_by, double* chain, double* log_prob, double* accepted);
+/* eb_step_store that also stores the state's blobs (backend.py:226-227): each stored step's records go to
+ * blobs[nstore, nwalkers, record_bytes] (host), through the same double-buffered pinned staging and drain as
+ * coords and log_prob, so a call stopped by the function leaves the blobs of every completed stored step in
+ * place.  blobs == NULL is eb_step_store; non-NULL needs a state with blobs (EB_ERR_STATE). */
+int eb_step_store_blobs(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
+                        uint64_t thin_by, double* chain, double* log_prob, double* accepted, void* blobs);
 
 /* ---- device chain storage (backends/backend.py:12-237 kept in HBM) ----- */
 /* A stored chain on one device: coords[slots, nwalkers, ndim], log_prob[slots,
