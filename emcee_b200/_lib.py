@@ -37,10 +37,11 @@ EB_COMM_ALLGATHER = 0
 EB_COMM_P2P = 1
 EB_CALLBACK_HOST = 0
 EB_CALLBACK_DEVICE = 1
+EB_MAX_PROPOSAL_SLOTS = 64  # user proposals one engine can hold (eb_move_set_proposal)
 EB_STREAM_UNKNOWN = 2**64 - 1  # eb_callback_result: the producer named no stream -> wait for the whole device
 
 MODEL_KINDS = {"gauss_iso": 0, "gauss_dense": 1, "rosenbrock": 2, "ring": 3}
-MOVE_KINDS = {"stretch": 0, "de": 1, "snooker": 2, "walk": 3, "gaussian": 4}
+MOVE_KINDS = {"stretch": 0, "de": 1, "snooker": 2, "walk": 3, "gaussian": 4, "user": 5, "user_mh": 6}
 
 
 class EbMove(C.Structure):
@@ -69,6 +70,9 @@ class EngineError(RuntimeError):
 _dp = C.POINTER(C.c_double)
 # eb_logprob_fn: (user, x, m, ndim, lp, stream) -> 0 | non-zero
 LOGPROB_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, _dp, C.c_int64, C.c_int64, _dp, C.c_void_p)
+# eb_proposal_fn: (user, step, split, s, ns, c, c_counts, nsets, ndim, q, factors, stream) -> 0 | non-zero
+PROPOSAL_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint64, C.c_int32, _dp, C.c_int64, _dp, C.POINTER(C.c_int64),
+                          C.c_int32, C.c_int64, _dp, _dp, C.c_void_p)
 _SIGNATURES = {
     "eb_abi_version": (C.c_int, []),
     "eb_device_count": (C.c_int, []),
@@ -80,6 +84,8 @@ _SIGNATURES = {
     "eb_model_set_callback": (C.c_int, [C.c_void_p, LOGPROB_FN, C.c_void_p, C.c_int]),
     "eb_callback_result": (C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_callback_blobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_uint64]),
+    "eb_move_set_proposal": (C.c_int, [C.c_void_p, C.c_int32, PROPOSAL_FN, C.c_void_p, C.c_int]),
+    "eb_proposal_result": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_set_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_get_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_set_state_blobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
@@ -235,6 +241,7 @@ class DeviceRows(object):
     only during the call; afterwards the interface raises ``RuntimeError``."""
 
     __slots__ = ("_cai",)
+    _what = "a log-probability callback"
 
     def __init__(self, ptr, m, ndim, stream):
         self._cai = {"shape": (int(m), int(ndim)), "typestr": "<f8", "data": (int(ptr or 0), False),
@@ -243,7 +250,7 @@ class DeviceRows(object):
     @property
     def __cuda_array_interface__(self):
         if self._cai is None:
-            raise RuntimeError("the rows of a log-probability callback are only valid during the call")
+            raise RuntimeError("the rows of %s are only valid during the call" % self._what)
         return dict(self._cai)
 
     @property
@@ -252,6 +259,109 @@ class DeviceRows(object):
 
     def _release(self):
         self._cai = None
+
+
+class ProposalRows(DeviceRows):
+    """The rows a device-mode user proposal receives (``s``, each ``c[j]``, or the ensemble): as
+    :class:`DeviceRows`, engine scratch valid only during the call."""
+
+    __slots__ = ()
+    _what = "a user proposal"
+
+
+def _proposal_arrays(out):
+    """``(q, factors)`` of a proposal's result, or the error for anything else."""
+    try:
+        q, f = out
+    except (TypeError, ValueError):
+        raise ValueError("the proposal must return (q, factors)") from None
+    return q, f
+
+
+def _check_proposal(shape, dtype, want, what):
+    if tuple(shape) != want:
+        raise ValueError("the proposal returned %s of shape %s; expected %s" % (what, tuple(shape), want))
+    if np.dtype(dtype) != np.float64:
+        raise TypeError("the proposal must return float64 %s, got %s" % (what, np.dtype(dtype)))
+
+
+def make_proposal_trampoline(h, propose, setup, where, failure, seed_box):
+    """The C proposal function of one schedule entry: calls ``propose(s, c, random)`` (host mode: fresh ndarrays the
+    function owns; device mode: :class:`ProposalRows`) and hands ``(q, factors)`` to the engine; ``setup(coords)``
+    for the setup call (split -1).  ``random`` = ``moves.user_random(seed_box[0], step, split)``.  Any exception is
+    stored as ``failure[0]`` and the engine is told to stop (``EB_ERR_CALLBACK``)."""
+    from .moves.user import user_random
+
+    def host(user, step, split, s, ns, c, counts, nsets, ndim, q, f):
+        S = np.ctypeslib.as_array(s, shape=(ns, ndim)).copy()
+        if split < 0:
+            setup(S)
+            return
+        sizes = [int(counts[j]) for j in range(nsets)]
+        cs = []
+        if nsets:
+            allc = np.ctypeslib.as_array(c, shape=(sum(sizes), ndim))
+            cs = [a.copy() for a in np.split(allc, np.cumsum(sizes)[:-1])]
+        qo, fo = _proposal_arrays(propose(S, cs, user_random(seed_box[0], step, split)))
+        qa, fa = np.asarray(qo), np.asarray(fo)
+        _check_proposal(qa.shape, qa.dtype, (ns, ndim), "q")
+        _check_proposal(fa.shape, fa.dtype, (ns,), "factors")
+        np.ctypeslib.as_array(q, shape=(ns, ndim))[:] = qa
+        np.ctypeslib.as_array(f, shape=(ns,))[:] = fa
+
+    def device(user, step, split, s, ns, c, counts, nsets, ndim, q, f, stream):
+        rows = [ProposalRows(C.cast(s, C.c_void_p).value, ns, ndim, stream)]
+        try:
+            if split < 0:
+                setup(rows[0])
+                return
+            base = C.cast(c, C.c_void_p).value or 0
+            off = 0
+            for j in range(nsets):
+                n = int(counts[j])
+                rows.append(ProposalRows(base + off * ndim * 8, n, ndim, stream))
+                off += n
+            qo, fo = _proposal_arrays(propose(rows[0], rows[1:], user_random(seed_box[0], step, split)))
+            ptrs, streams = [], set()
+            for a, want, what in ((qo, (ns, ndim), "q"), (fo, (ns,), "factors")):
+                cai = getattr(a, "__cuda_array_interface__", None)
+                if cai is None:
+                    a = np.ascontiguousarray(a)
+                    _check_proposal(a.shape, a.dtype, want, what)
+                    ptrs.append((a, a.ctypes.data, a.strides[0] if a.ndim else 8))
+                    continue
+                _check_proposal(cai["shape"], cai["typestr"], want, what)
+                if cai.get("mask") is not None:
+                    raise ValueError("masked CUDA arrays are not supported as proposals")
+                strides = cai.get("strides")
+                if strides is not None and len(want) == 2 and ndim > 1 and strides[1] != 8:
+                    raise ValueError("the rows of q must be contiguous; only the first axis may be strided")
+                stride = (8 * want[-1] if len(want) == 2 else 8) if strides is None else int(strides[0])
+                streams.add((cai["stream"] or 0) if "stream" in cai else EB_STREAM_UNKNOWN)
+                ptrs.append((a, cai["data"][0], stride))
+            streams.discard(0)
+            stream_id = streams.pop() if len(streams) == 1 else (EB_STREAM_UNKNOWN if streams else 0)
+            (_, qp, qs), (_, fp, fs) = ptrs
+            rc = lib().eb_proposal_result(h, C.c_void_p(qp), int(qs) if ns > 1 else ndim * 8, C.c_void_p(fp),
+                                          int(fs) if ns > 1 else 8, int(ns), int(stream_id))
+            if rc != EB_OK:
+                _raise(rc, lib().eb_last_error(h).decode())
+        finally:
+            for r in rows:
+                r._release()
+
+    def call(*args):
+        try:
+            if where == EB_CALLBACK_HOST:
+                host(*args[:-1])
+            else:
+                device(*args)
+            return 0
+        except BaseException as e:  # noqa: B902 -- re-raised unchanged when the ABI call returns
+            failure[0] = e
+            return 1
+
+    return PROPOSAL_FN(call)
 
 
 def _host_result(out, m):
@@ -520,6 +630,8 @@ class Engine(object):
         self._cb_failure = [None]
         self._blob_sink = None  # BlobSink of a callback that declares blobs_dtype
         self._blob_layout = None  # (dtype, shape) of the state's blob records, or None
+        self._props = {}  # slot -> the registered C proposal function (kept alive while the engine may call it)
+        self._seed_box = [int(seed) & (2**64 - 1)]  # the Philox key, read by the proposal trampolines
         self.nwalkers, self.ndim = int(nwalkers), int(ndim)
         rc = lib().eb_create(int(device), self.nwalkers, self.ndim, int(seed) & (2**64 - 1), C.byref(self._h))
         if rc != EB_OK:
@@ -708,6 +820,18 @@ class Engine(object):
     # -- rng -----------------------------------------------------------------
     def set_rng(self, seed, step):
         self._check(lib().eb_set_rng(self._h, int(seed) & (2**64 - 1), int(step)))
+        self._seed_box[0] = int(seed) & (2**64 - 1)
+
+    def set_proposal(self, slot, propose, where, setup=None):
+        """Make ``propose(s, c, random) -> (q, factors)`` proposal slot ``slot`` (``eb_move_set_proposal``), called
+        once per half-step of a schedule entry of kind ``"user"`` / ``"user_mh"`` whose ``p0`` is ``slot``;
+        ``where`` = ``"host"`` (numpy arrays) or ``"device"`` (:class:`ProposalRows`).  ``setup(coords)``, if given,
+        is called once per step before the splits of a ``"user"`` entry with ``mode`` 1.  Exceptions propagate
+        unchanged from the call that ran the function."""
+        mode = {"host": EB_CALLBACK_HOST, "device": EB_CALLBACK_DEVICE}[where]
+        fn = make_proposal_trampoline(self._h, propose, setup, mode, self._cb_failure, self._seed_box)
+        self._check(lib().eb_move_set_proposal(self._h, int(slot), fn, None, mode))
+        self._props[int(slot)] = fn
 
     def get_rng(self):
         seed, step = C.c_uint64(), C.c_uint64()
@@ -736,6 +860,8 @@ class Engine(object):
                 arr[k].ncov = cov.size
                 arr[k].mode = int(d.get("mode", 0))
                 arr[k].seq_index = int(d.get("seq_index", 0))
+            elif d["kind"] == "user":
+                arr[k].mode = int(d.get("mode", 0))  # EB_USER_SETUP
         return arr
 
     def move_picks(self, nmoves):

@@ -159,6 +159,22 @@ struct eb_ctx {
   uint8_t* stage_blob[2] = {nullptr, nullptr};  // eb_step_store_blobs: pinned [N, blob_bytes] staging
   size_t stage_blob_cap = 0;
 
+  // user proposals (eb_move_set_proposal), indexed by slot
+  struct ProposalSlot {
+    eb_proposal_fn fn = nullptr;
+    void* user = nullptr;
+    int where = EB_CALLBACK_HOST;
+  };
+  std::vector<ProposalSlot> props;
+  bool in_proposal = false;   // every other call on the context is refused while a proposal runs
+  int up_where = EB_CALLBACK_HOST;  // mode of the running proposal
+  int64_t up_m = 0;           // rows the running proposal returns
+  double* up_x = nullptr;     // device [N, D] rows handed to the proposal (s | c, or the ensemble)
+  double* up_f = nullptr;     // device [N] its Hastings factors
+  double* up_hx = nullptr;    // host mode: pinned [N, D] copy of up_x's rows
+  double* up_hq = nullptr;    // host mode: pinned [N, D] proposals
+  double* up_hf = nullptr;    // host mode: pinned [N] factors
+
   std::string err;
 };
 
@@ -174,8 +190,9 @@ static const char* const MSG_BLOBS_WITH_LOG_PROB =  // moves/move.py:38-42
 
 #define NOT_IN_CALLBACK(ctx)                                                      \
   do {                                                                            \
-    if ((ctx)->in_callback) {                                                     \
-      (ctx)->err = "engine is inside a log-probability callback";                 \
+    if ((ctx)->in_callback || (ctx)->in_proposal) {                               \
+      (ctx)->err = (ctx)->in_callback ? "engine is inside a log-probability callback" \
+                                      : "engine is inside a user proposal";       \
       return EB_ERR_STATE;                                                        \
     }                                                                             \
   } while (0)
@@ -355,6 +372,11 @@ int eb_destroy(eb_ctx* c) {
   cudaFreeHost(c->blob_host);
   cudaFreeHost(c->cmp_blobs);
   for (int k = 0; k < 2; ++k) cudaFreeHost(c->stage_blob[k]);
+  cudaFree(c->up_x);
+  cudaFree(c->up_f);
+  cudaFreeHost(c->up_hx);
+  cudaFreeHost(c->up_hq);
+  cudaFreeHost(c->up_hf);
   if (c->ev0) cudaEventDestroy(c->ev0);
   if (c->ev1) cudaEventDestroy(c->ev1);
   if (c->st) cudaStreamDestroy(c->st);
@@ -612,6 +634,42 @@ int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_by
          (long long)stride_bytes);
   if (m == 0) return EB_OK;
   return copy_records(c, lp, src, sizeof(double), (size_t)stride_bytes, (size_t)m, src_stream);
+}
+
+int eb_move_set_proposal(eb_ctx* c, int32_t slot, eb_proposal_fn fn, void* user, int where) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (slot < 0 || slot >= EB_MAX_PROPOSAL_SLOTS)
+    FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal: slot must be in [0, %d) (got %d)", EB_MAX_PROPOSAL_SLOTS, slot);
+  if (fn && where != EB_CALLBACK_HOST && where != EB_CALLBACK_DEVICE)
+    FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal: where must be EB_CALLBACK_HOST or EB_CALLBACK_DEVICE (got %d)", where);
+  if (fn && c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "user proposals are not sharded across GPUs");
+  if ((size_t)slot >= c->props.size()) c->props.resize((size_t)slot + 1);
+  c->props[(size_t)slot].fn = fn;
+  c->props[(size_t)slot].user = fn ? user : nullptr;
+  c->props[(size_t)slot].where = where;
+  return EB_OK;
+}
+
+int eb_proposal_result(eb_ctx* c, const void* q, int64_t q_row_stride_bytes, const void* factors,
+                       int64_t f_stride_bytes, int64_t m, uint64_t src_stream) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->in_proposal || c->up_where != EB_CALLBACK_DEVICE || c->up_m == 0)
+    FAIL(c, EB_ERR_STATE, "eb_proposal_result: only from inside a device-mode user proposal");
+  if (m != c->up_m)
+    FAIL(c, EB_ERR_INVALID, "the proposal returned %lld rows for %lld walkers", (long long)m, (long long)c->up_m);
+  if (!q || !factors) FAIL(c, EB_ERR_INVALID, "eb_proposal_result: null buffer");
+  const int64_t row = (int64_t)c->D * (int64_t)sizeof(double);
+  if ((m > 1 && q_row_stride_bytes < row) || q_row_stride_bytes <= 0 || q_row_stride_bytes % 8 != 0)
+    FAIL(c, EB_ERR_INVALID, "eb_proposal_result: the row stride of q must be a multiple of 8 bytes, at least %lld (got %lld)",
+         (long long)row, (long long)q_row_stride_bytes);
+  if (f_stride_bytes <= 0 || f_stride_bytes % 8 != 0)
+    FAIL(c, EB_ERR_INVALID, "eb_proposal_result: the stride of factors must be a positive multiple of 8 bytes (got %lld)",
+         (long long)f_stride_bytes);
+  int rc = copy_records(c, c->qbuf, q, (size_t)row, (size_t)q_row_stride_bytes, (size_t)m, src_stream);
+  if (rc) return rc;
+  // the first copy already waited for src_stream
+  return copy_records(c, c->up_f, factors, sizeof(double), (size_t)f_stride_bytes, (size_t)m, 0);
 }
 
 int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
@@ -998,8 +1056,22 @@ int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) 
   std::vector<double> ghost;  // host image of gauss_dev
   for (size_t mi = 0; mi < nmoves; ++mi) {
     eb_move& m = s.moves[mi];
-    if (m.kind < EB_MOVE_STRETCH || m.kind > EB_MOVE_GAUSSIAN)
+    if (m.kind == EB_MOVE_USER || m.kind == EB_MOVE_USER_MH) {
+      if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "user proposals are not sharded across GPUs");
+      if (c->debug) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: debug taps do not cover user proposals");
+      if (!(m.p0 >= 0.0 && m.p0 < (double)c->props.size()) || m.p0 != floor(m.p0) || !c->props[(size_t)m.p0].fn)
+        FAIL(c, EB_ERR_INVALID, "eb_step: proposal slot %g is not set (eb_move_set_proposal)", m.p0);
+      if (!(m.weight >= 0.0) || !isfinite(m.weight)) FAIL(c, EB_ERR_INVALID, "eb_step: bad move weight");
+      if (m.kind == EB_MOVE_USER_MH) {
+        m.nsplits = 1;  // the split table of such a step is never read
+        m.randomize_split = 0;
+        tot += m.weight;
+        continue;
+      }
+      if (m.mode != 0 && m.mode != EB_USER_SETUP) FAIL(c, EB_ERR_INVALID, "eb_step: unknown user-move mode %d", m.mode);
+    } else if (m.kind < EB_MOVE_STRETCH || m.kind > EB_MOVE_GAUSSIAN) {
       FAIL(c, EB_ERR_INVALID, "eb_step: unknown move kind %d", m.kind);
+    }
     if ((m.kind == EB_MOVE_WALK || m.kind == EB_MOVE_GAUSSIAN) && c->comm.nranks > 1)
       FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove / GaussianMove are not sharded across GPUs yet");
     if ((m.kind == EB_MOVE_WALK || m.kind == EB_MOVE_GAUSSIAN) && c->debug)
@@ -1339,6 +1411,156 @@ int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step,
   return EB_OK;
 }
 
+// ---- user proposals (eb_move_set_proposal) ----------------------------------------------------------
+int ensure_user_scratch(eb_ctx* c, bool host) {
+  const size_t N = (size_t)c->N, D = (size_t)c->D;
+  if (!c->qbuf) CK(c, cudaMalloc(&c->qbuf, N * D * sizeof(double)));
+  if (!c->up_x) CK(c, cudaMalloc(&c->up_x, N * D * sizeof(double)));
+  if (!c->up_f) CK(c, cudaMalloc(&c->up_f, N * sizeof(double)));
+  if (host && !c->up_hf) {
+    CK(c, cudaMallocHost(&c->up_hx, N * D * sizeof(double)));
+    CK(c, cudaMallocHost(&c->up_hq, N * D * sizeof(double)));
+    CK(c, cudaMallocHost(&c->up_hf, N * sizeof(double)));
+  }
+  return EB_OK;
+}
+
+// steps 2-5 of a user half-step (include/emcee_b200.h): rows[N, D] (device; s then c, or the ensemble) are
+// enqueued.  ns > 0: the proposal of ns rows lands in qbuf / up_f; ns == 0: the setup call, which returns nothing
+int user_proposal_call(eb_ctx* c, const eb_ctx::ProposalSlot& p, uint64_t step, int split, const double* rows,
+                       int64_t ns, const int64_t* counts, int nsets) {
+  const size_t N = (size_t)c->N, D = (size_t)c->D;
+  const bool host = p.where == EB_CALLBACK_HOST;
+  // the function gets its own copy of the rows
+  if (host)
+    CK(c, cudaMemcpyAsync(c->up_hx, rows, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  else if (rows != c->up_x)
+    CK(c, cudaMemcpyAsync(c->up_x, rows, N * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
+  // complete before fn runs (a device consumer may ignore the stream it is given)
+  CK(c, cudaStreamSynchronize(c->st));
+  const double* s = host ? c->up_hx : c->up_x;
+  const double* cset = nsets > 0 ? s + (size_t)ns * D : nullptr;
+  double* q = ns > 0 ? (host ? c->up_hq : c->qbuf) : nullptr;
+  double* f = ns > 0 ? (host ? c->up_hf : c->up_f) : nullptr;
+  c->up_m = ns;
+  c->up_where = p.where;
+  c->in_proposal = true;
+  const int r = p.fn(p.user, step, (int32_t)split, s, ns > 0 ? ns : (int64_t)N, cset, nsets > 0 ? counts : nullptr,
+                     nsets, (int64_t)D, q, f, host ? nullptr : (void*)c->st);
+  c->in_proposal = false;
+  c->up_m = 0;
+  if (r != 0) {
+    cudaStreamSynchronize(c->st);  // whatever the function enqueued before it failed
+    FAIL(c, EB_ERR_CALLBACK, "the user proposal failed (returned %d)", r);
+  }
+  if (ns == 0) return EB_OK;
+  if (host) {
+    CK(c, cudaMemcpyAsync(c->qbuf, c->up_hq, (size_t)ns * D * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    CK(c, cudaMemcpyAsync(c->up_f, c->up_hf, (size_t)ns * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  }
+  if (c->model.kind == MODEL_EXTERNAL) return EB_OK;  // run_callback scans the rows before the function sees them
+  // ensemble.py:476-479: a non-finite proposal stops the call before any log-probability is evaluated
+  CK(c, launch_scan_nonfinite(c->qbuf, (size_t)ns * D, 0, c->status_dev, c->st));
+  return fetch_status(c);
+}
+
+// step 6: the log-probability of qbuf's rows and the accept + update (kind EB_MOVE_USER / EB_MOVE_USER_MH)
+int user_accept(eb_ctx* c, int kind, const HalfStepArgs& a, uint64_t& launches) {
+  const ExternalBufs ext{c->qbuf, c->up_f, c->ext_lp};
+  if (c->model.kind == MODEL_EXTERNAL) {
+    c->cb_phase = CB_STEP;
+    int rc = run_callback(c, c->qbuf, (int64_t)a.i_hi - a.i_lo, c->ext_lp, true);
+    if (rc) return rc;
+    if (kind == EB_MOVE_USER)
+      CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st));
+    else
+      CK(c, launch_half_step_user(EB_MOVE_USER_MH, a, ext, c->st));
+    ++launches;
+    if (c->blobs_live) {
+      CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop, c->blob_live,
+                               c->blob_bytes, c->st));
+      ++launches;
+    }
+  } else {
+    CK(c, launch_half_step_user(kind, a, ext, c->st));
+    ++launches;
+  }
+  return EB_OK;
+}
+
+void note_user_kernel(eb_ctx* c, const eb_ctx::ProposalSlot& p) {
+  c->last_kernel = "user_move";
+  snprintf(c->last_variant, sizeof(c->last_variant), "user_move where=%s",
+           p.where == EB_CALLBACK_HOST ? "host" : "device");
+}
+
+// a RedBlueMove with a user get_proposal (red_blue.py:52-106): per split the gather, the function, the accept
+int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t* order, uint64_t& launches) {
+  int rc = check_walker_count(c, mv);
+  if (rc) return rc;
+  const eb_ctx::ProposalSlot p = c->props[(size_t)mv.p0];
+  rc = ensure_user_scratch(c, p.where == EB_CALLBACK_HOST);
+  if (rc) return rc;
+  c->chain_ok = false;
+  if (mv.mode == EB_USER_SETUP) {  // red_blue.py:73 setup(state.coords), once per step before the splits
+    rc = user_proposal_call(c, p, step, -1, c->coords, 0, nullptr, 0);
+    if (rc) return rc;
+  }
+  const int P = mv.nsplits;
+  int start[MAX_SPLITS + 1];
+  split_starts(c->N, P, start);
+  HalfStepArgs a;
+  fill_base_args(c, mv, a);
+  a.order = order;
+  a.step = step;
+  a.qbuf = c->qbuf;
+  int64_t counts[MAX_SPLITS];
+  for (int split = 0; split < P; ++split) {
+    a.split = split;
+    a.a_start = start[split];
+    a.a_count = start[split + 1] - start[split];
+    a.i_lo = 0;
+    a.i_hi = a.a_count;
+    a.range = nullptr;
+    int k = 0;
+    for (int j = 0; j < P; ++j)
+      if (j != split) counts[k++] = start[j + 1] - start[j];
+    CK(c, launch_split_gather(c->coords, order, c->N, c->D, a.a_start, a.a_count, c->up_x, c->st));
+    ++launches;
+    rc = user_proposal_call(c, p, step, split, c->up_x, a.a_count, counts, P - 1);
+    if (rc) return rc;
+    rc = user_accept(c, EB_MOVE_USER, a, launches);
+    if (rc) return rc;
+  }
+  note_user_kernel(c, p);
+  return EB_OK;
+}
+
+// MHMove with a user proposal_function (mh.py:35-65): the whole ensemble in walker order, one accept launch
+int launch_step_user_mh(eb_ctx* c, const eb_move& mv, uint64_t step, uint64_t& launches) {
+  const eb_ctx::ProposalSlot p = c->props[(size_t)mv.p0];
+  int rc = ensure_user_scratch(c, p.where == EB_CALLBACK_HOST);
+  if (rc) return rc;
+  c->chain_ok = false;
+  HalfStepArgs a;
+  fill_base_args(c, mv, a);
+  a.order = nullptr;  // the active set is every walker, in walker order
+  a.step = step;
+  a.split = 0;
+  a.a_start = 0;
+  a.a_count = (int)c->N;
+  a.i_lo = 0;
+  a.i_hi = (int)c->N;
+  a.range = nullptr;
+  a.qbuf = c->qbuf;
+  rc = user_proposal_call(c, p, step, 0, c->coords, c->N, nullptr, 0);
+  if (rc) return rc;
+  rc = user_accept(c, EB_MOVE_USER_MH, a, launches);
+  if (rc) return rc;
+  note_user_kernel(c, p);
+  return EB_OK;
+}
+
 constexpr int DMMA_TILE_SLOTS = 8;  // consumer warps per SM of the dense_dmma kernel
 
 // a run of consecutive half-steps handed to ONE persistent dense_dmma launch
@@ -1543,6 +1765,10 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
           rc = launch_step_walk(c, mv, c->step, c->order + (off + k) * (size_t)c->N, launches);
         else if (mv.kind == EB_MOVE_GAUSSIAN)
           rc = launch_step_gaussian(c, s, pick[k], c->step, launches);
+        else if (mv.kind == EB_MOVE_USER)
+          rc = launch_step_user(c, mv, c->step, c->order + (off + k) * (size_t)c->N, launches);
+        else if (mv.kind == EB_MOVE_USER_MH)
+          rc = launch_step_user_mh(c, mv, c->step, launches);
         else
           rc = launch_step_generic(c, mv, c->step, c->order + (off + k) * (size_t)c->N, off + k, launches);
         if (rc) return rc;

@@ -123,6 +123,15 @@ cudaError_t launch_half_step_external(int move_kind, const HalfStepArgs& a, cons
 // : i takes record i - i_lo of prop[rows, record_bytes] into live[w] when accepted[w] is set (packed records)
 cudaError_t launch_blob_select(const int32_t* order, int a_start, int i_lo, int i_hi, const uint8_t* accepted,
                                const void* prop, void* live, size_t record_bytes, cudaStream_t st);
+// user proposals (eb_move_set_proposal).  Accept launch of a half-step whose proposals a user function wrote: row i
+// - i_lo of HalfStepArgs::qbuf, Hastings factor f[i - i_lo].  move_kind EB_MOVE_USER: a device model, red-blue
+// order (f + lp_new) - lp_old (red_blue.py:99); EB_MOVE_USER_MH: a device model or MODEL_EXTERNAL (lp from ext.lp),
+// mh.py:57 order (lp_new - lp_old) + f, uniform indexed by walker (order == nullptr)
+cudaError_t launch_half_step_user(int move_kind, const HalfStepArgs& a, const ExternalBufs& ext, cudaStream_t st);
+// user_moves.cu: out[r] = coords row of walker order[a_start + r] for r < a_count, then the other sets in set order
+// (order[r - a_count] for the sets before, order[r] for the sets after): the rows s | c of red_blue.py:85-87
+cudaError_t launch_split_gather(const double* coords, const int32_t* order, int64_t N, int D, int a_start, int a_count,
+                                double* out, cudaStream_t st);
 // status |= FLAG_NAN_LOGPROB if any of x[n] is NaN (logprob != 0), else the non-finite parameter flags of x[n]
 cudaError_t launch_scan_nonfinite(const double* x, size_t n, int logprob, int* status, cudaStream_t st);
 // the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)

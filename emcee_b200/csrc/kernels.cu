@@ -207,6 +207,8 @@ template <int MOVE, int MODEL>
 __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepArgs a, const int G, const ExternalBufs ext) {
   extern __shared__ double smem[];
   constexpr int NROWS = (MOVE == EB_MOVE_SNOOKER ? 4 : 1) + (MODEL == EB_MODEL_GAUSS_DENSE ? 1 : 0);
+  // the proposal row comes from qbuf: written by a proposal kernel, a callback's propose phase or a user function
+  constexpr bool PRE = MOVE == MOVE_PRECOMPUTED || MOVE == EB_MOVE_USER || MOVE == EB_MOVE_USER_MH;
   const int D = a.D;
   const int groups = blockDim.x / G;
   const int gid = threadIdx.x / G, g = threadIdx.x % G;
@@ -263,16 +265,17 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
       if (!isfinite(v)) flag_nonfinite(v, a.status);
     }
     tap_scalar = gamma;
-  } else if (MOVE == MOVE_PRECOMPUTED) {
+  } else if (PRE) {
     // WalkMove / GaussianMove: the proposal was written by its own kernel (moves_extra.cu); factors = 0
-    // (accept phase of a callback model: written by the propose phase, factor from ext.f)
+    // (accept phase of a callback model: written by the propose phase, factor from ext.f; user proposals: row and
+    // factor written by the user function)
     const double* qrow = a.qbuf + (size_t)(i - i_lo) * D;
     for (int e = g; e < D; e += G) {
       const double v = qrow[e];
       q[e] = v;
       if (!isfinite(v)) flag_nonfinite(v, a.status);
     }
-    if (MODEL == MODEL_EXTERNAL && ext.f != nullptr) factor = ext.f[i - i_lo];
+    if ((MODEL == MODEL_EXTERNAL || MOVE != MOVE_PRECOMPUTED) && ext.f != nullptr) factor = ext.f[i - i_lo];
   } else {  // EB_MOVE_SNOOKER
     const u32x4 B = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_B, (uint32_t)i);
     int64_t cw[3];
@@ -330,7 +333,7 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
   }
   __syncwarp(mask);
 
-  if (MODEL == MODEL_EXTERNAL && MOVE != MOVE_PRECOMPUTED) {
+  if (MODEL == MODEL_EXTERNAL && !PRE) {
     // propose phase of a callback model: hand the staged row and its factor to the host, stop before the model
     double* dst = ext.q + (size_t)(i - i_lo) * D;
     for (int e = g; e < D; e += G) dst[e] = q[e];
@@ -359,7 +362,10 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
   // red_blue.py:96-101
   const u32x4 U = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_ACCEPT, (uint32_t)i);
   const double u_acc = u53(U.x, U.y);
-  const double lnpdiff = __dsub_rn(__dadd_rn(factor, lp_new), a.logp[w]);
+  // red_blue.py:99 (f + lp_new) - lp_old; a user MHMove keeps mh.py:57's order (lp_new - lp_old) + f, which rounds
+  // differently once f != 0
+  const double lnpdiff = MOVE == EB_MOVE_USER_MH ? __dadd_rn(__dsub_rn(lp_new, a.logp[w]), factor)
+                                                 : __dsub_rn(__dadd_rn(factor, lp_new), a.logp[w]);
   const bool acc = lnpdiff > log(u_acc);
 
   // red_blue.py:103-104 -> move.py:29-34
@@ -451,6 +457,29 @@ cudaError_t launch_half_step_external(int move_kind, const HalfStepArgs& a, cons
       return launch_generic_t<MOVE_PRECOMPUTED, MODEL_EXTERNAL>(a, st, ext);
   }
   return cudaErrorInvalidValue;
+}
+
+template <int MOVE>
+static cudaError_t launch_user_m(const HalfStepArgs& a, const ExternalBufs& ext, cudaStream_t st) {
+  switch (a.model.kind) {
+    case EB_MODEL_GAUSS_ISO:
+      return launch_generic_t<MOVE, EB_MODEL_GAUSS_ISO>(a, st, ext);
+    case EB_MODEL_GAUSS_DENSE:
+      return launch_generic_t<MOVE, EB_MODEL_GAUSS_DENSE>(a, st, ext);
+    case EB_MODEL_ROSENBROCK:
+      return launch_generic_t<MOVE, EB_MODEL_ROSENBROCK>(a, st, ext);
+    case EB_MODEL_RING:
+      return launch_generic_t<MOVE, EB_MODEL_RING>(a, st, ext);
+  }
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_half_step_user(int move_kind, const HalfStepArgs& a, const ExternalBufs& ext, cudaStream_t st) {
+  if (move_kind == EB_MOVE_USER) return launch_user_m<EB_MOVE_USER>(a, ext, st);
+  if (move_kind != EB_MOVE_USER_MH) return cudaErrorInvalidValue;
+  // a red-blue user move with a callback model is the callback's own accept launch, <MOVE_PRECOMPUTED, MODEL_EXTERNAL>
+  if (a.model.kind == MODEL_EXTERNAL) return launch_generic_t<EB_MOVE_USER_MH, MODEL_EXTERNAL>(a, st, ext);
+  return launch_user_m<EB_MOVE_USER_MH>(a, ext, st);
 }
 
 // non-finite scan of a callback's input rows (ensemble.py:476-479) or of its log-probabilities (:550-551)

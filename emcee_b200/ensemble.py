@@ -20,6 +20,7 @@ from .backend import Backend, DeviceBackend
 from .model import Model
 from .models import CallbackFunction, DeviceModel
 from .moves import StretchMove
+from .moves.user import user_move_spec
 from .rng import DeviceRandom
 from .state import State
 
@@ -134,6 +135,7 @@ class EnsembleSampler(object):
         self._engine = _lib.Engine(self.nwalkers, self.ndim, _seed_from_numpy() if seed is None else seed,
                                    device=device)
         self._load_model()
+        self._load_moves()
         self._random = DeviceRandom(self._engine)
         self._pinned = None
         if pinned_results:
@@ -174,6 +176,20 @@ class EnsembleSampler(object):
         box = m.bounds(self.ndim)
         if box is not None:
             self._engine.set_bounds(*box)
+
+    def _user_slots(self):
+        """``{schedule index: proposal slot}`` of the user moves, slots numbered densely in schedule order."""
+        idx = [k for k, m in enumerate(self._moves) if user_move_spec(m) is not None]
+        return {k: slot for slot, k in enumerate(idx)}
+
+    def _load_moves(self):
+        slots = self._user_slots()
+        if len(slots) > _lib.EB_MAX_PROPOSAL_SLOTS:
+            raise NotImplementedError("a move schedule holds at most %d user moves (got %d)"
+                                      % (_lib.EB_MAX_PROPOSAL_SLOTS, len(slots)))
+        for k, slot in slots.items():
+            _, where, propose, setup = user_move_spec(self._moves[k])
+            self._engine.set_proposal(slot, propose, where, setup)
 
     # ------------------------------------------------------------------ state
     @property
@@ -223,6 +239,7 @@ class EnsembleSampler(object):
         self.__dict__.update(d)
         self._engine = _lib.Engine(self.nwalkers, self.ndim, seed, device=self._device)
         self._load_model()
+        self._load_moves()
         self._engine.set_rng(seed, step)
         self._random = DeviceRandom(self._engine)
         self._pinned = None
@@ -245,6 +262,8 @@ class EnsembleSampler(object):
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
+        if any(user_move_spec(m) is not None for m in self._moves):
+            raise NotImplementedError("a user proposal runs on one GPU; a schedule with user moves cannot be sharded")
         dist.attach(self._engine, rdv, mode)
         self._rdv = rdv
         self._gather_results = bool(gather_results)
@@ -275,7 +294,15 @@ class EnsembleSampler(object):
 
     # ------------------------------------------------------------- the driver
     def _schedule(self):
-        return [(m.descriptor(), w) for m, w in zip(self._moves, self._raw_weights)]
+        sched, slots = [], self._user_slots()
+        for k, (m, w) in enumerate(zip(self._moves, self._raw_weights)):
+            d = m.descriptor()
+            if d["kind"] in ("user", "user_mh"):
+                if d["kind"] == "user_mh" and m.ndim is not None and m.ndim != self.ndim:
+                    raise ValueError("Dimension mismatch in proposal")  # mh.py:47-49
+                d["p0"] = float(slots[k])  # the proposal slot _load_moves registered
+            sched.append((d, w))
+        return sched
 
     def _stored_before_failure(self, step0, thin_by, k0):
         """A bulk run stopped by an exception: the backend keeps the stored steps that completed, blobs

@@ -1,8 +1,10 @@
 """Moves of the device path (reference: ``src/emcee/moves/__init__.py``).
 
 The red-blue family (``StretchMove``, ``DEMove``, ``DESnookerMove``, ``WalkMove``) and the
-Metropolis family with Gaussian proposals (``MHMove``, ``GaussianMove``); the reference's
-``KDEMove`` (SciPy kernel-density proposals) is out of scope (DESIGN.md)."""
+Metropolis family with Gaussian proposals (``MHMove``, ``GaussianMove``), and user-written proposals:
+``RedBlueMove`` subclasses that override ``get_proposal`` (``CudaArrayRedBlueMove`` for CUDA arrays) and
+``MHMove(HostProposal(fn))`` / ``MHMove(CudaArrayProposal(fn))``; the reference's ``KDEMove`` (SciPy
+kernel-density proposals) is out of scope (DESIGN.md)."""
 
 from .de import DEMove
 from .de_snooker import DESnookerMove
@@ -11,6 +13,8 @@ from .mh import MHMove
 from .move import Move
 from .red_blue import RedBlueMove
 from .stretch import StretchMove
+from .user import CudaArrayProposal, CudaArrayRedBlueMove, HostProposal, user_random
 from .walk import WalkMove
 
-__all__ = ["Move", "RedBlueMove", "StretchMove", "DEMove", "DESnookerMove", "WalkMove", "MHMove", "GaussianMove"]
+__all__ = ["Move", "RedBlueMove", "StretchMove", "DEMove", "DESnookerMove", "WalkMove", "MHMove", "GaussianMove",
+           "HostProposal", "CudaArrayProposal", "CudaArrayRedBlueMove", "user_random"]

@@ -1,12 +1,14 @@
 """Metropolis-Hastings move of the device path (reference: ``src/emcee/moves/mh.py:11-65``).
 
-The reference's ``MHMove`` takes an arbitrary host ``proposal_function(coords, rng)``; a GPU kernel
-cannot call back into Python, so the device path accepts the proposals it has a kernel for -- the
-Gaussian family of :class:`emcee_b200.moves.GaussianMove` -- and says so for anything else."""
+The reference's ``MHMove`` takes an arbitrary host ``proposal_function(coords, rng)``.  The device path runs
+the Gaussian family of :class:`emcee_b200.moves.GaussianMove` in its own kernels, and a user function wrapped
+as ``moves.HostProposal(fn)`` or ``moves.CudaArrayProposal(fn)`` once per step between the GPU's gather and its
+accept (DESIGN.md §5.9).  A bare callable is refused: the wrapper is the explicit opt-in."""
 
 import numpy as np
 
 from .move import Move
+from .user import _UserProposal
 
 __all__ = ["MHMove"]
 
@@ -20,10 +22,12 @@ class MHMove(Move):
     kind = "gaussian"
 
     def __init__(self, proposal_function, ndim=None):
-        if not isinstance(proposal_function, dict) or proposal_function.get("family") != "gaussian":
+        if isinstance(proposal_function, _UserProposal):
+            self.kind = "user_mh"
+        elif not isinstance(proposal_function, dict) or proposal_function.get("family") != "gaussian":
             raise NotImplementedError(
-                "MHMove on the device path needs a device proposal (use GaussianMove); an arbitrary host "
-                "proposal_function cannot be called from inside the step kernels"
+                "MHMove on the device path needs a device proposal (GaussianMove) or a wrapped user function: "
+                "MHMove(moves.HostProposal(fn)) for numpy arrays, MHMove(moves.CudaArrayProposal(fn)) for CUDA arrays"
             )
         self.ndim = ndim
         self.get_proposal = proposal_function
@@ -34,13 +38,16 @@ class MHMove(Move):
 
     def descriptor(self):
         p = self.get_proposal
+        if self.kind == "user_mh":  # the sampler fills in p0 = its proposal slot
+            return dict(kind=self.kind, nsplits=1, randomize_split=False, live_dangerously=True,
+                        p0=float("nan"), p1=float("nan"))
         return dict(kind=self.kind, nsplits=1, randomize_split=False, live_dangerously=True,
                     p0=float("nan"), p1=float("nan") if p["factor"] is None else float(p["factor"]),
                     mode=p["mode"], cov=p["cov"], seq_index=int(self.index))
 
     def _advance(self, picks, ndim):
         """The engine ran ``picks`` steps with this move: what ``gaussian.py:103`` does to ``index``."""
-        if self.get_proposal["mode"] == 2:  # "sequential"
+        if self.kind == "gaussian" and self.get_proposal["mode"] == 2:  # "sequential"
             self.index = (self.index + int(picks)) % int(ndim)
 
     def propose(self, model, state):
@@ -51,6 +58,8 @@ class MHMove(Move):
         nwalkers, ndim = state.coords.shape
         if self.ndim is not None and self.ndim != ndim:
             raise ValueError("Dimension mismatch in proposal")  # mh.py:47-48
+        if self.kind == "user_mh":
+            raise NotImplementedError("a user proposal_function runs inside EnsembleSampler.sample / run_mcmc")
         engine.set_state(state.coords, state.log_prob)
         accepted = engine.step([(self.descriptor(), 1.0)], 1)
         self._advance(1, ndim)

@@ -4,7 +4,11 @@
 The reference's ``propose`` loops over the splits on the host, calling
 ``get_proposal`` -> ``compute_log_prob_fn`` -> a per-walker Python accept loop
 -> ``update``.  Here one C-ABI call (``eb_step``) runs the whole split cycle in
-fused CUDA kernels; a subclass only describes itself (``descriptor``)."""
+fused CUDA kernels; a subclass only describes itself (``descriptor``).
+
+A subclass that overrides ``get_proposal`` is a user move: the engine calls its ``get_proposal(s, c, random)`` once
+per half-step with the split's walkers and the other sets, as ``red_blue.py:85-90`` does, and keeps everything else
+on the GPU (DESIGN.md §5.9)."""
 
 import numpy as np
 
@@ -15,9 +19,18 @@ __all__ = ["RedBlueMove"]
 
 class RedBlueMove(Move):
     """Args mirror ``red_blue.py:37-42``: ``nsplits`` (default 2),
-    ``randomize_split`` (default True), ``live_dangerously`` (default False)."""
+    ``randomize_split`` (default True), ``live_dangerously`` (default False).
+
+    Override ``get_proposal(s, c, random) -> (q, factors)`` to write a move of your own: ``s`` is
+    ``float64[Ns, ndim]``, the split's walkers in ascending walker order; ``c`` is the list of the ``nsplits - 1``
+    other sets, in set order, each in ascending walker order; ``random`` is a numpy ``RandomState``
+    (``moves.user_random``).  Return ``q`` (float64 ``[Ns, ndim]``) and ``factors`` (float64 ``[Ns]``, the log
+    Hastings ratios).  An overridden ``setup(coords)`` is called once per step with a copy of the whole ensemble
+    before the splits (``red_blue.py:73``), which costs one download of the state per step; without an override
+    nothing is downloaded."""
 
     kind = None
+    _where = "host"  # where a user get_proposal runs (moves.CudaArrayRedBlueMove: on CUDA arrays)
 
     def __init__(self, nsplits=2, randomize_split=True, live_dangerously=False):
         self.nsplits = int(nsplits)
@@ -37,6 +50,11 @@ class RedBlueMove(Move):
         raise NotImplementedError("The proposal must be implemented by subclasses")
 
     def descriptor(self):
+        if type(self).get_proposal is not RedBlueMove.get_proposal:
+            # a user move: the sampler fills in p0 = its proposal slot; mode 1 = EB_USER_SETUP
+            return dict(kind="user", nsplits=self.nsplits, randomize_split=bool(self.randomize_split),
+                        live_dangerously=bool(self.live_dangerously), p0=float("nan"), p1=float("nan"),
+                        mode=int(type(self).setup is not RedBlueMove.setup))
         p0, p1 = self._params()
         return dict(
             kind=self.kind,
@@ -60,6 +78,8 @@ class RedBlueMove(Move):
                 "model.random must be an emcee_b200 DeviceRandom (the device "
                 "path cannot consume a host RandomState)"
             )
+        if type(self).get_proposal is not RedBlueMove.get_proposal:
+            raise NotImplementedError("a user get_proposal runs inside EnsembleSampler.sample / run_mcmc")
         nwalkers, ndim = state.coords.shape
         if nwalkers < 2 * ndim and not self.live_dangerously:  # red_blue.py:64-70
             raise RuntimeError(

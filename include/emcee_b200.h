@@ -65,6 +65,14 @@ typedef enum eb_move_kind {
                           not a red-blue move: nsplits / randomize_split are ignored */
 } eb_move_kind;
 
+/* user-written proposals (eb_move_set_proposal below); not members of eb_move_kind so that the enum keeps its
+ * ABI 2 range */
+#define EB_MOVE_USER 5    /* red-blue move with a user proposal (red_blue.py:47,90); p0 = proposal slot;
+                             mode = EB_USER_SETUP: call the function once per step with the whole ensemble first */
+#define EB_MOVE_USER_MH 6 /* MHMove with a user proposal_function (mh.py:31-33,52); p0 = proposal slot;
+                             nsplits / randomize_split are ignored */
+#define EB_USER_SETUP 1
+
 typedef enum eb_gaussian_mode { /* gaussian.py:63,99-104 */
   EB_GAUSS_VECTOR = 0, EB_GAUSS_RANDOM = 1, EB_GAUSS_SEQUENTIAL = 2
 } eb_gaussian_mode;
@@ -167,6 +175,45 @@ int eb_callback_result(eb_ctx* ctx, double* lp, const void* src, int64_t stride_
  * synchronisation of their own.  Device mode copies them before returning. */
 int eb_callback_blobs(eb_ctx* ctx, const void* src, int64_t record_bytes, int64_t stride_bytes, int64_t m,
                       uint64_t src_stream);
+
+/* ---- user proposals (moves/red_blue.py:47,82-93; moves/mh.py:31-33,52) ------------------------------------ */
+/* A user proposal, called once per half-step of a schedule entry of kind EB_MOVE_USER / EB_MOVE_USER_MH:
+ *   EB_MOVE_USER (RedBlueMove.get_proposal(s, c, random), red_blue.py:85-90): split = the active set; s[ns, ndim]
+ *     is that set's walkers in ascending walker order; c holds the nsets = nsplits - 1 other sets back to back, in
+ *     set order, each in ascending walker order, c_counts[nsets] their sizes (red_blue.py:85-87);
+ *   EB_MOVE_USER_MH (proposal_function(coords, random), mh.py:52): split = 0, s = the whole ensemble in walker
+ *     order (ns = nwalkers), c = c_counts = NULL, nsets = 0;
+ *   setup call (EB_MOVE_USER with mode = EB_USER_SETUP; RedBlueMove.setup(coords), red_blue.py:73): once per step
+ *     before its splits, split = -1, s = the whole ensemble in walker order, c = c_counts = q = factors = NULL.
+ * The function writes q[ns, ndim] and factors[ns] (the log Hastings ratios) and returns 0, or returns non-zero to
+ * stop the calling ABI function with EB_ERR_CALLBACK.  `step` is the sampler step, so (seed, step, split) names the
+ * call for a generator of the caller's own (DESIGN.md "Draw specification", purpose 8).  Host mode (`where` =
+ * EB_CALLBACK_HOST): every pointer is pinned host staging owned by the engine, stream = NULL.  Device mode: s and
+ * c are device scratch, complete when fn is called; q and factors are the engine's device buffers, which fn fills
+ * with eb_proposal_result (or with work of its own on `stream`, the engine's cudaStream_t).  All pointers are valid
+ * only during the call. */
+typedef int (*eb_proposal_fn)(void* user, uint64_t step, int32_t split, const double* s, int64_t ns,
+                              const double* c, const int64_t* c_counts, int32_t nsets, int64_t ndim, double* q,
+                              double* factors, void* stream);
+#define EB_MAX_PROPOSAL_SLOTS 64
+/* register fn as proposal slot `slot` (0 <= slot < EB_MAX_PROPOSAL_SLOTS); fn == NULL clears it.  `user` is passed back unchanged;
+ * both must stay valid while the slot is set.  A half-step of a user move runs:
+ *   1. the gather of s and c from the live state, in one kernel (red_blue.py:85-87);
+ *   2. host mode: one copy to the host, then a stream synchronisation;  3. fn;
+ *   4. host mode: q and factors are copied to the device;
+ *   5. a non-finite q stops the call with EB_ERR_INF_PARAM / EB_ERR_NAN_PARAM before any log-probability is
+ *      evaluated (ensemble.py:476-479); NaN factors are no error: the comparison rejects them (red_blue.py:100);
+ *   6. the log-probability of q -- the device model, fused with the accept + update kernel, or the callback of
+ *      eb_model_set_callback with its own guards -- then the accept + update (red_blue.py:96-104, mh.py:57-62).
+ * A schedule naming an unset slot is refused with EB_ERR_INVALID.  Failures of fn stop the call inside a step
+ * exactly as a failing log-probability callback does; inside fn every other call on the context returns
+ * EB_ERR_STATE.  Sharded engines are refused with EB_ERR_UNSUPPORTED. */
+int eb_move_set_proposal(eb_ctx* ctx, int32_t slot, eb_proposal_fn fn, void* user, int where);
+/* device mode, from inside fn: copy m (= fn's ns) rows of ndim float64 values, q_row_stride_bytes apart (contiguous
+ * inside a row), from q, and m factors, f_stride_bytes apart, from factors (device or host memory) into fn's q and
+ * factors, ordered on src_stream as eb_callback_result orders its copy.  Complete when the call returns. */
+int eb_proposal_result(eb_ctx* ctx, const void* q, int64_t q_row_stride_bytes, const void* factors,
+                       int64_t f_stride_bytes, int64_t m, uint64_t src_stream);
 
 /* ---- state (state.py:10-45) ------------------------------------------- */
 /* State(initial_state, copy=True) + the initial compute_log_prob
@@ -366,7 +413,8 @@ const char* eb_last_kernel_name(const eb_ctx* ctx);
  * "tma_rows R=<walkers per tile> epl=<8 register path | 0 strided> own_reg=<0|1> warps=<per CTA>",
  * "dense_dmma nhalf_max=<most half-steps of one launch in the call> grid=<CTAs>", "generic G=<lanes per
  * walker>", "walk", "gaussian", "callback G=<lanes per walker> where=host|device" (eb_last_kernel_name
- * "callback": any move with a callback model) or "none". */
+ * "callback": any move with a callback model), "user_move where=host|device" (eb_last_kernel_name "user_move": a
+ * user proposal, with any model) or "none". */
 const char* eb_last_kernel_variant(const eb_ctx* ctx);
 
 /* device micro-benchmarks that anchor the FP64 roofline: what = 0 DFMA, 1 DMMA m8n8k4, 2 DMMA m16n8k8,
