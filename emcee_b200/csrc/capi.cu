@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -2364,14 +2365,26 @@ int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, 
   *c->status_host = 0;
   CK(c, cudaMemsetAsync(c->status_dev, 0, sizeof(int), c->st));
   CK(c, cudaStreamSynchronize(c->st));
-  // centred, column-normalised walkers C (ensemble.py:656-661): C^T C = M_jk / sqrt(M_jj M_kk); the
-  // max-abs scaling of :658-659 cancels, it only matters as the zero-span test
-  for (size_t j = 0; j < D; ++j)
-    if (!(acc[D + j * D + j] > 0.0)) f |= 2;
+  // centred, column-normalised walkers C (ensemble.py:656-661): C^T C = M_jk / (sqrt(M_jj) sqrt(M_kk)); the
+  // max-abs scaling of :658-659 cancels, it only matters as the zero-span test.  The square roots are taken
+  // before the product, so that the denominator stays normal whenever both sums are.  A sum M_jj that is
+  // zero, subnormal or not finite (coordinates near 1e-154 or 1e154 and beyond) has lost its digits: bit 2,
+  // and that column's entries are returned as 0 instead of a ratio of rounding noise or a NaN.
+  std::vector<double> rt(D);
+  for (size_t j = 0; j < D; ++j) {
+    const double m = acc[D + j * D + j];
+    if (!(m > 0.0)) f |= 2;
+    rt[j] = std::isnormal(m) && m > 0.0 ? sqrt(m) : 0.0;
+    if (rt[j] == 0.0) f |= 4;
+  }
   for (size_t j = 0; j < D; ++j)
     for (size_t k = 0; k < D; ++k) {
-      const double den = sqrt(acc[D + j * D + j] * acc[D + k * D + k]);
-      gram[j * D + k] = den > 0.0 ? acc[D + j * D + k] / den : 0.0;
+      double g = rt[j] > 0.0 && rt[k] > 0.0 ? acc[D + j * D + k] / (rt[j] * rt[k]) : 0.0;
+      if (!std::isfinite(g)) {
+        g = 0.0;
+        f |= 4;
+      }
+      gram[j * D + k] = g;
     }
   if (flags) *flags = f;
   return EB_OK;

@@ -513,18 +513,41 @@ class EnsembleSampler(object):
 
     def _walkers_independent(self, coords):
         """``walkers_independent`` (``ensemble.py:653-663``) with the O(N D^2) part on
-        the device: ``eb_walkers_gram`` returns ``C^T C`` of the centred,
-        column-normalised walkers, the host solves the ``D x D`` symmetric
-        eigen-problem, ``cond(C) = sqrt(l_max / l_min)``.  Squaring halves the
-        digits, so only a clearly well-conditioned ensemble (cond <= 1e6 by the
-        Gram matrix) is accepted here; anything nearer the reference's 1e8
-        threshold is decided by the reference's own SVD statement on the host."""
+        the device.  What is decided where:
+
+        * host, the reference's own first statements (O(N D)): a non-finite
+          coordinate gives False; ``C = coords - mean`` with numpy's mean and
+          ``span = amax(|C|, 0)``; a zero span gives False.  The zero-span test
+          is the reference's bit for bit, which a constant column needs: whether
+          ``C`` is zero there depends on the order the mean was summed in.
+        * device: ``eb_walkers_gram`` returns ``G = C^T C`` of ``C`` with column
+          ``j`` scaled by ``2**-frexp(span_j)[1]``, re-centred and
+          column-normalised.  The scaling is exact (or changes an entry by less
+          than 2**-1074) and puts every column's largest entry in [0.5, 1), so
+          the sums of squares neither underflow nor overflow at any scale of the
+          coordinates.  The host solves the D x D eigen-problem, ``cond(C) =
+          sqrt(l_max / l_min)``; squaring halves the digits, so only a clearly
+          well-conditioned ensemble (cond <= 1e6 by the Gram matrix) is accepted
+          here.
+        * host, the reference's SVD statement: everything else -- cond above 1e6
+          by the Gram matrix, a Gram matrix the device flags as unreliable, a
+          centring that overflows, ndim above 1024."""
         coords = np.asarray(coords, dtype=np.float64)
         if coords.ndim != 2 or coords.shape[1] != self.ndim or self.ndim > 1024:
             return walkers_independent(coords)
-        gram, flags = self._engine.walkers_gram(coords)
+        if not np.all(np.isfinite(coords)):
+            return False
+        # the same expressions as ensemble.py:656-659, so that the mean is numpy's, summed in its order
+        centred = coords - np.mean(coords, axis=0)[None, :]
+        span = np.amax(np.abs(centred), axis=0)
+        if not np.all(np.isfinite(span)):
+            return walkers_independent(coords)  # the centring overflowed
+        if np.any(span == 0):
+            return False
+        centred = np.ldexp(centred, -np.frexp(span)[1][None, :])  # not a product: 2**-k overflows for a subnormal span
+        gram, flags = self._engine.walkers_gram(centred)
         if flags:
-            return False  # non-finite coordinate or a column without span
+            return walkers_independent(coords)
         ev = np.linalg.eigvalsh(gram)
         if ev[0] > 0 and np.sqrt(ev[-1] / ev[0]) <= 1e6:
             return True

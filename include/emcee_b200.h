@@ -357,7 +357,13 @@ int eb_moments(eb_ctx* ctx, double* mean, double* cov, uint64_t* count, uint64_t
 /* walkers_independent (ensemble.py:653-663) on the device: gram[ndim*ndim] =
  * C^T C of the centred, column-normalised coords[rows, ndim] (:656-661), whose
  * extreme eigenvalues give cond(C)^2.  *flags: bit 0 = non-finite coordinate
- * (:655), bit 1 = a column with zero span (:659-660).  The D x D symmetric
+ * (:655), bit 1 = a column with zero span (:659-660), bit 2 (additive: earlier
+ * builds of ABI 2 never set it) = some column's sum of squares about its mean is not a positive,
+ * finite, normal double, or an entry overflowed: the Gram matrix is unreliable
+ * (its entries in such columns are 0) and the caller should decide on the host.
+ * Bits 1 and 2 are tested on the sums about the device's column mean, not the
+ * reference's: a caller that wants the reference's zero-span test applies it
+ * itself, and hands over coordinates of a moderate scale.  The D x D symmetric
  * eigen-solve stays on the host (numpy). */
 int eb_walkers_gram(eb_ctx* ctx, const double* coords, size_t rows, double* gram, int* flags);
 /* The device part of autocorr.integrated_time (autocorr.py:49-123, called from
