@@ -36,6 +36,8 @@ EB_IPC_BLOB_BYTES = 256
 EB_COMM_ALLGATHER = 0
 EB_COMM_P2P = 1
 EB_CALLBACK_HOST = 0
+EB_CHAIN_COORDS = 0
+EB_CHAIN_LOG_PROB = 1
 EB_CALLBACK_DEVICE = 1
 EB_MAX_PROPOSAL_SLOTS = 64  # user proposals one engine can hold (eb_move_set_proposal)
 EB_STREAM_UNKNOWN = 2**64 - 1  # eb_callback_result: the producer named no stream -> wait for the whole device
@@ -120,6 +122,12 @@ _SIGNATURES = {
     "eb_chain_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, _dp, _dp]),
     "eb_chain_accepted": (C.c_int, [C.c_void_p, _dp]),
     "eb_chain_autocorr": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, _dp]),
+    "eb_chain_select": (
+        C.c_int,
+        [C.c_void_p, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), C.c_size_t, _dp,
+         C.POINTER(C.c_uint8), C.POINTER(C.c_uint32)],
+    ),
+    "eb_chain_moments": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, _dp, _dp, C.POINTER(C.c_uint64)]),
     "eb_get_naccepted": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "eb_reset_counters": (C.c_int, [C.c_void_p]),
     "eb_move_picks": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_size_t]),
@@ -617,6 +625,31 @@ class Chain(object):
         out = np.empty((self.ndim, int(count)), dtype=np.float64)
         self._check(lib().eb_chain_autocorr(self._h, int(first), int(stride), int(count), _as_dp(out)))
         return np.ascontiguousarray(out.T)
+
+
+    def select(self, what, first, stride, count, ranks):
+        """``(values[len(ranks), D], has_nan[D], passes)``: the exact order statistics at 0-based ``ranks`` of
+        each parameter's ``count * nwalkers`` values in the stored slice (``eb_chain_select``); ``what`` is
+        ``"chain"`` (D = ndim) or ``"log_prob"`` (D = 1)."""
+        ranks = np.ascontiguousarray(ranks, dtype=np.uint64)
+        D = self.ndim if what == "chain" else 1
+        out = np.empty((ranks.size, D))
+        has_nan = np.zeros(D, dtype=np.uint8)
+        passes = C.c_uint32()
+        self._check(lib().eb_chain_select(
+            self._h, EB_CHAIN_COORDS if what == "chain" else EB_CHAIN_LOG_PROB, int(first), int(stride), int(count),
+            ranks.ctypes.data_as(C.POINTER(C.c_uint64)), ranks.size, _as_dp(out),
+            has_nan.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(passes)))
+        return out, has_nan.astype(bool), int(passes.value)
+
+    def moments(self, first, stride, count):
+        """``(mean[ndim], cov[ndim, ndim], n)`` of the stored slice (``eb_chain_moments``)."""
+        mean = np.empty(self.ndim)
+        cov = np.empty((self.ndim, self.ndim))
+        n = C.c_uint64()
+        self._check(lib().eb_chain_moments(self._h, int(first), int(stride), int(count), _as_dp(mean), _as_dp(cov),
+                                           C.byref(n)))
+        return mean, cov, int(n.value)
 
 
 class Engine(object):

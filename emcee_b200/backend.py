@@ -140,11 +140,31 @@ class Backend(object):
         x = self.get_chain(discard=discard, thin=thin)
         return thin * autocorr.integrated_time(x, **kwargs)
 
+    def get_percentile(self, q, discard=0, thin=1, name="chain"):
+        """``np.percentile(get_value(name, flat=True, discard=discard, thin=thin), q, axis=0)``."""
+        _check_summary_name(name)
+        return np.percentile(self.get_value(name, flat=True, discard=discard, thin=thin), q, axis=0)
+
+    def get_moments(self, discard=0, thin=1):
+        """``(mean[ndim], cov[ndim, ndim], count)`` of ``get_chain(flat=True, discard=discard, thin=thin)``:
+        ``np.mean(axis=0)``, ``np.cov(rowvar=False)`` (``ddof = 1``) and the number of samples, as
+        ``EnsembleSampler.moments()`` gives them; NaN for an empty slice."""
+        flat = self.get_chain(flat=True, discard=discard, thin=thin)
+        if len(flat) == 0:
+            return np.full(self.ndim, np.nan), np.full((self.ndim, self.ndim), np.nan), 0
+        cov = np.cov(flat, rowvar=False).reshape(self.ndim, self.ndim)
+        return np.mean(flat, axis=0), cov, len(flat)
+
     def __enter__(self):
         return self
 
     def __exit__(self, *exc):
         pass
+
+
+def _check_summary_name(name):
+    if name not in ("chain", "log_prob"):
+        raise ValueError("percentiles are taken of 'chain' or 'log_prob', not {0!r}".format(name))
 
 
 def slice_plan(iteration, discard=0, thin=1):
@@ -297,6 +317,31 @@ class DeviceBackend(object):
         ch, (first, stride, count) = self._plan(discard, thin)
         rho = ch.autocorr_function(first, stride, count)
         return thin * autocorr.integrated_time_from_acf(rho, **kwargs)
+
+    def get_percentile(self, q, discard=0, thin=1, name="chain"):
+        """``Backend.get_percentile``: ``np.percentile`` of the flat slice along the samples, equal with ``==``
+        (a zero comes back as +0.0).  The exact order statistics are selected on the device, where the chain is
+        (``eb_chain_select``); only they cross PCIe, and numpy's interpolation runs on the host."""
+        from .summary import percentile_finish, percentile_ranks
+
+        _check_summary_name(name)
+        ch, (first, stride, count) = self._plan(discard, thin)
+        plan = percentile_ranks(q, count * self.nwalkers)
+        shape = (0, self.ndim) if name == "chain" else (0,)
+        if count == 0:
+            return np.percentile(np.empty(shape), q, axis=0)  # numpy's own error for an empty slice
+        if plan.ranks.size == 0:
+            return percentile_finish(plan, np.empty(shape))
+        stats, has_nan, _ = ch.select(name, first, stride, count, plan.ranks)
+        if name == "log_prob":
+            stats, has_nan = stats[:, 0], has_nan[0]
+        return percentile_finish(plan, stats, has_nan)
+
+    def get_moments(self, discard=0, thin=1):
+        """``Backend.get_moments`` computed where the chain is (``eb_chain_moments``, the moment sums of
+        ``EnsembleSampler.moments()``); ``ndim`` up to 1024."""
+        ch, (first, stride, count) = self._plan(discard, thin)
+        return ch.moments(first, stride, count)
 
     def __enter__(self):
         return self

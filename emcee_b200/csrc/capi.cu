@@ -2035,6 +2035,53 @@ int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, s
   return EB_OK;
 }
 
+// mean[D], cov[D * D] of m samples from the sums acc = [S1 | S2] about `shift` (eb_moments, eb_chain_moments):
+// mean = shift + S1 / m, cov = (S2 - S1 S1^T / m) / (m - 1)   (np.cov(flatchain, rowvar=False)); NaN when m == 0
+void finish_moments(const double* acc, const double* shift, uint64_t count, size_t D, double* mean, double* cov) {
+  if (count == 0) {
+    if (mean) std::fill(mean, mean + D, NAN);
+    if (cov) std::fill(cov, cov + D * D, NAN);
+    return;
+  }
+  const double m = (double)count;
+  if (mean)
+    for (size_t d = 0; d < D; ++d) mean[d] = shift[d] + acc[d] / m;
+  if (cov)
+    for (size_t r = 0; r < D; ++r)
+      for (size_t k = 0; k < D; ++k)
+        cov[r * D + k] = (acc[D + r * D + k] - acc[r] * acc[k] / m) / (m - 1.0);
+}
+
+// the base of each stored step of the slice: coords ([N, D] blocks) or log_prob ([N] rows)
+std::vector<const double*> chain_slot_table(eb_chain* ch, bool coords, uint64_t first, uint64_t stride,
+                                            uint64_t count) {
+  std::vector<const double*> t;
+  t.reserve(count);
+  for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+                     [&](size_t s, uint64_t off, uint64_t, uint64_t n) {
+                       for (uint64_t j = 0; j < n; ++j)
+                         t.push_back(coords ? ch->segs[s].x + (off + j * stride) * ch->xs
+                                            : ch->segs[s].lp + (off + j * stride) * ch->ls);
+                     });
+  return t;
+}
+
+// scratch of `bytes` on the chain's device, refused before the allocation when it cannot fit
+int chain_scratch(eb_chain* ch, const char* who, size_t bytes, void** out) {
+  *out = nullptr;
+  size_t free_b = 0, total_b = 0;
+  CK(ch, cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > free_b)
+    FAIL(ch, EB_ERR_NOMEM, "%s: %zu bytes of scratch, %zu bytes free", who, bytes, free_b);
+  const cudaError_t e = cudaMalloc(out, bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    *out = nullptr;
+    FAIL(ch, EB_ERR_NOMEM, "%s: allocating %zu bytes of scratch failed (%s)", who, bytes, cudaGetErrorString(e));
+  }
+  return EB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2261,6 +2308,76 @@ int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t co
                    });
 }
 
+int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uint64_t count, const uint64_t* ranks,
+                    size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes) {
+  if (!ch) return EB_ERR_INVALID;
+  if (what != EB_CHAIN_COORDS && what != EB_CHAIN_LOG_PROB)
+    FAIL(ch, EB_ERR_INVALID, "eb_chain_select: what must be EB_CHAIN_COORDS or EB_CHAIN_LOG_PROB");
+  if (count == 0 || nranks == 0 || !ranks || !out || !has_nan)
+    FAIL(ch, EB_ERR_INVALID, "eb_chain_select: empty slice, no rank or null buffer");
+  int rc = chain_check_slice(ch, "eb_chain_select", first, stride, count);
+  if (rc) return rc;
+  const uint64_t n = count * (uint64_t)ch->N;
+  if (n / (uint64_t)ch->N != count) FAIL(ch, EB_ERR_INVALID, "eb_chain_select: slice of more than 2^64 values");
+  for (size_t r = 0; r < nranks; ++r)
+    if (ranks[r] >= n)
+      FAIL(ch, EB_ERR_INVALID, "eb_chain_select: rank %llu of a slice of %llu values per parameter",
+           (unsigned long long)ranks[r], (unsigned long long)n);
+  CK(ch, cudaSetDevice(ch->device));
+  const bool coords = what == EB_CHAIN_COORDS;
+  const int D = coords ? ch->D : 1;
+  uint32_t np = 0;
+  const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
+  const SelectScratch z = select_scratch(count, D, (size_t)D * nranks);
+  void* scratch = nullptr;
+  rc = chain_scratch(ch, "eb_chain_select", z.bytes, &scratch);
+  if (rc) return rc;
+  const cudaError_t e = select_run(slots.data(), count, (uint32_t)ch->N, D, ranks, nranks, out, has_nan, &np, z,
+                                   scratch, ch->sm_count, ch->st);
+  cudaStreamSynchronize(ch->st);
+  cudaFree(scratch);
+  CK(ch, e);
+  if (passes) *passes = np;
+  return EB_OK;
+}
+
+int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* mean, double* cov,
+                     uint64_t* n) {
+  if (!ch) return EB_ERR_INVALID;
+  if (ch->D > 1024) FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_moments is limited to ndim <= 1024");
+  int rc = chain_check_slice(ch, "eb_chain_moments", first, stride, count);
+  if (rc) return rc;
+  const size_t D = (size_t)ch->D, na = D + D * D;
+  if (n) *n = count * (uint64_t)ch->N;
+  if (count == 0) {
+    finish_moments(nullptr, nullptr, 0, D, mean, cov);
+    return EB_OK;
+  }
+  CK(ch, cudaSetDevice(ch->device));
+  // [D shift | D + D*D sums | CTA partials of launch_moments]
+  const size_t head = ((D + na) * sizeof(double) + 255) & ~(size_t)255;
+  void* scratch = nullptr;
+  rc = chain_scratch(ch, "eb_chain_moments", head + moments_partial_bytes(ch->D, ch->sm_count), &scratch);
+  if (rc) return rc;
+  double* shift = static_cast<double*>(scratch);
+  double* acc = shift + D;
+  double* partial = reinterpret_cast<double*>(static_cast<char*>(scratch) + head);
+  const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
+  // shift = the column mean of the slice's first stored step (as eb_moments takes the first accumulated state's);
+  // then every stored step is folded into one accumulator, in slot order
+  cudaError_t e = cudaMemsetAsync(acc, 0, na * sizeof(double), ch->st);
+  if (e == cudaSuccess) e = launch_colmean(slots[0], ch->N, ch->D, shift, nullptr, ch->st);
+  for (size_t k = 0; k < slots.size() && e == cudaSuccess; ++k)
+    e = launch_moments(slots[k], ch->N, ch->D, shift, partial, acc, ch->sm_count, ch->st);
+  std::vector<double> h(D + na);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), shift, (D + na) * sizeof(double), cudaMemcpyDeviceToHost, ch->st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ch->st);
+  cudaFree(scratch);
+  CK(ch, e);
+  finish_moments(h.data() + D, h.data(), count * (uint64_t)ch->N, D, mean, cov);
+  return EB_OK;
+}
+
 int eb_get_naccepted(eb_ctx* c, uint64_t* naccepted) {
   if (!c || !naccepted) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -2306,25 +2423,13 @@ int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* 
   }
   CK(c, cudaStreamSynchronize(c->st));
   c->chain_ok = false;
-  const double m = (double)c->mom_count;
   if (count) *count = c->mom_count;
   if (naccepted_total) {
     unsigned long long tot = 0;
     for (unsigned long long v : nacc) tot += v;
     *naccepted_total = tot;
   }
-  if (c->mom_count == 0) {
-    if (mean) std::fill(mean, mean + D, NAN);
-    if (cov) std::fill(cov, cov + D * D, NAN);
-    return EB_OK;
-  }
-  // mean = shift + S1 / m ; cov = (S2 - S1 S1^T / m) / (m - 1)   (np.cov(flatchain, rowvar=False))
-  if (mean)
-    for (size_t d = 0; d < D; ++d) mean[d] = shift[d] + acc[d] / m;
-  if (cov)
-    for (size_t r = 0; r < D; ++r)
-      for (size_t k = 0; k < D; ++k)
-        cov[r * D + k] = (acc[D + r * D + k] - acc[r] * acc[k] / m) / (m - 1.0);
+  finish_moments(acc.data(), shift.data(), c->mom_count, D, mean, cov);
   return EB_OK;
 }
 

@@ -210,6 +210,21 @@ cudaError_t launch_acf_scale(double* f, size_t n, double scale, cudaStream_t st)
 cudaError_t launch_chain_store(const double* x, const double* lp, const uint8_t* acc, double* cx, double* clp,
                                double* accepted, size_t nx, size_t nl, int64_t N, int sm_count, cudaStream_t st);
 
+// ---- exact order statistics of a stored slice (select.cu, eb_chain_select) ----------------------------------
+constexpr size_t SELECT_PAIR_BATCH = 16384;          // (parameter, rank) pairs planned at once
+constexpr uint64_t SELECT_CAND_MAX = (uint64_t)1 << 23;  // compacted candidates held at once (64 MiB)
+struct SelectScratch {
+  size_t batch = 0;     // pairs per batch
+  uint64_t budget = 0;  // candidate keys
+  size_t bytes = 0;     // device scratch select_run needs
+};
+SelectScratch select_scratch(uint64_t count, int D, size_t npairs);
+// slots[count] (host array of device pointers): each stored step's [N, D] block.  out[nranks, D] and has_nan[D]
+// on the host; *passes = full reads of the slice.  scratch: z.bytes of device memory.
+cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint64_t* ranks,
+                       size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes, const SelectScratch& z,
+                       void* scratch, int sm_count, cudaStream_t st);
+
 inline int lanes_per_walker(int D) {
   int g = 4;
   while (g < 32 && g * 4 < D) g <<= 1;

@@ -583,6 +583,15 @@ class EnsembleSampler(object):
     def get_value(self, name, **kwargs):
         return self.backend.get_value(name, **kwargs)
 
+    def get_percentile(self, q, **kwargs):
+        """``np.percentile`` of the flat stored slice along the samples (``backend.get_percentile``: on the
+        device for a ``DeviceBackend``)."""
+        return self.backend.get_percentile(q, **kwargs)
+
+    def get_moments(self, **kwargs):
+        """``(mean, cov, count)`` of the flat stored slice (``backend.get_moments``)."""
+        return self.backend.get_moments(**kwargs)
+
     def get_autocorr_time(self, discard=0, thin=1, **kwargs):
         """Integrated autocorrelation time of the stored chain (``ensemble.py:619-623``
         -> ``backends/backend.py:130-150``), the FFTs on the GPU (``eb_autocorr``; a

@@ -333,6 +333,27 @@ int eb_chain_accepted(eb_chain* ch, double* accepted);
  * is stored: acf[ndim, count], bit-identical to eb_autocorr of the same slice
  * copied to the host. */
 int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* acf);
+/* Exact order statistics of the stored slice first + k * stride, k < count, read
+ * where it is stored: for each parameter (what = EB_CHAIN_COORDS: ndim of them;
+ * EB_CHAIN_LOG_PROB: one) out[r * D + d] is the value np.partition puts at
+ * 0-based rank ranks[r] (nranks >= 1; each < count * nwalkers; any order, repeats allowed) of
+ * that parameter's count * nwalkers values, with -0.0 returned as +0.0.
+ * has_nan[D] flags the parameters holding a NaN; their entries of out are NaN.
+ * *passes (nullable) = full reads of the slice the call made (radix passes of
+ * SEL_DIGIT bits, select_keys.h).  Device scratch is bounded (about 100 MiB at
+ * most) and checked against the free memory first: EB_ERR_NOMEM. */
+#define EB_CHAIN_COORDS 0
+#define EB_CHAIN_LOG_PROB 1
+int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uint64_t count,
+                    const uint64_t* ranks, size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes);
+/* eb_moments of the stored slice: mean[ndim], cov[ndim*ndim] (np.mean /
+ * np.cov(rowvar=False, ddof=1) of get_chain(flat=True)) and their sample count
+ * count * nwalkers; the sums run about the column mean of the slice's first
+ * stored step, one accumulation per stored step in slot order.  ndim <= 1024
+ * (EB_ERR_UNSUPPORTED beyond); an empty slice gives NaN.  Scratch is checked
+ * against the free memory first: EB_ERR_NOMEM. */
+int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* mean, double* cov,
+                     uint64_t* n);
 
 /* per-walker number of accepted proposals since creation / eb_reset_counters
  * (numerator of acceptance_fraction, ensemble.py:555-558). */
