@@ -8,6 +8,10 @@ The engine's ``eb_step_store_blobs`` writes stored steps straight into the
 ``chain`` / ``log_prob`` / ``blobs`` arrays of this class (pinned double-buffered
 D2H), so ``store=True`` does not need a host round trip per step."""
 
+import builtins
+import itertools
+import operator
+
 import numpy as np
 
 from .state import State
@@ -155,6 +159,37 @@ class Backend(object):
         cov = np.cov(flat, rowvar=False).reshape(self.ndim, self.ndim)
         return np.mean(flat, axis=0), cov, len(flat)
 
+    def get_histogram(self, bins=10, range=None, discard=0, thin=1, name="chain"):
+        """``np.histogram`` of the flat slice: for ``name="chain"``, ``(hist[ndim, bins], edges[ndim, bins + 1])``
+        whose row ``d`` is ``np.histogram(flat[:, d], bins, range=None if range is None else range[d])``; for
+        ``"log_prob"``, ``np.histogram`` of the flat log-probabilities with ``range`` one pair."""
+        _check_histogram_name(name)
+        flat = self.get_value(name, flat=True, discard=discard, thin=thin)
+        if name == "log_prob":
+            return np.histogram(flat, bins=bins, range=range)
+        ranges = _histogram_ranges(range, self.ndim)
+        out = [np.histogram(flat[:, d], bins=bins, range=ranges[d]) for d in builtins.range(self.ndim)]
+        return np.array([h for h, _ in out]), np.array([e for _, e in out], dtype=np.float64)
+
+    def get_histogram2d(self, params=None, bins=10, range=None, discard=0, thin=1):
+        """``(hist[npairs, bins, bins], edges[len(params), bins + 1], pairs)``: ``pairs`` is
+        ``list(itertools.combinations(params, 2))`` and ``hist[p]`` is ``np.histogram2d(flat[:, i], flat[:, j], bins,
+        range=None if range is None else [range[i], range[j]])[0]`` for ``(i, j) = pairs[p]``; ``edges[k]`` are the
+        edges of ``params[k]``.  ``params`` (default: every parameter) are distinct, at least two, in any order;
+        ``range`` is indexed by parameter number."""
+        params = _histogram_params(params, self.ndim)
+        ranges = _histogram_ranges(range, self.ndim)
+        flat = self.get_chain(flat=True, discard=discard, thin=thin)
+        pairs = list(itertools.combinations(params, 2))
+        hist, edges = [], {}
+        for i, j in pairs:
+            h, ei, ej = np.histogram2d(flat[:, i], flat[:, j], bins=bins, range=None if range is None
+                                       else [ranges[i], ranges[j]])
+            hist.append(h)
+            edges.setdefault(i, ei)
+            edges.setdefault(j, ej)
+        return np.array(hist), np.array([edges[k] for k in params], dtype=np.float64), pairs
+
     def __enter__(self):
         return self
 
@@ -165,6 +200,32 @@ class Backend(object):
 def _check_summary_name(name):
     if name not in ("chain", "log_prob"):
         raise ValueError("percentiles are taken of 'chain' or 'log_prob', not {0!r}".format(name))
+
+
+def _check_histogram_name(name):
+    if name not in ("chain", "log_prob"):
+        raise ValueError("histograms are taken of 'chain' or 'log_prob', not {0!r}".format(name))
+
+
+def _histogram_ranges(range, ndim):
+    """``range`` (None, or one ``(lo, hi)`` pair or None per parameter) as a list of ``ndim`` entries"""
+    if range is None:
+        return [None] * ndim
+    ranges = list(range)
+    if len(ranges) != ndim:
+        raise ValueError("range must hold one (lo, hi) pair per parameter: {0} for ndim = {1}".format(
+            len(ranges), ndim))
+    return ranges
+
+
+def _histogram_params(params, ndim):
+    """``params`` of ``get_histogram2d`` as a list of ints: distinct, in ``[0, ndim)``, at least two"""
+    params = list(builtins.range(ndim)) if params is None else [operator.index(p) for p in params]
+    if len(params) < 2:
+        raise ValueError("get_histogram2d needs at least two parameters, got {0}".format(params))
+    if len(set(params)) != len(params) or min(params) < 0 or max(params) >= ndim:
+        raise ValueError("params must be distinct parameter numbers in [0, {0}), got {1}".format(ndim, params))
+    return params
 
 
 def slice_plan(iteration, discard=0, thin=1):
@@ -342,6 +403,67 @@ class DeviceBackend(object):
         ``EnsembleSampler.moments()``); ``ndim`` up to 1024."""
         ch, (first, stride, count) = self._plan(discard, thin)
         return ch.moments(first, stride, count)
+
+    def _column_extremes(self, ch, name, first, stride, count, ranges):
+        """``(lo, hi, has_nan)`` per column of the slice (ranks 0 and n - 1 of ``eb_chain_select``, one call for
+        every column), or None when every column has a given range"""
+        if all(r is not None for r in ranges):
+            return None
+        n = count * self.nwalkers
+        stats, has_nan, _ = ch.select(name, first, stride, count, np.array([0, n - 1], dtype=np.uint64))
+        return stats[0], stats[1], has_nan
+
+    def get_histogram(self, bins=10, range=None, discard=0, thin=1, name="chain"):
+        """``Backend.get_histogram``, equal with ``==``, counted where the chain is (``eb_chain_histogram``, one read
+        of the slice).  An autodetected range takes each column's minimum and maximum from ``eb_chain_select``;
+        numpy forms the edges from them on the host (``summary.uniform_edges``), so a bad ``bins`` or range raises
+        numpy's exception.  ``bins`` is an int of at most 4096; a finite range wider than the largest double
+        raises ``ValueError`` (numpy's own result there is not meaningful)."""
+        from .summary import HIST_BINS_MAX, histogram_bins, uniform_edges
+
+        _check_histogram_name(name)
+        ch, (first, stride, count) = self._plan(discard, thin)
+        D = self.ndim if name == "chain" else 1
+        ranges = [range] if name == "log_prob" else _histogram_ranges(range, D)
+        n = histogram_bins(bins, HIST_BINS_MAX)
+        if count == 0:  # numpy's empty-input result (edges over [0, 1] without a range), no device work
+            out = [np.histogram(np.empty(0), bins=n, range=r) for r in ranges]
+            hist, edges = np.array([h for h, _ in out]), np.array([e for _, e in out], dtype=np.float64)
+            return (hist[0], edges[0]) if name == "log_prob" else (hist, edges)
+        ext = self._column_extremes(ch, name, first, stride, count, ranges)
+        outer = np.empty((D, 3))
+        edges = np.empty((D, n + 1))
+        for d in builtins.range(D):
+            kw = {} if ext is None else dict(lo=ext[0][d], hi=ext[1][d], has_nan=ext[2][d])
+            outer[d], edges[d] = uniform_edges(n, ranges[d], **kw)
+        hist = ch.histogram(name, first, stride, count, n, outer, edges)
+        if name == "log_prob":
+            return hist[0], edges[0]
+        return hist, edges
+
+    def get_histogram2d(self, params=None, bins=10, range=None, discard=0, thin=1):
+        """``Backend.get_histogram2d``, equal with ``==``, counted where the chain is (``eb_chain_histogram2d``,
+        one read of the slice for every pair of a tile).  Edges come from numpy on each column's ``[min; max]``
+        (``summary.searched_edges``).  ``bins`` is an int of at most 128; a finite range wider than the largest
+        double raises ``ValueError``.  The counts of all pairs are held in device memory at once
+        (``npairs * bins^2 * 8`` bytes; ``MemoryError`` when they do not fit)."""
+        from .summary import HIST2_BINS_MAX, histogram_bins, searched_edges
+
+        ch, (first, stride, count) = self._plan(discard, thin)
+        params = _histogram_params(params, self.ndim)
+        ranges = _histogram_ranges(range, self.ndim)
+        n = histogram_bins(bins, HIST2_BINS_MAX, two_d=True)
+        pairs = list(itertools.combinations(params, 2))
+        if count == 0:  # numpy's empty-input result, no device work
+            e = [searched_edges(n, ranges[p], 0.0, 1.0) for p in params]
+            return np.zeros((len(pairs), n, n)), np.array(e, dtype=np.float64), pairs
+        ext = self._column_extremes(ch, "chain", first, stride, count, [ranges[p] for p in params])
+        edges = np.empty((len(params), n + 1))
+        for k, p in enumerate(params):
+            kw = {} if ext is None else dict(lo=ext[0][p], hi=ext[1][p], has_nan=ext[2][p])
+            edges[k] = searched_edges(n, ranges[p], **kw)
+        hist = ch.histogram2d(first, stride, count, params, n, edges)
+        return hist.astype(np.float64), edges, pairs
 
     def __enter__(self):
         return self

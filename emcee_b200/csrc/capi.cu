@@ -13,6 +13,7 @@
 #include "chain_map.h"
 #include "comm.h"
 #include "engine.cuh"
+#include "hist_bins.h"
 
 using namespace eb;
 
@@ -2375,6 +2376,85 @@ int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t cou
   cudaFree(scratch);
   CK(ch, e);
   finish_moments(h.data() + D, h.data(), count * (uint64_t)ch->N, D, mean, cov);
+  return EB_OK;
+}
+
+int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, uint64_t count, uint32_t bins,
+                       const double* outer, const double* edges, uint64_t* hist) {
+  if (!ch) return EB_ERR_INVALID;
+  if (what != EB_CHAIN_COORDS && what != EB_CHAIN_LOG_PROB)
+    FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram: what must be EB_CHAIN_COORDS or EB_CHAIN_LOG_PROB");
+  if (bins == 0 || !outer || !edges || !hist) FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram: bins == 0 or null buffer");
+  if (bins > (uint32_t)HIST_BINS_MAX)
+    FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram is limited to bins <= %d on the device, got %u", HIST_BINS_MAX,
+         bins);
+  int rc = chain_check_slice(ch, "eb_chain_histogram", first, stride, count);
+  if (rc) return rc;
+  const bool coords = what == EB_CHAIN_COORDS;
+  const int D = coords ? ch->D : 1;
+  if (count == 0) {
+    std::fill(hist, hist + (size_t)D * bins, (uint64_t)0);
+    return EB_OK;
+  }
+  const uint64_t n = count * (uint64_t)ch->N;
+  if (n / (uint64_t)ch->N != count || !hist_rows_fit(n))
+    FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram: slice of %llu stored steps is too long",
+         (unsigned long long)count);
+  CK(ch, cudaSetDevice(ch->device));
+  const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
+  void* scratch = nullptr;
+  rc = chain_scratch(ch, "eb_chain_histogram", hist1_scratch_bytes(count, D, (int)bins), &scratch);
+  if (rc) return rc;
+  bool bad = false;
+  const cudaError_t e = hist1_run(slots.data(), count, (uint32_t)ch->N, D, (int)bins, outer, edges, hist, &bad,
+                                  scratch, ch->sm_count, ch->st);
+  cudaStreamSynchronize(ch->st);
+  cudaFree(scratch);
+  CK(ch, e);
+  if (bad)
+    FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram: a value's truncated bin index is above bins (np.histogram raises "
+         "IndexError there); the span does not fit the edges");
+  return EB_OK;
+}
+
+int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, const uint32_t* params,
+                         size_t nparams, uint32_t bins, const double* edges, uint64_t* hist) {
+  if (!ch) return EB_ERR_INVALID;
+  if (bins == 0 || !params || !edges || !hist)
+    FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram2d: bins == 0 or null buffer");
+  if (bins > (uint32_t)HIST2_BINS_MAX)
+    FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram2d is limited to bins <= %d on the device, got %u",
+         HIST2_BINS_MAX, bins);
+  if (nparams < 2 || nparams > (size_t)ch->D)
+    FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram2d: need 2 <= nparams <= ndim = %d, got %zu", ch->D, nparams);
+  std::vector<uint8_t> seen((size_t)ch->D, 0);
+  for (size_t k = 0; k < nparams; ++k) {
+    if (params[k] >= (uint32_t)ch->D || seen[params[k]])
+      FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram2d: params must be distinct and < ndim = %d (params[%zu] = %u)",
+           ch->D, k, params[k]);
+    seen[params[k]] = 1;
+  }
+  int rc = chain_check_slice(ch, "eb_chain_histogram2d", first, stride, count);
+  if (rc) return rc;
+  const size_t out = nparams * (nparams - 1) / 2 * (size_t)bins * bins;
+  if (count == 0) {
+    std::fill(hist, hist + out, (uint64_t)0);
+    return EB_OK;
+  }
+  const uint64_t n = count * (uint64_t)ch->N;
+  if (n / (uint64_t)ch->N != count || !hist_rows_fit(n))
+    FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram2d: slice of %llu stored steps is too long",
+         (unsigned long long)count);
+  CK(ch, cudaSetDevice(ch->device));
+  const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
+  void* scratch = nullptr;
+  rc = chain_scratch(ch, "eb_chain_histogram2d", hist2_scratch_bytes(count, (int)nparams, (int)bins), &scratch);
+  if (rc) return rc;
+  const cudaError_t e = hist2_run(slots.data(), count, (uint32_t)ch->N, ch->D, params, (int)nparams, (int)bins, edges,
+                                  hist, scratch, ch->sm_count, ch->st);
+  cudaStreamSynchronize(ch->st);
+  cudaFree(scratch);
+  CK(ch, e);
   return EB_OK;
 }
 

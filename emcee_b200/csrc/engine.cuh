@@ -225,6 +225,19 @@ cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, i
                        size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes, const SelectScratch& z,
                        void* scratch, int sm_count, cudaStream_t st);
 
+// ---- histograms of a stored slice (histogram.cu, eb_chain_histogram / eb_chain_histogram2d) ----------------------
+// can count * N rows be split over grid y with fewer than 2^32 counted by one CTA?
+bool hist_rows_fit(uint64_t n);
+size_t hist1_scratch_bytes(uint64_t count, int D, int bins);
+// slots[count] (host array of device pointers); outer[D, 3] = (first, last, span), edges[D, bins + 1] and
+// hist[D, bins] on the host; *bad: some value's bin index fell outside the edges
+cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t N, int D, int bins, const double* outer,
+                      const double* edges, uint64_t* hist, bool* bad, void* scratch, int sm_count, cudaStream_t st);
+size_t hist2_scratch_bytes(uint64_t count, int m, int bins);
+// params[m] distinct columns; edges[m, bins + 1] and hist[m (m - 1) / 2, bins, bins] on the host
+cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint32_t* params, int m,
+                      int bins, const double* edges, uint64_t* hist, void* scratch, int sm_count, cudaStream_t st);
+
 inline int lanes_per_walker(int D) {
   int g = 4;
   while (g < 32 && g * 4 < D) g <<= 1;

@@ -592,6 +592,15 @@ class EnsembleSampler(object):
         """``(mean, cov, count)`` of the flat stored slice (``backend.get_moments``)."""
         return self.backend.get_moments(**kwargs)
 
+    def get_histogram(self, bins=10, range=None, discard=0, thin=1, name="chain"):
+        """``np.histogram`` of each parameter (or of the log-probabilities) of the flat stored slice
+        (``backend.get_histogram``: counted on the device for a ``DeviceBackend``)."""
+        return self.backend.get_histogram(bins, range, discard=discard, thin=thin, name=name)
+
+    def get_histogram2d(self, params=None, bins=10, range=None, discard=0, thin=1):
+        """``np.histogram2d`` of every pair of ``params`` of the flat stored slice (``backend.get_histogram2d``)."""
+        return self.backend.get_histogram2d(params, bins, range, discard=discard, thin=thin)
+
     def get_autocorr_time(self, discard=0, thin=1, **kwargs):
         """Integrated autocorrelation time of the stored chain (``ensemble.py:619-623``
         -> ``backends/backend.py:130-150``), the FFTs on the GPU (``eb_autocorr``; a

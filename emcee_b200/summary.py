@@ -5,11 +5,28 @@ array (``_get_indexes``: floor / floor + 1 of the virtual index ``(n - 1) q``, c
 raising numpy's exceptions for a bad ``q``; ``percentile_finish`` takes the values at those ranks and applies
 numpy's ``_lerp`` arithmetic.  Both follow numpy's statements one for one, so that a caller that finds the order
 statistics exactly (``DeviceBackend.get_percentile`` does so on the GPU, ``eb_chain_select``) returns what
-``np.percentile(x, q, axis=0)`` returns, compared with ``==``."""
+``np.percentile(x, q, axis=0)`` returns, compared with ``==``.
+
+The histogram plan (``histogram_bins``, ``uniform_edges``, ``searched_edges``) gives the edges of
+``np.histogram`` / ``np.histogram2d`` of a column from its minimum and maximum alone: numpy depends on the data
+only through them (``_get_outer_edges``, ``np.linspace``, the finite-bins check), so numpy's own functions called
+on the two-row array ``[min; max]`` return the edges, and raise the exceptions, that they would on the whole
+column.  ``DeviceBackend.get_histogram`` / ``get_histogram2d`` then count on the GPU with these edges."""
+
+import operator
 
 import numpy as np
 
-__all__ = ["percentile_ranks", "percentile_finish"]
+try:
+    from numpy.lib._histograms_impl import _get_outer_edges, _unsigned_subtract
+except ImportError:  # numpy < 2
+    from numpy.lib.histograms import _get_outer_edges, _unsigned_subtract
+
+__all__ = ["percentile_ranks", "percentile_finish", "histogram_bins", "uniform_edges", "searched_edges",
+           "HIST_BINS_MAX", "HIST2_BINS_MAX"]
+
+HIST_BINS_MAX = 4096  # eb_chain_histogram (hist_bins.h)
+HIST2_BINS_MAX = 128  # eb_chain_histogram2d: a 64 KiB uint32 pair histogram in shared memory
 
 
 def _quantile_is_valid(q):
@@ -81,3 +98,68 @@ def percentile_finish(plan, stats, has_nan=None):
         else:
             np.copyto(result, np.nan, where=np.asarray(has_nan, dtype=bool).reshape(stats.shape[1:]))
     return result
+
+
+def histogram_bins(bins, limit, two_d=False):
+    """``bins`` as the device takes it: numpy's own check first (``np.histogram``'s, or ``np.histogram2d``'s when
+    ``two_d``: its exception for a bad ``bins``), then an int of at most ``limit`` (``NotImplementedError`` beyond,
+    and for the string rules and explicit edge arrays numpy also accepts)."""
+    if two_d:
+        np.histogramdd(np.empty((0, 2)), bins)
+    else:
+        np.histogram_bin_edges(np.empty(0), bins)
+    if isinstance(bins, str) or np.ndim(bins) != 0:
+        raise NotImplementedError("the device histograms take an integer number of bins, not {0!r}".format(bins))
+    n = operator.index(bins)
+    if n > limit:
+        raise NotImplementedError("the device histogram is limited to bins <= {0}, got {1}".format(limit, n))
+    return n
+
+
+def _check_overflow(a2, rng):
+    """Refuse a finite range wider than the largest double: ``np.linspace`` overflows there and the edges numpy
+    returns are not all finite (numpy then indexes with a NaN-derived integer, or counts nonsense)."""
+    lo, hi = (a2[0], a2[1]) if rng is None else rng
+    try:
+        lo, hi = np.float64(lo), np.float64(hi)
+    except (TypeError, ValueError):
+        return  # numpy raises its own exception for this range
+    with np.errstate(over="ignore", invalid="ignore"):
+        if np.isfinite(lo) and np.isfinite(hi) and lo < hi and not np.isfinite(hi - lo):
+            raise ValueError("range of [{0}, {1}] is wider than the largest double: its histogram edges would not be "
+                             "finite".format(lo, hi))
+
+
+def _two_rows(lo, hi, has_nan):
+    """the ``[min; max]`` stand-in of a column: NaN for a column that holds one (numpy's ``min()`` propagates it)"""
+    return np.array([np.nan, np.nan]) if has_nan else np.array([lo, hi], dtype=np.float64)
+
+
+def uniform_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
+    """``(outer[3], edges[bins + 1])`` of ``np.histogram(column, bins, rng)`` for a column with minimum ``lo`` and
+    maximum ``hi`` (used only when ``rng`` is None): ``outer`` is numpy's ``(first_edge, last_edge, norm_denom)``
+    of its uniform-bin fast path, as float64.  numpy's exceptions for a bad range; ``ValueError`` for an
+    overflowing one."""
+    a2 = _two_rows(lo, hi, has_nan)
+    _check_overflow(a2, rng)
+    edges = np.histogram_bin_edges(a2, bins, rng)
+    first, last = _get_outer_edges(a2, rng)
+    span = _unsigned_subtract(last, first)
+    if not np.all(np.isfinite(edges)):
+        raise ValueError("histogram edges over [{0}, {1}] are not finite".format(first, last))
+    return np.array([first, last, span], dtype=np.float64), np.asarray(edges, dtype=np.float64)
+
+
+def searched_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
+    """``edges[bins + 1]`` of one axis of ``np.histogram2d`` / ``np.histogramdd`` for a column with minimum ``lo``
+    and maximum ``hi``: ``np.histogramdd`` of the column's ``[min; max]`` alone, which forms each axis's edges
+    independently of the others.  numpy's exceptions for a bad range; ``ValueError`` for an overflowing one.  A
+    finite range gives non-decreasing edges (``np.linspace`` rounds monotonically), so ``searchsorted`` is the count
+    of edges at or below a value."""
+    a2 = _two_rows(lo, hi, has_nan)
+    _check_overflow(a2, rng)
+    with np.errstate(invalid="ignore"):
+        _, (edges,) = np.histogramdd(a2[:, None], bins=bins, range=None if rng is None else [rng])
+    if not np.all(np.isfinite(edges)):
+        raise ValueError("histogram edges over [{0}, {1}] are not finite".format(edges[0], edges[-1]))
+    return np.asarray(edges, dtype=np.float64)

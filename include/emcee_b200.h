@@ -354,6 +354,30 @@ int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uin
  * against the free memory first: EB_ERR_NOMEM. */
 int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* mean, double* cov,
                      uint64_t* n);
+/* np.histogram of each parameter (what = EB_CHAIN_COORDS: ndim of them;
+ * EB_CHAIN_LOG_PROB: one) of the stored slice first + k * stride, k < count, read
+ * where it is stored, with numpy's edges given by the caller: outer[D * 3] holds
+ * each parameter's (first_edge, last_edge, norm_denom) and edges[D * (bins + 1)]
+ * its linspace, as np.histogram forms them.  hist[D * bins] gets the counts of
+ * numpy's uniform-bin rule (values outside [first_edge, last_edge] and NaN are
+ * dropped).  1 <= bins <= 4096 (EB_ERR_UNSUPPORTED beyond); a value whose
+ * truncated index ((x - first) / span) * bins is above bins (numpy indexes past
+ * its edges there and raises IndexError) gives EB_ERR_INVALID; count == 0 gives
+ * zero counts.  Scratch is checked against the
+ * free memory first: EB_ERR_NOMEM. */
+int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, uint64_t count, uint32_t bins,
+                       const double* outer, const double* edges, uint64_t* hist);
+/* np.histogram2d of every pair of the nparams >= 2 distinct coordinates
+ * params[] (each < ndim) of the stored slice: pair p is the p-th of
+ * itertools.combinations(params, 2) and hist[p * bins * bins + x * bins + y]
+ * counts its values in bin x of params[i] and bin y of params[j], with
+ * np.histogramdd's rule (searchsorted right, the last edge in the last bin,
+ * outliers and NaN dropped) against edges[k * (bins + 1) ...], the edges of
+ * params[k].  1 <= bins <= 128 (EB_ERR_UNSUPPORTED beyond); count == 0 gives
+ * zero counts.  hist holds nparams (nparams - 1) / 2 * bins^2 counts, all in
+ * device scratch at once, checked against the free memory first: EB_ERR_NOMEM. */
+int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, const uint32_t* params,
+                         size_t nparams, uint32_t bins, const double* edges, uint64_t* hist);
 
 /* per-walker number of accepted proposals since creation / eb_reset_counters
  * (numerator of acceptance_fraction, ensemble.py:555-558). */
