@@ -140,6 +140,11 @@ _SIGNATURES = {
     "eb_reset_counters": (C.c_int, [C.c_void_p]),
     "eb_move_picks": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_size_t]),
     "eb_moments": (C.c_int, [C.c_void_p, _dp, _dp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_histograms_config": (
+        C.c_int,
+        [C.c_void_p, C.c_uint64, C.c_uint32, _dp, _dp, C.c_int, C.POINTER(C.c_uint32), C.c_size_t, C.c_uint32, _dp],
+    ),
+    "eb_histograms": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "eb_walkers_gram": (C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp, C.POINTER(C.c_int)]),
     "eb_autocorr": (C.c_int, [C.c_void_p, _dp, C.c_size_t, C.c_size_t, C.c_size_t, _dp]),
     "eb_last_step_timing": (C.c_int, [C.c_void_p, _dp, C.POINTER(C.c_uint64)]),
@@ -830,6 +835,36 @@ class Engine(object):
         n, na = C.c_uint64(), C.c_uint64()
         self._check(lib().eb_moments(self._h, _as_dp(mean), _as_dp(cov), C.byref(n), C.byref(na)))
         return mean, cov, int(n.value), int(na.value)
+
+    def histograms_config(self, every, bins, outer, edges, log_prob=False, params2d=None, bins2d=0, edges2d=None):
+        """Count every ``every``-th step into running histograms (``eb_histograms_config``; zeroes the counts):
+        ``outer[ndim + log_prob, 3]`` / ``edges[ndim + log_prob, bins + 1]`` as :meth:`Chain.histogram` takes them,
+        the log-probabilities in the last row; ``params2d`` (or None) with ``edges2d[len(params2d), bins2d + 1]``."""
+        rows, bins = self.ndim + (1 if log_prob else 0), int(bins)
+        outer = _f64(outer, (rows, 3))
+        edges = _f64(edges, (rows, bins + 1))
+        p, m, e2 = None, 0, None
+        if params2d is not None:
+            params2d = np.ascontiguousarray(params2d, dtype=np.uint32)
+            m, bins2d = params2d.size, int(bins2d)
+            e2 = _f64(edges2d, (m, bins2d + 1))
+            p = params2d.ctypes.data_as(C.POINTER(C.c_uint32))
+        self._check(lib().eb_histograms_config(
+            self._h, int(every), bins, _as_dp(outer), _as_dp(edges), int(bool(log_prob)), p, m, int(bins2d),
+            None if e2 is None else _as_dp(e2)))
+        self._hist_shape = (rows, bins, m, int(bins2d))
+
+    def histograms(self, counts=True):
+        """``(hist[ndim + log_prob, bins] uint64, hist2d[npairs, bins2d, bins2d] uint64 or None, count)`` of the
+        running histograms (``eb_histograms``); ``counts=False`` reads only ``count``."""
+        rows, bins, m, bins2d = getattr(self, "_hist_shape", (self.ndim, 1, 0, 0))
+        hist = np.zeros((rows, bins), dtype=np.uint64) if counts else None
+        hist2 = np.zeros((m * (m - 1) // 2, bins2d, bins2d), dtype=np.uint64) if m and counts else None
+        n = C.c_uint64()
+        self._check(lib().eb_histograms(
+            self._h, None if hist is None else hist.ctypes.data_as(C.POINTER(C.c_uint64)),
+            None if hist2 is None else hist2.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(n)))
+        return hist, hist2, int(n.value)
 
     def walkers_gram(self, coords):
         """``(gram[D, D], flags)`` of ``eb_walkers_gram`` for ``coords[rows, D]``."""

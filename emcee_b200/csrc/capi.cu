@@ -124,6 +124,12 @@ struct eb_ctx {
   unsigned long long mom_count = 0;
   bool mom_have_shift = false;
 
+  // running histograms (eb_histograms): the owned rows of every `hist_every`-th step counted into hist.counts
+  uint64_t hist_every = 0;
+  bool hist_on = false;  // configured: hist holds tables and counts
+  LiveHist hist;
+  unsigned long long hist_count = 0;  // samples counted
+
   // WalkMove / GaussianMove scratch (moves_extra.cu)
   double* qbuf = nullptr;       // [N, D] proposals
   double* walk_work = nullptr;  // [D shift | D + D*D moment sums | D*D cov | D*D L]
@@ -358,6 +364,7 @@ int eb_destroy(eb_ctx* c) {
   cudaFree(c->mom_acc);
   cudaFree(c->mom_shift);
   cudaFree(c->mom_partial);
+  cudaFree(c->hist.mem);
   for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
   cudaFree(c->timeline);
   cudaFree(c->tap_partners);
@@ -1617,6 +1624,7 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
 // enqueue copies on the stream; `sync_every` > 0 tells how often it actually does (every
 // sync_every-th step), so that steps in between can share one persistent launch.
 int accumulate_moments(eb_ctx* c, uint64_t& launches);  // below
+int accumulate_histograms(eb_ctx* c, uint64_t& launches);  // below
 
 template <class F>
 int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every, F&& after_step) {
@@ -1753,7 +1761,8 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
           }
         }
         const bool moments_now = c->moments_every > 0 && (c->step + 1) % c->moments_every == 0;
-        const bool host_event = perstep || moments_now || (sync_every > 0 && (done + k + 1) % sync_every == 0);
+        const bool hist_now = c->hist_every > 0 && (c->step + 1) % c->hist_every == 0;
+        const bool host_event = perstep || moments_now || hist_now || (sync_every > 0 && (done + k + 1) % sync_every == 0);
         if (host_event || k + 1 == chunk || grp.nhalf >= c->dmma_group) {
           rc = flush_dmma(c, mv, grp, launches);
           if (rc) return rc;
@@ -1779,6 +1788,10 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
       c->step += 1;
       if (c->moments_every > 0 && c->step % c->moments_every == 0) {
         rc = accumulate_moments(c, launches);
+        if (rc) return rc;
+      }
+      if (c->hist_every > 0 && c->step % c->hist_every == 0) {
+        rc = accumulate_histograms(c, launches);
         if (rc) return rc;
       }
       if (perstep) {
@@ -1846,6 +1859,14 @@ int accumulate_moments(eb_ctx* c, uint64_t& launches) {
   CK(c, launch_moments(X, r1 - r0, c->D, c->mom_shift, c->mom_partial, c->mom_acc, c->sm_count, c->st));
   launches += 2;
   c->mom_count += (unsigned long long)(r1 - r0);
+  return EB_OK;
+}
+
+// count the CURRENT state into the running histograms (kernels only, enqueued on the stream)
+int accumulate_histograms(eb_ctx* c, uint64_t& launches) {
+  c->chain_ok = false;
+  CK(c, live_hist_launch(c->hist, c->st, launches));
+  c->hist_count += (unsigned long long)c->N;
   return EB_OK;
 }
 
@@ -2513,6 +2534,80 @@ int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* 
   return EB_OK;
 }
 
+int eb_histograms_config(eb_ctx* c, uint64_t every, uint32_t bins, const double* outer, const double* edges,
+                         int log_prob, const uint32_t* params2d, size_t nparams2d, uint32_t bins2d,
+                         const double* edges2d) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
+  if (bins == 0 || !outer || !edges) FAIL(c, EB_ERR_INVALID, "eb_histograms_config: bins == 0 or null buffer");
+  if (bins > (uint32_t)HIST_BINS_MAX)
+    FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are limited to bins <= %d on the device, got %u", HIST_BINS_MAX,
+         bins);
+  if (nparams2d > 0) {
+    if (!params2d || !edges2d || bins2d == 0)
+      FAIL(c, EB_ERR_INVALID, "eb_histograms_config: bins2d == 0 or null 2-D buffer");
+    if (bins2d > (uint32_t)HIST2_BINS_MAX)
+      FAIL(c, EB_ERR_UNSUPPORTED, "running 2-D histograms are limited to bins <= %d on the device, got %u",
+           HIST2_BINS_MAX, bins2d);
+    if (nparams2d < 2 || nparams2d > (size_t)c->D)
+      FAIL(c, EB_ERR_INVALID, "eb_histograms_config: need 2 <= nparams2d <= ndim = %d, got %zu", c->D, nparams2d);
+    std::vector<uint8_t> seen((size_t)c->D, 0);
+    for (size_t k = 0; k < nparams2d; ++k) {
+      if (params2d[k] >= (uint32_t)c->D || seen[params2d[k]])
+        FAIL(c, EB_ERR_INVALID, "eb_histograms_config: params2d must be distinct and < ndim = %d (params2d[%zu] = %u)",
+             c->D, k, params2d[k]);
+      seen[params2d[k]] = 1;
+    }
+  }
+  CK(c, cudaSetDevice(c->device));
+  // the old configuration goes first: its memory counts towards what the new one may take
+  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaFree(c->hist.mem));
+  c->hist = LiveHist{};
+  c->hist_on = false;
+  c->hist_every = 0;
+  c->hist_count = 0;
+  const int lp = log_prob ? 1 : 0, m = nparams2d > 0 ? (int)nparams2d : 0;
+  const size_t bytes = live_hist_bytes(c->D, (int)bins, lp, m, (int)bins2d);
+  size_t free_b = 0, total_b = 0;
+  CK(c, cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > free_b)
+    FAIL(c, EB_ERR_NOMEM, "eb_histograms_config: %zu bytes of counts and tables, %zu bytes free", bytes, free_b);
+  void* mem = nullptr;
+  const cudaError_t e = cudaMalloc(&mem, bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    FAIL(c, EB_ERR_NOMEM, "eb_histograms_config: allocating %zu bytes failed (%s)", bytes, cudaGetErrorString(e));
+  }
+  const cudaError_t s = live_hist_setup(&c->hist, mem, (uint32_t)c->N, c->D, (int)bins, lp, outer, edges, params2d, m,
+                                        (int)bins2d, edges2d, c->coords, c->logp, c->sm_count, c->st);
+  if (s != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(mem);
+    c->hist = LiveHist{};
+    FAIL(c, EB_ERR_CUDA, "eb_histograms_config: %s", cudaGetErrorString(s));
+  }
+  c->hist_on = true;
+  c->hist_every = every;
+  return EB_OK;
+}
+
+int eb_histograms(eb_ctx* c, uint64_t* hist, uint64_t* hist2d, uint64_t* count) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->hist_on) FAIL(c, EB_ERR_STATE, "eb_histograms: configure them with eb_histograms_config first");
+  CK(c, cudaSetDevice(c->device));
+  bool bad = false;
+  CK(c, live_hist_read(c->hist, hist, hist2d, &bad, c->st));
+  c->chain_ok = false;
+  if (count) *count = c->hist_count;
+  if (bad)
+    FAIL(c, EB_ERR_INVALID, "eb_histograms: a value's truncated bin index is above bins (np.histogram raises "
+         "IndexError there); the span does not fit the edges");
+  return EB_OK;
+}
+
 int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, int* flags) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -2719,6 +2814,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
   NOT_IN_CALLBACK(c);
   if (c->have_model && c->model.kind == MODEL_EXTERNAL && nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
+  if (c->hist_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path

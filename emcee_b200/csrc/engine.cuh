@@ -238,6 +238,39 @@ size_t hist2_scratch_bytes(uint64_t count, int m, int bins);
 cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint32_t* params, int m,
                       int bins, const double* edges, uint64_t* hist, void* scratch, int sm_count, cudaStream_t st);
 
+// ---- running histograms of the live state (histogram.cu, eb_histograms_config / eb_histograms) -------------------
+struct HistTile;
+// one configuration: device tables and persistent counts inside `mem` (live_hist_bytes of it), launch geometry
+struct LiveHist {
+  uint32_t N = 0;
+  int D = 0, bins = 0, lp = 0;  // lp: row D of the 1-D tables counts the log-probabilities
+  int m = 0, bins2 = 0;         // 2-D: m parameters (m >= 2), bins2 per axis
+  void* mem = nullptr;
+  const double** slots = nullptr;  // [coords, logp]
+  double* outer = nullptr;         // [D + lp, 3]
+  double* edges = nullptr;         // [D + lp, bins + 1]
+  unsigned long long* hist = nullptr;  // [D + lp, bins]
+  unsigned int* bad = nullptr;
+  HistTile* tiles = nullptr;
+  uint32_t ntiles = 0;
+  uint32_t* params = nullptr;           // [m]
+  double* edges2 = nullptr;             // [m, bins2 + 1]
+  unsigned long long* hist2 = nullptr;  // [m (m - 1) / 2, bins2, bins2]
+  int W1 = 1, Wlp = 1;
+  size_t smem1 = 0, smemlp = 0, smem2 = 0;
+  dim3 grid1, gridlp, grid2;
+  uint64_t rows1 = 0, rowslp = 0, rows2 = 0;
+};
+size_t live_hist_bytes(int D, int bins, int lp, int m, int bins2);
+// uploads the tables, zeroes the counts and synchronises; m < 2: no 2-D counts
+cudaError_t live_hist_setup(LiveHist* h, void* mem, uint32_t N, int D, int bins, int lp, const double* outer,
+                            const double* edges, const uint32_t* params, int m, int bins2, const double* edges2,
+                            const double* coords, const double* logp, int sm_count, cudaStream_t st);
+// adds the current state to the counts: kernels only, on `st` (launches += their number)
+cudaError_t live_hist_launch(const LiveHist& h, cudaStream_t st, uint64_t& launches);
+// hist[(D + lp) * bins], hist2 (nullable) to the host; *bad: some value fell past numpy's edge array
+cudaError_t live_hist_read(const LiveHist& h, uint64_t* hist, uint64_t* hist2, bool* bad, cudaStream_t st);
+
 inline int lanes_per_walker(int D) {
   int g = 4;
   while (g < 32 && g * 4 < D) g <<= 1;

@@ -278,8 +278,144 @@ cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t N, in
   HE(cudaGetLastError());
   HE(cudaMemcpyAsync(hist, d_hist, out * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   HE(cudaStreamSynchronize(st));
-#undef HE
   return cudaSuccess;
 }
+
+// ---- running histograms of the live state ---------------------------------------------------------------------
+// The same kernels over one "stored step": the engine's [N, D] coordinates (and [N] log-probabilities), read through
+// a two-entry slot table uploaded once.  The counts and the bad flag persist across launches; a launch only adds.
+
+namespace {
+
+// the layout of LiveHist::mem: slot table, 1-D tables and counts, bad flag, then the 2-D tables and counts
+struct LiveLayout {
+  size_t slots, outer, edges, hist, bad, tiles, params, edges2, hist2, bytes;
+};
+
+LiveLayout live_layout(int D, int bins, int lp, int m, int bins2, uint64_t ntiles) {
+  const size_t rows = (size_t)D + (size_t)lp, npairs = (size_t)m * (m > 0 ? m - 1 : 0) / 2;
+  LiveLayout l;
+  size_t at = 0;
+  auto take = [&](size_t bytes) {
+    const size_t q = at;
+    at += align256(bytes);
+    return q;
+  };
+  l.slots = take(2 * sizeof(double*));
+  l.outer = take(rows * 3 * sizeof(double));
+  l.edges = take(rows * (bins + 1) * sizeof(double));
+  l.hist = take(rows * bins * sizeof(uint64_t));
+  l.bad = take(sizeof(uint32_t));
+  l.tiles = take(ntiles * sizeof(HistTile));
+  l.params = take((size_t)m * sizeof(uint32_t));
+  l.edges2 = take((size_t)m * (bins2 + 1) * sizeof(double));
+  l.hist2 = take(npairs * bins2 * bins2 * sizeof(uint64_t));
+  l.bytes = at;
+  return l;
+}
+
+uint64_t live_ntiles(int m, int bins2) { return m >= 2 ? hist2_ntiles(m, hist2_geom(m, bins2).block) : 0; }
+
+// column block width, shared bytes and grid of the 1-D kernel over D columns of N rows
+void live_hist1_geom(uint32_t N, int D, int bins, int sm_count, int* W, size_t* smem, dim3* grid, uint64_t* rows_per) {
+  const size_t col = hist1_col_bytes(bins);
+  *W = (int)std::max<size_t>(1, std::min<size_t>({(size_t)32, (size_t)D, HIST1_SMEM / col}));
+  *smem = (size_t)*W * col;
+  const uint64_t nx = ((uint64_t)D + *W - 1) / *W;
+  uint64_t ys = 1;
+  split_rows(N, nx, (uint64_t)sm_count * 8, (uint64_t)(HIST_THREADS / *W) * 16, &ys, rows_per);
+  *grid = dim3((unsigned)nx, (unsigned)ys);
+}
+
+}  // namespace
+
+size_t live_hist_bytes(int D, int bins, int lp, int m, int bins2) {
+  return live_layout(D, bins, lp, m, bins2, live_ntiles(m, bins2)).bytes;
+}
+
+cudaError_t live_hist_setup(LiveHist* h, void* mem, uint32_t N, int D, int bins, int lp, const double* outer,
+                            const double* edges, const uint32_t* params, int m, int bins2, const double* edges2,
+                            const double* coords, const double* logp, int sm_count, cudaStream_t st) {
+  const std::vector<HistTile> tiles = m >= 2 ? hist2_tiles(m, hist2_geom(m, bins2).block) : std::vector<HistTile>();
+  const LiveLayout l = live_layout(D, bins, lp, m, bins2, tiles.size());
+  char* p = static_cast<char*>(mem);
+  *h = LiveHist{};
+  h->N = N;
+  h->D = D;
+  h->bins = bins;
+  h->lp = lp;
+  h->m = m;
+  h->bins2 = bins2;
+  h->mem = mem;
+  h->slots = reinterpret_cast<const double**>(p + l.slots);
+  h->outer = reinterpret_cast<double*>(p + l.outer);
+  h->edges = reinterpret_cast<double*>(p + l.edges);
+  h->hist = reinterpret_cast<unsigned long long*>(p + l.hist);
+  h->bad = reinterpret_cast<unsigned int*>(p + l.bad);
+  h->tiles = reinterpret_cast<HistTile*>(p + l.tiles);
+  h->ntiles = (uint32_t)tiles.size();
+  h->params = reinterpret_cast<uint32_t*>(p + l.params);
+  h->edges2 = reinterpret_cast<double*>(p + l.edges2);
+  h->hist2 = reinterpret_cast<unsigned long long*>(p + l.hist2);
+  const size_t rows = (size_t)D + (size_t)lp, npairs = (size_t)m * (m > 0 ? m - 1 : 0) / 2;
+  const double* table[2] = {coords, logp};
+  HE(cudaMemcpyAsync(h->slots, table, sizeof(table), cudaMemcpyHostToDevice, st));
+  HE(cudaMemcpyAsync(h->outer, outer, rows * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  HE(cudaMemcpyAsync(h->edges, edges, rows * (bins + 1) * sizeof(double), cudaMemcpyHostToDevice, st));
+  HE(cudaMemsetAsync(h->hist, 0, rows * bins * sizeof(uint64_t), st));
+  HE(cudaMemsetAsync(h->bad, 0, sizeof(uint32_t), st));
+  live_hist1_geom(N, D, bins, sm_count, &h->W1, &h->smem1, &h->grid1, &h->rows1);
+  live_hist1_geom(N, 1, bins, sm_count, &h->Wlp, &h->smemlp, &h->gridlp, &h->rowslp);
+  if (m >= 2) {
+    HE(cudaMemcpyAsync(h->tiles, tiles.data(), tiles.size() * sizeof(HistTile), cudaMemcpyHostToDevice, st));
+    HE(cudaMemcpyAsync(h->params, params, (size_t)m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    HE(cudaMemcpyAsync(h->edges2, edges2, (size_t)m * (bins2 + 1) * sizeof(double), cudaMemcpyHostToDevice, st));
+    HE(cudaMemsetAsync(h->hist2, 0, npairs * bins2 * bins2 * sizeof(uint64_t), st));
+    h->smem2 = hist2_geom(m, bins2).smem;
+    uint64_t ys = 1;
+    split_rows(N, tiles.size(), (uint64_t)sm_count * 2, (uint64_t)HIST2_ROWS * 4, &ys, &h->rows2);
+    h->grid2 = dim3((unsigned)tiles.size(), (unsigned)ys);
+  }
+  return cudaStreamSynchronize(st);
+}
+
+cudaError_t live_hist_launch(const LiveHist& h, cudaStream_t st, uint64_t& launches) {
+  // the attribute is set at every launch: eb_chain_histogram sets the same kernels' limits to its own sizes
+  HE(cudaFuncSetAttribute(hist1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                          (int)std::max(h.smem1, h.lp ? h.smemlp : 0)));
+  hist1_kernel<<<h.grid1, HIST_THREADS, h.smem1, st>>>(h.slots, h.N, h.D, h.N, h.rows1, h.W1, h.bins, h.outer,
+                                                       h.edges, h.hist, h.bad);
+  HE(cudaGetLastError());
+  ++launches;
+  if (h.lp) {  // the log-probabilities: row D of the tables, one column of stride 1
+    hist1_kernel<<<h.gridlp, HIST_THREADS, h.smemlp, st>>>(h.slots + 1, h.N, 1, h.N, h.rowslp, h.Wlp, h.bins,
+                                                           h.outer + 3 * (size_t)h.D,
+                                                           h.edges + (size_t)h.D * (h.bins + 1),
+                                                           h.hist + (size_t)h.D * h.bins, h.bad);
+    HE(cudaGetLastError());
+    ++launches;
+  }
+  if (h.m >= 2) {
+    HE(cudaFuncSetAttribute(hist2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h.smem2));
+    hist2_kernel<<<h.grid2, HIST2_THREADS, h.smem2, st>>>(h.slots, h.N, h.D, h.N, h.rows2, h.tiles, h.params,
+                                                          (uint32_t)h.m, h.bins2, h.edges2, h.hist2);
+    HE(cudaGetLastError());
+    ++launches;
+  }
+  return cudaSuccess;
+}
+
+cudaError_t live_hist_read(const LiveHist& h, uint64_t* hist, uint64_t* hist2, bool* bad, cudaStream_t st) {
+  const size_t rows = (size_t)h.D + (size_t)h.lp, npairs = (size_t)h.m * (h.m > 0 ? h.m - 1 : 0) / 2;
+  uint32_t hb = 0;
+  if (hist) HE(cudaMemcpyAsync(hist, h.hist, rows * h.bins * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if (hist2 && h.m >= 2)
+    HE(cudaMemcpyAsync(hist2, h.hist2, npairs * h.bins2 * h.bins2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  HE(cudaMemcpyAsync(&hb, h.bad, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  HE(cudaStreamSynchronize(st));
+  *bad = hb != 0;
+  return cudaSuccess;
+}
+#undef HE
 
 }  // namespace eb

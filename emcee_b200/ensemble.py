@@ -11,6 +11,7 @@ through pinned buffers.  ``pool`` / ``args`` / ``kwargs`` / ``vectorize``
 and ``blobs_dtype`` belong to ``models.HostFunction`` / ``models.CudaArrayFunction``;
 named parameters raise ``NotImplementedError``."""
 
+import operator
 from collections.abc import Iterable
 
 import numpy as np
@@ -32,6 +33,8 @@ _NO_SHARDED_DEVICE_CHAIN = (
     "of the other ranks' rows before each stored step is built for host chains only; use Backend()"
 )
 _NO_DEVICE_CHAIN_BLOBS = "a DeviceBackend does not store blobs; use Backend() with a function that returns blobs"
+_NO_SHARDED_HISTOGRAMS = "running histograms are counted on one GPU; they cannot be combined with a sharded ensemble"
+_NO_HISTOGRAMS = "running histograms are not enabled: call enable_histograms(range, ...) first"
 
 
 def _seed_from_numpy():
@@ -141,6 +144,7 @@ class EnsembleSampler(object):
         if pinned_results:
             self._pinned = (_lib.pinned_empty((self.nwalkers, self.ndim)), _lib.pinned_empty((self.nwalkers,)))
         self._rdv = None  # multi-GPU: the host rendezvous this sampler is attached to (``attach``)
+        self._hist = None  # running histograms: the configuration of enable_histograms (edges, pairs)
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
@@ -230,6 +234,7 @@ class EnsembleSampler(object):
         for k in ("_engine", "_random", "_pinned"):
             d.pop(k, None)
         d["_rdv"] = None  # a communicator does not survive pickling: re-attach after loading
+        d["_hist"] = None  # the running histograms live in the engine's memory: enable them again after loading
         d["pool"] = None
         return d
 
@@ -260,6 +265,8 @@ class EnsembleSampler(object):
 
         if isinstance(self.backend, DeviceBackend):
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
+        if getattr(self, "_hist", None) is not None:
+            raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
@@ -291,6 +298,66 @@ class EnsembleSampler(object):
         parts = [part] if self._rdv is None else self._rdv.allgather(part)
         mean, cov, n, _ = dist.combine_moments(parts)
         return mean, cov, n
+
+    def enable_histograms(self, range, bins=10, every=1, log_prob_range=None, params2d=None, bins2d=10):
+        """Count every walker's coordinates into fixed bins on the device after every ``every``-th step (the
+        cadence of :meth:`enable_moments`), for runs that store nothing.  :meth:`histogram` and
+        :meth:`histogram2d` then return what ``get_histogram(bins, range, thin=every)`` and
+        ``get_histogram2d(params2d, bins2d, range, thin=every)`` of a run that stored those steps return, when the
+        step counter (``random_state[2]``) is a multiple of ``every`` at this call.
+
+        ``range`` gives one ``(lo, hi)`` pair per parameter: the edges are fixed before any value is seen.
+        ``log_prob_range`` (a pair) adds a histogram of the log-probabilities with ``bins`` bins; ``params2d``
+        (distinct parameter numbers, at least two) adds ``np.histogram2d`` counts of every pair of them with
+        ``bins2d`` bins per axis.  ``bins <= 4096`` and ``bins2d <= 128`` (``NotImplementedError`` beyond); a bad
+        ``bins`` or range raises numpy's exception.  Every call zeroes the counts; ``every=0`` counts nothing.
+        The counts are not pickled, and a sharded ensemble is refused."""
+        from .summary import running_histogram_plan
+
+        if self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
+        every = operator.index(every)
+        if every < 0:
+            raise ValueError("every must be >= 0, got {0}".format(every))
+        cfg = running_histogram_plan(self.ndim, range, bins, log_prob_range, params2d, bins2d)
+        self._hist = None
+        self._engine.histograms_config(every, cfg["bins"], cfg["outer"], cfg["edges"], cfg["log_prob"],
+                                       cfg["params2d"], cfg["bins2d"], cfg["edges2d"])
+        self._hist = cfg
+
+    def _histogram_counts(self, counts=True):
+        if getattr(self, "_hist", None) is None:
+            raise RuntimeError(_NO_HISTOGRAMS)
+        return self._engine.histograms(counts)
+
+    def histogram(self, name="chain"):
+        """``(hist, edges)`` of the running histograms (:meth:`enable_histograms`), as ``get_histogram`` returns
+        them: ``hist[ndim, bins]`` (int64) and ``edges[ndim, bins + 1]`` for ``name="chain"``, ``hist[bins]`` and
+        ``edges[bins + 1]`` for ``"log_prob"``."""
+        if name not in ("chain", "log_prob"):
+            raise ValueError("histograms are taken of 'chain' or 'log_prob', not {0!r}".format(name))
+        hist, _, _ = self._histogram_counts()
+        cfg = self._hist
+        if name == "log_prob":
+            if not cfg["log_prob"]:
+                raise RuntimeError("no running histogram of the log-probabilities: pass log_prob_range to "
+                                   "enable_histograms")
+            return hist[self.ndim].astype(np.int64), cfg["edges"][self.ndim].copy()
+        return hist[: self.ndim].astype(np.int64), cfg["edges"][: self.ndim].copy()
+
+    def histogram2d(self):
+        """``(hist[npairs, bins2d, bins2d], edges[len(params2d), bins2d + 1], pairs)`` of the running pair
+        histograms (:meth:`enable_histograms` with ``params2d``), as ``get_histogram2d`` returns them."""
+        _, hist2, _ = self._histogram_counts()
+        cfg = self._hist
+        if cfg["params2d"] is None:
+            raise RuntimeError("no running pair histograms: pass params2d to enable_histograms")
+        return hist2.astype(np.float64), cfg["edges2d"].copy(), list(cfg["pairs"])
+
+    @property
+    def histogram_count(self):
+        """Samples counted per parameter by the running histograms: counted steps times ``nwalkers``."""
+        return self._histogram_counts(counts=False)[2]
 
     # ------------------------------------------------------------- the driver
     def _schedule(self):

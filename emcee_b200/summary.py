@@ -13,6 +13,7 @@ only through them (``_get_outer_edges``, ``np.linspace``, the finite-bins check)
 on the two-row array ``[min; max]`` return the edges, and raise the exceptions, that they would on the whole
 column.  ``DeviceBackend.get_histogram`` / ``get_histogram2d`` then count on the GPU with these edges."""
 
+import itertools
 import operator
 
 import numpy as np
@@ -23,7 +24,7 @@ except ImportError:  # numpy < 2
     from numpy.lib.histograms import _get_outer_edges, _unsigned_subtract
 
 __all__ = ["percentile_ranks", "percentile_finish", "histogram_bins", "uniform_edges", "searched_edges",
-           "HIST_BINS_MAX", "HIST2_BINS_MAX"]
+           "running_histogram_plan", "HIST_BINS_MAX", "HIST2_BINS_MAX"]
 
 HIST_BINS_MAX = 4096  # eb_chain_histogram (hist_bins.h)
 HIST2_BINS_MAX = 128  # eb_chain_histogram2d: a 64 KiB uint32 pair histogram in shared memory
@@ -163,3 +164,35 @@ def searched_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
     if not np.all(np.isfinite(edges)):
         raise ValueError("histogram edges over [{0}, {1}] are not finite".format(edges[0], edges[-1]))
     return np.asarray(edges, dtype=np.float64)
+
+
+def running_histogram_plan(ndim, range, bins=10, log_prob_range=None, params2d=None, bins2d=10):
+    """The configuration of ``EnsembleSampler.enable_histograms``, formed on the host before anything is counted:
+    ``bins``, ``outer[rows, 3]`` / ``edges[rows, bins + 1]`` (``uniform_edges`` of each parameter's range and,
+    with ``log_prob_range``, a last row for the log-probabilities), and with ``params2d`` the pair list and
+    ``edges2d[len(params2d), bins2d + 1]`` (``searched_edges``).  A streaming count cannot see the data before it
+    bins it, so every parameter needs a range (``ValueError``); otherwise numpy's exceptions, the device limits and
+    ``params2d``'s checks are those of ``get_histogram`` / ``get_histogram2d``."""
+    from .backend import _histogram_params
+
+    if range is None or any(r is None for r in range):
+        raise ValueError("running histograms need a (lo, hi) range for every parameter: the edges are fixed "
+                         "before the first value is counted, so they cannot be taken from the data")
+    ranges = list(range)
+    if len(ranges) != ndim:
+        raise ValueError("range must hold one (lo, hi) pair per parameter: {0} for ndim = {1}".format(
+            len(ranges), ndim))
+    n = histogram_bins(bins, HIST_BINS_MAX)
+    rows = ranges + ([] if log_prob_range is None else [log_prob_range])
+    outer = np.empty((len(rows), 3))
+    edges = np.empty((len(rows), n + 1))
+    for d, r in enumerate(rows):
+        outer[d], edges[d] = uniform_edges(n, r)
+    cfg = dict(bins=n, outer=outer, edges=edges, log_prob=log_prob_range is not None, params2d=None, bins2d=0,
+               edges2d=None, pairs=None)
+    if params2d is not None:
+        params2d = _histogram_params(params2d, ndim)
+        n2 = histogram_bins(bins2d, HIST2_BINS_MAX, two_d=True)
+        edges2d = np.array([searched_edges(n2, ranges[p]) for p in params2d], dtype=np.float64)
+        cfg.update(params2d=params2d, bins2d=n2, edges2d=edges2d, pairs=list(itertools.combinations(params2d, 2)))
+    return cfg

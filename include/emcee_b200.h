@@ -399,6 +399,32 @@ int eb_reset_counters(eb_ctx* ctx);
  * of accepted proposals of the owned walkers; any output may be NULL.  On a
  * sharded ensemble the values are per rank (the host combines them). */
 int eb_moments(eb_ctx* ctx, double* mean, double* cov, uint64_t* count, uint64_t* naccepted_total);
+/* Running histograms of the chain for store=False runs: eb_chain_histogram /
+ * eb_chain_histogram2d of the steps a store with thin_by = every would keep,
+ * without storing them.  After every step whose counter is a multiple of
+ * `every` (the cadence of "moments_every"), each walker's coordinates are
+ * counted into device counts by kernels behind the step on the engine's stream
+ * (no synchronisation or copy per count); every == 0 counts nothing.
+ * 1-D: outer[(ndim + log_prob) * 3] and edges[(ndim + log_prob) * (bins + 1)]
+ * as eb_chain_histogram takes them, one row per parameter and, when log_prob is
+ * non-zero, a last row for the log-probabilities; 1 <= bins <= 4096.  2-D
+ * (nparams2d == 0: none): the 2 <= nparams2d <= ndim distinct params2d[] with
+ * edges2d[nparams2d * (bins2d + 1)], as eb_chain_histogram2d takes them;
+ * 1 <= bins2d <= 128.  Each call replaces the configuration and zeroes the
+ * counts.  The tables are uploaded and the uint64 counts allocated here, checked
+ * against the free memory first (EB_ERR_NOMEM); the 2-D counts take
+ * nparams2d (nparams2d - 1) / 2 * bins2d^2 * 8 bytes.  Sharded engines are
+ * refused with EB_ERR_UNSUPPORTED, both ways round (eb_comm_init). */
+int eb_histograms_config(eb_ctx* ctx, uint64_t every, uint32_t bins, const double* outer, const double* edges,
+                         int log_prob, const uint32_t* params2d, size_t nparams2d, uint32_t bins2d,
+                         const double* edges2d);
+/* the counts since eb_histograms_config: hist[(ndim + log_prob) * bins] and
+ * hist2d[npairs * bins2d^2] in eb_chain_histogram / eb_chain_histogram2d's
+ * layout (either may be NULL), and the number of samples counted per parameter
+ * (*count: counted steps * nwalkers).  EB_ERR_STATE before any configuration; a
+ * value whose truncated index is above bins (see eb_chain_histogram) gives
+ * EB_ERR_INVALID, with the counts written. */
+int eb_histograms(eb_ctx* ctx, uint64_t* hist, uint64_t* hist2d, uint64_t* count);
 /* walkers_independent (ensemble.py:653-663) on the device: gram[ndim*ndim] =
  * C^T C of the centred, column-normalised coords[rows, ndim] (:656-661), whose
  * extreme eigenvalues give cond(C)^2.  *flags: bit 0 = non-finite coordinate
