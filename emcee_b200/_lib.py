@@ -145,6 +145,10 @@ _SIGNATURES = {
         [C.c_void_p, C.c_uint64, C.c_uint32, _dp, _dp, C.c_int, C.POINTER(C.c_uint32), C.c_size_t, C.c_uint32, _dp],
     ),
     "eb_histograms": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_trace_config": (C.c_int, [C.c_void_p, C.c_uint64]),
+    "eb_trace_count": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
+    "eb_trace_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), _dp]),
+    "eb_trace_best": (C.c_int, [C.c_void_p, _dp, _dp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "eb_walkers_gram": (C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp, C.POINTER(C.c_int)]),
     "eb_autocorr": (C.c_int, [C.c_void_p, _dp, C.c_size_t, C.c_size_t, C.c_size_t, _dp]),
     "eb_last_step_timing": (C.c_int, [C.c_void_p, _dp, C.POINTER(C.c_uint64)]),
@@ -865,6 +869,32 @@ class Engine(object):
             self._h, None if hist is None else hist.ctypes.data_as(C.POINTER(C.c_uint64)),
             None if hist2 is None else hist2.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(n)))
         return hist, hist2, int(n.value)
+
+    def trace_config(self, every):
+        """Record one row of ensemble statistics after every ``every``-th step (``eb_trace_config``)."""
+        self._check(lib().eb_trace_config(self._h, int(every)))
+
+    def trace_count(self):
+        n = C.c_uint64()
+        self._check(lib().eb_trace_count(self._h, C.byref(n)))
+        return int(n.value)
+
+    def trace_read(self, first=0):
+        """``(step[n] uint64, rows[n, 2 ndim + 4])`` of the recorded rows from ``first`` on (``eb_trace_read``)."""
+        n = max(self.trace_count() - int(first), 0)
+        step = np.zeros(n, dtype=np.uint64)
+        rows = np.zeros((n, 2 * self.ndim + 4), dtype=np.float64)
+        if n:
+            self._check(lib().eb_trace_read(self._h, int(first), n, step.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            _as_dp(rows)))
+        return step, rows
+
+    def trace_best(self):
+        """``(coords[ndim], log_prob, step, walker)`` of ``eb_trace_best``."""
+        coords = np.zeros(self.ndim, dtype=np.float64)
+        lp, step, walker = C.c_double(), C.c_uint64(), C.c_uint64()
+        self._check(lib().eb_trace_best(self._h, _as_dp(coords), C.byref(lp), C.byref(step), C.byref(walker)))
+        return coords, float(lp.value), int(step.value), int(walker.value)
 
     def walkers_gram(self, coords):
         """``(gram[D, D], flags)`` of ``eb_walkers_gram`` for ``coords[rows, D]``."""

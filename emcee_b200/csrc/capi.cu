@@ -14,6 +14,7 @@
 #include "comm.h"
 #include "engine.cuh"
 #include "hist_bins.h"
+#include "trace_sum.h"
 
 using namespace eb;
 
@@ -129,6 +130,14 @@ struct eb_ctx {
   bool hist_on = false;  // configured: hist holds tables and counts
   LiveHist hist;
   unsigned long long hist_count = 0;  // samples counted
+
+  // running trace (eb_trace_read): one row [2 D + 4] of ensemble statistics per `trace_every`-th step
+  uint64_t trace_every = 0;
+  bool trace_on = false;  // configured: trace holds its fixed part
+  LiveTrace trace;
+  double* trace_rows = nullptr;       // [trace_cap, 2 D + 4], device
+  uint64_t trace_cap = 0;
+  std::vector<uint64_t> trace_steps;  // the step counter of each recorded row
 
   // WalkMove / GaussianMove scratch (moves_extra.cu)
   double* qbuf = nullptr;       // [N, D] proposals
@@ -365,6 +374,8 @@ int eb_destroy(eb_ctx* c) {
   cudaFree(c->mom_shift);
   cudaFree(c->mom_partial);
   cudaFree(c->hist.mem);
+  cudaFree(c->trace.mem);
+  cudaFree(c->trace_rows);
   for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
   cudaFree(c->timeline);
   cudaFree(c->tap_partners);
@@ -1625,6 +1636,8 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
 // sync_every-th step), so that steps in between can share one persistent launch.
 int accumulate_moments(eb_ctx* c, uint64_t& launches);  // below
 int accumulate_histograms(eb_ctx* c, uint64_t& launches);  // below
+int reserve_trace(eb_ctx* c, uint64_t nsteps);             // below
+int accumulate_trace(eb_ctx* c, uint64_t& launches);       // below
 
 template <class F>
 int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every, F&& after_step) {
@@ -1638,6 +1651,10 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
       CK(c, cudaEventCreate(&e));
       c->ev_pool.push_back(e);
     }
+  }
+  if (c->trace_every > 0) {
+    const int rc = reserve_trace(c, nsteps);
+    if (rc) return rc;
   }
   c->chain_ok = false;
   c->dmma_nhalf_max = 0;
@@ -1762,7 +1779,9 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         }
         const bool moments_now = c->moments_every > 0 && (c->step + 1) % c->moments_every == 0;
         const bool hist_now = c->hist_every > 0 && (c->step + 1) % c->hist_every == 0;
-        const bool host_event = perstep || moments_now || hist_now || (sync_every > 0 && (done + k + 1) % sync_every == 0);
+        const bool trace_now = c->trace_every > 0 && (c->step + 1) % c->trace_every == 0;
+        const bool host_event =
+            perstep || moments_now || hist_now || trace_now || (sync_every > 0 && (done + k + 1) % sync_every == 0);
         if (host_event || k + 1 == chunk || grp.nhalf >= c->dmma_group) {
           rc = flush_dmma(c, mv, grp, launches);
           if (rc) return rc;
@@ -1792,6 +1811,10 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
       }
       if (c->hist_every > 0 && c->step % c->hist_every == 0) {
         rc = accumulate_histograms(c, launches);
+        if (rc) return rc;
+      }
+      if (c->trace_every > 0 && c->step % c->trace_every == 0) {
+        rc = accumulate_trace(c, launches);
         if (rc) return rc;
       }
       if (perstep) {
@@ -1867,6 +1890,45 @@ int accumulate_histograms(eb_ctx* c, uint64_t& launches) {
   c->chain_ok = false;
   CK(c, live_hist_launch(c->hist, c->st, launches));
   c->hist_count += (unsigned long long)c->N;
+  return EB_OK;
+}
+
+// Room for the rows the next `nsteps` steps record, made before the first launch: the rows already recorded move
+// into a larger allocation (half as large again when that fits, so that a run of many short calls grows a few times).
+int reserve_trace(eb_ctx* c, uint64_t nsteps) {
+  const uint64_t add = (c->step + nsteps) / c->trace_every - c->step / c->trace_every;
+  const uint64_t have = c->trace_steps.size(), need = have + add;
+  if (need <= c->trace_cap) return EB_OK;
+  const size_t row = (2 * (size_t)c->D + TRACE_EXTRA) * sizeof(double);
+  size_t free_b = 0, total_b = 0;
+  CK(c, cudaMemGetInfo(&free_b, &total_b));
+  uint64_t cap = std::max(need, c->trace_cap + c->trace_cap / 2);
+  if (cap > free_b / row) cap = need;
+  if (cap > free_b / row)
+    FAIL(c, EB_ERR_NOMEM, "the trace needs room for %llu rows of %zu bytes, %zu bytes free", (unsigned long long)need,
+         row, free_b);
+  double* rows = nullptr;
+  const cudaError_t e = cudaMalloc(&rows, (size_t)cap * row);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    FAIL(c, EB_ERR_NOMEM, "the trace: allocating %llu rows of %zu bytes failed (%s)", (unsigned long long)cap, row,
+         cudaGetErrorString(e));
+  }
+  if (have) CK(c, cudaMemcpyAsync(rows, c->trace_rows, (size_t)have * row, cudaMemcpyDeviceToDevice, c->st));
+  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaFree(c->trace_rows));
+  c->trace_rows = rows;
+  c->trace_cap = cap;
+  c->trace_steps.reserve((size_t)cap);
+  return EB_OK;
+}
+
+// record the CURRENT state as one row of the trace (kernels only, enqueued on the stream)
+int accumulate_trace(eb_ctx* c, uint64_t& launches) {
+  c->chain_ok = false;
+  double* row = c->trace_rows + c->trace_steps.size() * (2 * (size_t)c->D + TRACE_EXTRA);
+  CK(c, live_trace_launch(c->trace, row, c->step, c->st, launches));
+  c->trace_steps.push_back(c->step);
   return EB_OK;
 }
 
@@ -2608,6 +2670,85 @@ int eb_histograms(eb_ctx* c, uint64_t* hist, uint64_t* hist2d, uint64_t* count) 
   return EB_OK;
 }
 
+int eb_trace_config(eb_ctx* c, uint64_t every) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st));
+  if (every > 0 || !c->trace_on) {  // every == 0 after a configuration keeps what was recorded readable
+    CK(c, cudaFree(c->trace_rows));
+    c->trace_rows = nullptr;
+    c->trace_cap = 0;
+    c->trace_steps.clear();
+    if (!c->trace_on) {
+      const size_t bytes = live_trace_fixed_bytes((uint32_t)c->N, c->D);
+      size_t free_b = 0, total_b = 0;
+      CK(c, cudaMemGetInfo(&free_b, &total_b));
+      if (bytes > free_b) FAIL(c, EB_ERR_NOMEM, "eb_trace_config: %zu bytes of partial sums, %zu bytes free", bytes, free_b);
+      void* mem = nullptr;
+      const cudaError_t e = cudaMalloc(&mem, bytes);
+      if (e != cudaSuccess) {
+        cudaGetLastError();
+        FAIL(c, EB_ERR_NOMEM, "eb_trace_config: allocating %zu bytes failed (%s)", bytes, cudaGetErrorString(e));
+      }
+      c->trace.mem = mem;
+    }
+    const cudaError_t s =
+        live_trace_setup(&c->trace, c->trace.mem, (uint32_t)c->N, c->D, c->coords, c->logp, c->accepted, c->st);
+    if (s != cudaSuccess) {
+      cudaGetLastError();
+      FAIL(c, EB_ERR_CUDA, "eb_trace_config: %s", cudaGetErrorString(s));
+    }
+    c->trace_on = true;
+  }
+  c->trace_every = every;
+  return EB_OK;
+}
+
+int eb_trace_count(eb_ctx* c, uint64_t* rows) {
+  if (!c || !rows) return EB_ERR_INVALID;
+  if (!c->trace_on) FAIL(c, EB_ERR_STATE, "eb_trace_count: configure the trace with eb_trace_config first");
+  *rows = c->trace_steps.size();
+  return EB_OK;
+}
+
+int eb_trace_read(eb_ctx* c, uint64_t first, uint64_t count, uint64_t* step, double* rows_out) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->trace_on) FAIL(c, EB_ERR_STATE, "eb_trace_read: configure the trace with eb_trace_config first");
+  const uint64_t have = c->trace_steps.size();
+  if (first > have || count > have - first)
+    FAIL(c, EB_ERR_INVALID, "eb_trace_read: rows %llu .. %llu + %llu of %llu recorded", (unsigned long long)first,
+         (unsigned long long)first, (unsigned long long)count, (unsigned long long)have);
+  if (count == 0) return EB_OK;
+  if (step) std::copy(c->trace_steps.begin() + first, c->trace_steps.begin() + first + count, step);
+  if (rows_out) {
+    const size_t W = 2 * (size_t)c->D + TRACE_EXTRA;
+    CK(c, cudaSetDevice(c->device));
+    CK(c, cudaMemcpyAsync(rows_out, c->trace_rows + first * W, (size_t)count * W * sizeof(double),
+                          cudaMemcpyDeviceToHost, c->st));
+    CK(c, cudaStreamSynchronize(c->st));
+    c->chain_ok = false;
+  }
+  return EB_OK;
+}
+
+int eb_trace_best(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, uint64_t* walker) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->trace_on) FAIL(c, EB_ERR_STATE, "eb_trace_best: configure the trace with eb_trace_config first");
+  if (c->trace_steps.empty()) FAIL(c, EB_ERR_STATE, "eb_trace_best: no step has been recorded yet");
+  CK(c, cudaSetDevice(c->device));
+  TraceBest b;
+  CK(c, live_trace_best(c->trace, &b, coords, c->st));
+  c->chain_ok = false;
+  if (log_prob) *log_prob = b.log_prob;
+  if (step) *step = b.step;
+  if (walker) *walker = b.walker;
+  return EB_OK;
+}
+
 int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, int* flags) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -2815,6 +2956,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
   if (c->have_model && c->model.kind == MODEL_EXTERNAL && nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
   if (c->hist_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
+  if (c->trace_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path

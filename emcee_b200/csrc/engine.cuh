@@ -271,6 +271,33 @@ cudaError_t live_hist_launch(const LiveHist& h, cudaStream_t st, uint64_t& launc
 // hist[(D + lp) * bins], hist2 (nullable) to the host; *bad: some value fell past numpy's edge array
 cudaError_t live_hist_read(const LiveHist& h, uint64_t* hist, uint64_t* hist2, bool* bad, cudaStream_t st);
 
+// ---- running trace of the live state (trace.cu, eb_trace_config / eb_trace_read / eb_trace_best) -----------------
+struct TraceBest {
+  double log_prob;
+  unsigned long long step, walker;
+  unsigned long long have;  // 0 until a step has been recorded
+};
+// the fixed part of a trace inside `mem` (live_trace_fixed_bytes of it); the rows are the engine's to grow
+struct LiveTrace {
+  uint32_t N = 0;
+  int D = 0;
+  const double* coords = nullptr;
+  const double* logp = nullptr;
+  const uint8_t* accepted = nullptr;
+  void* mem = nullptr;
+  double* partial = nullptr;      // [trace_nchunks(N), 2 D + 4] chunk sums, folded in place
+  TraceBest* best = nullptr;
+  double* best_coords = nullptr;  // [D]
+};
+size_t live_trace_fixed_bytes(uint32_t N, int D);
+// lays the pointers out, clears the best sample and synchronises
+cudaError_t live_trace_setup(LiveTrace* t, void* mem, uint32_t N, int D, const double* coords, const double* logp,
+                             const uint8_t* accepted, cudaStream_t st);
+// row[2 D + 4] (device) = the statistics of the current state, recorded as `step`: two kernels on `st`
+cudaError_t live_trace_launch(const LiveTrace& t, double* row, uint64_t step, cudaStream_t st, uint64_t& launches);
+// the best sample so far to the host (coords nullable); synchronises
+cudaError_t live_trace_best(const LiveTrace& t, TraceBest* best, double* coords, cudaStream_t st);
+
 inline int lanes_per_walker(int D) {
   int g = 4;
   while (g < 32 && g * 4 < D) g <<= 1;

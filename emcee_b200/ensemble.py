@@ -12,6 +12,7 @@ and ``blobs_dtype`` belong to ``models.HostFunction`` / ``models.CudaArrayFuncti
 named parameters raise ``NotImplementedError``."""
 
 import operator
+from collections import namedtuple
 from collections.abc import Iterable
 
 import numpy as np
@@ -35,6 +36,11 @@ _NO_SHARDED_DEVICE_CHAIN = (
 _NO_DEVICE_CHAIN_BLOBS = "a DeviceBackend does not store blobs; use Backend() with a function that returns blobs"
 _NO_SHARDED_HISTOGRAMS = "running histograms are counted on one GPU; they cannot be combined with a sharded ensemble"
 _NO_HISTOGRAMS = "running histograms are not enabled: call enable_histograms(range, ...) first"
+_NO_SHARDED_TRACE = "the running trace is recorded on one GPU; it cannot be combined with a sharded ensemble"
+_NO_TRACE = "the running trace is not enabled: call enable_trace() first"
+
+#: what :meth:`EnsembleSampler.trace` returns: one entry per recorded step
+Trace = namedtuple("Trace", ["step", "mean", "var", "log_prob_mean", "log_prob_max", "accepted"])
 
 
 def _seed_from_numpy():
@@ -145,6 +151,7 @@ class EnsembleSampler(object):
             self._pinned = (_lib.pinned_empty((self.nwalkers, self.ndim)), _lib.pinned_empty((self.nwalkers,)))
         self._rdv = None  # multi-GPU: the host rendezvous this sampler is attached to (``attach``)
         self._hist = None  # running histograms: the configuration of enable_histograms (edges, pairs)
+        self._trace_every = None  # running trace: the cadence its rows were recorded with (enable_trace)
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
@@ -235,6 +242,7 @@ class EnsembleSampler(object):
             d.pop(k, None)
         d["_rdv"] = None  # a communicator does not survive pickling: re-attach after loading
         d["_hist"] = None  # the running histograms live in the engine's memory: enable them again after loading
+        d["_trace_every"] = None  # and so do the rows of the running trace
         d["pool"] = None
         return d
 
@@ -267,6 +275,8 @@ class EnsembleSampler(object):
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
         if getattr(self, "_hist", None) is not None:
             raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
+        if getattr(self, "_trace_every", None) is not None:
+            raise NotImplementedError(_NO_SHARDED_TRACE)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
@@ -358,6 +368,63 @@ class EnsembleSampler(object):
     def histogram_count(self):
         """Samples counted per parameter by the running histograms: counted steps times ``nwalkers``."""
         return self._histogram_counts(counts=False)[2]
+
+    def enable_trace(self, every=1):
+        """Record one row of ensemble statistics on the device after every ``every``-th step (the cadence of
+        :meth:`enable_histograms`), for runs that store nothing: each parameter's mean and variance over the
+        walkers, the mean and maximum log-probability and the number of accepted proposals of that step
+        (:meth:`trace`), and the best sample of all recorded steps (:meth:`best_sample`).  A row is about
+        ``16 * ndim`` bytes where a stored step is ``8 * nwalkers * ndim``.
+
+        Every call with ``every > 0`` drops the rows and the best sample recorded so far; ``every=0`` records nothing
+        more and leaves them readable.  The initial state is never recorded.  The rows are not pickled, and a
+        sharded ensemble is refused."""
+        if self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_TRACE)
+        every = operator.index(every)
+        if every < 0:
+            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._engine.trace_config(every)
+        if every > 0 or self._trace_every is None:
+            self._trace_every = every
+
+    def _trace_on(self):
+        if getattr(self, "_trace_every", None) is None:
+            raise RuntimeError(_NO_TRACE)
+
+    def trace(self, discard=0):
+        """The rows recorded since :meth:`enable_trace`, from row ``discard`` on, as a :data:`Trace` of ``n`` rows:
+        ``step[n]`` (uint64, the step counter), ``mean[n, ndim]`` and ``var[n, ndim]`` (``np.mean(x, axis=0)`` and
+        ``np.var(x, axis=0, ddof=1)`` of that step's ensemble), ``log_prob_mean[n]``, ``log_prob_max[n]`` and
+        ``accepted[n]`` (int64: the walkers that accepted their proposal in that step).  The sums are taken in a
+        fixed order that depends on ``nwalkers`` alone, so the same steps give the same bytes however they were
+        run."""
+        self._trace_on()
+        discard = operator.index(discard)
+        if discard < 0:
+            raise ValueError("discard must be >= 0, got {0}".format(discard))
+        step, rows = self._engine.trace_read(discard)
+        D = self.ndim
+        return Trace(step, rows[:, :D].copy(), rows[:, D:2 * D].copy(), rows[:, 2 * D].copy(),
+                     rows[:, 2 * D + 1].copy(), rows[:, 2 * D + 2].astype(np.int64))
+
+    def best_sample(self):
+        """``(coords[ndim], log_prob, step, walker)`` of the largest log-probability among the steps the running
+        trace recorded (:meth:`enable_trace`); ties go to the earliest step, then the lowest walker, as
+        ``np.argmax(get_log_prob(thin=every, flat=True))`` of a run that stored those steps picks."""
+        self._trace_on()
+        if self._engine.trace_count() == 0:
+            raise RuntimeError("the running trace has recorded no step yet")
+        return self._engine.trace_best()
+
+    def trace_autocorr_time(self, discard=0, **kwargs):
+        """Integrated autocorrelation time, in steps, of each parameter's ensemble mean (Goodman & Weare 2010):
+        ``every * autocorr.integrated_time(trace(discard).mean[:, None, :], **kwargs)`` with ``c``, ``tol`` and
+        ``quiet`` as there, and its :class:`~emcee_b200.autocorr.AutocorrError` / warning for a short series."""
+        from . import autocorr
+
+        mean = self.trace(discard).mean
+        return self._trace_every * autocorr.integrated_time(mean[:, None, :], **kwargs)
 
     # ------------------------------------------------------------- the driver
     def _schedule(self):

@@ -425,6 +425,39 @@ int eb_histograms_config(eb_ctx* ctx, uint64_t every, uint32_t bins, const doubl
  * value whose truncated index is above bins (see eb_chain_histogram) gives
  * EB_ERR_INVALID, with the counts written. */
 int eb_histograms(eb_ctx* ctx, uint64_t* hist, uint64_t* hist2d, uint64_t* count);
+/* Running trace for store=False runs: the time axis that eb_moments and
+ * eb_histograms pool away.  After every step whose counter is a multiple of
+ * `every` (the cadence of eb_histograms_config) one row of 2 ndim + 4 doubles is
+ * recorded in device memory by two kernels behind the step on the engine's
+ * stream: the mean and the ddof = 1 variance of each parameter over the
+ * ensemble, the mean and the maximum of the log-probabilities, the number of
+ * walkers that accepted their proposal in that step, and the lowest walker
+ * holding the maximum.  The sums are taken in a fixed order that depends on
+ * nwalkers alone (csrc/trace_sum.h), so a row does not depend on how the steps
+ * were launched.  The largest log-probability of all recorded steps is kept
+ * with its coordinates (eb_trace_best).  every > 0 drops the rows and the best
+ * sample recorded so far; every == 0 records nothing more and leaves them
+ * readable.  The rows are not allocated here: each stepping call knows how many
+ * it will add and makes room once before its first launch, checked against the
+ * free memory (EB_ERR_NOMEM, with nothing enqueued); recorded rows survive the
+ * growth.  Nothing is allocated, copied to the host, cleared or synchronised per
+ * recorded step.  Sharded engines are refused with EB_ERR_UNSUPPORTED, both ways
+ * round (eb_comm_init). */
+int eb_trace_config(eb_ctx* ctx, uint64_t every);
+/* rows recorded since the last eb_trace_config with every > 0; EB_ERR_STATE
+ * before any configuration (as eb_trace_read and eb_trace_best) */
+int eb_trace_count(eb_ctx* ctx, uint64_t* rows);
+/* rows first .. first + count - 1 in one download: step[count] their step
+ * counters and rows_out[count * (2 ndim + 4)], a row being mean[ndim],
+ * var[ndim], log_prob_mean, log_prob_max, accepted, argmax walker (the last two
+ * whole numbers).  Either output may be NULL; a range past eb_trace_count gives
+ * EB_ERR_INVALID. */
+int eb_trace_read(eb_ctx* ctx, uint64_t first, uint64_t count, uint64_t* step, double* rows_out);
+/* the largest log-probability among the recorded steps: coords[ndim], its
+ * value, the step counter and the walker; ties go to the earliest step, then
+ * the lowest walker.  Any output may be NULL; EB_ERR_STATE while no step has
+ * been recorded. */
+int eb_trace_best(eb_ctx* ctx, double* coords, double* log_prob, uint64_t* step, uint64_t* walker);
 /* walkers_independent (ensemble.py:653-663) on the device: gram[ndim*ndim] =
  * C^T C of the centred, column-normalised coords[rows, ndim] (:656-661), whose
  * extreme eigenvalues give cond(C)^2.  *flags: bit 0 = non-finite coordinate
