@@ -14,14 +14,19 @@
 #include "comm.h"
 #include "engine.cuh"
 #include "hist_bins.h"
+#include "owners.h"
 #include "trace_sum.h"
 
 using namespace eb;
 
+// Every buffer, event and stream of an engine or a chain is held by an owner (owners.h), so deleting the object
+// releases them.  A group of buffers that is tested through one of its members is allocated into local owners and
+// moved in only once the whole group exists: a failed call never leaves half a group behind.
+
 // a stored chain in device memory (eb_chain_*): segments of [n, N, D] coords and [n, N] log-probs, one per grow
 struct ChainSeg {
-  double* x = nullptr;
-  double* lp = nullptr;
+  DevPtr<double> x;
+  DevPtr<double> lp;
 };
 
 struct eb_chain {
@@ -31,11 +36,11 @@ struct eb_chain {
   int D = 0;
   size_t xs = 0, ls = 0;  // slot pitches in doubles: N * D and N rounded up to even (16-byte aligned slots)
   size_t max_pitch = 0;   // cudaMemcpy2D limit; larger strides are copied row by row
-  cudaStream_t st = nullptr;
+  StreamPtr st;           // declared first among the owners: destroyed after the memory
   std::vector<ChainSeg> segs;
   std::vector<uint64_t> start{0};  // segment s holds slots [start[s], start[s + 1])
-  double* accepted = nullptr;      // [N] float64 (backend.py:31)
-  uint8_t* mask = nullptr;         // [N] eb_chain_write's accept mask
+  DevPtr<double> accepted;         // [N] float64 (backend.py:31)
+  DevPtr<uint8_t> mask;            // [N] eb_chain_write's accept mask
   std::string err;
 };
 
@@ -45,57 +50,57 @@ struct eb_ctx {
   int64_t N = 0;
   int D = 0;
   uint64_t seed = 0, step = 0;
-  cudaStream_t st = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  StreamPtr st;  // declared first among the owners: destroyed after the events and the memory
+  EventPtr ev0, ev1;
 
-  double* coords = nullptr;
-  double* logp = nullptr;
-  uint8_t* accepted = nullptr;
-  unsigned long long* nacc = nullptr;
-  int* status_dev = nullptr;
-  int* status_host = nullptr;  // pinned
+  DevPtr<double> coords;  // [N, D], then the peer-memory barrier flags (exported to the peers, comm.h)
+  DevPtr<double> logp;
+  DevPtr<uint8_t> accepted;
+  DevPtr<unsigned long long> nacc;
+  DevPtr<int> status_dev;
+  HostPtr<int> status_host;
 
   ModelDev model{};
-  double* model_params = nullptr;
-  double* model_chol = nullptr;
-  double* model_box = nullptr;  // [lo[D] | hi[D]] of eb_model_set_bounds, or null
+  DevPtr<double> model_params;
+  DevPtr<double> model_chol;
+  DevPtr<double> model_box;  // [lo[D] | hi[D]] of eb_model_set_bounds, or null
   bool have_model = false, have_state = false;
 
-  int32_t* order = nullptr;  // [table_cap, N]
+  DevPtr<int32_t> order;  // [table_cap, N]
   size_t table_cap = 0;
-  StepInfo* info_dev = nullptr;
-  StepInfo* info_host = nullptr;  // pinned
-  HalfDesc* descs_dev = nullptr;  // [table_cap * MAX_SPLITS] half-step descriptors of a chunk (dense_dmma)
-  HalfDesc* descs_host = nullptr;  // pinned
-  unsigned long long* gbar = nullptr;  // grid-barrier counter of the persistent dense_dmma kernel
+  DevPtr<StepInfo> info_dev;
+  HostPtr<StepInfo> info_host;
+  DevPtr<HalfDesc> descs_dev;  // [table_cap * MAX_SPLITS] half-step descriptors of a chunk (dense_dmma)
+  HostPtr<HalfDesc> descs_host;
+  DevPtr<unsigned long long> gbar;  // grid-barrier counter of the persistent dense_dmma kernel
   unsigned long long gbar_count = 0;   // arrivals issued so far
   // split tables already on the device: steps [tbl_step0, tbl_step0 + tbl_n) of key tbl_seed, built with tbl_info
   uint64_t tbl_seed = 0, tbl_step0 = 0;
   size_t tbl_n = 0;
   std::vector<StepInfo> tbl_info;
 
-  double* scratch_x = nullptr;
-  double* scratch_lp = nullptr;
+  DevPtr<double> scratch_x;
+  DevPtr<double> scratch_lp;
   size_t scratch_rows = 0;
 
   // pinned staging for eb_step_store
-  double* stage[2] = {nullptr, nullptr};
-  uint8_t* stage_acc[2] = {nullptr, nullptr};
-  cudaEvent_t stage_ev[2] = {nullptr, nullptr};
+  HostPtr<double> stage[2];
+  HostPtr<uint8_t> stage_acc[2];
+  EventPtr stage_ev[2];
 
   bool debug = false;
-  int64_t* tap_partners = nullptr;
-  double* tap_scalar = nullptr;
-  double* tap_u = nullptr;
-  int64_t* tap_active = nullptr;
+  DevPtr<int64_t> tap_partners;
+  DevPtr<double> tap_scalar;
+  DevPtr<double> tap_u;
+  DevPtr<int64_t> tap_active;
   int64_t tap_count = 0;
-  long long* timeline = nullptr;  // dense_dmma instrumentation buffer (option "dmma_timeline")
+  DevPtr<long long> timeline;  // dense_dmma instrumentation buffer (option "dmma_timeline")
 
   // optional L2 flush between steps (benchmark hygiene): per-step event pairs
   bool l2_flush = false;
-  void* flush_buf = nullptr;
+  DevPtr<void> flush_buf;
   size_t flush_bytes = (size_t)256 << 20;
-  std::vector<cudaEvent_t> ev_pool;
+  std::vector<EventPtr> ev_pool;
 
   double last_ms = 0.0;
   uint64_t last_launches = 0;
@@ -119,9 +124,9 @@ struct eb_ctx {
   // running chain moments (eb_moments): sum of (x - shift) and of its outer product over the owned
   // rows of every `moments_every`-th step
   uint64_t moments_every = 0;
-  double* mom_acc = nullptr;      // [D + D*D] accumulators
-  double* mom_shift = nullptr;    // [D]
-  double* mom_partial = nullptr;  // per-CTA partials of one accumulation
+  DevPtr<double> mom_acc;      // [D + D*D] accumulators
+  DevPtr<double> mom_shift;    // [D]
+  DevPtr<double> mom_partial;  // per-CTA partials of one accumulation
   unsigned long long mom_count = 0;
   bool mom_have_shift = false;
 
@@ -129,20 +134,22 @@ struct eb_ctx {
   uint64_t hist_every = 0;
   bool hist_on = false;  // configured: hist holds tables and counts
   LiveHist hist;
+  DevPtr<void> hist_mem;  // hist.mem
   unsigned long long hist_count = 0;  // samples counted
 
   // running trace (eb_trace_read): one row [2 D + 4] of ensemble statistics per `trace_every`-th step
   uint64_t trace_every = 0;
   bool trace_on = false;  // configured: trace holds its fixed part
   LiveTrace trace;
-  double* trace_rows = nullptr;       // [trace_cap, 2 D + 4], device
+  DevPtr<void> trace_mem;           // trace.mem
+  DevPtr<double> trace_rows;        // [trace_cap, 2 D + 4], device
   uint64_t trace_cap = 0;
   std::vector<uint64_t> trace_steps;  // the step counter of each recorded row
 
   // WalkMove / GaussianMove scratch (moves_extra.cu)
-  double* qbuf = nullptr;       // [N, D] proposals
-  double* walk_work = nullptr;  // [D shift | D + D*D moment sums | D*D cov | D*D L]
-  double* gauss_dev = nullptr;  // per schedule entry: scale / factor L of GaussianMove
+  DevPtr<double> qbuf;       // [N, D] proposals
+  DevPtr<double> walk_work;  // [D shift | D + D*D moment sums | D*D cov | D*D L]
+  DevPtr<double> gauss_dev;  // per schedule entry: scale / factor L of GaussianMove
   size_t gauss_cap = 0;
   std::vector<uint64_t> picks;  // per schedule entry: steps of the last call that ran it
 
@@ -153,27 +160,27 @@ struct eb_ctx {
   void* cb_user = nullptr;
   int cb_where = EB_CALLBACK_HOST;
   bool in_callback = false;        // every other call on the context is refused while fn runs
-  double* cb_x = nullptr;          // host mode: pinned [cb_rows, D] proposals
-  double* cb_lp = nullptr;         // host mode: pinned [cb_rows] results
-  double* cb_xdev = nullptr;       // device mode: [cb_rows, D] copy of the rows, the function's to overwrite
+  HostPtr<double> cb_x;            // host mode: pinned [cb_rows, D] proposals
+  HostPtr<double> cb_lp;           // host mode: pinned [cb_rows] results
+  DevPtr<double> cb_xdev;          // device mode: [cb_rows, D] copy of the rows, the function's to overwrite
   size_t cb_rows = 0;
-  double* ext_f = nullptr;         // device [N] Hastings factors of the propose phase
-  double* ext_lp = nullptr;        // device [N] the callback's log-probabilities
+  DevPtr<double> ext_f;            // device [N] Hastings factors of the propose phase
+  DevPtr<double> ext_lp;           // device [N] the callback's log-probabilities
   int cb_phase = 0;                // CB_STEP / CB_SET_STATE / CB_COMPUTE: what the running callback evaluates
   int64_t cb_m = 0;                // rows of the running callback
 
   // blobs of a callback model (eb_callback_blobs): packed records of blob_bytes bytes, one per walker
   size_t blob_bytes = 0;           // the live layout (0: none)
   bool blobs_live = false;         // blob_live holds the records of the current state
-  uint8_t* blob_live = nullptr;    // device [N, blob_bytes]
-  uint8_t* blob_prop = nullptr;    // device [N, blob_bytes] the records of the running half-step's proposals
-  uint8_t* blob_host = nullptr;    // host mode: pinned [N, blob_bytes] staging of the function's records
+  DevPtr<uint8_t> blob_live;       // device [N, blob_bytes]
+  DevPtr<uint8_t> blob_prop;       // device [N, blob_bytes] the records of the running half-step's proposals
+  HostPtr<uint8_t> blob_host;      // host mode: pinned [N, blob_bytes] staging of the function's records
   size_t blob_cap = 0;             // bytes of each of the three buffers
   int64_t cb_blob_rows = -1;       // records the running callback delivered (-1: none)
   size_t cb_blob_bytes = 0;        // their size
   uint8_t* cb_blob_dst = nullptr;  // host mode: where run_callback copies blob_host to, next to the lp copy-back
-  uint8_t* cmp_blobs = nullptr;    // CB_COMPUTE: pinned [m, record] records handed to the caller
-  uint8_t* stage_blob[2] = {nullptr, nullptr};  // eb_step_store_blobs: pinned [N, blob_bytes] staging
+  HostPtr<uint8_t> cmp_blobs;      // CB_COMPUTE: pinned [m, record] records handed to the caller
+  HostPtr<uint8_t> stage_blob[2];  // eb_step_store_blobs: pinned [N, blob_bytes] staging
   size_t stage_blob_cap = 0;
 
   // user proposals (eb_move_set_proposal), indexed by slot
@@ -186,11 +193,11 @@ struct eb_ctx {
   bool in_proposal = false;   // every other call on the context is refused while a proposal runs
   int up_where = EB_CALLBACK_HOST;  // mode of the running proposal
   int64_t up_m = 0;           // rows the running proposal returns
-  double* up_x = nullptr;     // device [N, D] rows handed to the proposal (s | c, or the ensemble)
-  double* up_f = nullptr;     // device [N] its Hastings factors
-  double* up_hx = nullptr;    // host mode: pinned [N, D] copy of up_x's rows
-  double* up_hq = nullptr;    // host mode: pinned [N, D] proposals
-  double* up_hf = nullptr;    // host mode: pinned [N] factors
+  DevPtr<double> up_x;        // device [N, D] rows handed to the proposal (s | c, or the ensemble)
+  DevPtr<double> up_f;        // device [N] its Hastings factors
+  HostPtr<double> up_hx;      // host mode: pinned [N, D] copy of up_x's rows
+  HostPtr<double> up_hq;      // host mode: pinned [N, D] proposals
+  HostPtr<double> up_hf;      // host mode: pinned [N] factors
 
   std::string err;
 };
@@ -232,14 +239,25 @@ static const char* const MSG_BLOBS_WITH_LOG_PROB =  // moves/move.py:38-42
     }                                                                                      \
   } while (0)
 
+// an allocation into an owner (dev_alloc / host_alloc) that fails makes the call fail with EB_ERR_NOMEM; the
+// message may name the CUDA error as cudaGetErrorString(alloc_err)
+#define CK_NOMEM(ctx, call, ...)            \
+  do {                                      \
+    const cudaError_t alloc_err = (call);   \
+    if (alloc_err != cudaSuccess) {         \
+      cudaGetLastError();                   \
+      FAIL(ctx, EB_ERR_NOMEM, __VA_ARGS__); \
+    }                                       \
+  } while (0)
+
 // map (and clear) the device status word to the reference's exceptions, in the
 // order compute_log_prob raises them (ensemble.py:476-479, 550-551)
 static int check_status(eb_ctx* c) {
   const int f = *c->status_host;
   if (f == 0) return EB_OK;
   *c->status_host = 0;
-  cudaMemsetAsync(c->status_dev, 0, sizeof(int), c->st);
-  cudaStreamSynchronize(c->st);
+  cudaMemsetAsync(c->status_dev.get(), 0, sizeof(int), c->st.get());
+  cudaStreamSynchronize(c->st.get());
   if (f & FLAG_COMM_TIMEOUT) FAIL(c, EB_ERR_COMM, "peer-memory barrier timed out: another rank did not arrive");
   if (f & FLAG_INF_PARAM) FAIL(c, EB_ERR_INF_PARAM, "At least one parameter value was infinite");
   if (f & FLAG_NAN_PARAM) FAIL(c, EB_ERR_NAN_PARAM, "At least one parameter value was NaN");
@@ -247,10 +265,42 @@ static int check_status(eb_ctx* c) {
 }
 
 static int fetch_status(eb_ctx* c) {
-  CK(c, cudaMemcpyAsync(c->status_host, c->status_dev, sizeof(int), cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return check_status(c);
 }
+
+// the arguments eb_create and eb_chain_create (`who`) share
+static int check_create_args(const char* who, int device, int64_t nwalkers, int64_t ndim) {
+  if (nwalkers < 2 || ndim < 1 || nwalkers > (int64_t)0x7fffffff || ndim > 16384) {
+    g_create_err = std::string(who) + ": need 2 <= nwalkers < 2^31 and 1 <= ndim <= 16384";
+    return EB_ERR_INVALID;
+  }
+  int ndev = 0;
+  const cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    g_create_err =
+        std::string(who) + ": no CUDA device (" + cudaGetErrorString(e) + "); this engine has no CPU fallback";
+    return EB_ERR_CUDA;
+  }
+  if (device < 0 || device >= ndev) {
+    g_create_err = std::string(who) + ": device index out of range";
+    return EB_ERR_INVALID;
+  }
+  return EB_OK;
+}
+
+// a failed step of eb_create / eb_chain_create; the owner the object is built in frees what exists of it
+#define CREATE_CK(call)                                                                       \
+  do {                                                                                        \
+    const cudaError_t _e = (call);                                                            \
+    if (_e != cudaSuccess) {                                                                  \
+      cudaGetLastError();                                                                     \
+      g_create_err = std::string(__func__) + ": " + #call + ": " + cudaGetErrorString(_e);    \
+      return EB_ERR_CUDA;                                                                     \
+    }                                                                                         \
+  } while (0)
 
 extern "C" {
 
@@ -270,71 +320,47 @@ const char* eb_last_error(const eb_ctx* ctx) { return ctx ? ctx->err.c_str() : g
 int eb_create(int device, int64_t nwalkers, int64_t ndim, uint64_t seed, eb_ctx** out) {
   if (!out) return EB_ERR_INVALID;
   *out = nullptr;
-  if (nwalkers < 2 || ndim < 1 || nwalkers > (int64_t)0x7fffffff || ndim > 16384) {
-    g_create_err = "eb_create: need 2 <= nwalkers < 2^31 and 1 <= ndim <= 16384";
-    return EB_ERR_INVALID;
-  }
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    g_create_err = std::string("eb_create: no CUDA device (") + cudaGetErrorString(e) +
-                   "); this engine has no CPU fallback";
-    return EB_ERR_CUDA;
-  }
-  if (device < 0 || device >= ndev) {
-    g_create_err = "eb_create: device index out of range";
-    return EB_ERR_INVALID;
-  }
-  eb_ctx* c = new eb_ctx();
+  const int rc = check_create_args("eb_create", device, nwalkers, ndim);
+  if (rc) return rc;
+  std::unique_ptr<eb_ctx> c(new eb_ctx());
   c->device = device;
   c->N = nwalkers;
   c->D = (int)ndim;
   c->seed = seed;
   if (const char* e = getenv("EMCEE_B200_TMA_ROWS")) c->allow_tma = atoi(e);  // developer override
-  auto fail = [&](const char* what, cudaError_t err) {
-    g_create_err = std::string("eb_create: ") + what + ": " + cudaGetErrorString(err);
-    eb_destroy(c);
-    return EB_ERR_CUDA;
-  };
-#define CC(call)                             \
-  do {                                       \
-    cudaError_t _e = (call);                 \
-    if (_e != cudaSuccess) return fail(#call, _e); \
-  } while (0)
-  CC(cudaSetDevice(device));
+  CREATE_CK(cudaSetDevice(device));
   cudaDeviceProp prop;
-  CC(cudaGetDeviceProperties(&prop, device));
+  CREATE_CK(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
-  CC(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
-  CC(cudaEventCreate(&c->ev0));
-  CC(cudaEventCreate(&c->ev1));
+  CREATE_CK(stream_create(c->st, cudaStreamNonBlocking));
+  CREATE_CK(event_create(c->ev0));
+  CREATE_CK(event_create(c->ev1));
+  cudaStream_t st = c->st.get();
   const size_t nd = (size_t)nwalkers * (size_t)ndim;
   // the tail holds the peer-memory barrier flags so one IPC handle exports both
-  CC(cudaMalloc(&c->coords, nd * sizeof(double) + MAX_RANKS * sizeof(unsigned)));
-  CC(cudaMalloc(&c->logp, (size_t)nwalkers * sizeof(double)));
-  CC(cudaMalloc(&c->accepted, (size_t)nwalkers));
-  CC(cudaMalloc(&c->nacc, (size_t)nwalkers * sizeof(unsigned long long)));
-  CC(cudaMalloc(&c->status_dev, sizeof(int)));
-  CC(cudaMallocHost(&c->status_host, sizeof(int)));
+  CREATE_CK(dev_alloc(c->coords, nd * sizeof(double) + MAX_RANKS * sizeof(unsigned)));
+  CREATE_CK(dev_alloc(c->logp, (size_t)nwalkers * sizeof(double)));
+  CREATE_CK(dev_alloc(c->accepted, (size_t)nwalkers));
+  CREATE_CK(dev_alloc(c->nacc, (size_t)nwalkers * sizeof(unsigned long long)));
+  CREATE_CK(dev_alloc(c->status_dev, sizeof(int)));
+  CREATE_CK(host_alloc(c->status_host, sizeof(int)));
   *c->status_host = 0;
-  CC(cudaMemsetAsync(c->status_dev, 0, sizeof(int), c->st));
-  CC(cudaMemsetAsync(c->accepted, 0, (size_t)nwalkers, c->st));
-  CC(cudaMemsetAsync(c->nacc, 0, (size_t)nwalkers * sizeof(unsigned long long), c->st));
+  CREATE_CK(cudaMemsetAsync(c->status_dev.get(), 0, sizeof(int), st));
+  CREATE_CK(cudaMemsetAsync(c->accepted.get(), 0, (size_t)nwalkers, st));
+  CREATE_CK(cudaMemsetAsync(c->nacc.get(), 0, (size_t)nwalkers * sizeof(unsigned long long), st));
   // split tables for a chunk of steps: <= 64 MiB, 1..512 steps
   size_t cap = (64u << 20) / ((size_t)nwalkers * sizeof(int32_t));
   cap = std::max<size_t>(1, std::min<size_t>(cap, 512));
   c->table_cap = cap;
-  CC(cudaMalloc(&c->order, cap * (size_t)nwalkers * sizeof(int32_t)));
-  CC(cudaMalloc(&c->info_dev, cap * sizeof(StepInfo)));
-  CC(cudaMallocHost(&c->info_host, cap * sizeof(StepInfo)));
-  CC(cudaMalloc(&c->descs_dev, cap * MAX_SPLITS * sizeof(HalfDesc)));
-  CC(cudaMallocHost(&c->descs_host, cap * MAX_SPLITS * sizeof(HalfDesc)));
-  CC(cudaMalloc(&c->gbar, sizeof(unsigned long long)));
-  CC(cudaMemsetAsync(c->gbar, 0, sizeof(unsigned long long), c->st));
-  CC(cudaStreamSynchronize(c->st));
-#undef CC
-  *out = c;
+  CREATE_CK(dev_alloc(c->order, cap * (size_t)nwalkers * sizeof(int32_t)));
+  CREATE_CK(dev_alloc(c->info_dev, cap * sizeof(StepInfo)));
+  CREATE_CK(host_alloc(c->info_host, cap * sizeof(StepInfo)));
+  CREATE_CK(dev_alloc(c->descs_dev, cap * MAX_SPLITS * sizeof(HalfDesc)));
+  CREATE_CK(host_alloc(c->descs_host, cap * MAX_SPLITS * sizeof(HalfDesc)));
+  CREATE_CK(dev_alloc(c->gbar, sizeof(unsigned long long)));
+  CREATE_CK(cudaMemsetAsync(c->gbar.get(), 0, sizeof(unsigned long long), st));
+  CREATE_CK(cudaStreamSynchronize(st));
+  *out = c.release();
   return EB_OK;
 }
 
@@ -342,66 +368,10 @@ int eb_destroy(eb_ctx* c) {
   if (!c) return EB_OK;
   NOT_IN_CALLBACK(c);
   cudaSetDevice(c->device);
-  comm_destroy(c->comm);
-  if (c->st) cudaStreamSynchronize(c->st);
-  cudaFree(c->coords);
-  cudaFree(c->logp);
-  cudaFree(c->accepted);
-  cudaFree(c->nacc);
-  cudaFree(c->status_dev);
-  cudaFreeHost(c->status_host);
-  cudaFree(c->model_params);
-  cudaFree(c->model_chol);
-  cudaFree(c->model_box);
-  cudaFree(c->order);
-  cudaFree(c->info_dev);
-  cudaFreeHost(c->info_host);
-  cudaFree(c->descs_dev);
-  cudaFreeHost(c->descs_host);
-  cudaFree(c->gbar);
-  cudaFree(c->scratch_x);
-  cudaFree(c->scratch_lp);
-  for (int k = 0; k < 2; ++k) {
-    cudaFreeHost(c->stage[k]);
-    cudaFreeHost(c->stage_acc[k]);
-    if (c->stage_ev[k]) cudaEventDestroy(c->stage_ev[k]);
-  }
-  cudaFree(c->flush_buf);
-  cudaFree(c->qbuf);
-  cudaFree(c->walk_work);
-  cudaFree(c->gauss_dev);
-  cudaFree(c->mom_acc);
-  cudaFree(c->mom_shift);
-  cudaFree(c->mom_partial);
-  cudaFree(c->hist.mem);
-  cudaFree(c->trace.mem);
-  cudaFree(c->trace_rows);
-  for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
-  cudaFree(c->timeline);
-  cudaFree(c->tap_partners);
-  cudaFree(c->tap_scalar);
-  cudaFree(c->tap_u);
-  cudaFree(c->tap_active);
-  cudaFreeHost(c->cb_x);
-  cudaFreeHost(c->cb_lp);
-  cudaFree(c->cb_xdev);
-  cudaFree(c->ext_f);
-  cudaFree(c->ext_lp);
-  cudaFree(c->blob_live);
-  cudaFree(c->blob_prop);
-  cudaFreeHost(c->blob_host);
-  cudaFreeHost(c->cmp_blobs);
-  for (int k = 0; k < 2; ++k) cudaFreeHost(c->stage_blob[k]);
-  cudaFree(c->up_x);
-  cudaFree(c->up_f);
-  cudaFreeHost(c->up_hx);
-  cudaFreeHost(c->up_hq);
-  cudaFreeHost(c->up_hf);
-  if (c->ev0) cudaEventDestroy(c->ev0);
-  if (c->ev1) cudaEventDestroy(c->ev1);
-  if (c->st) cudaStreamDestroy(c->st);
+  comm_destroy(c->comm);  // before any free: coords is exported to the peers
+  cudaStreamSynchronize(c->st.get());
+  delete c;  // the owners release the buffers, then the events and the stream
   cudaGetLastError();
-  delete c;
   return EB_OK;
 }
 
@@ -457,29 +427,26 @@ int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
     default:
       FAIL(c, EB_ERR_INVALID, "unknown model kind %d", kind);
   }
-  CK(c, cudaStreamSynchronize(c->st));
-  cudaFree(c->model_params);
-  cudaFree(c->model_chol);
-  cudaFree(c->model_box);  // a new model starts unbounded
-  c->model_params = nullptr;
-  c->model_chol = nullptr;
-  c->model_box = nullptr;
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  DevPtr<double> dparams, dchol;
   if (!host.empty()) {
-    CK(c, cudaMalloc(&c->model_params, host.size() * sizeof(double)));
-    CK(c, cudaMemcpy(c->model_params, host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice));
-    m.params = c->model_params;
+    CK(c, dev_alloc(dparams, host.size() * sizeof(double)));
+    CK(c, cudaMemcpy(dparams.get(), host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice));
+    m.params = dparams.get();
     if (kind == EB_MODEL_GAUSS_DENSE && dense_dmma_supported(c->D)) {
       std::vector<double> L;
       if (cholesky_lower(host.data() + D, c->D, L)) {
         std::vector<double> packed(dense_dmma_factor_doubles(c->D));
         dense_dmma_pack_factor(L.data(), c->D, packed.data());
-        CK(c, cudaMalloc(&c->model_chol, packed.size() * sizeof(double)));
-        CK(c, cudaMemcpy(c->model_chol, packed.data(), packed.size() * sizeof(double),
-                         cudaMemcpyHostToDevice));
-        m.chol = c->model_chol;
+        CK(c, dev_alloc(dchol, packed.size() * sizeof(double)));
+        CK(c, cudaMemcpy(dchol.get(), packed.data(), packed.size() * sizeof(double), cudaMemcpyHostToDevice));
+        m.chol = dchol.get();
       }
     }
   }
+  c->model_params = std::move(dparams);
+  c->model_chol = std::move(dchol);
+  c->model_box.reset();  // a new model starts unbounded
   c->model = m;
   c->have_model = true;
   c->cb_fn = nullptr;
@@ -497,16 +464,13 @@ int eb_model_set_callback(eb_ctx* c, eb_logprob_fn fn, void* user, int where) {
     FAIL(c, EB_ERR_INVALID, "eb_model_set_callback: where must be EB_CALLBACK_HOST or EB_CALLBACK_DEVICE (got %d)", where);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st));
-  cudaFree(c->model_params);
-  cudaFree(c->model_chol);
-  cudaFree(c->model_box);
-  c->model_params = nullptr;
-  c->model_chol = nullptr;
-  c->model_box = nullptr;
-  if (!c->ext_f) CK(c, cudaMalloc(&c->ext_f, (size_t)c->N * sizeof(double)));
-  if (!c->ext_lp) CK(c, cudaMalloc(&c->ext_lp, (size_t)c->N * sizeof(double)));
-  if (!c->qbuf) CK(c, cudaMalloc(&c->qbuf, (size_t)c->N * c->D * sizeof(double)));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  if (!c->ext_f) CK(c, dev_alloc(c->ext_f, (size_t)c->N * sizeof(double)));
+  if (!c->ext_lp) CK(c, dev_alloc(c->ext_lp, (size_t)c->N * sizeof(double)));
+  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, (size_t)c->N * c->D * sizeof(double)));
+  c->model_params.reset();
+  c->model_chol.reset();
+  c->model_box.reset();
   c->model = ModelDev{};
   c->model.kind = MODEL_EXTERNAL;
   c->cb_fn = fn;
@@ -528,28 +492,27 @@ static int ensure_blob_buffers(eb_ctx* c, size_t record_bytes) {
     FAIL(c, EB_ERR_NOMEM, "blob records of %zu bytes for %zu walkers do not fit in device memory", record_bytes, N);
   const size_t need = N * record_bytes;
   if (need <= c->blob_cap && (!host || c->blob_host)) return EB_OK;
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   size_t free_b = 0, total_b = 0;
   CK(c, cudaMemGetInfo(&free_b, &total_b));
   const size_t held = 2 * c->blob_cap;  // freed below before the new buffers are allocated
   if (2 * need > free_b + held)
     FAIL(c, EB_ERR_NOMEM, "blob buffers need %zu bytes of device memory, %zu are free", 2 * need, free_b + held);
-  cudaFree(c->blob_live);
-  cudaFree(c->blob_prop);
-  cudaFreeHost(c->blob_host);
-  c->blob_live = c->blob_prop = c->blob_host = nullptr;
+  c->blob_live.reset();
+  c->blob_prop.reset();
+  c->blob_host.reset();
   c->blob_cap = 0;
   c->blobs_live = false;
-  const size_t cap = need;
-  if (cudaMalloc(&c->blob_live, cap) != cudaSuccess || cudaMalloc(&c->blob_prop, cap) != cudaSuccess ||
-      (host && cudaMallocHost(&c->blob_host, cap) != cudaSuccess)) {
-    cudaGetLastError();
-    cudaFree(c->blob_live);
-    cudaFree(c->blob_prop);
-    c->blob_live = c->blob_prop = nullptr;
-    FAIL(c, EB_ERR_NOMEM, "allocating %zu bytes of blob buffers failed", 2 * cap);
-  }
-  c->blob_cap = cap;
+  DevPtr<uint8_t> live, prop;
+  HostPtr<uint8_t> staging;
+  cudaError_t e = dev_alloc(live, need);
+  if (e == cudaSuccess) e = dev_alloc(prop, need);
+  if (e == cudaSuccess && host) e = host_alloc(staging, need);
+  CK_NOMEM(c, e, "allocating %zu bytes of blob buffers failed", 2 * need);
+  c->blob_live = std::move(live);
+  c->blob_prop = std::move(prop);
+  c->blob_host = std::move(staging);
+  c->blob_cap = need;
   return EB_OK;
 }
 
@@ -566,18 +529,16 @@ static int copy_records(eb_ctx* c, void* dst, const void* src, size_t width, siz
     cudaStream_t s = src_stream == 1 ? cudaStreamLegacy
                      : src_stream == 2 ? cudaStreamPerThread
                                        : reinterpret_cast<cudaStream_t>((uintptr_t)src_stream);
-    cudaEvent_t ev;
-    CK(c, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    cudaError_t e = cudaEventRecord(ev, s);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->st, ev, 0);
-    cudaEventDestroy(ev);
-    CK(c, e);
+    EventPtr ev;
+    CK(c, event_create(ev, cudaEventDisableTiming));
+    CK(c, cudaEventRecord(ev.get(), s));
+    CK(c, cudaStreamWaitEvent(c->st.get(), ev.get(), 0));
   }
   if (spitch == width || m == 1)
-    CK(c, cudaMemcpyAsync(dst, src, width * m, cudaMemcpyDefault, c->st));
+    CK(c, cudaMemcpyAsync(dst, src, width * m, cudaMemcpyDefault, c->st.get()));
   else
-    CK(c, cudaMemcpy2DAsync(dst, width, src, spitch, width, m, cudaMemcpyDefault, c->st));
-  CK(c, cudaStreamSynchronize(c->st));  // the caller may free or reuse src as soon as this returns
+    CK(c, cudaMemcpy2DAsync(dst, width, src, spitch, width, m, cudaMemcpyDefault, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));  // the caller may free or reuse src as soon as this returns
   return EB_OK;
 }
 
@@ -600,7 +561,7 @@ int eb_callback_blobs(eb_ctx* c, const void* src, int64_t record_bytes, int64_t 
     case CB_SET_STATE: {  // the initial evaluation fixes the live layout
       int rc = ensure_blob_buffers(c, R);
       if (rc) return rc;
-      dst = c->blob_live;
+      dst = c->blob_live.get();
       break;
     }
     case CB_STEP:
@@ -608,20 +569,16 @@ int eb_callback_blobs(eb_ctx* c, const void* src, int64_t record_bytes, int64_t 
       if (R != c->blob_bytes)
         FAIL(c, EB_ERR_INVALID, "the function returned blob records of %zu bytes; the state's records have %zu", R,
              c->blob_bytes);
-      dst = c->blob_prop;
+      dst = c->blob_prop.get();
       break;
     default:  // CB_COMPUTE: straight to the caller's pinned buffer
       if (c->blob_bytes && R != c->blob_bytes)
         FAIL(c, EB_ERR_INVALID, "the function returned blob records of %zu bytes; the state's records have %zu", R,
              c->blob_bytes);
-      cudaFreeHost(c->cmp_blobs);
-      c->cmp_blobs = nullptr;
-      if (cudaMallocHost(&c->cmp_blobs, std::max<size_t>(1, (size_t)m * R)) != cudaSuccess) {
-        cudaGetLastError();
-        c->cmp_blobs = nullptr;
-        FAIL(c, EB_ERR_NOMEM, "allocating %zu bytes of pinned host memory for blobs failed", (size_t)m * R);
-      }
-      dst = c->cmp_blobs;
+      c->cmp_blobs.reset();
+      CK_NOMEM(c, host_alloc(c->cmp_blobs, std::max<size_t>(1, (size_t)m * R)),
+               "allocating %zu bytes of pinned host memory for blobs failed", (size_t)m * R);
+      dst = c->cmp_blobs.get();
       to_host = false;  // copied below, whatever the mode
   }
   if (m > 0) {
@@ -629,9 +586,9 @@ int eb_callback_blobs(eb_ctx* c, const void* src, int64_t record_bytes, int64_t 
       // host mode: into the pinned staging; run_callback copies it to dst next to the lp copy-back
       const uint8_t* s = static_cast<const uint8_t*>(src);
       if ((size_t)stride_bytes == R)
-        memcpy(c->blob_host, s, (size_t)m * R);
+        memcpy(c->blob_host.get(), s, (size_t)m * R);
       else
-        for (int64_t r = 0; r < m; ++r) memcpy(c->blob_host + (size_t)r * R, s + (size_t)r * stride_bytes, R);
+        for (int64_t r = 0; r < m; ++r) memcpy(c->blob_host.get() + (size_t)r * R, s + (size_t)r * stride_bytes, R);
       c->cb_blob_dst = dst;
     } else {
       int rc = copy_records(c, dst, src, R, (size_t)stride_bytes, (size_t)m, src_stream);
@@ -686,10 +643,10 @@ int eb_proposal_result(eb_ctx* c, const void* q, int64_t q_row_stride_bytes, con
   if (f_stride_bytes <= 0 || f_stride_bytes % 8 != 0)
     FAIL(c, EB_ERR_INVALID, "eb_proposal_result: the stride of factors must be a positive multiple of 8 bytes (got %lld)",
          (long long)f_stride_bytes);
-  int rc = copy_records(c, c->qbuf, q, (size_t)row, (size_t)q_row_stride_bytes, (size_t)m, src_stream);
+  int rc = copy_records(c, c->qbuf.get(), q, (size_t)row, (size_t)q_row_stride_bytes, (size_t)m, src_stream);
   if (rc) return rc;
   // the first copy already waited for src_stream
-  return copy_records(c, c->up_f, factors, sizeof(double), (size_t)f_stride_bytes, (size_t)m, 0);
+  return copy_records(c, c->up_f.get(), factors, sizeof(double), (size_t)f_stride_bytes, (size_t)m, 0);
 }
 
 int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
@@ -710,18 +667,17 @@ int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
     }
   }
   CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   c->chain_ok = false;
-  cudaFree(c->model_box);
-  c->model_box = nullptr;
-  c->model.lo = c->model.hi = nullptr;
+  DevPtr<double> box;
   if (lower) {
-    CK(c, cudaMalloc(&c->model_box, 2 * D * sizeof(double)));
-    CK(c, cudaMemcpy(c->model_box, lower, D * sizeof(double), cudaMemcpyHostToDevice));
-    CK(c, cudaMemcpy(c->model_box + D, upper, D * sizeof(double), cudaMemcpyHostToDevice));
-    c->model.lo = c->model_box;
-    c->model.hi = c->model_box + D;
+    CK(c, dev_alloc(box, 2 * D * sizeof(double)));
+    CK(c, cudaMemcpy(box.get(), lower, D * sizeof(double), cudaMemcpyHostToDevice));
+    CK(c, cudaMemcpy(box.get() + D, upper, D * sizeof(double), cudaMemcpyHostToDevice));
   }
+  c->model.lo = box.get();
+  c->model.hi = lower ? box.get() + D : nullptr;
+  c->model_box = std::move(box);
   return EB_OK;
 }
 
@@ -731,20 +687,18 @@ static int ensure_callback_staging(eb_ctx* c, size_t rows) {
   const bool host = c->cb_where == EB_CALLBACK_HOST;
   if (rows <= c->cb_rows && (host ? c->cb_x != nullptr : c->cb_xdev != nullptr)) return EB_OK;
   rows = std::max(rows, c->cb_rows);
-  CK(c, cudaStreamSynchronize(c->st));
-  cudaFreeHost(c->cb_x);
-  cudaFreeHost(c->cb_lp);
-  cudaFree(c->cb_xdev);
-  c->cb_x = nullptr;
-  c->cb_lp = nullptr;
-  c->cb_xdev = nullptr;
-  c->cb_rows = 0;
+  HostPtr<double> x, lp;
+  DevPtr<double> xdev;
   if (host) {
-    CK(c, cudaMallocHost(&c->cb_x, rows * (size_t)c->D * sizeof(double)));
-    CK(c, cudaMallocHost(&c->cb_lp, rows * sizeof(double)));
+    CK(c, host_alloc(x, rows * (size_t)c->D * sizeof(double)));
+    CK(c, host_alloc(lp, rows * sizeof(double)));
   } else {
-    CK(c, cudaMalloc(&c->cb_xdev, rows * (size_t)c->D * sizeof(double)));
+    CK(c, dev_alloc(xdev, rows * (size_t)c->D * sizeof(double)));
   }
+  CK(c, cudaStreamSynchronize(c->st.get()));  // the old buffers may still be in use
+  c->cb_x = std::move(x);
+  c->cb_lp = std::move(lp);
+  c->cb_xdev = std::move(xdev);
   c->cb_rows = rows;
   return EB_OK;
 }
@@ -754,7 +708,7 @@ static int ensure_callback_staging(eb_ctx* c, size_t rows) {
 // non-finite flags (WalkMove / GaussianMove proposals, the caller's coordinates)
 static int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x) {
   const size_t D = (size_t)c->D;
-  if (scan_x) CK(c, launch_scan_nonfinite(x, (size_t)m * D, 0, c->status_dev, c->st));
+  if (scan_x) CK(c, launch_scan_nonfinite(x, (size_t)m * D, 0, c->status_dev.get(), c->st.get()));
   int rc = fetch_status(c);  // synchronises; ensemble.py:476-479: the function never sees a non-finite row
   if (rc) return rc;
   rc = ensure_callback_staging(c, (size_t)m);
@@ -762,53 +716,52 @@ static int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool 
   const bool host = c->cb_where == EB_CALLBACK_HOST;
   // the function gets its own copy of the rows: writing to it cannot change the proposals the update reads
   if (host) {
-    CK(c, cudaMemcpyAsync(c->cb_x, x, (size_t)m * D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaStreamSynchronize(c->st));
+    CK(c, cudaMemcpyAsync(c->cb_x.get(), x, (size_t)m * D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
+    CK(c, cudaStreamSynchronize(c->st.get()));
   } else {
-    CK(c, cudaMemcpyAsync(c->cb_xdev, x, (size_t)m * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
+    CK(c, cudaMemcpyAsync(c->cb_xdev.get(), x, (size_t)m * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st.get()));
     // complete before fn runs: a consumer may ignore the stream it is given (torch does) and read x from any
     // stream of its own
-    CK(c, cudaStreamSynchronize(c->st));
+    CK(c, cudaStreamSynchronize(c->st.get()));
   }
   c->cb_m = m;
   c->cb_blob_rows = -1;
   c->cb_blob_dst = nullptr;
   c->in_callback = true;
-  const int r = host ? c->cb_fn(c->cb_user, c->cb_x, m, (int64_t)D, c->cb_lp, nullptr)
-                     : c->cb_fn(c->cb_user, c->cb_xdev, m, (int64_t)D, lp, (void*)c->st);
+  const int r = host ? c->cb_fn(c->cb_user, c->cb_x.get(), m, (int64_t)D, c->cb_lp.get(), nullptr)
+                     : c->cb_fn(c->cb_user, c->cb_xdev.get(), m, (int64_t)D, lp, (void*)c->st.get());
   c->in_callback = false;
   if (r != 0) {
-    cudaStreamSynchronize(c->st);  // whatever the function enqueued before it failed
+    cudaStreamSynchronize(c->st.get());  // whatever the function enqueued before it failed
     FAIL(c, EB_ERR_CALLBACK, "the log-probability callback failed (returned %d)", r);
   }
   if (c->cb_phase == CB_STEP && c->blobs_live && c->cb_blob_rows < 0)
     FAIL(c, EB_ERR_INVALID, "the log-probability function returned no blobs; the state has blob records of %zu bytes",
          c->blob_bytes);
-  if (host) CK(c, cudaMemcpyAsync(lp, c->cb_lp, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  if (host) CK(c, cudaMemcpyAsync(lp, c->cb_lp.get(), (size_t)m * sizeof(double), cudaMemcpyHostToDevice, c->st.get()));
   // host-mode blob records ride with the lp copy-back: no synchronisation of their own
   if (c->cb_blob_dst)
-    CK(c, cudaMemcpyAsync(c->cb_blob_dst, c->blob_host, (size_t)m * c->cb_blob_bytes, cudaMemcpyHostToDevice, c->st));
-  CK(c, launch_scan_nonfinite(lp, (size_t)m, 1, c->status_dev, c->st));
+    CK(c, cudaMemcpyAsync(c->cb_blob_dst, c->blob_host.get(), (size_t)m * c->cb_blob_bytes, cudaMemcpyHostToDevice,
+                          c->st.get()));
+  CK(c, launch_scan_nonfinite(lp, (size_t)m, 1, c->status_dev.get(), c->st.get()));
   return fetch_status(c);  // ensemble.py:550-551, before any update
 }
 
 // rows of x -> out with the kernel that matches the stepping path of the model
 static cudaError_t launch_logprob(eb_ctx* c, const double* x, int64_t rows, double* out) {
   if (c->allow_dmma && c->model.kind == EB_MODEL_GAUSS_DENSE && c->model.chol != nullptr)
-    return launch_logprob_dense_dmma(c->model, c->D, x, rows, out, c->status_dev, c->sm_count, c->st);
-  return launch_logprob_generic(c->model, x, rows, c->D, out, c->status_dev, c->st);
+    return launch_logprob_dense_dmma(c->model, c->D, x, rows, out, c->status_dev.get(), c->sm_count, c->st.get());
+  return launch_logprob_generic(c->model, x, rows, c->D, out, c->status_dev.get(), c->st.get());
 }
 
 static int ensure_scratch(eb_ctx* c, size_t rows) {
   if (rows <= c->scratch_rows) return EB_OK;
-  CK(c, cudaStreamSynchronize(c->st));
-  cudaFree(c->scratch_x);
-  cudaFree(c->scratch_lp);
-  c->scratch_x = nullptr;
-  c->scratch_lp = nullptr;
-  c->scratch_rows = 0;
-  CK(c, cudaMalloc(&c->scratch_x, rows * (size_t)c->D * sizeof(double)));
-  CK(c, cudaMalloc(&c->scratch_lp, rows * sizeof(double)));
+  DevPtr<double> x, lp;
+  CK(c, dev_alloc(x, rows * (size_t)c->D * sizeof(double)));
+  CK(c, dev_alloc(lp, rows * sizeof(double)));
+  CK(c, cudaStreamSynchronize(c->st.get()));  // the old buffers may still be in use
+  c->scratch_x = std::move(x);
+  c->scratch_lp = std::move(lp);
   c->scratch_rows = rows;
   return EB_OK;
 }
@@ -822,16 +775,16 @@ int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) 
   CK(c, cudaSetDevice(c->device));
   int rc = ensure_scratch(c, m);
   if (rc) return rc;
-  CK(c, cudaMemcpyAsync(c->scratch_x, coords, m * (size_t)c->D * sizeof(double), cudaMemcpyHostToDevice,
-                        c->st));
+  CK(c, cudaMemcpyAsync(c->scratch_x.get(), coords, m * (size_t)c->D * sizeof(double), cudaMemcpyHostToDevice,
+                        c->st.get()));
   if (c->model.kind == MODEL_EXTERNAL) {
     c->cb_phase = CB_COMPUTE;
-    rc = run_callback(c, c->scratch_x, (int64_t)m, c->scratch_lp, true);
+    rc = run_callback(c, c->scratch_x.get(), (int64_t)m, c->scratch_lp.get(), true);
     if (rc) return rc;
   } else {
-    CK(c, launch_logprob(c, c->scratch_x, (int64_t)m, c->scratch_lp));
+    CK(c, launch_logprob(c, c->scratch_x.get(), (int64_t)m, c->scratch_lp.get()));
   }
-  CK(c, cudaMemcpyAsync(out, c->scratch_lp, m * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  CK(c, cudaMemcpyAsync(out, c->scratch_lp.get(), m * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
   return fetch_status(c);
 }
 
@@ -844,17 +797,14 @@ int eb_compute_log_prob_blobs(eb_ctx* c, const double* coords, size_t m, double*
   *record_bytes = 0;
   if (c->have_model && c->model.kind != MODEL_EXTERNAL)
     FAIL(c, EB_ERR_UNSUPPORTED, "eb_compute_log_prob_blobs: only log-probability callbacks return blobs");
-  cudaFreeHost(c->cmp_blobs);
-  c->cmp_blobs = nullptr;
+  c->cmp_blobs.reset();
   c->cb_blob_rows = -1;
   const int rc = eb_compute_log_prob(c, coords, m, out);
   if (rc == EB_OK && c->cb_blob_rows >= 0 && c->cmp_blobs) {
-    *blobs_out = c->cmp_blobs;
+    *blobs_out = c->cmp_blobs.release();  // the caller frees them with eb_host_free
     *record_bytes = c->cb_blob_bytes;
-  } else {
-    cudaFreeHost(c->cmp_blobs);
   }
-  c->cmp_blobs = nullptr;
+  c->cmp_blobs.reset();
   return rc;
 }
 
@@ -875,10 +825,11 @@ static int sync_replicas(eb_ctx* c) {
   if (c->comm.nranks == 1 || !c->replicas_dirty) return EB_OK;
   uint64_t launches = 0;
   c->chain_ok = false;
-  if (comm_sync_state(c->comm, c->st, c->status_dev, c->logp, c->accepted, c->nacc, launches))
+  if (comm_sync_state(c->comm, c->st.get(), c->status_dev.get(), c->logp.get(), c->accepted.get(), c->nacc.get(),
+                      launches))
     FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   c->fused_last = false;
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   c->replicas_dirty = false;
   return EB_OK;
 }
@@ -907,29 +858,31 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   uint64_t launches = 0;
   if (c->comm.nranks > 1 && c->comm.mode == EB_COMM_P2P && c->comm.imported) {
     // no peer may still be pulling the rows that are about to be overwritten
-    if (comm_barrier(c->comm, c->st, c->status_dev, launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
+    if (comm_barrier(c->comm, c->st.get(), c->status_dev.get(), launches))
+      FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
     c->fused_last = false;
   }
-  CK(c, cudaMemcpyAsync(c->coords + (size_t)r0 * D, coords + (size_t)r0 * D, rows * D * sizeof(double),
-                        cudaMemcpyHostToDevice, c->st));
+  CK(c, cudaMemcpyAsync(c->coords.get() + (size_t)r0 * D, coords + (size_t)r0 * D, rows * D * sizeof(double),
+                        cudaMemcpyHostToDevice, c->st.get()));
   if (log_prob) {
-    CK(c, cudaMemcpyAsync(c->logp + r0, log_prob + r0, rows * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    CK(c, cudaMemcpyAsync(c->logp.get() + r0, log_prob + r0, rows * sizeof(double), cudaMemcpyHostToDevice,
+                          c->st.get()));
   } else if (c->model.kind == MODEL_EXTERNAL) {
     c->cb_phase = CB_SET_STATE;
-    int rc = run_callback(c, c->coords, (int64_t)rows, c->logp, true);  // one GPU: rows == nwalkers
+    int rc = run_callback(c, c->coords.get(), (int64_t)rows, c->logp.get(), true);  // one GPU: rows == nwalkers
     if (rc) return rc;
     if (c->cb_blob_rows >= 0) {  // the records went to blob_live: they fix the live layout
       c->blob_bytes = c->cb_blob_bytes;
       c->blobs_live = true;
     }
   } else {
-    CK(c, launch_logprob(c, c->coords + (size_t)r0 * D, (int64_t)rows, c->logp + r0));
+    CK(c, launch_logprob(c, c->coords.get() + (size_t)r0 * D, (int64_t)rows, c->logp.get() + r0));
   }
   if (c->comm.nranks > 1) {
-    if (c->comm.mode == EB_COMM_ALLGATHER && comm_gather_coords(c->comm, c->st, launches))
+    if (c->comm.mode == EB_COMM_ALLGATHER && comm_gather_coords(c->comm, c->st.get(), launches))
       FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
     if (c->comm.mode == EB_COMM_P2P && c->comm.imported &&
-        comm_barrier(c->comm, c->st, c->status_dev, launches))  // every rank's block is in place
+        comm_barrier(c->comm, c->st.get(), c->status_dev.get(), launches))  // every rank's block is in place
       FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
     c->replicas_dirty = true;
   }
@@ -948,11 +901,11 @@ int eb_get_state(eb_ctx* c, double* coords, double* log_prob) {
   if (rc) return rc;
   c->chain_ok = false;
   if (coords)
-    CK(c, cudaMemcpyAsync(coords, c->coords, (size_t)c->N * c->D * sizeof(double), cudaMemcpyDeviceToHost,
-                          c->st));
+    CK(c, cudaMemcpyAsync(coords, c->coords.get(), (size_t)c->N * c->D * sizeof(double), cudaMemcpyDeviceToHost,
+                          c->st.get()));
   if (log_prob)
-    CK(c, cudaMemcpyAsync(log_prob, c->logp, (size_t)c->N * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+    CK(c, cudaMemcpyAsync(log_prob, c->logp.get(), (size_t)c->N * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
 
@@ -970,8 +923,8 @@ int eb_set_state_blobs(eb_ctx* c, const void* blobs, size_t record_bytes) {
   CK(c, cudaSetDevice(c->device));
   int rc = ensure_blob_buffers(c, record_bytes);
   if (rc) return rc;
-  CK(c, cudaMemcpyAsync(c->blob_live, blobs, (size_t)c->N * record_bytes, cudaMemcpyHostToDevice, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemcpyAsync(c->blob_live.get(), blobs, (size_t)c->N * record_bytes, cudaMemcpyHostToDevice, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   c->blob_bytes = record_bytes;
   c->blobs_live = true;
   return EB_OK;
@@ -983,8 +936,8 @@ int eb_get_blobs(eb_ctx* c, void* out) {
   if (!c->blobs_live) FAIL(c, EB_ERR_STATE, "eb_get_blobs: the state has no blobs");
   if (!out) FAIL(c, EB_ERR_INVALID, "eb_get_blobs: null buffer");
   CK(c, cudaSetDevice(c->device));
-  CK(c, cudaMemcpyAsync(out, c->blob_live, (size_t)c->N * c->blob_bytes, cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemcpyAsync(out, c->blob_live.get(), (size_t)c->N * c->blob_bytes, cudaMemcpyDeviceToHost, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
 
@@ -1011,11 +964,12 @@ int eb_get_state_rows(eb_ctx* c, int64_t row0, int64_t nrows, double* coords, do
   CK(c, cudaSetDevice(c->device));
   c->chain_ok = false;
   if (coords && nrows)
-    CK(c, cudaMemcpyAsync(coords, c->coords + (size_t)row0 * c->D, (size_t)nrows * c->D * sizeof(double),
-                          cudaMemcpyDeviceToHost, c->st));
+    CK(c, cudaMemcpyAsync(coords, c->coords.get() + (size_t)row0 * c->D, (size_t)nrows * c->D * sizeof(double),
+                          cudaMemcpyDeviceToHost, c->st.get()));
   if (log_prob && nrows)
-    CK(c, cudaMemcpyAsync(log_prob, c->logp + row0, (size_t)nrows * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+    CK(c, cudaMemcpyAsync(log_prob, c->logp.get() + row0, (size_t)nrows * sizeof(double), cudaMemcpyDeviceToHost,
+                          c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
 
@@ -1153,15 +1107,13 @@ int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) 
   if (!(tot > 0.0)) FAIL(c, EB_ERR_INVALID, "eb_step: move weights sum to zero");
   if (!ghost.empty()) {
     if (ghost.size() > c->gauss_cap) {
-      CK(c, cudaStreamSynchronize(c->st));
-      cudaFree(c->gauss_dev);
-      c->gauss_dev = nullptr;
-      c->gauss_cap = 0;
-      CK(c, cudaMalloc(&c->gauss_dev, ghost.size() * sizeof(double)));
+      CK(c, cudaStreamSynchronize(c->st.get()));
+      CK(c, dev_alloc(c->gauss_dev, ghost.size() * sizeof(double)));
       c->gauss_cap = ghost.size();
     }
-    CK(c, cudaMemcpyAsync(c->gauss_dev, ghost.data(), ghost.size() * sizeof(double), cudaMemcpyHostToDevice, c->st));
-    CK(c, cudaStreamSynchronize(c->st));  // ghost is a local
+    CK(c, cudaMemcpyAsync(c->gauss_dev.get(), ghost.data(), ghost.size() * sizeof(double), cudaMemcpyHostToDevice,
+                          c->st.get()));
+    CK(c, cudaStreamSynchronize(c->st.get()));  // ghost is a local
   }
   c->picks.assign(nmoves, 0);
   // ensemble.py:128-129 then RandomState.choice(p=...): cdf = cumsum(p); cdf /= cdf[-1]
@@ -1192,20 +1144,20 @@ void split_starts(int64_t N, int P, int* start) {
 
 void fill_base_args(eb_ctx* c, const eb_move& mv, HalfStepArgs& a) {
   a = HalfStepArgs{};
-  a.coords = c->coords;
-  a.logp = c->logp;
-  a.accepted = c->accepted;
-  a.nacc = c->nacc;
-  a.status = c->status_dev;
+  a.coords = c->coords.get();
+  a.logp = c->logp.get();
+  a.accepted = c->accepted.get();
+  a.nacc = c->nacc.get();
+  a.status = c->status_dev.get();
   a.N = c->N;
   a.D = c->D;
   a.seed = c->seed;
   a.model = c->model;
   if (c->debug) {
-    a.tap_partners = c->tap_partners;
-    a.tap_scalar = c->tap_scalar;
-    a.tap_u = c->tap_u;
-    a.tap_active = c->tap_active;
+    a.tap_partners = c->tap_partners.get();
+    a.tap_scalar = c->tap_scalar.get();
+    a.tap_u = c->tap_u.get();
+    a.tap_active = c->tap_active.get();
   }
   switch (mv.kind) {
     case EB_MOVE_STRETCH:
@@ -1218,7 +1170,7 @@ void fill_base_args(eb_ctx* c, const eb_move& mv, HalfStepArgs& a) {
     default:
       a.p0 = mv.p0;  // gammas
   }
-  a.timeline = c->timeline;
+  a.timeline = c->timeline.get();
   a.dmma_stagger = c->dmma_stagger;
   comm_fill_args(c->comm, a);
 }
@@ -1239,21 +1191,21 @@ int check_walker_count(eb_ctx* c, const eb_move& mv) {
 // SNOOKER) -- or the proposals a move's own kernels left in qbuf (MOVE_PRECOMPUTED) --, the callback, then the
 // accept phase.  The proposal rows are the fused kernel's by construction: the same code stages them.
 int callback_half_step(eb_ctx* c, int move_kind, HalfStepArgs a, uint64_t& launches) {
-  ExternalBufs ext{c->qbuf, nullptr, c->ext_lp};
+  ExternalBufs ext{c->qbuf.get(), nullptr, c->ext_lp.get()};
   if (move_kind != MOVE_PRECOMPUTED) {
-    ext.f = c->ext_f;
-    CK(c, launch_half_step_external(move_kind, a, ext, c->st));
+    ext.f = c->ext_f.get();
+    CK(c, launch_half_step_external(move_kind, a, ext, c->st.get()));
     ++launches;
   }
   c->cb_phase = CB_STEP;
-  int rc = run_callback(c, c->qbuf, (int64_t)a.i_hi - a.i_lo, c->ext_lp, move_kind == MOVE_PRECOMPUTED);
+  int rc = run_callback(c, c->qbuf.get(), (int64_t)a.i_hi - a.i_lo, c->ext_lp.get(), move_kind == MOVE_PRECOMPUTED);
   if (rc) return rc;
-  a.qbuf = c->qbuf;
-  CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st));
+  a.qbuf = c->qbuf.get();
+  CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st.get()));
   ++launches;
   if (c->blobs_live) {  // accepted walkers take their proposal's record (moves/move.py:36-43)
-    CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop, c->blob_live,
-                             c->blob_bytes, c->st));
+    CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop.get(), c->blob_live.get(),
+                             c->blob_bytes, c->st.get()));
     ++launches;
   }
   c->last_kernel = "callback";
@@ -1289,7 +1241,8 @@ int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, const int32
     if (c->fused_last) {
       // the previous launch was a dense_dmma kernel that carried the peer barrier itself (signal at its end);
       // this kernel does not wait on its own, so the ranks meet explicitly before it reads peer rows
-      if (comm_barrier(c->comm, c->st, c->status_dev, launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
+      if (comm_barrier(c->comm, c->st.get(), c->status_dev.get(), launches))
+        FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
       c->fused_last = false;
     }
     c->chain_ok = false;
@@ -1302,28 +1255,30 @@ int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, const int32
     bool used_tma = false;
     TmaVariant tv{};
     if (c->allow_tma && !c->debug)
-      CK(c, launch_half_step_tma(mv.kind, a, c->sm_count, c->allow_tma >= 2, c->tma_own_reg, c->st, &used_tma, &tv));
+      CK(c, launch_half_step_tma(mv.kind, a, c->sm_count, c->allow_tma >= 2, c->tma_own_reg, c->st.get(), &used_tma,
+                                 &tv));
     if (used_tma) {
       c->last_kernel = "tma_rows";
       snprintf(c->last_variant, sizeof(c->last_variant), "tma_rows R=%d epl=%d own_reg=%d warps=%d", tv.R, tv.epl,
                tv.own_reg, tv.warps);
     } else {
-      CK(c, launch_half_step_generic(mv.kind, a, c->st));
+      CK(c, launch_half_step_generic(mv.kind, a, c->st.get()));
       c->last_kernel = "generic";
       snprintf(c->last_variant, sizeof(c->last_variant), "generic G=%d", lanes_per_walker(c->D));
     }
     ++launches;
     c->tap_count = a.a_count;
-    if (comm_after_split(c->comm, c->st, c->status_dev, launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
+    if (comm_after_split(c->comm, c->st.get(), c->status_dev.get(), launches))
+      FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   }
   return EB_OK;
 }
 
 int ensure_move_scratch(eb_ctx* c) {
   const size_t D = (size_t)c->D;
-  if (!c->qbuf) CK(c, cudaMalloc(&c->qbuf, (size_t)c->N * D * sizeof(double)));
-  if (!c->walk_work && D <= 1024) CK(c, cudaMalloc(&c->walk_work, (2 * D + 3 * D * D) * sizeof(double)));
-  if (!c->mom_partial && D <= 1024) CK(c, cudaMalloc(&c->mom_partial, moments_partial_bytes(c->D, c->sm_count)));
+  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, (size_t)c->N * D * sizeof(double)));
+  if (!c->walk_work && D <= 1024) CK(c, dev_alloc(c->walk_work, (2 * D + 3 * D * D) * sizeof(double)));
+  if (!c->mom_partial && D <= 1024) CK(c, dev_alloc(c->mom_partial, moments_partial_bytes(c->D, c->sm_count)));
   return EB_OK;
 }
 
@@ -1341,10 +1296,10 @@ int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
   fill_base_args(c, mv, a);
   a.order = order;
   a.step = step;
-  a.qbuf = c->qbuf;
+  a.qbuf = c->qbuf.get();
   c->chain_ok = false;
   const size_t D = (size_t)c->D;
-  double* shift = c->walk_work;
+  double* shift = c->walk_work.get();
   double* acc = shift + D;
   double* cov = acc + D + D * D;
   double* L = cov + D * D;
@@ -1360,15 +1315,16 @@ int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
     if (s0 == Nc) {
       // every walker of the split draws from the covariance of the WHOLE complement (walk.py:34-35 with a
       // permutation of all Nc rows): computed once -- moment sums on the tensor pipe, then a D x D factorisation
-      CK(c, launch_colmean(c->coords, c->N, c->D, shift, nullptr, c->st));  // any shift will do: the ensemble mean
-      CK(c, cudaMemsetAsync(acc, 0, (D + D * D) * sizeof(double), c->st));
-      CK(c, launch_moments(c->coords, Nc, c->D, shift, c->mom_partial, acc, c->sm_count, c->st, order, a.a_start,
-                           a.a_count));
-      CK(c, launch_cov_chol(acc, (double)Nc, c->D, cov, L, c->st));
-      CK(c, launch_walk_shared_propose(a, L, c->qbuf, c->st));
+      // any shift will do: the ensemble mean
+      CK(c, launch_colmean(c->coords.get(), c->N, c->D, shift, nullptr, c->st.get()));
+      CK(c, cudaMemsetAsync(acc, 0, (D + D * D) * sizeof(double), c->st.get()));
+      CK(c, launch_moments(c->coords.get(), Nc, c->D, shift, c->mom_partial.get(), acc, c->sm_count, c->st.get(), order,
+                           a.a_start, a.a_count));
+      CK(c, launch_cov_chol(acc, (double)Nc, c->D, cov, L, c->st.get()));
+      CK(c, launch_walk_shared_propose(a, L, c->qbuf.get(), c->st.get()));
       launches += 5;
     } else {
-      CK(c, launch_walk_subset_propose(a, (int)s0, c->qbuf, c->st));
+      CK(c, launch_walk_subset_propose(a, (int)s0, c->qbuf.get(), c->st.get()));
       ++launches;
     }
     if (c->model.kind == MODEL_EXTERNAL) {
@@ -1376,7 +1332,7 @@ int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
       if (rc) return rc;
       continue;
     }
-    CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st));
+    CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st.get()));
     ++launches;
   }
   if (c->model.kind == MODEL_EXTERNAL) return EB_OK;
@@ -1398,17 +1354,18 @@ int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step,
     f = exp(-lf + (lf - (-lf)) * u53(w.x, w.y));
   }
   const int seq_dim = (int)(((uint64_t)mv.seq_index + c->picks[mi]) % (uint64_t)D);  // gaussian.py:102-103
-  const double* dev = c->gauss_dev + s.goff[mi];
+  const double* dev = c->gauss_dev.get() + s.goff[mi];
   const int form = s.gform[mi];
   const double* scale = dev;
   c->chain_ok = false;
   if (form == 2) {
-    double* v = c->gauss_dev + s.goff[mi] + (size_t)D * D;
-    CK(c, launch_gaussian_shift(dev, D, f, c->seed, step, v, c->st));
+    double* v = c->gauss_dev.get() + s.goff[mi] + (size_t)D * D;
+    CK(c, launch_gaussian_shift(dev, D, f, c->seed, step, v, c->st.get()));
     scale = v;
     ++launches;
   }
-  CK(c, launch_gaussian_propose(c->coords, 0, c->N, D, form, scale, f, mv.mode, seq_dim, c->seed, step, c->qbuf, c->st));
+  CK(c, launch_gaussian_propose(c->coords.get(), 0, c->N, D, form, scale, f, mv.mode, seq_dim, c->seed, step,
+                                c->qbuf.get(), c->st.get()));
   HalfStepArgs a;
   fill_base_args(c, mv, a);
   a.order = nullptr;  // the active set is every walker, in walker order
@@ -1419,12 +1376,12 @@ int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step,
   a.i_lo = 0;
   a.i_hi = (int)c->N;
   a.range = nullptr;
-  a.qbuf = c->qbuf;
+  a.qbuf = c->qbuf.get();
   if (c->model.kind == MODEL_EXTERNAL) {
     ++launches;
     return callback_half_step(c, MOVE_PRECOMPUTED, a, launches);
   }
-  CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st));
+  CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st.get()));
   launches += 2;
   c->last_kernel = "gaussian";
   snprintf(c->last_variant, sizeof(c->last_variant), "gaussian");
@@ -1434,13 +1391,17 @@ int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step,
 // ---- user proposals (eb_move_set_proposal) ----------------------------------------------------------
 int ensure_user_scratch(eb_ctx* c, bool host) {
   const size_t N = (size_t)c->N, D = (size_t)c->D;
-  if (!c->qbuf) CK(c, cudaMalloc(&c->qbuf, N * D * sizeof(double)));
-  if (!c->up_x) CK(c, cudaMalloc(&c->up_x, N * D * sizeof(double)));
-  if (!c->up_f) CK(c, cudaMalloc(&c->up_f, N * sizeof(double)));
+  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, N * D * sizeof(double)));
+  if (!c->up_x) CK(c, dev_alloc(c->up_x, N * D * sizeof(double)));
+  if (!c->up_f) CK(c, dev_alloc(c->up_f, N * sizeof(double)));
   if (host && !c->up_hf) {
-    CK(c, cudaMallocHost(&c->up_hx, N * D * sizeof(double)));
-    CK(c, cudaMallocHost(&c->up_hq, N * D * sizeof(double)));
-    CK(c, cudaMallocHost(&c->up_hf, N * sizeof(double)));
+    HostPtr<double> hx, hq, hf;
+    CK(c, host_alloc(hx, N * D * sizeof(double)));
+    CK(c, host_alloc(hq, N * D * sizeof(double)));
+    CK(c, host_alloc(hf, N * sizeof(double)));
+    c->up_hx = std::move(hx);
+    c->up_hq = std::move(hq);
+    c->up_hf = std::move(hf);
   }
   return EB_OK;
 }
@@ -1453,56 +1414,58 @@ int user_proposal_call(eb_ctx* c, const eb_ctx::ProposalSlot& p, uint64_t step, 
   const bool host = p.where == EB_CALLBACK_HOST;
   // the function gets its own copy of the rows
   if (host)
-    CK(c, cudaMemcpyAsync(c->up_hx, rows, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  else if (rows != c->up_x)
-    CK(c, cudaMemcpyAsync(c->up_x, rows, N * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
+    CK(c, cudaMemcpyAsync(c->up_hx.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
+  else if (rows != c->up_x.get())
+    CK(c, cudaMemcpyAsync(c->up_x.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st.get()));
   // complete before fn runs (a device consumer may ignore the stream it is given)
-  CK(c, cudaStreamSynchronize(c->st));
-  const double* s = host ? c->up_hx : c->up_x;
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  const double* s = host ? c->up_hx.get() : c->up_x.get();
   const double* cset = nsets > 0 ? s + (size_t)ns * D : nullptr;
-  double* q = ns > 0 ? (host ? c->up_hq : c->qbuf) : nullptr;
-  double* f = ns > 0 ? (host ? c->up_hf : c->up_f) : nullptr;
+  double* q = ns > 0 ? (host ? c->up_hq.get() : c->qbuf.get()) : nullptr;
+  double* f = ns > 0 ? (host ? c->up_hf.get() : c->up_f.get()) : nullptr;
   c->up_m = ns;
   c->up_where = p.where;
   c->in_proposal = true;
   const int r = p.fn(p.user, step, (int32_t)split, s, ns > 0 ? ns : (int64_t)N, cset, nsets > 0 ? counts : nullptr,
-                     nsets, (int64_t)D, q, f, host ? nullptr : (void*)c->st);
+                     nsets, (int64_t)D, q, f, host ? nullptr : (void*)c->st.get());
   c->in_proposal = false;
   c->up_m = 0;
   if (r != 0) {
-    cudaStreamSynchronize(c->st);  // whatever the function enqueued before it failed
+    cudaStreamSynchronize(c->st.get());  // whatever the function enqueued before it failed
     FAIL(c, EB_ERR_CALLBACK, "the user proposal failed (returned %d)", r);
   }
   if (ns == 0) return EB_OK;
   if (host) {
-    CK(c, cudaMemcpyAsync(c->qbuf, c->up_hq, (size_t)ns * D * sizeof(double), cudaMemcpyHostToDevice, c->st));
-    CK(c, cudaMemcpyAsync(c->up_f, c->up_hf, (size_t)ns * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    CK(c, cudaMemcpyAsync(c->qbuf.get(), c->up_hq.get(), (size_t)ns * D * sizeof(double), cudaMemcpyHostToDevice,
+                          c->st.get()));
+    CK(c, cudaMemcpyAsync(c->up_f.get(), c->up_hf.get(), (size_t)ns * sizeof(double), cudaMemcpyHostToDevice,
+                          c->st.get()));
   }
   if (c->model.kind == MODEL_EXTERNAL) return EB_OK;  // run_callback scans the rows before the function sees them
   // ensemble.py:476-479: a non-finite proposal stops the call before any log-probability is evaluated
-  CK(c, launch_scan_nonfinite(c->qbuf, (size_t)ns * D, 0, c->status_dev, c->st));
+  CK(c, launch_scan_nonfinite(c->qbuf.get(), (size_t)ns * D, 0, c->status_dev.get(), c->st.get()));
   return fetch_status(c);
 }
 
 // step 6: the log-probability of qbuf's rows and the accept + update (kind EB_MOVE_USER / EB_MOVE_USER_MH)
 int user_accept(eb_ctx* c, int kind, const HalfStepArgs& a, uint64_t& launches) {
-  const ExternalBufs ext{c->qbuf, c->up_f, c->ext_lp};
+  const ExternalBufs ext{c->qbuf.get(), c->up_f.get(), c->ext_lp.get()};
   if (c->model.kind == MODEL_EXTERNAL) {
     c->cb_phase = CB_STEP;
-    int rc = run_callback(c, c->qbuf, (int64_t)a.i_hi - a.i_lo, c->ext_lp, true);
+    int rc = run_callback(c, c->qbuf.get(), (int64_t)a.i_hi - a.i_lo, c->ext_lp.get(), true);
     if (rc) return rc;
     if (kind == EB_MOVE_USER)
-      CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st));
+      CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st.get()));
     else
-      CK(c, launch_half_step_user(EB_MOVE_USER_MH, a, ext, c->st));
+      CK(c, launch_half_step_user(EB_MOVE_USER_MH, a, ext, c->st.get()));
     ++launches;
     if (c->blobs_live) {
-      CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop, c->blob_live,
-                               c->blob_bytes, c->st));
+      CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop.get(), c->blob_live.get(),
+                               c->blob_bytes, c->st.get()));
       ++launches;
     }
   } else {
-    CK(c, launch_half_step_user(kind, a, ext, c->st));
+    CK(c, launch_half_step_user(kind, a, ext, c->st.get()));
     ++launches;
   }
   return EB_OK;
@@ -1523,7 +1486,7 @@ int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
   if (rc) return rc;
   c->chain_ok = false;
   if (mv.mode == EB_USER_SETUP) {  // red_blue.py:73 setup(state.coords), once per step before the splits
-    rc = user_proposal_call(c, p, step, -1, c->coords, 0, nullptr, 0);
+    rc = user_proposal_call(c, p, step, -1, c->coords.get(), 0, nullptr, 0);
     if (rc) return rc;
   }
   const int P = mv.nsplits;
@@ -1533,7 +1496,7 @@ int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
   fill_base_args(c, mv, a);
   a.order = order;
   a.step = step;
-  a.qbuf = c->qbuf;
+  a.qbuf = c->qbuf.get();
   int64_t counts[MAX_SPLITS];
   for (int split = 0; split < P; ++split) {
     a.split = split;
@@ -1545,9 +1508,9 @@ int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t*
     int k = 0;
     for (int j = 0; j < P; ++j)
       if (j != split) counts[k++] = start[j + 1] - start[j];
-    CK(c, launch_split_gather(c->coords, order, c->N, c->D, a.a_start, a.a_count, c->up_x, c->st));
+    CK(c, launch_split_gather(c->coords.get(), order, c->N, c->D, a.a_start, a.a_count, c->up_x.get(), c->st.get()));
     ++launches;
-    rc = user_proposal_call(c, p, step, split, c->up_x, a.a_count, counts, P - 1);
+    rc = user_proposal_call(c, p, step, split, c->up_x.get(), a.a_count, counts, P - 1);
     if (rc) return rc;
     rc = user_accept(c, EB_MOVE_USER, a, launches);
     if (rc) return rc;
@@ -1572,8 +1535,8 @@ int launch_step_user_mh(eb_ctx* c, const eb_move& mv, uint64_t step, uint64_t& l
   a.i_lo = 0;
   a.i_hi = (int)c->N;
   a.range = nullptr;
-  a.qbuf = c->qbuf;
-  rc = user_proposal_call(c, p, step, 0, c->coords, c->N, nullptr, 0);
+  a.qbuf = c->qbuf.get();
+  rc = user_proposal_call(c, p, step, 0, c->coords.get(), c->N, nullptr, 0);
   if (rc) return rc;
   rc = user_accept(c, EB_MOVE_USER_MH, a, launches);
   if (rc) return rc;
@@ -1594,7 +1557,7 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
   if (grp.nhalf == 0) return EB_OK;
   HalfStepArgs a;
   fill_base_args(c, mv, a);
-  a.order = c->order;  // chunk base; HalfDesc::order_step selects the table
+  a.order = c->order.get();  // chunk base; HalfDesc::order_step selects the table
   a.range = c->comm.nranks > 1 ? c->comm.ranges : nullptr;
   int bound = grp.max_count;
   if (c->comm.nranks > 1 && c->comm.rows_per_rank < bound) bound = (int)c->comm.rows_per_rank;
@@ -1612,20 +1575,20 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
   // The predecessor ran only earlier splits of the same step, the last one being split - 1: they write only
   // their own active walkers, so this split's rows may be requested before the predecessor has finished.
   // Not across a step boundary (a randomised split can write any row), not sharded (peer GPUs write rows too).
-  const HalfDesc& d0 = c->descs_host[grp.first];
+  const HalfDesc& d0 = c->descs_host.get()[grp.first];
   a.dmma_early_own = pdl && c->comm.nranks == 1 && d0.split > 0 && c->dmma_first.step == d0.step &&
                      c->dmma_first.order_step == d0.order_step && c->dmma_last.step == d0.step &&
                      c->dmma_last.split == d0.split - 1;
   int grid = 0;
-  CK(c, launch_dense_dmma(a, c->descs_host[grp.first], c->descs_dev + grp.first, grp.nhalf, bound, c->gbar, c->gbar_count, c->sm_count, pdl,
-                          &grid, c->st));
+  CK(c, launch_dense_dmma(a, c->descs_host.get()[grp.first], c->descs_dev.get() + grp.first, grp.nhalf, bound,
+                          c->gbar.get(), c->gbar_count, c->sm_count, pdl, &grid, c->st.get()));
   c->gbar_count += (unsigned long long)(grp.nhalf - 1) * (unsigned long long)grid;
   c->last_kernel = "dense_dmma";
   c->dmma_nhalf_max = std::max(c->dmma_nhalf_max, grp.nhalf);
   snprintf(c->last_variant, sizeof(c->last_variant), "dense_dmma nhalf_max=%d grid=%d", c->dmma_nhalf_max, grid);
   c->chain_ok = grid > 0;
-  c->dmma_first = c->descs_host[grp.first];
-  c->dmma_last = c->descs_host[grp.first + grp.nhalf - 1];
+  c->dmma_first = c->descs_host.get()[grp.first];
+  c->dmma_last = c->descs_host.get()[grp.first + grp.nhalf - 1];
   ++launches;
   grp = DmmaGroup{};
   return EB_OK;
@@ -1645,11 +1608,11 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
   const bool perstep = c->l2_flush;  // flush L2 before every step, time each step on its own
   if (perstep) {
     if (nsteps > 16384) FAIL(c, EB_ERR_INVALID, "l2_flush mode times each step separately; use nsteps <= 16384");
-    if (!c->flush_buf) CK(c, cudaMalloc(&c->flush_buf, c->flush_bytes));
+    if (!c->flush_buf) CK(c, dev_alloc(c->flush_buf, c->flush_bytes));
     while (c->ev_pool.size() < 2 * nsteps) {
-      cudaEvent_t e;
-      CK(c, cudaEventCreate(&e));
-      c->ev_pool.push_back(e);
+      EventPtr e;
+      CK(c, event_create(e));
+      c->ev_pool.push_back(std::move(e));
     }
   }
   if (c->trace_every > 0) {
@@ -1658,8 +1621,8 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
   }
   c->chain_ok = false;
   c->dmma_nhalf_max = 0;
-  CK(c, cudaEventRecord(c->ev0, c->st));
-  if (comm_begin(c->comm, c->st, c->status_dev, launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
+  CK(c, cudaEventRecord(c->ev0.get(), c->st.get()));
+  if (comm_begin(c->comm, c->st.get(), c->status_dev.get(), launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   c->fused_last = false;
   const bool multi = c->comm.nranks > 1;
   // sharded ensembles run one half-step per launch: NCCL exchanges whole row blocks after every split, and the
@@ -1672,13 +1635,13 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
   while (done < nsteps) {
     const size_t chunk = (size_t)std::min<uint64_t>(nsteps - done, c->table_cap);
     pick.resize(chunk);
-    CK(c, cudaStreamSynchronize(c->st));  // info_host / descs_host are reused per chunk
+    CK(c, cudaStreamSynchronize(c->st.get()));  // info_host / descs_host are reused per chunk
     size_t ndesc = 0;
     for (size_t k = 0; k < chunk; ++k) {
       pick[k] = choose_move(c, s, c->step + k);
       const eb_move& mv = s.moves[pick[k]];
-      c->info_host[k].nsplits = mv.nsplits;
-      c->info_host[k].randomize = mv.randomize_split;
+      c->info_host.get()[k].nsplits = mv.nsplits;
+      c->info_host.get()[k].randomize = mv.randomize_split;
     }
     // Split tables depend only on (seed, step, nsplits, randomize): reuse the ones already on the
     // device when they cover this chunk, else build them -- looking ahead with the same schedule, so
@@ -1689,21 +1652,21 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
     if (hit) {
       off = (size_t)(c->step - c->tbl_step0);
       for (size_t k = 0; k < chunk && hit; ++k)
-        hit = c->tbl_info[off + k].nsplits == c->info_host[k].nsplits &&
-              c->tbl_info[off + k].randomize == c->info_host[k].randomize;
+        hit = c->tbl_info[off + k].nsplits == c->info_host.get()[k].nsplits &&
+              c->tbl_info[off + k].randomize == c->info_host.get()[k].randomize;
     }
     if (!hit) {
       off = 0;
       build = std::min<size_t>(c->table_cap, std::max<size_t>(chunk, 64));
       for (size_t k = chunk; k < build; ++k) {
         const eb_move& mv = s.moves[choose_move(c, s, c->step + k)];
-        c->info_host[k].nsplits = mv.nsplits;
-        c->info_host[k].randomize = mv.randomize_split;
+        c->info_host.get()[k].nsplits = mv.nsplits;
+        c->info_host.get()[k].randomize = mv.randomize_split;
       }
       c->tbl_seed = c->seed;
       c->tbl_step0 = c->step;
       c->tbl_n = build;
-      c->tbl_info.assign(c->info_host, c->info_host + build);
+      c->tbl_info.assign(c->info_host.get(), c->info_host.get() + build);
     }
     for (size_t k = 0; k < chunk; ++k) {
       const eb_move& mv = s.moves[pick[k]];
@@ -1711,7 +1674,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         int start[MAX_SPLITS + 1];
         split_starts(c->N, mv.nsplits, start);
         for (int split = 0; split < mv.nsplits; ++split) {
-          HalfDesc& d = c->descs_host[ndesc++];
+          HalfDesc& d = c->descs_host.get()[ndesc++];
           d.step = c->step + k;
           d.order_step = (int32_t)(off + k);
           d.split = split;
@@ -1726,27 +1689,29 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
     for (size_t k = 0; k < chunk; ++k) {
       const eb_move& mv = s.moves[pick[k]];
       if (perstep) {
-        CK(c, cudaMemsetAsync(c->flush_buf, (int)(k & 0xff), c->flush_bytes, c->st));
-        CK(c, cudaEventRecord(c->ev_pool[2 * (done + k)], c->st));
+        CK(c, cudaMemsetAsync(c->flush_buf.get(), (int)(k & 0xff), c->flush_bytes, c->st.get()));
+        CK(c, cudaEventRecord(c->ev_pool[2 * (done + k)].get(), c->st.get()));
         c->chain_ok = false;
       }
       if (k == 0) {
         // dense_dmma descriptors of the chunk and, when needed, the split tables (charged to this step)
         if (ndesc) {
-          CK(c, cudaMemcpyAsync(c->descs_dev, c->descs_host, ndesc * sizeof(HalfDesc), cudaMemcpyHostToDevice, c->st));
+          CK(c, cudaMemcpyAsync(c->descs_dev.get(), c->descs_host.get(), ndesc * sizeof(HalfDesc),
+                                cudaMemcpyHostToDevice, c->st.get()));
           c->chain_ok = false;
         }
         if (build) {
-          CK(c, cudaMemcpyAsync(c->info_dev, c->info_host, build * sizeof(StepInfo), cudaMemcpyHostToDevice, c->st));
+          CK(c, cudaMemcpyAsync(c->info_dev.get(), c->info_host.get(), build * sizeof(StepInfo), cudaMemcpyHostToDevice,
+                                c->st.get()));
           const Comm& cm = c->comm;
-          CK(c, launch_split_tables(c->order, c->info_dev, (int)build, c->N, c->seed, c->step,
+          CK(c, launch_split_tables(c->order.get(), c->info_dev.get(), (int)build, c->N, c->seed, c->step,
                                     cm.rows_per_rank * cm.rank, cm.rows_per_rank * (cm.rank + 1),
-                                    cm.nranks > 1 ? cm.ranges : nullptr, c->st));
+                                    cm.nranks > 1 ? cm.ranges : nullptr, c->st.get()));
           ++launches;
           if (cm.nranks > 1 && cm.aperm) {
             // front group = one tile (8 walkers) for each of the 8 consumer warps of every SM: the first round
-            CK(c, launch_locality_tables(c->order, c->info_dev, cm.ranges, (int)build, c->N, c->seed, c->step,
-                                         cm.rows_per_rank, cm.rank, 64 * c->sm_count, cm.aperm, c->st));
+            CK(c, launch_locality_tables(c->order.get(), c->info_dev.get(), cm.ranges, (int)build, c->N, c->seed,
+                                         c->step, cm.rows_per_rank, cm.rank, 64 * c->sm_count, cm.aperm, c->st.get()));
             ++launches;
           }
           c->chain_ok = false;
@@ -1762,7 +1727,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         }
         grp_move = &mv;
         for (int split = 0; split < mv.nsplits; ++split) {
-          const HalfDesc& d = c->descs_host[desc_cursor];
+          const HalfDesc& d = c->descs_host.get()[desc_cursor];
           if (grp.nhalf == 0) grp.first = desc_cursor;
           grp.nhalf += 1;
           grp.max_count = std::max(grp.max_count, (int)d.a_count);
@@ -1772,7 +1737,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
             if (rc) return rc;
             if (exchange_each) {
               c->chain_ok = false;
-              if (comm_after_split(c->comm, c->st, c->status_dev, launches))
+              if (comm_after_split(c->comm, c->st.get(), c->status_dev.get(), launches))
                 FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
             }
           }
@@ -1792,15 +1757,15 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
           if (rc) return rc;
         }
         if (mv.kind == EB_MOVE_WALK)
-          rc = launch_step_walk(c, mv, c->step, c->order + (off + k) * (size_t)c->N, launches);
+          rc = launch_step_walk(c, mv, c->step, c->order.get() + (off + k) * (size_t)c->N, launches);
         else if (mv.kind == EB_MOVE_GAUSSIAN)
           rc = launch_step_gaussian(c, s, pick[k], c->step, launches);
         else if (mv.kind == EB_MOVE_USER)
-          rc = launch_step_user(c, mv, c->step, c->order + (off + k) * (size_t)c->N, launches);
+          rc = launch_step_user(c, mv, c->step, c->order.get() + (off + k) * (size_t)c->N, launches);
         else if (mv.kind == EB_MOVE_USER_MH)
           rc = launch_step_user_mh(c, mv, c->step, launches);
         else
-          rc = launch_step_generic(c, mv, c->step, c->order + (off + k) * (size_t)c->N, off + k, launches);
+          rc = launch_step_generic(c, mv, c->step, c->order.get() + (off + k) * (size_t)c->N, off + k, launches);
         if (rc) return rc;
       }
       c->picks[pick[k]] += 1;
@@ -1818,7 +1783,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         if (rc) return rc;
       }
       if (perstep) {
-        CK(c, cudaEventRecord(c->ev_pool[2 * (done + k) + 1], c->st));
+        CK(c, cudaEventRecord(c->ev_pool[2 * (done + k) + 1].get(), c->st.get()));
         c->chain_ok = false;
       }
       rc = after_step(done + k);
@@ -1826,23 +1791,23 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
     }
     done += chunk;
   }
-  CK(c, cudaEventRecord(c->ev1, c->st));
+  CK(c, cudaEventRecord(c->ev1.get(), c->st.get()));
   c->chain_ok = false;
   // multi-GPU: the rows of other ranks are NOT replicated here; collective readers (eb_get_state,
   // eb_get_naccepted, the accept mask of eb_step) do that on demand, sharded readers never need it
   if (multi) c->replicas_dirty = true;
-  CK(c, cudaMemcpyAsync(c->status_host, c->status_dev, sizeof(int), cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   float ms = 0.f;
   if (perstep) {
     double tot = 0.0;
     for (uint64_t k = 0; k < nsteps; ++k) {
-      CK(c, cudaEventElapsedTime(&ms, c->ev_pool[2 * k], c->ev_pool[2 * k + 1]));
+      CK(c, cudaEventElapsedTime(&ms, c->ev_pool[2 * k].get(), c->ev_pool[2 * k + 1].get()));
       tot += ms;
     }
     c->last_ms = tot;
   } else {
-    CK(c, cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+    CK(c, cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
     c->last_ms = ms;
   }
   c->last_launches = launches;
@@ -1855,15 +1820,19 @@ int moments_config(eb_ctx* c, uint64_t every) {
   if (every > 0 && c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "chain moments are limited to ndim <= 1024");
   const size_t n = (size_t)c->D + (size_t)c->D * c->D;
   if (every > 0 && !c->mom_acc) {
-    CK(c, cudaMalloc(&c->mom_acc, n * sizeof(double)));
-    CK(c, cudaMalloc(&c->mom_shift, (size_t)c->D * sizeof(double)));
-    if (!c->mom_partial) CK(c, cudaMalloc(&c->mom_partial, moments_partial_bytes(c->D, c->sm_count)));
+    DevPtr<double> acc, shift, partial;
+    CK(c, dev_alloc(acc, n * sizeof(double)));
+    CK(c, dev_alloc(shift, (size_t)c->D * sizeof(double)));
+    if (!c->mom_partial) CK(c, dev_alloc(partial, moments_partial_bytes(c->D, c->sm_count)));
+    c->mom_acc = std::move(acc);
+    c->mom_shift = std::move(shift);
+    if (partial) c->mom_partial = std::move(partial);
   }
-  if (c->mom_acc) CK(c, cudaMemsetAsync(c->mom_acc, 0, n * sizeof(double), c->st));
+  if (c->mom_acc) CK(c, cudaMemsetAsync(c->mom_acc.get(), 0, n * sizeof(double), c->st.get()));
   c->mom_count = 0;
   c->mom_have_shift = false;
   c->moments_every = every;
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
 
@@ -1871,15 +1840,16 @@ int moments_config(eb_ctx* c, uint64_t every) {
 int accumulate_moments(eb_ctx* c, uint64_t& launches) {
   int64_t r0, r1;
   owned_rows(c, r0, r1);
-  const double* X = c->coords + (size_t)r0 * c->D;
+  const double* X = c->coords.get() + (size_t)r0 * c->D;
   c->chain_ok = false;
   if (!c->mom_have_shift) {
     // shift = the ensemble mean at the first accumulation: keeps the raw second moments well conditioned
-    CK(c, launch_colmean(X, r1 - r0, c->D, c->mom_shift, nullptr, c->st));
+    CK(c, launch_colmean(X, r1 - r0, c->D, c->mom_shift.get(), nullptr, c->st.get()));
     c->mom_have_shift = true;
     ++launches;
   }
-  CK(c, launch_moments(X, r1 - r0, c->D, c->mom_shift, c->mom_partial, c->mom_acc, c->sm_count, c->st));
+  CK(c, launch_moments(X, r1 - r0, c->D, c->mom_shift.get(), c->mom_partial.get(), c->mom_acc.get(), c->sm_count,
+                       c->st.get()));
   launches += 2;
   c->mom_count += (unsigned long long)(r1 - r0);
   return EB_OK;
@@ -1888,7 +1858,7 @@ int accumulate_moments(eb_ctx* c, uint64_t& launches) {
 // count the CURRENT state into the running histograms (kernels only, enqueued on the stream)
 int accumulate_histograms(eb_ctx* c, uint64_t& launches) {
   c->chain_ok = false;
-  CK(c, live_hist_launch(c->hist, c->st, launches));
+  CK(c, live_hist_launch(c->hist, c->st.get(), launches));
   c->hist_count += (unsigned long long)c->N;
   return EB_OK;
 }
@@ -1907,17 +1877,13 @@ int reserve_trace(eb_ctx* c, uint64_t nsteps) {
   if (cap > free_b / row)
     FAIL(c, EB_ERR_NOMEM, "the trace needs room for %llu rows of %zu bytes, %zu bytes free", (unsigned long long)need,
          row, free_b);
-  double* rows = nullptr;
-  const cudaError_t e = cudaMalloc(&rows, (size_t)cap * row);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    FAIL(c, EB_ERR_NOMEM, "the trace: allocating %llu rows of %zu bytes failed (%s)", (unsigned long long)cap, row,
-         cudaGetErrorString(e));
-  }
-  if (have) CK(c, cudaMemcpyAsync(rows, c->trace_rows, (size_t)have * row, cudaMemcpyDeviceToDevice, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
-  CK(c, cudaFree(c->trace_rows));
-  c->trace_rows = rows;
+  DevPtr<double> rows;
+  CK_NOMEM(c, dev_alloc(rows, (size_t)cap * row), "the trace: allocating %llu rows of %zu bytes failed (%s)",
+           (unsigned long long)cap, row, cudaGetErrorString(alloc_err));
+  if (have)
+    CK(c, cudaMemcpyAsync(rows.get(), c->trace_rows.get(), (size_t)have * row, cudaMemcpyDeviceToDevice, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  c->trace_rows = std::move(rows);
   c->trace_cap = cap;
   c->trace_steps.reserve((size_t)cap);
   return EB_OK;
@@ -1926,8 +1892,8 @@ int reserve_trace(eb_ctx* c, uint64_t nsteps) {
 // record the CURRENT state as one row of the trace (kernels only, enqueued on the stream)
 int accumulate_trace(eb_ctx* c, uint64_t& launches) {
   c->chain_ok = false;
-  double* row = c->trace_rows + c->trace_steps.size() * (2 * (size_t)c->D + TRACE_EXTRA);
-  CK(c, live_trace_launch(c->trace, row, c->step, c->st, launches));
+  double* row = c->trace_rows.get() + c->trace_steps.size() * (2 * (size_t)c->D + TRACE_EXTRA);
+  CK(c, live_trace_launch(c->trace, row, c->step, c->st.get(), launches));
   c->trace_steps.push_back(c->step);
   return EB_OK;
 }
@@ -1958,8 +1924,8 @@ int eb_step(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uin
   if (accepted_last) {
     rc = sync_replicas(c);  // multi-GPU: the mask of every rank's rows (collective)
     if (rc) return rc;
-    CK(c, cudaMemcpyAsync(accepted_last, c->accepted, (size_t)c->N, cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaStreamSynchronize(c->st));
+    CK(c, cudaMemcpyAsync(accepted_last, c->accepted.get(), (size_t)c->N, cudaMemcpyDeviceToHost, c->st.get()));
+    CK(c, cudaStreamSynchronize(c->st.get()));
   }
   return EB_OK;
 }
@@ -1984,20 +1950,22 @@ int eb_step_store_blobs(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
   const size_t N = (size_t)c->N, D = (size_t)c->D;
   const size_t row = N * D + N;  // coords then log_prob, staged together
   for (int k = 0; k < 2; ++k) {
-    if (!c->stage[k]) {
-      CK(c, cudaMallocHost(&c->stage[k], row * sizeof(double)));
-      CK(c, cudaMallocHost(&c->stage_acc[k], N));
-      CK(c, cudaEventCreateWithFlags(&c->stage_ev[k], cudaEventDisableTiming));
-    }
+    if (c->stage[k]) continue;
+    HostPtr<double> x;
+    HostPtr<uint8_t> acc;
+    EventPtr ev;
+    CK(c, host_alloc(x, row * sizeof(double)));
+    CK(c, host_alloc(acc, N));
+    CK(c, event_create(ev, cudaEventDisableTiming));
+    c->stage[k] = std::move(x);
+    c->stage_acc[k] = std::move(acc);
+    c->stage_ev[k] = std::move(ev);
   }
   const size_t blob_row = blobs ? N * c->blob_bytes : 0;  // the blob records of a stored step, staged beside them
   if (blob_row > c->stage_blob_cap) {
-    for (int k = 0; k < 2; ++k) {
-      cudaFreeHost(c->stage_blob[k]);
-      c->stage_blob[k] = nullptr;
-    }
+    for (HostPtr<uint8_t>& b : c->stage_blob) b.reset();
     c->stage_blob_cap = 0;
-    for (int k = 0; k < 2; ++k) CK(c, cudaMallocHost(&c->stage_blob[k], blob_row));
+    for (HostPtr<uint8_t>& b : c->stage_blob) CK(c, host_alloc(b, blob_row));
     c->stage_blob_cap = blob_row;
   }
   uint8_t* blob_out = static_cast<uint8_t*>(blobs);
@@ -2007,13 +1975,13 @@ int eb_step_store_blobs(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
   int64_t pending[2] = {-1, -1};
   auto drain = [&](int slot) -> int {
     if (pending[slot] < 0) return EB_OK;
-    CK(c, cudaEventSynchronize(c->stage_ev[slot]));
+    CK(c, cudaEventSynchronize(c->stage_ev[slot].get()));
     const size_t k = (size_t)pending[slot];
-    memcpy(chain + k * N * D, c->stage[slot], N * D * sizeof(double));          // backend.py:224
-    memcpy(log_prob + k * N, c->stage[slot] + N * D, N * sizeof(double));        // backend.py:225
-    if (blob_out) memcpy(blob_out + k * blob_row, c->stage_blob[slot], blob_row);  // backend.py:226-227
+    memcpy(chain + k * N * D, c->stage[slot].get(), N * D * sizeof(double));          // backend.py:224
+    memcpy(log_prob + k * N, c->stage[slot].get() + N * D, N * sizeof(double));        // backend.py:225
+    if (blob_out) memcpy(blob_out + k * blob_row, c->stage_blob[slot].get(), blob_row);  // backend.py:226-227
     if (accepted)
-      for (size_t w = 0; w < N; ++w) accepted[w] += (double)c->stage_acc[slot][w];  // backend.py:229
+      for (size_t w = 0; w < N; ++w) accepted[w] += (double)c->stage_acc[slot].get()[w];  // backend.py:229
     pending[slot] = -1;
     return EB_OK;
   };
@@ -2027,15 +1995,18 @@ int eb_step_store_blobs(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
       // a stored step holds EVERY walker: replicate the other ranks' rows (log_prob, accept mask and, in
       // P2P mode, coords) before the copy -- the in-run exchange only moves what the kernels need
       uint64_t l = 0;
-      if (comm_sync_state(c->comm, c->st, c->status_dev, c->logp, c->accepted, nullptr, l))
+      if (comm_sync_state(c->comm, c->st.get(), c->status_dev.get(), c->logp.get(), c->accepted.get(), nullptr, l))
         FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
       c->fused_last = false;
     }
-    CK(c, cudaMemcpyAsync(c->stage[slot], c->coords, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaMemcpyAsync(c->stage[slot] + N * D, c->logp, N * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaMemcpyAsync(c->stage_acc[slot], c->accepted, N, cudaMemcpyDeviceToHost, c->st));
-    if (blob_out) CK(c, cudaMemcpyAsync(c->stage_blob[slot], c->blob_live, blob_row, cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaEventRecord(c->stage_ev[slot], c->st));
+    CK(c, cudaMemcpyAsync(c->stage[slot].get(), c->coords.get(), N * D * sizeof(double), cudaMemcpyDeviceToHost,
+                          c->st.get()));
+    CK(c, cudaMemcpyAsync(c->stage[slot].get() + N * D, c->logp.get(), N * sizeof(double), cudaMemcpyDeviceToHost,
+                          c->st.get()));
+    CK(c, cudaMemcpyAsync(c->stage_acc[slot].get(), c->accepted.get(), N, cudaMemcpyDeviceToHost, c->st.get()));
+    if (blob_out) CK(c, cudaMemcpyAsync(c->stage_blob[slot].get(), c->blob_live.get(), blob_row, cudaMemcpyDeviceToHost,
+                                        c->st.get()));
+    CK(c, cudaEventRecord(c->stage_ev[slot].get(), c->st.get()));
     pending[slot] = (int64_t)stored;
     ++stored;
     return EB_OK;
@@ -2081,41 +2052,23 @@ int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, s
   const int M = acf_fft_length(n_t);
   const size_t wb = acf_slab_walkers(n_t, nw, nd);  // slab of walkers sized to ~1 GiB of scratch
   const size_t S = wb * nd;
-  double *xin = nullptr, *mean = nullptr, *f = nullptr;
-  double2 *z = nullptr, *tw = nullptr;
-  auto release = [&]() {
-    cudaFree(xin);
-    cudaFree(mean);
-    cudaFree(f);
-    cudaFree(z);
-    cudaFree(tw);
-  };
-#define AC(call)                                                                             \
-  do {                                                                                       \
-    cudaError_t _e = (call);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      cudaGetLastError();                                                                    \
-      release();                                                                             \
-      FAIL(c, EB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
-    }                                                                                        \
-  } while (0)
-  AC(cudaMalloc(&xin, n_t * S * sizeof(double)));
-  AC(cudaMalloc(&mean, S * sizeof(double)));
-  AC(cudaMalloc(&f, nd * n_t * sizeof(double)));
-  AC(cudaMalloc(&z, S * (size_t)M * sizeof(double2)));
-  AC(cudaMalloc(&tw, (size_t)std::max(1, M / 2) * sizeof(double2)));
-  AC(cudaMemsetAsync(f, 0, nd * n_t * sizeof(double), st));
-  AC(launch_acf_twiddles(tw, M, st));
+  DevPtr<double> xin, mean, f;
+  DevPtr<double2> z, tw;
+  CK(c, dev_alloc(xin, n_t * S * sizeof(double)));
+  CK(c, dev_alloc(mean, S * sizeof(double)));
+  CK(c, dev_alloc(f, nd * n_t * sizeof(double)));
+  CK(c, dev_alloc(z, S * (size_t)M * sizeof(double2)));
+  CK(c, dev_alloc(tw, (size_t)std::max(1, M / 2) * sizeof(double2)));
+  CK(c, cudaMemsetAsync(f.get(), 0, nd * n_t * sizeof(double), st));
+  CK(c, launch_acf_twiddles(tw.get(), M, st));
   for (size_t w0 = 0; w0 < nw; w0 += wb) {
     const size_t wn = std::min(wb, nw - w0);
-    AC(fill(xin, w0, wn));
-    AC(launch_acf_slab(xin, (int)n_t, (int)wn, (int)nd, M, tw, z, mean, f, st));
+    CK(c, fill(xin.get(), w0, wn));
+    CK(c, launch_acf_slab(xin.get(), (int)n_t, (int)wn, (int)nd, M, tw.get(), z.get(), mean.get(), f.get(), st));
   }
-  AC(launch_acf_scale(f, nd * n_t, 1.0 / (double)nw, st));  // autocorr.py:106  f /= n_w
-  AC(cudaMemcpyAsync(acf, f, nd * n_t * sizeof(double), cudaMemcpyDeviceToHost, st));
-  AC(cudaStreamSynchronize(st));
-#undef AC
-  release();
+  CK(c, launch_acf_scale(f.get(), nd * n_t, 1.0 / (double)nw, st));  // autocorr.py:106  f /= n_w
+  CK(c, cudaMemcpyAsync(acf, f.get(), nd * n_t * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(c, cudaStreamSynchronize(st));
   return EB_OK;
 }
 
@@ -2144,25 +2097,20 @@ std::vector<const double*> chain_slot_table(eb_chain* ch, bool coords, uint64_t 
   for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
                      [&](size_t s, uint64_t off, uint64_t, uint64_t n) {
                        for (uint64_t j = 0; j < n; ++j)
-                         t.push_back(coords ? ch->segs[s].x + (off + j * stride) * ch->xs
-                                            : ch->segs[s].lp + (off + j * stride) * ch->ls);
+                         t.push_back(coords ? ch->segs[s].x.get() + (off + j * stride) * ch->xs
+                                            : ch->segs[s].lp.get() + (off + j * stride) * ch->ls);
                      });
   return t;
 }
 
 // scratch of `bytes` on the chain's device, refused before the allocation when it cannot fit
-int chain_scratch(eb_chain* ch, const char* who, size_t bytes, void** out) {
-  *out = nullptr;
+int chain_scratch(eb_chain* ch, const char* who, size_t bytes, DevPtr<void>& out) {
   size_t free_b = 0, total_b = 0;
   CK(ch, cudaMemGetInfo(&free_b, &total_b));
   if (bytes > free_b)
     FAIL(ch, EB_ERR_NOMEM, "%s: %zu bytes of scratch, %zu bytes free", who, bytes, free_b);
-  const cudaError_t e = cudaMalloc(out, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    *out = nullptr;
-    FAIL(ch, EB_ERR_NOMEM, "%s: allocating %zu bytes of scratch failed (%s)", who, bytes, cudaGetErrorString(e));
-  }
+  CK_NOMEM(ch, dev_alloc(out, bytes), "%s: allocating %zu bytes of scratch failed (%s)", who, bytes,
+           cudaGetErrorString(alloc_err));
   return EB_OK;
 }
 
@@ -2202,8 +2150,9 @@ int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
     while (slot >= ch->start[seg + 1]) ++seg;
     const uint64_t off = slot - ch->start[seg];
     c->chain_ok = false;
-    CK(c, launch_chain_store(c->coords, c->logp, c->accepted, ch->segs[seg].x + off * ch->xs,
-                             ch->segs[seg].lp + off * ch->ls, ch->accepted, nx, (size_t)c->N, c->N, c->sm_count, c->st));
+    CK(c, launch_chain_store(c->coords.get(), c->logp.get(), c->accepted.get(), ch->segs[seg].x.get() + off * ch->xs,
+                             ch->segs[seg].lp.get() + off * ch->ls, ch->accepted.get(), nx, (size_t)c->N, c->N,
+                             c->sm_count, c->st.get()));
     ++slot;
     return EB_OK;
   });
@@ -2214,68 +2163,35 @@ const char* eb_chain_last_error(const eb_chain* ch) { return ch ? ch->err.c_str(
 int eb_chain_create(int device, int64_t nwalkers, int64_t ndim, eb_chain** out) {
   if (!out) return EB_ERR_INVALID;
   *out = nullptr;
-  if (nwalkers < 2 || ndim < 1 || nwalkers > (int64_t)0x7fffffff || ndim > 16384) {
-    g_create_err = "eb_chain_create: need 2 <= nwalkers < 2^31 and 1 <= ndim <= 16384";
-    return EB_ERR_INVALID;
-  }
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    g_create_err = std::string("eb_chain_create: no CUDA device (") + cudaGetErrorString(e) +
-                   "); this engine has no CPU fallback";
-    return EB_ERR_CUDA;
-  }
-  if (device < 0 || device >= ndev) {
-    g_create_err = "eb_chain_create: device index out of range";
-    return EB_ERR_INVALID;
-  }
-  eb_chain* ch = new eb_chain();
+  const int rc = check_create_args("eb_chain_create", device, nwalkers, ndim);
+  if (rc) return rc;
+  std::unique_ptr<eb_chain> ch(new eb_chain());
   ch->device = device;
   ch->N = nwalkers;
   ch->D = (int)ndim;
   ch->xs = ((size_t)nwalkers * (size_t)ndim + 1) & ~(size_t)1;
   ch->ls = ((size_t)nwalkers + 1) & ~(size_t)1;
-  auto fail = [&](const char* what, cudaError_t err) {
-    g_create_err = std::string("eb_chain_create: ") + what + ": " + cudaGetErrorString(err);
-    cudaGetLastError();
-    eb_chain_destroy(ch);
-    return EB_ERR_CUDA;
-  };
-#define CC(call)                                   \
-  do {                                             \
-    cudaError_t _e = (call);                       \
-    if (_e != cudaSuccess) return fail(#call, _e); \
-  } while (0)
-  CC(cudaSetDevice(device));
+  CREATE_CK(cudaSetDevice(device));
   int v = 0;
-  CC(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device));
+  CREATE_CK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device));
   ch->sm_count = v;
-  CC(cudaDeviceGetAttribute(&v, cudaDevAttrMaxPitch, device));
+  CREATE_CK(cudaDeviceGetAttribute(&v, cudaDevAttrMaxPitch, device));
   ch->max_pitch = (size_t)v;
-  CC(cudaStreamCreateWithFlags(&ch->st, cudaStreamNonBlocking));
-  CC(cudaMalloc(&ch->accepted, (size_t)nwalkers * sizeof(double)));
-  CC(cudaMalloc(&ch->mask, (size_t)nwalkers));
-  CC(cudaMemsetAsync(ch->accepted, 0, (size_t)nwalkers * sizeof(double), ch->st));
-  CC(cudaStreamSynchronize(ch->st));
-#undef CC
-  *out = ch;
+  CREATE_CK(stream_create(ch->st, cudaStreamNonBlocking));
+  CREATE_CK(dev_alloc(ch->accepted, (size_t)nwalkers * sizeof(double)));
+  CREATE_CK(dev_alloc(ch->mask, (size_t)nwalkers));
+  CREATE_CK(cudaMemsetAsync(ch->accepted.get(), 0, (size_t)nwalkers * sizeof(double), ch->st.get()));
+  CREATE_CK(cudaStreamSynchronize(ch->st.get()));
+  *out = ch.release();
   return EB_OK;
 }
 
 int eb_chain_destroy(eb_chain* ch) {
   if (!ch) return EB_OK;
   cudaSetDevice(ch->device);
-  if (ch->st) cudaStreamSynchronize(ch->st);
-  for (ChainSeg& s : ch->segs) {
-    cudaFree(s.x);
-    cudaFree(s.lp);
-  }
-  cudaFree(ch->accepted);
-  cudaFree(ch->mask);
-  if (ch->st) cudaStreamDestroy(ch->st);
+  cudaStreamSynchronize(ch->st.get());
+  delete ch;  // the owners release the segments and buffers, then the stream
   cudaGetLastError();
-  delete ch;
   return EB_OK;
 }
 
@@ -2293,16 +2209,15 @@ int eb_chain_grow(eb_chain* ch, uint64_t nslots) {
          "eb_chain_grow: %llu more slots need %.0f bytes, more than the device's %zu bytes in total (%zu free)",
          (unsigned long long)add, (double)add * (double)per_slot, total_b, free_b);
   ChainSeg seg;
-  cudaError_t e = cudaMalloc(&seg.x, add * ch->xs * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&seg.lp, add * ch->ls * sizeof(double));
-  if (e != cudaSuccess) {  // the chain stays as it was
-    cudaGetLastError();
-    cudaFree(seg.x);
+  cudaError_t e = dev_alloc(seg.x, add * ch->xs * sizeof(double));
+  if (e == cudaSuccess) e = dev_alloc(seg.lp, add * ch->ls * sizeof(double));
+  if (e != cudaSuccess) {  // the chain stays as it was; the free bytes are counted without the half-made segment
+    seg = ChainSeg{};
     cudaMemGetInfo(&free_b, &total_b);
-    FAIL(ch, EB_ERR_NOMEM, "eb_chain_grow: %llu more slots need %zu bytes, %zu bytes free (%s)",
-         (unsigned long long)add, (size_t)add * per_slot, free_b, cudaGetErrorString(e));
   }
-  ch->segs.push_back(seg);
+  CK_NOMEM(ch, e, "eb_chain_grow: %llu more slots need %zu bytes, %zu bytes free (%s)", (unsigned long long)add,
+           (size_t)add * per_slot, free_b, cudaGetErrorString(alloc_err));
+  ch->segs.push_back(std::move(seg));
   ch->start.push_back(nslots);
   return EB_OK;
 }
@@ -2325,15 +2240,16 @@ int eb_chain_write(eb_chain* ch, uint64_t slot, const double* coords, const doub
   const size_t s = (size_t)(std::upper_bound(ch->start.begin(), ch->start.end(), slot) - ch->start.begin()) - 1;
   const uint64_t off = slot - ch->start[s];
   const size_t N = (size_t)ch->N;
-  CK(ch, cudaMemcpyAsync(ch->segs[s].x + off * ch->xs, coords, N * ch->D * sizeof(double), cudaMemcpyHostToDevice,
-                         ch->st));
-  CK(ch, cudaMemcpyAsync(ch->segs[s].lp + off * ch->ls, log_prob, N * sizeof(double), cudaMemcpyHostToDevice, ch->st));
+  CK(ch, cudaMemcpyAsync(ch->segs[s].x.get() + off * ch->xs, coords, N * ch->D * sizeof(double), cudaMemcpyHostToDevice,
+                         ch->st.get()));
+  CK(ch, cudaMemcpyAsync(ch->segs[s].lp.get() + off * ch->ls, log_prob, N * sizeof(double), cudaMemcpyHostToDevice,
+                         ch->st.get()));
   if (accepted) {
-    CK(ch, cudaMemcpyAsync(ch->mask, accepted, N, cudaMemcpyHostToDevice, ch->st));
-    CK(ch, launch_chain_store(nullptr, nullptr, ch->mask, nullptr, nullptr, ch->accepted, 0, 0, ch->N, ch->sm_count,
-                              ch->st));
+    CK(ch, cudaMemcpyAsync(ch->mask.get(), accepted, N, cudaMemcpyHostToDevice, ch->st.get()));
+    CK(ch, launch_chain_store(nullptr, nullptr, ch->mask.get(), nullptr, nullptr, ch->accepted.get(), 0, 0, ch->N,
+                              ch->sm_count, ch->st.get()));
   }
-  CK(ch, cudaStreamSynchronize(ch->st));
+  CK(ch, cudaStreamSynchronize(ch->st.get()));
   return EB_OK;
 }
 
@@ -2347,24 +2263,25 @@ int eb_chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count,
   for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
                      [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
                        if (coords && e == cudaSuccess)
-                         e = copy_rows(coords + k0 * nx, nx * sizeof(double), ch->segs[s].x + off * ch->xs,
+                         e = copy_rows(coords + k0 * nx, nx * sizeof(double), ch->segs[s].x.get() + off * ch->xs,
                                        stride * ch->xs * sizeof(double), nx * sizeof(double), n,
-                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st);
+                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st.get());
                        if (log_prob && e == cudaSuccess)
-                         e = copy_rows(log_prob + k0 * N, N * sizeof(double), ch->segs[s].lp + off * ch->ls,
+                         e = copy_rows(log_prob + k0 * N, N * sizeof(double), ch->segs[s].lp.get() + off * ch->ls,
                                        stride * ch->ls * sizeof(double), N * sizeof(double), n,
-                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st);
+                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st.get());
                      });
   CK(ch, e);
-  CK(ch, cudaStreamSynchronize(ch->st));
+  CK(ch, cudaStreamSynchronize(ch->st.get()));
   return EB_OK;
 }
 
 int eb_chain_accepted(eb_chain* ch, double* accepted) {
   if (!ch || !accepted) return EB_ERR_INVALID;
   CK(ch, cudaSetDevice(ch->device));
-  CK(ch, cudaMemcpyAsync(accepted, ch->accepted, (size_t)ch->N * sizeof(double), cudaMemcpyDeviceToHost, ch->st));
-  CK(ch, cudaStreamSynchronize(ch->st));
+  CK(ch, cudaMemcpyAsync(accepted, ch->accepted.get(), (size_t)ch->N * sizeof(double), cudaMemcpyDeviceToHost,
+                         ch->st.get()));
+  CK(ch, cudaStreamSynchronize(ch->st.get()));
   return EB_OK;
 }
 
@@ -2377,16 +2294,16 @@ int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t co
   const size_t nw = (size_t)ch->N, nd = (size_t)ch->D;
   // the slab is filled from the stored slots in place (one strided copy per run of steps inside a segment), so
   // the FFT kernels see the numbers eb_autocorr gets from the host copy of the same slice
-  return acf_slabs(ch, "eb_chain_autocorr", ch->st, (size_t)count, nw, nd, acf,
+  return acf_slabs(ch, "eb_chain_autocorr", ch->st.get(), (size_t)count, nw, nd, acf,
                    [&](double* xin, size_t w0, size_t wn) {
                      cudaError_t e = cudaSuccess;
                      for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
                                         [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
                                           if (e == cudaSuccess)
                                             e = copy_rows(xin + k0 * wn * nd, wn * nd * sizeof(double),
-                                                          ch->segs[s].x + off * ch->xs + w0 * nd,
+                                                          ch->segs[s].x.get() + off * ch->xs + w0 * nd,
                                                           stride * ch->xs * sizeof(double), wn * nd * sizeof(double),
-                                                          n, cudaMemcpyDeviceToDevice, ch->max_pitch, ch->st);
+                                                          n, cudaMemcpyDeviceToDevice, ch->max_pitch, ch->st.get());
                                         });
                      return e;
                    });
@@ -2413,13 +2330,12 @@ int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uin
   uint32_t np = 0;
   const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
   const SelectScratch z = select_scratch(count, D, (size_t)D * nranks);
-  void* scratch = nullptr;
-  rc = chain_scratch(ch, "eb_chain_select", z.bytes, &scratch);
+  DevPtr<void> scratch;
+  rc = chain_scratch(ch, "eb_chain_select", z.bytes, scratch);
   if (rc) return rc;
   const cudaError_t e = select_run(slots.data(), count, (uint32_t)ch->N, D, ranks, nranks, out, has_nan, &np, z,
-                                   scratch, ch->sm_count, ch->st);
-  cudaStreamSynchronize(ch->st);
-  cudaFree(scratch);
+                                   scratch.get(), ch->sm_count, ch->st.get());
+  cudaStreamSynchronize(ch->st.get());
   CK(ch, e);
   if (passes) *passes = np;
   return EB_OK;
@@ -2440,23 +2356,23 @@ int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t cou
   CK(ch, cudaSetDevice(ch->device));
   // [D shift | D + D*D sums | CTA partials of launch_moments]
   const size_t head = ((D + na) * sizeof(double) + 255) & ~(size_t)255;
-  void* scratch = nullptr;
-  rc = chain_scratch(ch, "eb_chain_moments", head + moments_partial_bytes(ch->D, ch->sm_count), &scratch);
+  DevPtr<void> scratch;
+  rc = chain_scratch(ch, "eb_chain_moments", head + moments_partial_bytes(ch->D, ch->sm_count), scratch);
   if (rc) return rc;
-  double* shift = static_cast<double*>(scratch);
+  double* shift = static_cast<double*>(scratch.get());
   double* acc = shift + D;
-  double* partial = reinterpret_cast<double*>(static_cast<char*>(scratch) + head);
+  double* partial = reinterpret_cast<double*>(static_cast<char*>(scratch.get()) + head);
   const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
   // shift = the column mean of the slice's first stored step (as eb_moments takes the first accumulated state's);
   // then every stored step is folded into one accumulator, in slot order
-  cudaError_t e = cudaMemsetAsync(acc, 0, na * sizeof(double), ch->st);
-  if (e == cudaSuccess) e = launch_colmean(slots[0], ch->N, ch->D, shift, nullptr, ch->st);
+  cudaStream_t st = ch->st.get();
+  cudaError_t e = cudaMemsetAsync(acc, 0, na * sizeof(double), st);
+  if (e == cudaSuccess) e = launch_colmean(slots[0], ch->N, ch->D, shift, nullptr, st);
   for (size_t k = 0; k < slots.size() && e == cudaSuccess; ++k)
-    e = launch_moments(slots[k], ch->N, ch->D, shift, partial, acc, ch->sm_count, ch->st);
+    e = launch_moments(slots[k], ch->N, ch->D, shift, partial, acc, ch->sm_count, st);
   std::vector<double> h(D + na);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), shift, (D + na) * sizeof(double), cudaMemcpyDeviceToHost, ch->st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ch->st);
-  cudaFree(scratch);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), shift, (D + na) * sizeof(double), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   CK(ch, e);
   finish_moments(h.data() + D, h.data(), count * (uint64_t)ch->N, D, mean, cov);
   return EB_OK;
@@ -2485,14 +2401,13 @@ int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, 
          (unsigned long long)count);
   CK(ch, cudaSetDevice(ch->device));
   const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
-  void* scratch = nullptr;
-  rc = chain_scratch(ch, "eb_chain_histogram", hist1_scratch_bytes(count, D, (int)bins), &scratch);
+  DevPtr<void> scratch;
+  rc = chain_scratch(ch, "eb_chain_histogram", hist1_scratch_bytes(count, D, (int)bins), scratch);
   if (rc) return rc;
   bool bad = false;
   const cudaError_t e = hist1_run(slots.data(), count, (uint32_t)ch->N, D, (int)bins, outer, edges, hist, &bad,
-                                  scratch, ch->sm_count, ch->st);
-  cudaStreamSynchronize(ch->st);
-  cudaFree(scratch);
+                                  scratch.get(), ch->sm_count, ch->st.get());
+  cudaStreamSynchronize(ch->st.get());
   CK(ch, e);
   if (bad)
     FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram: a value's truncated bin index is above bins (np.histogram raises "
@@ -2530,13 +2445,12 @@ int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t
          (unsigned long long)count);
   CK(ch, cudaSetDevice(ch->device));
   const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
-  void* scratch = nullptr;
-  rc = chain_scratch(ch, "eb_chain_histogram2d", hist2_scratch_bytes(count, (int)nparams, (int)bins), &scratch);
+  DevPtr<void> scratch;
+  rc = chain_scratch(ch, "eb_chain_histogram2d", hist2_scratch_bytes(count, (int)nparams, (int)bins), scratch);
   if (rc) return rc;
   const cudaError_t e = hist2_run(slots.data(), count, (uint32_t)ch->N, ch->D, params, (int)nparams, (int)bins, edges,
-                                  hist, scratch, ch->sm_count, ch->st);
-  cudaStreamSynchronize(ch->st);
-  cudaFree(scratch);
+                                  hist, scratch.get(), ch->sm_count, ch->st.get());
+  cudaStreamSynchronize(ch->st.get());
   CK(ch, e);
   return EB_OK;
 }
@@ -2547,8 +2461,9 @@ int eb_get_naccepted(eb_ctx* c, uint64_t* naccepted) {
   CK(c, cudaSetDevice(c->device));
   int rc = sync_replicas(c);  // multi-GPU: every rank's counters (collective)
   if (rc) return rc;
-  CK(c, cudaMemcpyAsync(naccepted, c->nacc, (size_t)c->N * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemcpyAsync(naccepted, c->nacc.get(), (size_t)c->N * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                        c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
 
@@ -2562,8 +2477,8 @@ int eb_reset_counters(eb_ctx* c) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
-  CK(c, cudaMemsetAsync(c->nacc, 0, (size_t)c->N * sizeof(unsigned long long), c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemsetAsync(c->nacc.get(), 0, (size_t)c->N * sizeof(unsigned long long), c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
 
@@ -2574,17 +2489,17 @@ int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* 
   CK(c, cudaSetDevice(c->device));
   const size_t D = (size_t)c->D, n = D + D * D;
   std::vector<double> acc(n), shift(D);
-  CK(c, cudaMemcpyAsync(acc.data(), c->mom_acc, n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  CK(c, cudaMemcpyAsync(shift.data(), c->mom_shift, D * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  CK(c, cudaMemcpyAsync(acc.data(), c->mom_acc.get(), n * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
+  CK(c, cudaMemcpyAsync(shift.data(), c->mom_shift.get(), D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
   std::vector<unsigned long long> nacc;
   int64_t r0, r1;
   owned_rows(c, r0, r1);
   if (naccepted_total) {
     nacc.resize((size_t)(r1 - r0));
-    CK(c, cudaMemcpyAsync(nacc.data(), c->nacc + r0, nacc.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
-                          c->st));
+    CK(c, cudaMemcpyAsync(nacc.data(), c->nacc.get() + r0, nacc.size() * sizeof(unsigned long long),
+                          cudaMemcpyDeviceToHost, c->st.get()));
   }
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   c->chain_ok = false;
   if (count) *count = c->mom_count;
   if (naccepted_total) {
@@ -2624,8 +2539,8 @@ int eb_histograms_config(eb_ctx* c, uint64_t every, uint32_t bins, const double*
   }
   CK(c, cudaSetDevice(c->device));
   // the old configuration goes first: its memory counts towards what the new one may take
-  CK(c, cudaStreamSynchronize(c->st));
-  CK(c, cudaFree(c->hist.mem));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  c->hist_mem.reset();
   c->hist = LiveHist{};
   c->hist_on = false;
   c->hist_every = 0;
@@ -2636,20 +2551,18 @@ int eb_histograms_config(eb_ctx* c, uint64_t every, uint32_t bins, const double*
   CK(c, cudaMemGetInfo(&free_b, &total_b));
   if (bytes > free_b)
     FAIL(c, EB_ERR_NOMEM, "eb_histograms_config: %zu bytes of counts and tables, %zu bytes free", bytes, free_b);
-  void* mem = nullptr;
-  const cudaError_t e = cudaMalloc(&mem, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    FAIL(c, EB_ERR_NOMEM, "eb_histograms_config: allocating %zu bytes failed (%s)", bytes, cudaGetErrorString(e));
-  }
-  const cudaError_t s = live_hist_setup(&c->hist, mem, (uint32_t)c->N, c->D, (int)bins, lp, outer, edges, params2d, m,
-                                        (int)bins2d, edges2d, c->coords, c->logp, c->sm_count, c->st);
+  DevPtr<void> mem;
+  CK_NOMEM(c, dev_alloc(mem, bytes), "eb_histograms_config: allocating %zu bytes failed (%s)", bytes,
+           cudaGetErrorString(alloc_err));
+  const cudaError_t s = live_hist_setup(&c->hist, mem.get(), (uint32_t)c->N, c->D, (int)bins, lp, outer, edges,
+                                        params2d, m, (int)bins2d, edges2d, c->coords.get(), c->logp.get(), c->sm_count,
+                                        c->st.get());
   if (s != cudaSuccess) {
     cudaGetLastError();
-    cudaFree(mem);
     c->hist = LiveHist{};
     FAIL(c, EB_ERR_CUDA, "eb_histograms_config: %s", cudaGetErrorString(s));
   }
+  c->hist_mem = std::move(mem);
   c->hist_on = true;
   c->hist_every = every;
   return EB_OK;
@@ -2661,7 +2574,7 @@ int eb_histograms(eb_ctx* c, uint64_t* hist, uint64_t* hist2d, uint64_t* count) 
   if (!c->hist_on) FAIL(c, EB_ERR_STATE, "eb_histograms: configure them with eb_histograms_config first");
   CK(c, cudaSetDevice(c->device));
   bool bad = false;
-  CK(c, live_hist_read(c->hist, hist, hist2d, &bad, c->st));
+  CK(c, live_hist_read(c->hist, hist, hist2d, &bad, c->st.get()));
   c->chain_ok = false;
   if (count) *count = c->hist_count;
   if (bad)
@@ -2675,10 +2588,9 @@ int eb_trace_config(eb_ctx* c, uint64_t every) {
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   if (every > 0 || !c->trace_on) {  // every == 0 after a configuration keeps what was recorded readable
-    CK(c, cudaFree(c->trace_rows));
-    c->trace_rows = nullptr;
+    c->trace_rows.reset();
     c->trace_cap = 0;
     c->trace_steps.clear();
     if (!c->trace_on) {
@@ -2686,16 +2598,11 @@ int eb_trace_config(eb_ctx* c, uint64_t every) {
       size_t free_b = 0, total_b = 0;
       CK(c, cudaMemGetInfo(&free_b, &total_b));
       if (bytes > free_b) FAIL(c, EB_ERR_NOMEM, "eb_trace_config: %zu bytes of partial sums, %zu bytes free", bytes, free_b);
-      void* mem = nullptr;
-      const cudaError_t e = cudaMalloc(&mem, bytes);
-      if (e != cudaSuccess) {
-        cudaGetLastError();
-        FAIL(c, EB_ERR_NOMEM, "eb_trace_config: allocating %zu bytes failed (%s)", bytes, cudaGetErrorString(e));
-      }
-      c->trace.mem = mem;
+      CK_NOMEM(c, dev_alloc(c->trace_mem, bytes), "eb_trace_config: allocating %zu bytes failed (%s)", bytes,
+               cudaGetErrorString(alloc_err));
     }
-    const cudaError_t s =
-        live_trace_setup(&c->trace, c->trace.mem, (uint32_t)c->N, c->D, c->coords, c->logp, c->accepted, c->st);
+    const cudaError_t s = live_trace_setup(&c->trace, c->trace_mem.get(), (uint32_t)c->N, c->D, c->coords.get(),
+                                           c->logp.get(), c->accepted.get(), c->st.get());
     if (s != cudaSuccess) {
       cudaGetLastError();
       FAIL(c, EB_ERR_CUDA, "eb_trace_config: %s", cudaGetErrorString(s));
@@ -2726,9 +2633,9 @@ int eb_trace_read(eb_ctx* c, uint64_t first, uint64_t count, uint64_t* step, dou
   if (rows_out) {
     const size_t W = 2 * (size_t)c->D + TRACE_EXTRA;
     CK(c, cudaSetDevice(c->device));
-    CK(c, cudaMemcpyAsync(rows_out, c->trace_rows + first * W, (size_t)count * W * sizeof(double),
-                          cudaMemcpyDeviceToHost, c->st));
-    CK(c, cudaStreamSynchronize(c->st));
+    CK(c, cudaMemcpyAsync(rows_out, c->trace_rows.get() + first * W, (size_t)count * W * sizeof(double),
+                          cudaMemcpyDeviceToHost, c->st.get()));
+    CK(c, cudaStreamSynchronize(c->st.get()));
     c->chain_ok = false;
   }
   return EB_OK;
@@ -2741,7 +2648,7 @@ int eb_trace_best(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, u
   if (c->trace_steps.empty()) FAIL(c, EB_ERR_STATE, "eb_trace_best: no step has been recorded yet");
   CK(c, cudaSetDevice(c->device));
   TraceBest b;
-  CK(c, live_trace_best(c->trace, &b, coords, c->st));
+  CK(c, live_trace_best(c->trace, &b, coords, c->st.get()));
   c->chain_ok = false;
   if (log_prob) *log_prob = b.log_prob;
   if (step) *step = b.step;
@@ -2758,34 +2665,30 @@ int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, 
   int rc = ensure_scratch(c, rows);
   if (rc) return rc;
   const size_t D = (size_t)c->D, n = D + D * D;
-  double* work = nullptr;  // [D mean | D + D*D accumulators]
-  CK(c, cudaMalloc(&work, (D + n) * sizeof(double)));
-  if (!c->mom_partial) {
-    cudaError_t e = cudaMalloc(&c->mom_partial, moments_partial_bytes(c->D, c->sm_count));
-    if (e != cudaSuccess) {
-      cudaFree(work);
-      CK(c, e);
-    }
-  }
+  DevPtr<double> dwork;  // [D mean | D + D*D accumulators]
+  CK(c, dev_alloc(dwork, (D + n) * sizeof(double)));
+  if (!c->mom_partial) CK(c, dev_alloc(c->mom_partial, moments_partial_bytes(c->D, c->sm_count)));
   c->chain_ok = false;
   std::vector<double> acc(n);
   int f = 0;
-  cudaError_t e = cudaMemcpyAsync(c->scratch_x, coords, rows * D * sizeof(double), cudaMemcpyHostToDevice, c->st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(work, 0, (D + n) * sizeof(double), c->st);
-  if (e == cudaSuccess) e = launch_colmean(c->scratch_x, (int64_t)rows, c->D, work, c->status_dev, c->st);
+  double* work = dwork.get();
+  double* x = c->scratch_x.get();
+  cudaStream_t st = c->st.get();
+  cudaError_t e = cudaMemcpyAsync(x, coords, rows * D * sizeof(double), cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(work, 0, (D + n) * sizeof(double), st);
+  if (e == cudaSuccess) e = launch_colmean(x, (int64_t)rows, c->D, work, c->status_dev.get(), st);
   if (e == cudaSuccess)
-    e = launch_moments(c->scratch_x, (int64_t)rows, c->D, work, c->mom_partial, work + D, c->sm_count, c->st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(acc.data(), work + D, n * sizeof(double), cudaMemcpyDeviceToHost, c->st);
+    e = launch_moments(x, (int64_t)rows, c->D, work, c->mom_partial.get(), work + D, c->sm_count, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(acc.data(), work + D, n * sizeof(double), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess)
-    e = cudaMemcpyAsync(c->status_host, c->status_dev, sizeof(int), cudaMemcpyDeviceToHost, c->st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(c->st);
-  cudaFree(work);
+    e = cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   CK(c, e);
   // the non-finite flags are an ANSWER here (walkers_independent returns False), not an error
   if (*c->status_host & (FLAG_INF_PARAM | FLAG_NAN_PARAM)) f |= 1;
   *c->status_host = 0;
-  CK(c, cudaMemsetAsync(c->status_dev, 0, sizeof(int), c->st));
-  CK(c, cudaStreamSynchronize(c->st));
+  CK(c, cudaMemsetAsync(c->status_dev.get(), 0, sizeof(int), c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
   // centred, column-normalised walkers C (ensemble.py:656-661): C^T C = M_jk / (sqrt(M_jj) sqrt(M_kk)); the
   // max-abs scaling of :658-659 cancels, it only matters as the zero-span test.  The square roots are taken
   // before the product, so that the denominator stays normal whenever both sums are.  A sum M_jj that is
@@ -2817,10 +2720,10 @@ int eb_autocorr(eb_ctx* c, const double* chain, size_t n_t, size_t nw, size_t nd
   if (!chain || !acf || n_t == 0 || nw == 0 || nd == 0) FAIL(c, EB_ERR_INVALID, "eb_autocorr: empty chain or null buffer");
   CK(c, cudaSetDevice(c->device));
   c->chain_ok = false;
-  return acf_slabs(c, "eb_autocorr", c->st, n_t, nw, nd, acf, [&](double* xin, size_t w0, size_t wn) {
+  return acf_slabs(c, "eb_autocorr", c->st.get(), n_t, nw, nd, acf, [&](double* xin, size_t w0, size_t wn) {
     // chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd]: one strided copy (rows of the slab are contiguous in a step)
     return cudaMemcpy2DAsync(xin, wn * nd * sizeof(double), chain + w0 * nd, nw * nd * sizeof(double),
-                             wn * nd * sizeof(double), n_t, cudaMemcpyHostToDevice, c->st);
+                             wn * nd * sizeof(double), n_t, cudaMemcpyHostToDevice, c->st.get());
   });
 }
 
@@ -2842,10 +2745,16 @@ int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
     CK(c, cudaSetDevice(c->device));
     if (value && !c->tap_scalar) {
       const size_t N = (size_t)c->N;
-      CK(c, cudaMalloc(&c->tap_partners, 3 * N * sizeof(int64_t)));
-      CK(c, cudaMalloc(&c->tap_scalar, N * sizeof(double)));
-      CK(c, cudaMalloc(&c->tap_u, N * sizeof(double)));
-      CK(c, cudaMalloc(&c->tap_active, N * sizeof(int64_t)));
+      DevPtr<int64_t> partners, active;
+      DevPtr<double> scalar, u;
+      CK(c, dev_alloc(partners, 3 * N * sizeof(int64_t)));
+      CK(c, dev_alloc(scalar, N * sizeof(double)));
+      CK(c, dev_alloc(u, N * sizeof(double)));
+      CK(c, dev_alloc(active, N * sizeof(int64_t)));
+      c->tap_partners = std::move(partners);
+      c->tap_scalar = std::move(scalar);
+      c->tap_u = std::move(u);
+      c->tap_active = std::move(active);
     }
     c->debug = value != 0;
     return EB_OK;
@@ -2854,11 +2763,12 @@ int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
     CK(c, cudaSetDevice(c->device));
     const size_t n = (size_t)c->sm_count * 8 * TL_TILES * TL_EVENTS;
     if (value && !c->timeline) {
-      CK(c, cudaMalloc(&c->timeline, n * sizeof(long long)));
-      CK(c, cudaMemset(c->timeline, 0, n * sizeof(long long)));
-    } else if (!value && c->timeline) {
-      cudaFree(c->timeline);
-      c->timeline = nullptr;
+      DevPtr<long long> tl;
+      CK(c, dev_alloc(tl, n * sizeof(long long)));
+      CK(c, cudaMemset(tl.get(), 0, n * sizeof(long long)));
+      c->timeline = std::move(tl);
+    } else if (!value) {
+      c->timeline.reset();
     }
     return EB_OK;
   }
@@ -2909,7 +2819,7 @@ int eb_debug_timeline(eb_ctx* c, int64_t* out, size_t capacity, size_t* written)
   CK(c, cudaSetDevice(c->device));
   const size_t n = (size_t)c->sm_count * 8 * TL_TILES * TL_EVENTS;
   if (capacity < n) FAIL(c, EB_ERR_INVALID, "eb_debug_timeline: need room for %zu values", n);
-  CK(c, cudaMemcpy(out, c->timeline, n * sizeof(long long), cudaMemcpyDeviceToHost));
+  CK(c, cudaMemcpy(out, c->timeline.get(), n * sizeof(long long), cudaMemcpyDeviceToHost));
   if (written) *written = n;
   return EB_OK;
 }
@@ -2921,10 +2831,10 @@ int eb_debug_taps(eb_ctx* c, int64_t* partners, double* scalar, double* u_accept
   if (!c->debug || !c->tap_scalar) FAIL(c, EB_ERR_STATE, "eb_debug_taps: enable with eb_set_option(\"debug_taps\", 1)");
   CK(c, cudaSetDevice(c->device));
   const size_t N = (size_t)c->N;
-  if (partners) CK(c, cudaMemcpy(partners, c->tap_partners, 3 * N * sizeof(int64_t), cudaMemcpyDeviceToHost));
-  if (scalar) CK(c, cudaMemcpy(scalar, c->tap_scalar, N * sizeof(double), cudaMemcpyDeviceToHost));
-  if (u_accept) CK(c, cudaMemcpy(u_accept, c->tap_u, N * sizeof(double), cudaMemcpyDeviceToHost));
-  if (active) CK(c, cudaMemcpy(active, c->tap_active, N * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (partners) CK(c, cudaMemcpy(partners, c->tap_partners.get(), 3 * N * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (scalar) CK(c, cudaMemcpy(scalar, c->tap_scalar.get(), N * sizeof(double), cudaMemcpyDeviceToHost));
+  if (u_accept) CK(c, cudaMemcpy(u_accept, c->tap_u.get(), N * sizeof(double), cudaMemcpyDeviceToHost));
+  if (active) CK(c, cudaMemcpy(active, c->tap_active.get(), N * sizeof(int64_t), cudaMemcpyDeviceToHost));
   if (nactive) *nactive = c->tap_count;
   return EB_OK;
 }
@@ -2960,8 +2870,8 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path
-  unsigned* flags = reinterpret_cast<unsigned*>(c->coords + (size_t)c->N * c->D);
-  if (comm_init(c->comm, id, rank, nranks, mode, c->N, c->D, c->coords, flags, c->table_cap, c->st))
+  unsigned* flags = reinterpret_cast<unsigned*>(c->coords.get() + (size_t)c->N * c->D);
+  if (comm_init(c->comm, id, rank, nranks, mode, c->N, c->D, c->coords.get(), flags, c->table_cap, c->st.get()))
     FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   return EB_OK;
 }
@@ -2978,7 +2888,7 @@ int eb_comm_probe(eb_ctx* c, int peer, int what, double* gbs) {
   if (!c || !gbs) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
-  if (comm_probe(c->comm, peer, what, c->D, c->st, gbs)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
+  if (comm_probe(c->comm, peer, what, c->D, c->st.get(), gbs)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   return EB_OK;
 }
 

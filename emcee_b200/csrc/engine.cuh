@@ -101,8 +101,6 @@ struct ExternalBufs {
   const double* lp;  // accept: [a_count] log-probabilities of the proposals
 };
 
-struct Engine;  // defined in capi.cu
-
 // ---- kernel launchers (implemented in the .cu files) ----------------------
 // ranges (nullable): [nsteps_chunk, MAX_SPLITS] int2 = active ranks of each set owned by walkers [w_lo, w_hi)
 cudaError_t launch_split_tables(int32_t* order, const StepInfo* info_dev, int nsteps_chunk, int64_t N,
