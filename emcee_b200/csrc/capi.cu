@@ -95,6 +95,7 @@ struct eb_ctx {
   DevPtr<int64_t> tap_active;
   int64_t tap_count = 0;
   DevPtr<long long> timeline;  // dense_dmma instrumentation buffer (option "dmma_timeline")
+  bool timeline_first_split = false;  // option "dmma_timeline" = 2: stamp only launches that start a step
 
   // optional L2 flush between steps (benchmark hygiene): per-step event pairs
   bool l2_flush = false;
@@ -259,6 +260,7 @@ static int check_status(eb_ctx* c) {
   cudaMemsetAsync(c->status_dev.get(), 0, sizeof(int), c->st.get());
   cudaStreamSynchronize(c->st.get());
   if (f & FLAG_COMM_TIMEOUT) FAIL(c, EB_ERR_COMM, "peer-memory barrier timed out: another rank did not arrive");
+  if (f & FLAG_WAIT_TIMEOUT) FAIL(c, EB_ERR_CUDA, "kernel stalled: a warp waited ~2 minutes for a hand-off in its block");
   if (f & FLAG_INF_PARAM) FAIL(c, EB_ERR_INF_PARAM, "At least one parameter value was infinite");
   if (f & FLAG_NAN_PARAM) FAIL(c, EB_ERR_NAN_PARAM, "At least one parameter value was NaN");
   FAIL(c, EB_ERR_NAN_LOGPROB, "Probability function returned NaN");
@@ -1579,6 +1581,8 @@ int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches)
   a.dmma_early_own = pdl && c->comm.nranks == 1 && d0.split > 0 && c->dmma_first.step == d0.step &&
                      c->dmma_first.order_step == d0.order_step && c->dmma_last.step == d0.step &&
                      c->dmma_last.split == d0.split - 1;
+  // "dmma_timeline" = 2: the other launches run uninstrumented, so the stamps left are those of a first split
+  if (c->timeline_first_split && d0.split != 0) a.timeline = nullptr;
   int grid = 0;
   CK(c, launch_dense_dmma(a, c->descs_host.get()[grp.first], c->descs_dev.get() + grp.first, grp.nhalf, bound,
                           c->gbar.get(), c->gbar_count, c->sm_count, pdl, &grid, c->st.get()));
@@ -2770,6 +2774,7 @@ int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
     } else if (!value) {
       c->timeline.reset();
     }
+    c->timeline_first_split = value == 2;
     return EB_OK;
   }
   if (!strcmp(name, "l2_flush")) {

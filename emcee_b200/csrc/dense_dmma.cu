@@ -42,6 +42,19 @@ namespace {
 constexpr int DMMA_CONSUMERS = 8;
 constexpr int DMMA_THREADS = 64 * DMMA_CONSUMERS;  // consumers are warps 0..7, producers 8..15
 constexpr int NI = 2;  // 16-column tiles of y in flight per consumer (NI independent accumulator chains)
+// per-thread registers after the rebalance that follows the prologue (setmaxnreg: multiples of 8, and the 256 producer and
+// 256 consumer threads together hold no more than the 65 536 registers of the SM)
+constexpr int DMMA_PRODUCER_REGS = 64;
+constexpr int DMMA_CONSUMER_REGS = 192;
+static_assert((DMMA_THREADS / 2) * (DMMA_PRODUCER_REGS + DMMA_CONSUMER_REGS) <= 65536, "register file of one SM");
+// Which instantiations rebalance.  The producers spill below 128 registers at every D (64 is the fastest split
+// measured at D = 128: 56 starves the consumers, 72 leaves them spilling), so the rebalance pays only where
+// the consumer spilled more at the launch's 128: it is applied where it lowers the spill instructions of the
+// whole kernel (cuobjdump -sass, CUDA 12.9; DESIGN §5.3), i.e. without a box prior at D > 112, and with a mean
+// from D = 88 on.  The others keep 128 registers in both roles.
+__host__ __device__ constexpr bool dmma_rebalance(int KB, bool HAS_MEAN, bool BOUNDED) {
+  return !BOUNDED && (KB >= 15 || (HAS_MEAN && KB >= 11));
+}
 
 // C[16x8] += A[16x8] B[8x8]: lane (g,t) holds a = {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]},
 // b = {B[t][g], B[t+4][g]}, c = {C[g][2t], C[g][2t+1], C[g+8][2t], C[g+8][2t+1]}
@@ -224,11 +237,6 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   if (HAS_MEAN)
     for (int k = tid; k < D; k += DMMA_THREADS) sMu[k] = a.model.params[k];
   __syncthreads();
-  if (tid == 0) {  // one bulk copy brings the whole packed factor, once per launch
-    constexpr unsigned bytes = (unsigned)(SL::L_doubles * sizeof(double));
-    mbar_arrive_expect_tx(barL, bytes);
-    bulk_g2s(sL, a.model.chol, bytes, barL);
-  }
 
   // tile indices fit 32 bits: a half-step has at most 2^31 / 8 tiles (HalfDesc::a_count is an int32)
   const int tstride = (int)gridDim.x * DMMA_CONSUMERS;
@@ -240,7 +248,14 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   const bool multi = a.p2p_peer_flags != nullptr;
   unsigned k = 0;  // tiles this pair has handled so far in the launch (mbarrier phase counter)
 
+  // Register rebalance (dmma_rebalance).  The launch gives every thread 128 registers (512 threads, one CTA per
+  // SM); at large D the consumer spills more there (q, the factor fragments in flight, the accepted-row store), so the
+  // producers give up 64 of theirs.  Consumers are warpgroups 0-1 and producers 2-3, so each setmaxnreg is
+  // warpgroup-uniform; every warp arrives here converged, straight from the CTA barrier, and ptxas allocates
+  // each role's code under its own limit because the two paths never join again.
+  constexpr bool REBALANCE = dmma_rebalance(KB, HAS_MEAN, BOUNDED);
   if (is_producer) {
+    if constexpr (REBALANCE) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DMMA_PRODUCER_REGS));
     // ================= producer: draws, lookups, TMA row gather, proposal =================
     // optional stamps of the LAST half-step, events 6..8 of the tile's record (cycles since this warp entered
     // the kernel): 6 rows requested, 7 rows landed, 8 proposal published
@@ -454,6 +469,12 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   }
 
   // ================================ consumer: DMMA, accept, update ================================
+  if constexpr (REBALANCE) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(DMMA_CONSUMER_REGS));
+  if (tid == 0) {  // one bulk copy brings the whole packed factor, once per launch
+    constexpr unsigned bytes = (unsigned)(SL::L_doubles * sizeof(double));
+    mbar_arrive_expect_tx(barL, bytes);
+    bulk_g2s(sL, a.model.chol, bytes, barL);
+  }
   // optional per-tile timestamps of the LAST half-step (cycles since this warp entered the kernel):
   // 1 wait start, 2 proposal ready, 3 proposal in registers, 4 DMMA block done, 5 tile done
   const long long t_entry = clock64();
@@ -462,7 +483,8 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   pdl_launch_dependents();
   // On an abort a consumer stops working but keeps walking the same sequence of named barriers as its
   // siblings, so nobody is left waiting for a warp that left.
-  bool alive = mbar_wait_abortable(barL, 0, sAbort);
+  // (the consumer's waits have no trap: with one, ptxas would not let this code use the raised register limit)
+  bool alive = mbar_wait_abortable_notrap(barL, 0, sAbort, a.status, FLAG_WAIT_TIMEOUT);
   for (int h = 0; h < nhalf; ++h) {
     const HalfDesc d = (h == 0) ? d0 : descs[h];
     const int2 rg = a.range ? a.range[(size_t)d.order_step * MAX_SPLITS + d.split] : make_int2(0, d.a_count);
@@ -476,7 +498,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         tlk[0] = (long long)tile;
         tlk[1] = clock64() - t_entry;
       }
-      if (!mbar_wait_abortable(barReady + pair, k & 1u, sAbort)) {
+      if (!mbar_wait_abortable_notrap(barReady + pair, k & 1u, sAbort, a.status, FLAG_WAIT_TIMEOUT)) {
         alive = false;
         break;
       }
@@ -693,7 +715,7 @@ cudaError_t launch_t(const HalfStepArgs& a, const HalfDesc& d0, const HalfDesc* 
   if (nhalf == 1) {
     // no grid barrier inside: a plain launch (cooperative launches cost ~2 us more each).  With `pdl`
     // the kernel is a programmatic dependent of the previous kernel in the stream: its prologue
-    // (barrier set-up, factor copy, first draws, L2 prefetch of its own rows) overlaps that kernel's tail.
+    // (barrier set-up, factor copy, first draws) overlaps that kernel's tail.
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(DMMA_THREADS);

@@ -22,6 +22,7 @@ enum : int {
   FLAG_INF_PARAM = 2,
   FLAG_NAN_PARAM = 4,
   FLAG_COMM_TIMEOUT = 8,
+  FLAG_WAIT_TIMEOUT = 16,  // a warp gave up on an in-kernel hand-off (shared-memory barrier) of its own CTA
 };
 
 struct ModelDev {

@@ -50,6 +50,23 @@ __device__ __forceinline__ bool mbar_wait_abortable(uint64_t* bar, unsigned pari
   }
   return true;
 }
+// The same wait without the trap, for code that runs under a limit raised by setmaxnreg.inc: ptxas (CUDA 12.9)
+// does not give code from which a trap is reachable the raised limit.  At the last-resort bound it ORs
+// `timeout_flag` into the status word and raises `abort` itself, so the other warps leave as well.
+__device__ __forceinline__ bool mbar_wait_abortable_notrap(uint64_t* bar, unsigned parity, volatile int* abort,
+                                                           int* status, int timeout_flag) {
+  if (mbar_try_wait(bar, parity)) return true;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (*abort) return false;
+    if (clock64() - t0 > 240000000000ll) {
+      atomicOr(status, timeout_flag);
+      *abort = 1;
+      return false;
+    }
+  }
+  return true;
+}
 // best-effort wait of at most `cycles`: for orderings that are optimisations, not dependencies
 __device__ __forceinline__ void mbar_wait_for(uint64_t* bar, unsigned parity, long long cycles) {
   const long long t0 = clock64();

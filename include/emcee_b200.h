@@ -510,8 +510,9 @@ int eb_debug_timeline(eb_ctx* ctx, int64_t* out, size_t capacity, size_t* writte
  * in registers and stages only the partner rows; default 1), "dmma_local_first" (0/1/2: sharded dense_dmma -- build the first round of tiles from walkers whose
  * partner is local and take the peer barrier behind them; 0 never (default: the measured effect changes sign with the
  * number of GPUs), 1 when a consumer warp has at most two tiles per half-step, 2 always), "moments_every" (n >= 0: see
- * eb_moments; setting it resets the accumulators), "dmma_timeline" (0/1: record consumer cycle stamps
- * for eb_debug_timeline; 1 runs a separately compiled, instrumented kernel), "l2_flush"
+ * eb_moments; setting it resets the accumulators), "dmma_timeline" (0/1/2: record consumer cycle stamps
+ * for eb_debug_timeline in a separately compiled, instrumented kernel; 1 keeps those of the last launch of a call,
+ * 2 those of the last launch that starts a step, i.e. runs its first split), "l2_flush"
  * (0/1: benchmark hygiene -- write a 256 MiB buffer before every step and time
  * each step with its own CUDA-event pair, so eb_last_step_timing excludes the
  * flush). */

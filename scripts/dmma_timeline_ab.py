@@ -5,9 +5,10 @@
     python scripts/dmma_timeline_ab.py [--lib PATH] [--label NAME] [--steps K]
 
 `--lib` loads another build of the library (EMCEE_B200_LIB), so two builds can be compared from the same
-tree: run the script once per build.  The library keeps the stamps of the last dense_dmma launch of a
-call, i.e. the second split of the last step; with the flush that launch is the programmatic dependent of
-the first split.  Each of K one-step calls contributes one launch.  Segments, in cycles of a consumer warp:
+tree: run the script once per build.  Both launches of the step are reported.  Option "dmma_timeline" = 1
+keeps the stamps of the last launch of a call, the second split, which with the flush is the programmatic
+dependent of the first; = 2 keeps those of the first split, the launch after the flush that pulls the state
+from HBM.  Each of K one-step calls contributes one launch to each.  Segments, in cycles of a consumer warp:
 first-tile wait (wait for the first proposal, counted from the warp's entry into the kernel, so it includes
 griddepcontrol.wait), later waits, q-load (proposal into registers + slot release), DMMA block, epilogue
 (reduction, accept test, stores).  One JSON line goes to stdout."""
@@ -43,30 +44,31 @@ def main():
     eng.set_state(w["p0"])
     sched = s._schedule()
     eng.step(sched, args.warmup, want_accepted=False)
-    eng.set_option("dmma_timeline", 1)
-    seg = {k: [] for k in ("first_wait", "later_wait", "qload", "dmma", "epilogue")}
-    first_ready, end = [], []
-    for _ in range(args.steps):
-        eng.step(sched, 1, want_accepted=False)
-        tl = eng.debug_timeline()  # [SM, consumer, tile, event]
-        valid = tl[..., 5] > 0
-        wait = tl[..., 2] - tl[..., 1]
-        seg["first_wait"].append(tl[:, :, 0, 2][valid[:, :, 0]])  # from the warp's entry
-        seg["later_wait"].append(wait[:, :, 1:][valid[:, :, 1:]])
-        seg["qload"].append((tl[..., 3] - tl[..., 2])[valid])
-        seg["dmma"].append((tl[..., 4] - tl[..., 3])[valid])
-        seg["epilogue"].append((tl[..., 5] - tl[..., 4])[valid])
-        end.append(tl[..., 5].max(axis=(1, 2)))
-    eng.set_option("dmma_timeline", 0)
-    med = {k: float(np.median(np.concatenate(v))) for k, v in seg.items()}
-    ends = np.concatenate(end)
-    out = {"label": args.label or (args.lib or "in-tree"), "launch": "second split (PDL dependent of the first)",
-           "median_cycles": med, "kernel_end_per_sm_median": float(np.median(ends)),
-           "kernel_end_per_sm_max_median": float(np.median([e.max() for e in end])), "calls": args.steps,
-           "kernel": eng.last_kernel_name()}
-    print("%-10s first-wait %6.0f  later-wait %6.0f  q-load %5.0f  dmma %5.0f  epilogue %5.0f  | end/SM %6.0f"
-          % (out["label"], med["first_wait"], med["later_wait"], med["qload"], med["dmma"], med["epilogue"],
-             out["kernel_end_per_sm_median"]), file=sys.stderr)
+    out = {"label": args.label or (args.lib or "in-tree"), "calls": args.steps, "launches": {}}
+    for mode, launch in ((2, "first split (after the L2 flush)"), (1, "second split (PDL dependent of the first)")):
+        eng.set_option("dmma_timeline", mode)
+        seg = {k: [] for k in ("first_wait", "later_wait", "qload", "dmma", "epilogue")}
+        end = []
+        for _ in range(args.steps):
+            eng.step(sched, 1, want_accepted=False)
+            tl = eng.debug_timeline()  # [SM, consumer, tile, event]
+            valid = tl[..., 5] > 0
+            wait = tl[..., 2] - tl[..., 1]
+            seg["first_wait"].append(tl[:, :, 0, 2][valid[:, :, 0]])  # from the warp's entry
+            seg["later_wait"].append(wait[:, :, 1:][valid[:, :, 1:]])
+            seg["qload"].append((tl[..., 3] - tl[..., 2])[valid])
+            seg["dmma"].append((tl[..., 4] - tl[..., 3])[valid])
+            seg["epilogue"].append((tl[..., 5] - tl[..., 4])[valid])
+            end.append(tl[..., 5].max(axis=(1, 2)))
+        eng.set_option("dmma_timeline", 0)
+        med = {k: float(np.median(np.concatenate(v))) for k, v in seg.items()}
+        r = {"median_cycles": med, "kernel_end_per_sm_median": float(np.median(np.concatenate(end))),
+             "kernel_end_per_sm_max_median": float(np.median([e.max() for e in end]))}
+        out["launches"][launch] = r
+        print("%-10s %-6s first-wait %6.0f  later-wait %6.0f  q-load %5.0f  dmma %5.0f  epilogue %5.0f  | end/SM %6.0f"
+              % (out["label"], launch.split()[0], med["first_wait"], med["later_wait"], med["qload"], med["dmma"],
+                 med["epilogue"], r["kernel_end_per_sm_median"]), file=sys.stderr)
+    out["kernel"] = eng.last_kernel_name()
     print(json.dumps(out))
     eng.close()
 
