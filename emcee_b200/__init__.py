@@ -6,9 +6,10 @@ that the hot path covers."""
 __version__ = "0.1.0"
 
 from . import autocorr, models, moves
+from ._lib import DeviceArray
 from .backend import Backend, DeviceBackend
 from .ensemble import EnsembleSampler, walkers_independent
 from .model import Model
 from .state import State
 
-__all__ = ["EnsembleSampler", "walkers_independent", "State", "Model", "Backend", "DeviceBackend", "moves", "models", "autocorr", "__version__"]
+__all__ = ["EnsembleSampler", "walkers_independent", "State", "Model", "Backend", "DeviceBackend", "DeviceArray", "moves", "models", "autocorr", "__version__"]

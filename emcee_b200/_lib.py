@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-__all__ = ["lib", "Engine", "Chain", "EngineError", "device_count", "LIB_PATH", "EbMove", "DeviceRows"]
+__all__ = ["lib", "Engine", "Chain", "EngineError", "device_count", "LIB_PATH", "EbMove", "DeviceRows", "DeviceArray"]
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 # EMCEE_B200_LIB: developer override (A/B of two builds); the product always loads the in-tree library
@@ -168,6 +168,13 @@ _SIGNATURES = {
     "eb_comm_export": (C.c_int, [C.c_void_p, C.c_char_p]),
     "eb_comm_import": (C.c_int, [C.c_void_p, C.c_char_p]),
     "eb_comm_probe": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _dp]),
+    "eb_device_alloc": (C.c_int, [C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]),
+    "eb_device_free": (C.c_int, [C.c_int, C.c_void_p]),
+    "eb_device_copy": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_uint64]),
+    "eb_set_state_from": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_uint64]),
+    "eb_get_state_to": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "eb_compute_log_prob_from": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_uint64]),
+    "eb_chain_read_to": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -256,6 +263,189 @@ def _raise(rc, msg):
     if rc == EB_ERR_NOMEM:
         raise MemoryError(msg)
     raise EngineError("%s (eb_status %d)" % (msg, rc))
+
+
+def _raise_no_ctx(rc):
+    """The error of a failing call without a context (``eb_device_alloc``, ...): its message is eb_last_error(NULL)."""
+    _raise(rc, lib().eb_last_error(None).decode())
+
+
+class DeviceArray(object):
+    """A C-contiguous float64 array in device memory owned by the package: what ``cuda_results=True`` states and the
+    ``cuda=True`` reads of a ``DeviceBackend`` return.
+
+    It exposes the CUDA Array Interface (v3) with ``stream: None``: the data is complete when the array is handed
+    out, so a consumer needs no synchronisation.  ``torch.as_tensor(a, device="cuda")`` and ``cupy.asarray(a)``
+    wrap it without a copy and keep it alive; the memory is freed when the last reference goes.  ``get()``
+    returns a numpy copy.  A zero-size array has data pointer 0.  Pickling goes through the host."""
+
+    __slots__ = ("_ptr", "_shape", "_device")
+
+    def __init__(self, shape, device=0):
+        self._ptr = 0
+        self._shape = tuple(int(n) for n in shape)
+        self._device = int(device)
+        ptr = C.c_void_p()
+        rc = lib().eb_device_alloc(self._device, self.nbytes, C.byref(ptr))
+        if rc != EB_OK:
+            _raise_no_ctx(rc)
+        self._ptr = ptr.value or 0
+
+    def __del__(self):
+        if self._ptr:
+            try:
+                lib().eb_device_free(self._device, C.c_void_p(self._ptr))
+            except Exception:
+                pass
+            self._ptr = 0
+
+    @property
+    def __cuda_array_interface__(self):
+        return {"shape": self._shape, "typestr": "<f8", "data": (self._ptr, False), "strides": None, "version": 3,
+                "stream": None}
+
+    @property
+    def shape(self):
+        return self._shape
+
+    @property
+    def dtype(self):
+        return np.dtype(np.float64)
+
+    @property
+    def device(self):
+        """The CUDA device ordinal the memory lives on."""
+        return self._device
+
+    @property
+    def ndim(self):
+        return len(self._shape)
+
+    @property
+    def size(self):
+        return int(np.prod(self._shape, dtype=np.int64))
+
+    @property
+    def nbytes(self):
+        return 8 * self.size
+
+    def __len__(self):
+        if not self._shape:
+            raise TypeError("len() of a 0-d DeviceArray")
+        return self._shape[0]
+
+    def _copy_from(self, src, stream=0):
+        if self.nbytes:
+            rc = lib().eb_device_copy(self._device, C.c_void_p(self._ptr), C.c_void_p(src), self.nbytes, self.nbytes,
+                                      1, int(stream))
+            if rc != EB_OK:
+                _raise_no_ctx(rc)
+
+    def get(self):
+        """A numpy copy of the array."""
+        out = np.empty(self._shape, dtype=np.float64)
+        if self.nbytes:
+            rc = lib().eb_device_copy(self._device, C.c_void_p(out.ctypes.data), C.c_void_p(self._ptr), self.nbytes,
+                                      self.nbytes, 1, 0)
+            if rc != EB_OK:
+                _raise_no_ctx(rc)
+        return out
+
+    def copy(self):
+        """A new DeviceArray with the same values (a device-to-device copy)."""
+        out = DeviceArray(self._shape, self._device)
+        out._copy_from(self._ptr)
+        return out
+
+    def __deepcopy__(self, memo):
+        return self.copy()
+
+    def __reduce__(self):
+        return _device_array_from_host, (self.get(), self._device)
+
+    def __repr__(self):
+        return "DeviceArray(shape=%s, dtype=float64, device=%d)" % (self._shape, self._device)
+
+
+def _device_array_from_host(a, device):
+    """Unpickling: upload a host array into a new :class:`DeviceArray`."""
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    out = DeviceArray(a.shape, device)
+    out._copy_from(a.ctypes.data)
+    return out
+
+
+def is_cuda_array(obj):
+    """Whether ``obj`` exposes the CUDA Array Interface (a torch / CuPy / Numba device array, a :class:`DeviceArray`)."""
+    return obj is not None and hasattr(obj, "__cuda_array_interface__")
+
+
+def cuda_array_device(obj):
+    """The CUDA device ordinal an array object names -- ``DeviceArray.device``, a torch ``device.index``, a CuPy
+    ``device.id`` -- or None when it names none (the engine then checks the pointer itself)."""
+    dev = getattr(obj, "device", None)
+    if isinstance(dev, (int, np.integer)) and not isinstance(dev, bool):
+        return int(dev)
+    if getattr(dev, "type", None) == "cuda" and getattr(dev, "index", None) is not None:
+        return int(dev.index)
+    if isinstance(getattr(dev, "id", None), int):
+        return int(dev.id)
+    return None
+
+
+class CudaRows(object):
+    """A validated CUDA array for the device-memory transfers: its data pointer, first-axis stride in bytes and
+    the stream its producer names (the ``eb_callback_result`` encoding)."""
+
+    __slots__ = ("ptr", "stride", "stream", "shape")
+
+    def __init__(self, obj, shape, device, what):
+        cai = obj.__cuda_array_interface__
+        got = tuple(int(n) for n in cai["shape"])
+        if got != tuple(shape):
+            raise ValueError("incompatible input dimensions {0}".format(got))
+        if np.dtype(cai["typestr"]) != np.float64:
+            raise TypeError("%s must be a float64 CUDA array, got %s" % (what, np.dtype(cai["typestr"])))
+        if cai.get("mask") is not None:
+            raise ValueError("masked CUDA arrays are not supported as %s" % what)
+        dev = cuda_array_device(obj)
+        if dev is not None and dev != int(device):
+            raise ValueError("%s is on CUDA device %d; the sampler runs on device %d" % (what, dev, int(device)))
+        row = 8 * int(np.prod(got[1:], dtype=np.int64))
+        stride = row
+        strides = cai.get("strides")
+        if strides is not None:
+            strides = tuple(int(n) for n in strides)
+            if any(n > 1 and st != 8 for n, st in zip(got[1:], strides[1:])):
+                raise ValueError("the rows of %s must be contiguous; only the first axis may be strided" % what)
+            if got[0] > 1:
+                stride = strides[0]
+                if stride < row or stride % 8:
+                    raise ValueError("the first-axis stride of %s (%d bytes) must be a multiple of 8 bytes and at "
+                                     "least a row (%d bytes)" % (what, stride, row))
+        self.ptr = int(cai["data"][0] or 0)
+        self.stride = stride
+        # a "stream" entry is the producer's word on ordering (None: none needed); without one (interface v2, which
+        # torch exports) the data may still be in flight on any stream, so the engine waits for all of them
+        self.stream = (cai["stream"] or 0) if "stream" in cai else EB_STREAM_UNKNOWN
+        self.shape = got
+
+    def download(self, device):
+        """A numpy copy of the rows, ordered after the producer's stream (``eb_device_copy``)."""
+        out = np.empty(self.shape, dtype=np.float64)
+        width = out.itemsize * int(np.prod(self.shape[1:], dtype=np.int64))
+        if out.size:
+            rc = lib().eb_device_copy(int(device), C.c_void_p(out.ctypes.data), C.c_void_p(self.ptr), width,
+                                      self.stride, self.shape[0], int(self.stream))
+            if rc != EB_OK:
+                _raise_no_ctx(rc)
+        return out
+
+
+def _one_stream(*streams):
+    """The stream one copy of several producers' arrays waits for: the one they name, or the whole device."""
+    named = set(streams) - {0}
+    return named.pop() if len(named) == 1 else (EB_STREAM_UNKNOWN if named else 0)
 
 
 class DeviceRows(object):
@@ -631,6 +821,16 @@ class Chain(object):
         )
         return x, lp
 
+    def read_to(self, first, stride, count, coords_shape=None, log_prob_shape=None):
+        """:meth:`read` into new :class:`DeviceArray` s of the given shapes (None: not read), device to device
+        (``eb_chain_read_to``); a shape holds ``count * nwalkers * ndim`` or ``count * nwalkers`` values."""
+        x = None if coords_shape is None else DeviceArray(coords_shape, self.device)
+        lp = None if log_prob_shape is None else DeviceArray(log_prob_shape, self.device)
+        self._check(lib().eb_chain_read_to(
+            self._h, int(first), int(stride), int(count),
+            None if x is None else C.c_void_p(x._ptr), None if lp is None else C.c_void_p(lp._ptr)))
+        return x, lp
+
     def accepted(self):
         out = np.empty(self.nwalkers)
         self._check(lib().eb_chain_accepted(self._h, _as_dp(out)))
@@ -708,8 +908,8 @@ class Engine(object):
         self._blob_layout = None  # (dtype, shape) of the state's blob records, or None
         self._props = {}  # slot -> the registered C proposal function (kept alive while the engine may call it)
         self._seed_box = [int(seed) & (2**64 - 1)]  # the Philox key, read by the proposal trampolines
-        self.nwalkers, self.ndim = int(nwalkers), int(ndim)
-        rc = lib().eb_create(int(device), self.nwalkers, self.ndim, int(seed) & (2**64 - 1), C.byref(self._h))
+        self.nwalkers, self.ndim, self.device = int(nwalkers), int(ndim), int(device)
+        rc = lib().eb_create(self.device, self.nwalkers, self.ndim, int(seed) & (2**64 - 1), C.byref(self._h))
         if rc != EB_OK:
             msg = lib().eb_last_error(None).decode()
             self._h = C.c_void_p()
@@ -796,6 +996,26 @@ class Engine(object):
         elif blobs is not None:
             self._check(lib().eb_set_state_blobs(self._h, C.c_void_p(blobs.ctypes.data), blobs.nbytes // self.nwalkers))
             self._blob_layout = (blobs.dtype, _squeeze(blobs.shape[1:]))
+
+    def set_state_from(self, coords, log_prob=None):
+        """:meth:`set_state` from device memory (``eb_set_state_from``): ``coords`` and ``log_prob`` (or None) are
+        :class:`CudaRows`; the copy waits for the producers' stream.  ``log_prob=None``: evaluated by the model,
+        and a blob function's records become the state's blobs."""
+        stream = _one_stream(coords.stream, 0 if log_prob is None else log_prob.stream)
+        self._blob_layout = None
+        self._expect_blobs()
+        self._check(lib().eb_set_state_from(
+            self._h, C.c_void_p(coords.ptr), coords.stride, None if log_prob is None else C.c_void_p(log_prob.ptr),
+            8 if log_prob is None else log_prob.stride, stream))
+        if log_prob is None:
+            self._blob_layout = None if self._blob_sink is None else self._blob_sink.last
+
+    def get_state_to(self):
+        """``(coords, log_prob)`` of the live state as new :class:`DeviceArray` s (``eb_get_state_to``)."""
+        x = DeviceArray((self.nwalkers, self.ndim), self.device)
+        lp = DeviceArray((self.nwalkers,), self.device)
+        self._check(lib().eb_get_state_to(self._h, C.c_void_p(x._ptr), C.c_void_p(lp._ptr)))
+        return x, lp
 
     def get_blobs(self):
         """The state's blobs ``[nwalkers, *shape]`` (a fresh array), or None when it has none."""
@@ -925,6 +1145,18 @@ class Engine(object):
         out = np.empty(flat.shape[0], dtype=np.float64)
         self._check(lib().eb_compute_log_prob(self._h, _as_dp(flat), flat.shape[0], _as_dp(out)))
         return out.reshape(coords.shape[:-1])
+
+    def compute_log_prob_from(self, coords):
+        """:meth:`compute_log_prob` of a CUDA array ``coords[m, ndim]`` into a new :class:`DeviceArray` ``[m]``
+        (``eb_compute_log_prob_from``)."""
+        shape = tuple(int(n) for n in coords.__cuda_array_interface__["shape"])
+        if len(shape) != 2 or shape[1] != self.ndim:
+            raise ValueError("incompatible input dimensions {0}".format(shape))
+        rows = CudaRows(coords, shape, self.device, "coords")
+        out = DeviceArray((shape[0],), self.device)
+        self._check(lib().eb_compute_log_prob_from(self._h, C.c_void_p(rows.ptr), rows.stride, shape[0],
+                                                   C.c_void_p(out._ptr), rows.stream))
+        return out
 
     def compute_log_prob_blobs(self, coords):
         """``(log_prob[...], blobs[..., *shape] or None)`` of a blob function for ``coords[..., ndim]``."""

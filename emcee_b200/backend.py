@@ -248,6 +248,11 @@ class DeviceBackend(object):
     crosses PCIe.  Capacity is bounded by device memory, not host RAM: a
     ``grow`` that cannot fit raises ``MemoryError``.
 
+    ``cuda=True`` on ``get_chain`` / ``get_log_prob`` / ``get_value`` /
+    ``get_last_sample`` returns the same values as
+    :class:`~emcee_b200.DeviceArray` s, copied inside the GPU's memory: a caller
+    who keeps working on the device (torch, CuPy) never pays the two PCIe trips.
+
     Nothing is allocated before ``reset`` (the sampler calls it), so the
     object can be built without a GPU.  ``close()`` frees the device memory;
     pickling downloads the contents, and loading uploads them again.
@@ -342,13 +347,21 @@ class DeviceBackend(object):
             )
         return ch, slice_plan(self.iteration, discard, thin)
 
-    def get_value(self, name, flat=False, thin=1, discard=0):
+    def get_value(self, name, flat=False, thin=1, discard=0, cuda=False):
+        """``Backend.get_value``; ``cuda=True``: a :class:`~emcee_b200.DeviceArray` of the same shape and values,
+        device to device (``eb_chain_read_to``)."""
         ch, (first, stride, count) = self._plan(discard, thin)
         if name == "blobs":
             return None
         if name not in ("chain", "log_prob"):
             raise AttributeError(name)
         want_chain = name == "chain"
+        if cuda:
+            shape = (count, self.nwalkers, self.ndim) if want_chain else (count, self.nwalkers)
+            if flat:
+                shape = (shape[0] * shape[1],) + shape[2:]
+            x, lp = ch.read_to(first, stride, count, shape if want_chain else None, None if want_chain else shape)
+            return x if want_chain else lp
         x, lp = ch.read(first, stride, count, coords=want_chain, log_prob=not want_chain)
         v = x if want_chain else lp
         if flat:
@@ -356,7 +369,7 @@ class DeviceBackend(object):
         return v
 
     def get_chain(self, **kwargs):
-        """``[nsteps, nwalkers, ndim]`` (or flattened over walkers), downloaded."""
+        """``[nsteps, nwalkers, ndim]`` (or flattened over walkers), downloaded (``cuda=True``: in device memory)."""
         return self.get_value("chain", **kwargs)
 
     def get_log_prob(self, **kwargs):
@@ -365,8 +378,13 @@ class DeviceBackend(object):
     def get_blobs(self, **kwargs):
         return self.get_value("blobs", **kwargs)
 
-    def get_last_sample(self):
+    def get_last_sample(self, cuda=False):
+        """The last stored step as a ``State``: host arrays, or :class:`~emcee_b200.DeviceArray` s with
+        ``cuda=True``."""
         ch, _ = self._plan(0, 1)
+        if cuda:
+            x, lp = ch.read_to(self.iteration - 1, 1, 1, (self.nwalkers, self.ndim), (self.nwalkers,))
+            return State(x, log_prob=lp, blobs=None, random_state=self.random_state)
         x, lp = ch.read(self.iteration - 1, 1, 1)
         return State(x[0], log_prob=lp[0], blobs=None, random_state=self.random_state)
 

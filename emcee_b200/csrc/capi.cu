@@ -261,6 +261,7 @@ static int check_status(eb_ctx* c) {
   cudaStreamSynchronize(c->st.get());
   if (f & FLAG_COMM_TIMEOUT) FAIL(c, EB_ERR_COMM, "peer-memory barrier timed out: another rank did not arrive");
   if (f & FLAG_WAIT_TIMEOUT) FAIL(c, EB_ERR_CUDA, "kernel stalled: a warp waited ~2 minutes for a hand-off in its block");
+  if (f & FLAG_NAN_INITIAL) FAIL(c, EB_ERR_NAN_INITIAL, "The initial log_prob was NaN");  // ensemble.py:357-358
   if (f & FLAG_INF_PARAM) FAIL(c, EB_ERR_INF_PARAM, "At least one parameter value was infinite");
   if (f & FLAG_NAN_PARAM) FAIL(c, EB_ERR_NAN_PARAM, "At least one parameter value was NaN");
   FAIL(c, EB_ERR_NAN_LOGPROB, "Probability function returned NaN");
@@ -518,9 +519,13 @@ static int ensure_blob_buffers(eb_ctx* c, size_t record_bytes) {
   return EB_OK;
 }
 
-// m records of `width` bytes, `spitch` apart in src (device or host memory), packed into dst (eb_callback_result,
-// eb_callback_blobs): ordered after the producer's work, complete when this returns
-static int copy_records(eb_ctx* c, void* dst, const void* src, size_t width, size_t spitch, size_t m,
+}  // extern "C"
+
+// m records of `width` bytes, `spitch` apart in src (device or host memory), packed into dst on stream st
+// (eb_callback_result, eb_callback_blobs, the device-memory transfers): ordered after the producer's work, complete
+// when this returns.  Obj: anything with an `err` string (FAIL / CK)
+template <class Obj>
+static int copy_ordered(Obj* c, cudaStream_t st, void* dst, const void* src, size_t width, size_t spitch, size_t m,
                         uint64_t src_stream) {
   if (src_stream == EB_STREAM_UNKNOWN) {
     // a producer that names no stream (CUDA Array Interface v2, e.g. torch): its last kernel may be on any
@@ -534,15 +539,42 @@ static int copy_records(eb_ctx* c, void* dst, const void* src, size_t width, siz
     EventPtr ev;
     CK(c, event_create(ev, cudaEventDisableTiming));
     CK(c, cudaEventRecord(ev.get(), s));
-    CK(c, cudaStreamWaitEvent(c->st.get(), ev.get(), 0));
+    CK(c, cudaStreamWaitEvent(st, ev.get(), 0));
   }
   if (spitch == width || m == 1)
-    CK(c, cudaMemcpyAsync(dst, src, width * m, cudaMemcpyDefault, c->st.get()));
+    CK(c, cudaMemcpyAsync(dst, src, width * m, cudaMemcpyDefault, st));
   else
-    CK(c, cudaMemcpy2DAsync(dst, width, src, spitch, width, m, cudaMemcpyDefault, c->st.get()));
-  CK(c, cudaStreamSynchronize(c->st.get()));  // the caller may free or reuse src as soon as this returns
+    CK(c, cudaMemcpy2DAsync(dst, width, src, spitch, width, m, cudaMemcpyDefault, st));
+  CK(c, cudaStreamSynchronize(st));  // the caller may free or reuse src as soon as this returns
   return EB_OK;
 }
+
+static int copy_records(eb_ctx* c, void* dst, const void* src, size_t width, size_t spitch, size_t m,
+                        uint64_t src_stream) {
+  return copy_ordered(c, c->st.get(), dst, src, width, spitch, m, src_stream);
+}
+
+// a pointer the device-memory transfers take (eb_set_state_from, ...): device or managed memory of `device`
+template <class Obj>
+static int check_device_ptr(Obj* c, int device, const void* p, const char* who, const char* what) {
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    FAIL(c, EB_ERR_INVALID, "%s: %s is not CUDA memory (%s)", who, what, cudaGetErrorString(e));
+  }
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+    FAIL(c, EB_ERR_INVALID, "%s: %s is not device memory", who, what);
+  if (a.device != device) FAIL(c, EB_ERR_INVALID, "%s: %s is on device %d, not on device %d", who, what, a.device, device);
+  return EB_OK;
+}
+
+// the first-axis stride of m rows of `row` bytes in device memory: a positive multiple of 8, at least a row
+static bool row_stride_ok(int64_t stride, int64_t row, int64_t m) {
+  return m <= 1 || (stride >= row && stride % 8 == 0);
+}
+
+extern "C" {
 
 int eb_callback_blobs(eb_ctx* c, const void* src, int64_t record_bytes, int64_t stride_bytes, int64_t m,
                       uint64_t src_stream) {
@@ -768,6 +800,16 @@ static int ensure_scratch(eb_ctx* c, size_t rows) {
   return EB_OK;
 }
 
+// scratch_lp[m] = the log-probabilities of scratch_x[m] (compute_log_prob): the model's kernel, or the function
+static int evaluate_scratch(eb_ctx* c, size_t m) {
+  if (c->model.kind == MODEL_EXTERNAL) {
+    c->cb_phase = CB_COMPUTE;
+    return run_callback(c, c->scratch_x.get(), (int64_t)m, c->scratch_lp.get(), true);
+  }
+  CK(c, launch_logprob(c, c->scratch_x.get(), (int64_t)m, c->scratch_lp.get()));
+  return EB_OK;
+}
+
 int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -779,14 +821,34 @@ int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) 
   if (rc) return rc;
   CK(c, cudaMemcpyAsync(c->scratch_x.get(), coords, m * (size_t)c->D * sizeof(double), cudaMemcpyHostToDevice,
                         c->st.get()));
-  if (c->model.kind == MODEL_EXTERNAL) {
-    c->cb_phase = CB_COMPUTE;
-    rc = run_callback(c, c->scratch_x.get(), (int64_t)m, c->scratch_lp.get(), true);
-    if (rc) return rc;
-  } else {
-    CK(c, launch_logprob(c, c->scratch_x.get(), (int64_t)m, c->scratch_lp.get()));
-  }
+  rc = evaluate_scratch(c, m);
+  if (rc) return rc;
   CK(c, cudaMemcpyAsync(out, c->scratch_lp.get(), m * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
+  return fetch_status(c);
+}
+
+int eb_compute_log_prob_from(eb_ctx* c, const void* coords, int64_t row_stride_bytes, int64_t m, double* out_dst,
+                             uint64_t src_stream) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1)
+    FAIL(c, EB_ERR_UNSUPPORTED, "eb_compute_log_prob_from: sharded ensembles take coordinates from host memory");
+  if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_compute_log_prob_from: no model set");
+  if (m < 0) FAIL(c, EB_ERR_INVALID, "eb_compute_log_prob_from: negative row count");
+  if (m == 0) return EB_OK;
+  if (!coords || !out_dst) FAIL(c, EB_ERR_INVALID, "eb_compute_log_prob_from: null buffer");
+  const int64_t row = (int64_t)c->D * (int64_t)sizeof(double);
+  if (!row_stride_ok(row_stride_bytes, row, m))
+    FAIL(c, EB_ERR_INVALID, "eb_compute_log_prob_from: the row stride must be a multiple of 8 bytes, at least %lld (got %lld)",
+         (long long)row, (long long)row_stride_bytes);
+  CK(c, cudaSetDevice(c->device));
+  int rc = check_device_ptr(c, c->device, coords, "eb_compute_log_prob_from", "coords");
+  if (!rc) rc = check_device_ptr(c, c->device, out_dst, "eb_compute_log_prob_from", "out_dst");
+  if (!rc) rc = ensure_scratch(c, (size_t)m);
+  if (!rc) rc = copy_records(c, c->scratch_x.get(), coords, (size_t)row, (size_t)row_stride_bytes, (size_t)m, src_stream);
+  if (!rc) rc = evaluate_scratch(c, (size_t)m);
+  if (rc) return rc;
+  CK(c, cudaMemcpyAsync(out_dst, c->scratch_lp.get(), (size_t)m * sizeof(double), cudaMemcpyDefault, c->st.get()));
   return fetch_status(c);
 }
 
@@ -836,6 +898,23 @@ static int sync_replicas(eb_ctx* c) {
   return EB_OK;
 }
 
+// the initial log-probabilities of the uploaded rows [r0, r0 + rows) (ensemble.py:350-358); a user function's
+// records of that evaluation become the state's blobs
+static int evaluate_initial(eb_ctx* c, int64_t r0, size_t rows) {
+  if (c->model.kind != MODEL_EXTERNAL) {
+    CK(c, launch_logprob(c, c->coords.get() + (size_t)r0 * c->D, (int64_t)rows, c->logp.get() + r0));
+    return EB_OK;
+  }
+  c->cb_phase = CB_SET_STATE;
+  int rc = run_callback(c, c->coords.get(), (int64_t)rows, c->logp.get(), true);  // one GPU: rows == nwalkers
+  if (rc) return rc;
+  if (c->cb_blob_rows >= 0) {  // the records went to blob_live: they fix the live layout
+    c->blob_bytes = c->cb_blob_bytes;
+    c->blobs_live = true;
+  }
+  return EB_OK;
+}
+
 int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -869,16 +948,9 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   if (log_prob) {
     CK(c, cudaMemcpyAsync(c->logp.get() + r0, log_prob + r0, rows * sizeof(double), cudaMemcpyHostToDevice,
                           c->st.get()));
-  } else if (c->model.kind == MODEL_EXTERNAL) {
-    c->cb_phase = CB_SET_STATE;
-    int rc = run_callback(c, c->coords.get(), (int64_t)rows, c->logp.get(), true);  // one GPU: rows == nwalkers
-    if (rc) return rc;
-    if (c->cb_blob_rows >= 0) {  // the records went to blob_live: they fix the live layout
-      c->blob_bytes = c->cb_blob_bytes;
-      c->blobs_live = true;
-    }
   } else {
-    CK(c, launch_logprob(c, c->coords.get() + (size_t)r0 * D, (int64_t)rows, c->logp.get() + r0));
+    int rc = evaluate_initial(c, r0, rows);
+    if (rc) return rc;
   }
   if (c->comm.nranks > 1) {
     if (c->comm.mode == EB_COMM_ALLGATHER && comm_gather_coords(c->comm, c->st.get(), launches))
@@ -907,6 +979,67 @@ int eb_get_state(eb_ctx* c, double* coords, double* log_prob) {
                           c->st.get()));
   if (log_prob)
     CK(c, cudaMemcpyAsync(log_prob, c->logp.get(), (size_t)c->N * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  return EB_OK;
+}
+
+int eb_set_state_from(eb_ctx* c, const void* coords, int64_t coords_row_stride_bytes, const void* log_prob,
+                      int64_t lp_stride_bytes, uint64_t src_stream) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1)
+    FAIL(c, EB_ERR_UNSUPPORTED, "eb_set_state_from: sharded ensembles take their state from host memory (eb_set_state)");
+  if (!coords) FAIL(c, EB_ERR_INVALID, "eb_set_state_from: coords is null");
+  if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_set_state_from: no model set");
+  const int64_t row = (int64_t)c->D * (int64_t)sizeof(double);
+  if (!row_stride_ok(coords_row_stride_bytes, row, c->N))
+    FAIL(c, EB_ERR_INVALID, "eb_set_state_from: the row stride of coords must be a multiple of 8 bytes, at least %lld (got %lld)",
+         (long long)row, (long long)coords_row_stride_bytes);
+  if (log_prob && !row_stride_ok(lp_stride_bytes, (int64_t)sizeof(double), c->N))
+    FAIL(c, EB_ERR_INVALID, "eb_set_state_from: the stride of log_prob must be a positive multiple of 8 bytes (got %lld)",
+         (long long)lp_stride_bytes);
+  CK(c, cudaSetDevice(c->device));
+  int rc = check_device_ptr(c, c->device, coords, "eb_set_state_from", "coords");
+  if (!rc && log_prob) rc = check_device_ptr(c, c->device, log_prob, "eb_set_state_from", "log_prob");
+  if (rc) return rc;
+  const size_t N = (size_t)c->N;
+  c->have_state = false;
+  c->chain_ok = false;
+  c->blobs_live = false;  // as eb_set_state: a given log_prob comes without blobs
+  c->blob_bytes = 0;
+  rc = copy_records(c, c->coords.get(), coords, (size_t)row, (size_t)coords_row_stride_bytes, N, src_stream);
+  if (rc) return rc;
+  if (log_prob) {
+    // the first copy already waited for src_stream
+    rc = copy_records(c, c->logp.get(), log_prob, sizeof(double), (size_t)lp_stride_bytes, N, 0);
+    if (rc) return rc;
+    CK(c, launch_flag_nan(c->logp.get(), N, FLAG_NAN_INITIAL, c->status_dev.get(), c->st.get()));
+  } else {
+    rc = evaluate_initial(c, 0, N);
+    if (rc) return rc;
+  }
+  rc = fetch_status(c);
+  if (rc) return rc;
+  c->have_state = true;
+  return EB_OK;
+}
+
+int eb_get_state_to(eb_ctx* c, double* coords_dst, double* log_prob_dst) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1)
+    FAIL(c, EB_ERR_UNSUPPORTED, "eb_get_state_to: sharded ensembles return their state in host memory (eb_get_state)");
+  if (!c->have_state) FAIL(c, EB_ERR_STATE, "eb_get_state_to: no state set");
+  CK(c, cudaSetDevice(c->device));
+  int rc = coords_dst ? check_device_ptr(c, c->device, coords_dst, "eb_get_state_to", "coords_dst") : EB_OK;
+  if (!rc && log_prob_dst) rc = check_device_ptr(c, c->device, log_prob_dst, "eb_get_state_to", "log_prob_dst");
+  if (rc) return rc;
+  c->chain_ok = false;
+  if (coords_dst)
+    CK(c, cudaMemcpyAsync(coords_dst, c->coords.get(), (size_t)c->N * c->D * sizeof(double), cudaMemcpyDefault,
+                          c->st.get()));
+  if (log_prob_dst)
+    CK(c, cudaMemcpyAsync(log_prob_dst, c->logp.get(), (size_t)c->N * sizeof(double), cudaMemcpyDefault, c->st.get()));
   CK(c, cudaStreamSynchronize(c->st.get()));
   return EB_OK;
 }
@@ -2257,11 +2390,10 @@ int eb_chain_write(eb_chain* ch, uint64_t slot, const double* coords, const doub
   return EB_OK;
 }
 
-int eb_chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* coords, double* log_prob) {
-  if (!ch) return EB_ERR_INVALID;
-  int rc = chain_check_slice(ch, "eb_chain_read", first, stride, count);
-  if (rc) return rc;
-  CK(ch, cudaSetDevice(ch->device));
+// eb_chain_read (kind = cudaMemcpyDeviceToHost) and eb_chain_read_to (cudaMemcpyDefault, device to device): one copy
+// per run of the slice inside a segment
+static int chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* coords, double* log_prob,
+                      cudaMemcpyKind kind) {
   const size_t N = (size_t)ch->N, nx = N * ch->D;
   cudaError_t e = cudaSuccess;
   for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
@@ -2269,15 +2401,35 @@ int eb_chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count,
                        if (coords && e == cudaSuccess)
                          e = copy_rows(coords + k0 * nx, nx * sizeof(double), ch->segs[s].x.get() + off * ch->xs,
                                        stride * ch->xs * sizeof(double), nx * sizeof(double), n,
-                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st.get());
+                                       kind, ch->max_pitch, ch->st.get());
                        if (log_prob && e == cudaSuccess)
                          e = copy_rows(log_prob + k0 * N, N * sizeof(double), ch->segs[s].lp.get() + off * ch->ls,
                                        stride * ch->ls * sizeof(double), N * sizeof(double), n,
-                                       cudaMemcpyDeviceToHost, ch->max_pitch, ch->st.get());
+                                       kind, ch->max_pitch, ch->st.get());
                      });
   CK(ch, e);
   CK(ch, cudaStreamSynchronize(ch->st.get()));
   return EB_OK;
+}
+
+int eb_chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* coords, double* log_prob) {
+  if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_slice(ch, "eb_chain_read", first, stride, count);
+  if (rc) return rc;
+  CK(ch, cudaSetDevice(ch->device));
+  return chain_read(ch, first, stride, count, coords, log_prob, cudaMemcpyDeviceToHost);
+}
+
+int eb_chain_read_to(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* coords_dst,
+                     double* log_prob_dst) {
+  if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_slice(ch, "eb_chain_read_to", first, stride, count);
+  if (rc || count == 0) return rc;
+  CK(ch, cudaSetDevice(ch->device));
+  if (coords_dst) rc = check_device_ptr(ch, ch->device, coords_dst, "eb_chain_read_to", "coords_dst");
+  if (!rc && log_prob_dst) rc = check_device_ptr(ch, ch->device, log_prob_dst, "eb_chain_read_to", "log_prob_dst");
+  if (rc) return rc;
+  return chain_read(ch, first, stride, count, coords_dst, log_prob_dst, cudaMemcpyDefault);
 }
 
 int eb_chain_accepted(eb_chain* ch, double* accepted) {
@@ -2860,6 +3012,93 @@ int eb_host_free(void* ptr) {
     return EB_ERR_CUDA;
   }
   return EB_OK;
+}
+
+}  // extern "C"
+
+// the device-memory calls without a context (eb_device_alloc, ...): FAIL / CK write here, and the entry point hands
+// the message to eb_last_error(NULL)
+struct NoCtx {
+  std::string err;
+};
+
+static int no_ctx_result(const NoCtx& o, int rc) {
+  if (rc) g_create_err = o.err;
+  return rc;
+}
+
+static int select_device(NoCtx* o, const char* who, int device) {
+  int ndev = 0;
+  CK(o, cudaGetDeviceCount(&ndev));
+  if (device < 0 || device >= ndev) FAIL(o, EB_ERR_INVALID, "%s: device index %d out of range", who, device);
+  CK(o, cudaSetDevice(device));
+  return EB_OK;
+}
+
+static int device_alloc(NoCtx* o, int device, size_t bytes, void** out) {
+  if (bytes == 0) return EB_OK;  // NULL, as the CUDA Array Interface allows for an empty array
+  int rc = select_device(o, "eb_device_alloc", device);
+  if (rc) return rc;
+  size_t free_b = 0, total_b = 0;
+  CK(o, cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > total_b)  // decided before any allocation
+    FAIL(o, EB_ERR_NOMEM, "eb_device_alloc: %zu bytes, more than the device's %zu bytes in total (%zu free)", bytes,
+         total_b, free_b);
+  DevPtr<void> p;
+  const cudaError_t e = dev_alloc(p, bytes);
+  if (e != cudaSuccess) cudaMemGetInfo(&free_b, &total_b);
+  CK_NOMEM(o, e, "eb_device_alloc: %zu bytes, %zu bytes free (%s)", bytes, free_b, cudaGetErrorString(alloc_err));
+  *out = p.release();
+  return EB_OK;
+}
+
+static int device_copy(NoCtx* o, int device, void* dst, const void* src, int64_t width, int64_t src_pitch,
+                       int64_t rows, uint64_t src_stream) {
+  if (width < 0 || rows < 0) FAIL(o, EB_ERR_INVALID, "eb_device_copy: negative size");
+  if (width == 0 || rows == 0) return EB_OK;
+  if (!dst || !src) FAIL(o, EB_ERR_INVALID, "eb_device_copy: null buffer");
+  if (rows > 1 && src_pitch < width)
+    FAIL(o, EB_ERR_INVALID, "eb_device_copy: the source pitch (%lld bytes) is shorter than a row (%lld bytes)",
+         (long long)src_pitch, (long long)width);
+  int rc = select_device(o, "eb_device_copy", device);
+  if (rc) return rc;
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, src) != cudaSuccess) cudaGetLastError();  // not CUDA memory: a host source
+  if ((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device != device)
+    FAIL(o, EB_ERR_INVALID, "eb_device_copy: src is on device %d, not on device %d", a.device, device);
+  StreamPtr st;
+  CK(o, stream_create(st, cudaStreamNonBlocking));
+  return copy_ordered(o, st.get(), dst, src, (size_t)width, (size_t)src_pitch, (size_t)rows, src_stream);
+}
+
+extern "C" {
+
+int eb_device_alloc(int device, size_t bytes, void** out) {
+  if (!out) return EB_ERR_INVALID;
+  *out = nullptr;
+  NoCtx o;
+  return no_ctx_result(o, device_alloc(&o, device, bytes, out));
+}
+
+int eb_device_free(int device, void* p) {
+  if (!p) return EB_OK;
+  NoCtx o;
+  int rc = select_device(&o, "eb_device_free", device);
+  if (!rc) {
+    const cudaError_t e = cudaFree(p);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      o.err = std::string("eb_device_free: ") + cudaGetErrorString(e);
+      rc = EB_ERR_CUDA;
+    }
+  }
+  return no_ctx_result(o, rc);
+}
+
+int eb_device_copy(int device, void* dst, const void* src, int64_t width, int64_t src_pitch, int64_t rows,
+                   uint64_t src_stream) {
+  NoCtx o;
+  return no_ctx_result(o, device_copy(&o, device, dst, src, width, src_pitch, rows, src_stream));
 }
 
 // ---- multi-GPU ---------------------------------------------------------------

@@ -23,6 +23,7 @@ enum : int {
   FLAG_NAN_PARAM = 4,
   FLAG_COMM_TIMEOUT = 8,
   FLAG_WAIT_TIMEOUT = 16,  // a warp gave up on an in-kernel hand-off (shared-memory barrier) of its own CTA
+  FLAG_NAN_INITIAL = 32,   // a NaN in an initial log_prob given in device memory (eb_set_state_from)
 };
 
 struct ModelDev {
@@ -133,6 +134,8 @@ cudaError_t launch_split_gather(const double* coords, const int32_t* order, int6
                                 double* out, cudaStream_t st);
 // status |= FLAG_NAN_LOGPROB if any of x[n] is NaN (logprob != 0), else the non-finite parameter flags of x[n]
 cudaError_t launch_scan_nonfinite(const double* x, size_t n, int logprob, int* status, cudaStream_t st);
+// cuda_arrays.cu: status |= flag if any of x[n] is NaN
+cudaError_t launch_flag_nan(const double* x, size_t n, int flag, int* status, cudaStream_t st);
 // the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)
 struct TmaVariant {
   int R;        // walkers per tile (G = 32 / R lanes per walker)

@@ -38,6 +38,18 @@ _NO_SHARDED_HISTOGRAMS = "running histograms are counted on one GPU; they cannot
 _NO_HISTOGRAMS = "running histograms are not enabled: call enable_histograms(range, ...) first"
 _NO_SHARDED_TRACE = "the running trace is recorded on one GPU; it cannot be combined with a sharded ensemble"
 _NO_TRACE = "the running trace is not enabled: call enable_trace() first"
+_NO_SHARDED_CUDA_ARRAYS = (
+    "CUDA arrays in and out are copied on one GPU; a sharded ensemble takes and returns host arrays"
+)
+_NO_CUDA_STATE_BLOBS = (
+    "a state given as CUDA arrays cannot carry blobs; pass host arrays, or leave log_prob out so that the "
+    "function's blobs of the initial evaluation become the state's"
+)
+_NOT_INDEPENDENT = (
+    "Initial state has a large condition number. "
+    "Make sure that your walkers are linearly independent for the "
+    "best performance"
+)
 
 #: what :meth:`EnsembleSampler.trace` returns: one entry per recorded step
 Trace = namedtuple("Trace", ["step", "mean", "var", "log_prob_mean", "log_prob_max", "accepted"])
@@ -59,7 +71,15 @@ class EnsembleSampler(object):
     ``pinned_results`` (the yielded / returned ``State`` arrays are views of two
     page-locked buffers owned by the sampler and are overwritten by the next
     step -- full-speed D2H for callers that consume each state before asking for
-    the next; default ``False`` = fresh arrays, as the reference returns)."""
+    the next; default ``False`` = fresh arrays, as the reference returns) and
+    ``cuda_results`` (every yielded / returned ``State`` holds fresh
+    :class:`~emcee_b200.DeviceArray` coords and log_prob, copied inside the GPU's
+    memory; blobs still come back as host arrays; not with ``pinned_results``, and
+    not on a sharded ensemble).
+
+    ``sample`` / ``run_mcmc`` and ``compute_log_prob`` also take CUDA arrays
+    (anything with the CUDA Array Interface: torch, CuPy, Numba, ``DeviceArray``),
+    uploaded inside the GPU's memory after the work of the stream they name."""
 
     def __init__(
         self,
@@ -84,6 +104,7 @@ class EnsembleSampler(object):
         seed=None,
         device=0,
         pinned_results=False,
+        cuda_results=False,
     ):
         for name, val in (("a", a), ("postargs", postargs), ("threads", threads),
                           ("live_dangerously", live_dangerously), ("runtime_sortingfn", runtime_sortingfn)):
@@ -108,6 +129,9 @@ class EnsembleSampler(object):
                 "blobs_dtype: pass it to models.HostFunction / models.CudaArrayFunction(fn, blobs_dtype=...)")
         if isinstance(backend, DeviceBackend) and getattr(log_prob_fn, "blobs_dtype", None) is not None:
             raise NotImplementedError(_NO_DEVICE_CHAIN_BLOBS)
+        if cuda_results and pinned_results:
+            raise ValueError("cuda_results and pinned_results exclude each other: a state is returned in device "
+                             "memory or in page-locked host memory")
 
         # move schedule (ensemble.py:115-129)
         if moves is None:
@@ -149,6 +173,7 @@ class EnsembleSampler(object):
         self._pinned = None
         if pinned_results:
             self._pinned = (_lib.pinned_empty((self.nwalkers, self.ndim)), _lib.pinned_empty((self.nwalkers,)))
+        self._cuda_results = bool(cuda_results)
         self._rdv = None  # multi-GPU: the host rendezvous this sampler is attached to (``attach``)
         self._hist = None  # running histograms: the configuration of enable_histograms (edges, pairs)
         self._trace_every = None  # running trace: the cadence its rows were recorded with (enable_trace)
@@ -273,6 +298,8 @@ class EnsembleSampler(object):
 
         if isinstance(self.backend, DeviceBackend):
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
+        if getattr(self, "_cuda_results", False):
+            raise NotImplementedError("cuda_results=True: " + _NO_SHARDED_CUDA_ARRAYS)
         if getattr(self, "_hist", None) is not None:
             raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
         if getattr(self, "_trace_every", None) is not None:
@@ -507,26 +534,25 @@ class EnsembleSampler(object):
         # the yielded State gets its own arrays from the first device read-back
         state = State(initial_state)
         state = State(state.coords, log_prob=state.log_prob, blobs=state.blobs, random_state=state.random_state)
-        state_shape = np.shape(state.coords)
-        if state_shape != (self.nwalkers, self.ndim):
-            raise ValueError("incompatible input dimensions {0}".format(state_shape))
-        if state.blobs is not None and not has_blobs:
-            raise NotImplementedError(
-                "the state carries blobs, but the log-probability function declares none "
-                "(models.HostFunction / models.CudaArrayFunction(fn, blobs_dtype=...))")
-        if (not skip_initial_state_check) and (not self._walkers_independent(state.coords)):
-            raise ValueError(
-                "Initial state has a large condition number. "
-                "Make sure that your walkers are linearly independent for the "
-                "best performance"
-            )
-        self.random_state = state.random_state  # ensemble.py:335 (ignored if None/foreign)
+        if _lib.is_cuda_array(state.coords) or _lib.is_cuda_array(state.log_prob):
+            self._set_cuda_state(state, skip_initial_state_check)
+        else:
+            state_shape = np.shape(state.coords)
+            if state_shape != (self.nwalkers, self.ndim):
+                raise ValueError("incompatible input dimensions {0}".format(state_shape))
+            if state.blobs is not None and not has_blobs:
+                raise NotImplementedError(
+                    "the state carries blobs, but the log-probability function declares none "
+                    "(models.HostFunction / models.CudaArrayFunction(fn, blobs_dtype=...))")
+            if (not skip_initial_state_check) and (not self._walkers_independent(state.coords)):
+                raise ValueError(_NOT_INDEPENDENT)
+            self.random_state = state.random_state  # ensemble.py:335 (ignored if None/foreign)
 
-        if state.log_prob is not None and np.shape(state.log_prob) != (self.nwalkers,):
-            raise ValueError("incompatible input dimensions")
-        # upload; a missing log_prob is evaluated on the device (ensemble.py:350-358), and a blob function's
-        # records of that evaluation become the state's blobs
-        self._engine.set_state(state.coords, state.log_prob, state.blobs if state.log_prob is not None else None)
+            if state.log_prob is not None and np.shape(state.log_prob) != (self.nwalkers,):
+                raise ValueError("incompatible input dimensions")
+            # upload; a missing log_prob is evaluated on the device (ensemble.py:350-358), and a blob function's
+            # records of that evaluation become the state's blobs
+            self._engine.set_state(state.coords, state.log_prob, state.blobs if state.log_prob is not None else None)
         eng = self._engine
         if has_blobs:
             state.blobs = eng.get_blobs()
@@ -553,7 +579,9 @@ class EnsembleSampler(object):
         def refresh():
             bufs = self._pinned if self._pinned is not None else (
                 np.empty((self.nwalkers, self.ndim)), np.empty(self.nwalkers))
-            if self._rdv is not None and not self._gather_results:
+            if getattr(self, "_cuda_results", False):
+                state.coords, state.log_prob = eng.get_state_to()  # device to device: nothing crosses PCIe
+            elif self._rdv is not None and not self._gather_results:
                 r0, n = eng.owned_rows()  # sharded: only the owned block crosses PCIe
                 state.coords, state.log_prob = eng.get_state_rows(r0, n, *bufs)
             else:
@@ -632,6 +660,26 @@ class EnsembleSampler(object):
         if pbar is not None:
             pbar.close()
 
+    def _set_cuda_state(self, state, skip_initial_state_check):
+        """The upload of a state given as CUDA arrays (``eb_set_state_from``), with the host path's checks in its
+        order.  With ``skip_initial_state_check=False`` the coordinates are downloaded once for
+        :meth:`_walkers_independent`: that check is the reference's numpy on the host, bit for bit.  With ``True``
+        nothing crosses PCIe."""
+        if self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_CUDA_ARRAYS)
+        if not _lib.is_cuda_array(state.coords) or not (state.log_prob is None or _lib.is_cuda_array(state.log_prob)):
+            raise TypeError("the initial coords and log_prob must both be CUDA arrays, or both host arrays")
+        coords = _lib.CudaRows(state.coords, (self.nwalkers, self.ndim), self._device, "coords")
+        if state.blobs is not None:
+            raise NotImplementedError(_NO_CUDA_STATE_BLOBS)
+        if (not skip_initial_state_check) and (not self._walkers_independent(coords.download(self._device))):
+            raise ValueError(_NOT_INDEPENDENT)
+        self.random_state = state.random_state  # ensemble.py:335 (ignored if None/foreign)
+        lp = None
+        if state.log_prob is not None:
+            lp = _lib.CudaRows(state.log_prob, (self.nwalkers,), self._device, "log_prob")
+        self._engine.set_state_from(coords, lp)
+
     def run_mcmc(self, initial_state, nsteps, **kwargs):
         """Iterate :func:`sample` for ``nsteps`` iterations and return the last
         state (``ensemble.py:426-456``); ``initial_state=None`` resumes."""
@@ -691,7 +739,18 @@ class EnsembleSampler(object):
         """``(log_prob, blobs)`` for ``coords[..., ndim]`` evaluated on the device, or by the user
         function in one call (``ensemble.py:458-553``); ``blobs`` is None unless the function declares
         ``blobs_dtype``.  Raises ``ValueError`` for non-finite parameters or a NaN log-probability like
-        the reference."""
+        the reference.
+
+        ``coords`` may be a CUDA array of shape ``[m, ndim]`` (rows contiguous, the first axis may be strided):
+        the result is then ``(DeviceArray[m], None)``, and nothing crosses PCIe.  A function declared with
+        ``blobs_dtype`` takes host arrays only."""
+        if _lib.is_cuda_array(coords):
+            if self._rdv is not None:
+                raise NotImplementedError(_NO_SHARDED_CUDA_ARRAYS)
+            if self.blobs_dtype is not None:
+                raise NotImplementedError("compute_log_prob of a function with blobs_dtype takes host arrays: blobs "
+                                          "do not come back as CUDA arrays")
+            return self._engine.compute_log_prob_from(coords), None
         coords = np.asarray(coords, dtype=np.float64)
         if self.blobs_dtype is not None:
             return self._engine.compute_log_prob_blobs(coords)
@@ -712,6 +771,10 @@ class EnsembleSampler(object):
         return self.get_value("log_prob", **kwargs)
 
     def get_last_sample(self, **kwargs):
+        """The backend's last stored ``State``; ``cuda=True`` (a ``DeviceBackend``) returns it as
+        :class:`~emcee_b200.DeviceArray` s."""
+        if "cuda" in kwargs:
+            return self.backend.get_last_sample(cuda=kwargs["cuda"])
         return self.backend.get_last_sample()
 
     def get_value(self, name, **kwargs):

@@ -1,9 +1,11 @@
 """Host mirror of the ensemble state (reference: ``src/emcee/state.py:10-75``).
 
 The live walker positions and log-probabilities stay in HBM inside the engine;
-a ``State`` is the host-side snapshot handed to / received from the user, with
-the reference's attribute names, copy semantics and tuple-unpacking
-back-compat."""
+a ``State`` is the snapshot handed to / received from the user, with the
+reference's attribute names, copy semantics and tuple-unpacking back-compat.
+Its arrays are host arrays, or CUDA arrays (anything with the CUDA Array
+Interface, such as ``emcee_b200.DeviceArray`` or a torch tensor on the GPU)
+for callers that keep their data on the device."""
 
 import copy as _copy
 
@@ -15,7 +17,8 @@ __all__ = ["State"]
 class State(object):
     """Snapshot of the ensemble: ``coords[nwalkers, ndim]``, ``log_prob[nwalkers]``,
     ``blobs`` (``[nwalkers, ...]`` records of a user function declared with ``blobs_dtype``, else ``None``)
-    and ``random_state``.
+    and ``random_state``.  ``coords`` and ``log_prob`` may be CUDA arrays: they are kept as they are (the
+    reference's ``np.atleast_2d`` would copy them to the host).
 
     Iterating yields ``coords, log_prob, random_state`` (plus ``blobs`` when
     present), as the reference does for pre-3.0 callers (``state.py:47-75``)."""
@@ -27,7 +30,9 @@ class State(object):
         if other is not None:
             fields = (other.coords, other.log_prob, other.blobs, other.random_state)
         else:
-            fields = (np.atleast_2d(coords), log_prob, blobs, random_state)  # state.py:42
+            if not hasattr(coords, "__cuda_array_interface__"):
+                coords = np.atleast_2d(coords)  # state.py:42
+            fields = (coords, log_prob, blobs, random_state)
         if copy:
             fields = tuple(_copy.deepcopy(f) for f in fields)
         self.coords, self.log_prob, self.blobs, self.random_state = fields

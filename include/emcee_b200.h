@@ -379,6 +379,47 @@ int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, 
 int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, const uint32_t* params,
                          size_t nparams, uint32_t bins, const double* edges, uint64_t* hist);
 
+/* ---- device memory in and out (CUDA Array Interface) --------------------- */
+/* The device twins of the state, log-probability and chain transfers above, for callers that keep their arrays
+ * in GPU memory (torch, CuPy, Numba, ...).  Sources are ordered after the producer's work on src_stream with the
+ * encoding of eb_callback_result (CUDA Array Interface v3: 0 = none, 1 = legacy default stream, 2 = per-thread
+ * default stream, else a cudaStream_t; EB_STREAM_UNKNOWN = after all work on the device).  Rows must be
+ * contiguous; only the first axis may be strided (a positive multiple of 8 bytes, at least a row).  Every call
+ * is complete when it returns.  Device pointers must be device (or managed) memory of the context's or chain's
+ * device: another device, or host memory, gives EB_ERR_INVALID.  Sharded engines (eb_comm_init) are refused
+ * with EB_ERR_UNSUPPORTED.  The data moves on the copy engines (cudaMemcpy2DAsync, cudaMemcpyDefault). */
+/* device memory for arrays the caller hands out: bytes on device `device` (0 gives NULL, touching no
+ * device).  More than the device's total memory is refused before cudaMalloc, and a failed allocation is
+ * refused too: both EB_ERR_NOMEM (as eb_chain_grow).  Messages of these three calls: eb_last_error(NULL). */
+int eb_device_alloc(int device, size_t bytes, void** out);
+/* frees what eb_device_alloc returned (NULL is a no-op). */
+int eb_device_free(int device, void* p);
+/* rows of width bytes, src_pitch apart in src (memory of `device`, or host memory), packed into dst (host or
+ * device memory), ordered after src_stream: a CUDA array read back (DeviceArray.get, the host check of an
+ * initial state given on the device), copied or uploaded. */
+int eb_device_copy(int device, void* dst, const void* src, int64_t width, int64_t src_pitch, int64_t rows,
+                   uint64_t src_stream);
+/* eb_set_state from device memory (State(initial_state, copy=True) + the initial compute_log_prob,
+ * ensemble.py:312,350-358; state.py:10-45): coords[nwalkers] rows coords_row_stride_bytes apart, log_prob
+ * (nullable) lp_stride_bytes apart.  log_prob == NULL: evaluated on the device with eb_set_state's guards and
+ * callback / blob behaviour.  A given log_prob is checked for NaN on the device (EB_ERR_NAN_INITIAL, "The
+ * initial log_prob was NaN", ensemble.py:357-358). */
+int eb_set_state_from(eb_ctx* ctx, const void* coords, int64_t coords_row_stride_bytes, const void* log_prob,
+                      int64_t lp_stride_bytes, uint64_t src_stream);
+/* eb_get_state into device memory: coords_dst[nwalkers * ndim], log_prob_dst[nwalkers], either may be NULL
+ * (state.py:10-45, the State yielded by ensemble.py:403-424). */
+int eb_get_state_to(eb_ctx* ctx, double* coords_dst, double* log_prob_dst);
+/* eb_compute_log_prob (ensemble.py:458-553) of m rows of device memory, row_stride_bytes apart, into
+ * out_dst[m] (device), with the same guards on the input (:476-479) and the output (:550-551); m == 0 is a
+ * no-op. */
+int eb_compute_log_prob_from(eb_ctx* ctx, const void* coords, int64_t row_stride_bytes, int64_t m, double* out_dst,
+                             uint64_t src_stream);
+/* eb_chain_read into device memory (Backend.get_value, backend.py:42-58): the slots first + k * stride, k <
+ * count, into coords_dst[count, nwalkers, ndim] / log_prob_dst[count, nwalkers] (either may be NULL), device to
+ * device. */
+int eb_chain_read_to(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* coords_dst,
+                     double* log_prob_dst);
+
 /* per-walker number of accepted proposals since creation / eb_reset_counters
  * (numerator of acceptance_fraction, ensemble.py:555-558). */
 int eb_get_naccepted(eb_ctx* ctx, uint64_t* naccepted);
