@@ -1,5 +1,5 @@
-// C ABI of the engine (include/emcee_b200.h): context, host-side step loop,
-// state / model transfer, error mapping.  No torch, no CPU fallback.
+// C ABI of the engine (include/emcee_b200.h): context, state / model transfer, error mapping; the step driver
+// is in step.cu.  No torch, no CPU fallback.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -11,249 +11,17 @@
 #include <vector>
 
 #include "chain_map.h"
-#include "comm.h"
-#include "engine.cuh"
-#include "hist_bins.h"
-#include "owners.h"
-#include "trace_sum.h"
-
-using namespace eb;
-
-// Every buffer, event and stream of an engine or a chain is held by an owner (owners.h), so deleting the object
-// releases them.  A group of buffers that is tested through one of its members is allocated into local owners and
-// moved in only once the whole group exists: a failed call never leaves half a group behind.
-
-// a stored chain in device memory (eb_chain_*): segments of [n, N, D] coords and [n, N] log-probs, one per grow
-struct ChainSeg {
-  DevPtr<double> x;
-  DevPtr<double> lp;
-};
-
-struct eb_chain {
-  int device = 0;
-  int sm_count = 0;
-  int64_t N = 0;
-  int D = 0;
-  size_t xs = 0, ls = 0;  // slot pitches in doubles: N * D and N rounded up to even (16-byte aligned slots)
-  size_t max_pitch = 0;   // cudaMemcpy2D limit; larger strides are copied row by row
-  StreamPtr st;           // declared first among the owners: destroyed after the memory
-  std::vector<ChainSeg> segs;
-  std::vector<uint64_t> start{0};  // segment s holds slots [start[s], start[s + 1])
-  DevPtr<double> accepted;         // [N] float64 (backend.py:31)
-  DevPtr<uint8_t> mask;            // [N] eb_chain_write's accept mask
-  std::string err;
-};
-
-struct eb_ctx {
-  int device = 0;
-  int sm_count = 0;
-  int64_t N = 0;
-  int D = 0;
-  uint64_t seed = 0, step = 0;
-  StreamPtr st;  // declared first among the owners: destroyed after the events and the memory
-  EventPtr ev0, ev1;
-
-  DevPtr<double> coords;  // [N, D], then the peer-memory barrier flags (exported to the peers, comm.h)
-  DevPtr<double> logp;
-  DevPtr<uint8_t> accepted;
-  DevPtr<unsigned long long> nacc;
-  DevPtr<int> status_dev;
-  HostPtr<int> status_host;
-
-  ModelDev model{};
-  DevPtr<double> model_params;
-  DevPtr<double> model_chol;
-  DevPtr<double> model_box;  // [lo[D] | hi[D]] of eb_model_set_bounds, or null
-  bool have_model = false, have_state = false;
-
-  DevPtr<int32_t> order;  // [table_cap, N]
-  size_t table_cap = 0;
-  DevPtr<StepInfo> info_dev;
-  HostPtr<StepInfo> info_host;
-  DevPtr<HalfDesc> descs_dev;  // [table_cap * MAX_SPLITS] half-step descriptors of a chunk (dense_dmma)
-  HostPtr<HalfDesc> descs_host;
-  DevPtr<unsigned long long> gbar;  // grid-barrier counter of the persistent dense_dmma kernel
-  unsigned long long gbar_count = 0;   // arrivals issued so far
-  // split tables already on the device: steps [tbl_step0, tbl_step0 + tbl_n) of key tbl_seed, built with tbl_info
-  uint64_t tbl_seed = 0, tbl_step0 = 0;
-  size_t tbl_n = 0;
-  std::vector<StepInfo> tbl_info;
-
-  DevPtr<double> scratch_x;
-  DevPtr<double> scratch_lp;
-  size_t scratch_rows = 0;
-
-  // pinned staging for eb_step_store
-  HostPtr<double> stage[2];
-  HostPtr<uint8_t> stage_acc[2];
-  EventPtr stage_ev[2];
-
-  bool debug = false;
-  DevPtr<int64_t> tap_partners;
-  DevPtr<double> tap_scalar;
-  DevPtr<double> tap_u;
-  DevPtr<int64_t> tap_active;
-  int64_t tap_count = 0;
-  DevPtr<long long> timeline;  // dense_dmma instrumentation buffer (option "dmma_timeline")
-  bool timeline_first_split = false;  // option "dmma_timeline" = 2: stamp only launches that start a step
-
-  // optional L2 flush between steps (benchmark hygiene): per-step event pairs
-  bool l2_flush = false;
-  DevPtr<void> flush_buf;
-  size_t flush_bytes = (size_t)256 << 20;
-  std::vector<EventPtr> ev_pool;
-
-  double last_ms = 0.0;
-  uint64_t last_launches = 0;
-  const char* last_kernel = "none";
-  char last_variant[96] = "none";  // eb_last_kernel_variant: the parameters the last half-step launch chose
-  int dmma_nhalf_max = 0;          // most half-steps one dense_dmma launch ran in the current stepping call
-  bool allow_dmma = true;
-  int allow_tma = 2;  // TMA row-gather kernel for the HBM-bound models: 0 off, 1 short rows only, 2 long rows too
-  bool tma_own_reg = true;  // tma_rows, stretch rows <= 512 B: own rows through registers instead of the TMA unit
-  bool fused_last = false;  // the last dense_dmma launch carried the P2P barrier itself
-  int dmma_stagger = 1;
-  int dmma_group = 1;  // half-steps per persistent dense_dmma launch (1: a launch per half-step)
-  int pdl = 1;           // dense_dmma launches chain as programmatic dependents (1: one GPU only, 2: sharded too)
-  int local_first = 0;  // sharded dense_dmma: local-partner tiles first, peer barrier behind them (0 never, 1 auto, 2 always)
-  bool chain_ok = false; // the last operation enqueued on the stream is a dense_dmma kernel of this run
-  HalfDesc dmma_first{}, dmma_last{};  // first and last half-step of the last dense_dmma launch (while chain_ok)
-  // multi-GPU: log_prob / accept mask / counters (and, P2P, coords) of rows owned by OTHER ranks are stale
-  // on this rank until the next collective read (eb_get_state, eb_get_naccepted, ...) replicates them
-  bool replicas_dirty = false;
-
-  // running chain moments (eb_moments): sum of (x - shift) and of its outer product over the owned
-  // rows of every `moments_every`-th step
-  uint64_t moments_every = 0;
-  DevPtr<double> mom_acc;      // [D + D*D] accumulators
-  DevPtr<double> mom_shift;    // [D]
-  DevPtr<double> mom_partial;  // per-CTA partials of one accumulation
-  unsigned long long mom_count = 0;
-  bool mom_have_shift = false;
-
-  // running histograms (eb_histograms): the owned rows of every `hist_every`-th step counted into hist.counts
-  uint64_t hist_every = 0;
-  bool hist_on = false;  // configured: hist holds tables and counts
-  LiveHist hist;
-  DevPtr<void> hist_mem;  // hist.mem
-  unsigned long long hist_count = 0;  // samples counted
-
-  // running trace (eb_trace_read): one row [2 D + 4] of ensemble statistics per `trace_every`-th step
-  uint64_t trace_every = 0;
-  bool trace_on = false;  // configured: trace holds its fixed part
-  LiveTrace trace;
-  DevPtr<void> trace_mem;           // trace.mem
-  DevPtr<double> trace_rows;        // [trace_cap, 2 D + 4], device
-  uint64_t trace_cap = 0;
-  std::vector<uint64_t> trace_steps;  // the step counter of each recorded row
-
-  // WalkMove / GaussianMove scratch (moves_extra.cu)
-  DevPtr<double> qbuf;       // [N, D] proposals
-  DevPtr<double> walk_work;  // [D shift | D + D*D moment sums | D*D cov | D*D L]
-  DevPtr<double> gauss_dev;  // per schedule entry: scale / factor L of GaussianMove
-  size_t gauss_cap = 0;
-  std::vector<uint64_t> picks;  // per schedule entry: steps of the last call that ran it
-
-  Comm comm;  // multi-GPU (comm.h)
-
-  // log-probability callback (eb_model_set_callback; model.kind == MODEL_EXTERNAL)
-  eb_logprob_fn cb_fn = nullptr;
-  void* cb_user = nullptr;
-  int cb_where = EB_CALLBACK_HOST;
-  bool in_callback = false;        // every other call on the context is refused while fn runs
-  HostPtr<double> cb_x;            // host mode: pinned [cb_rows, D] proposals
-  HostPtr<double> cb_lp;           // host mode: pinned [cb_rows] results
-  DevPtr<double> cb_xdev;          // device mode: [cb_rows, D] copy of the rows, the function's to overwrite
-  size_t cb_rows = 0;
-  DevPtr<double> ext_f;            // device [N] Hastings factors of the propose phase
-  DevPtr<double> ext_lp;           // device [N] the callback's log-probabilities
-  int cb_phase = 0;                // CB_STEP / CB_SET_STATE / CB_COMPUTE: what the running callback evaluates
-  int64_t cb_m = 0;                // rows of the running callback
-
-  // blobs of a callback model (eb_callback_blobs): packed records of blob_bytes bytes, one per walker
-  size_t blob_bytes = 0;           // the live layout (0: none)
-  bool blobs_live = false;         // blob_live holds the records of the current state
-  DevPtr<uint8_t> blob_live;       // device [N, blob_bytes]
-  DevPtr<uint8_t> blob_prop;       // device [N, blob_bytes] the records of the running half-step's proposals
-  HostPtr<uint8_t> blob_host;      // host mode: pinned [N, blob_bytes] staging of the function's records
-  size_t blob_cap = 0;             // bytes of each of the three buffers
-  int64_t cb_blob_rows = -1;       // records the running callback delivered (-1: none)
-  size_t cb_blob_bytes = 0;        // their size
-  uint8_t* cb_blob_dst = nullptr;  // host mode: where run_callback copies blob_host to, next to the lp copy-back
-  HostPtr<uint8_t> cmp_blobs;      // CB_COMPUTE: pinned [m, record] records handed to the caller
-  HostPtr<uint8_t> stage_blob[2];  // eb_step_store_blobs: pinned [N, blob_bytes] staging
-  size_t stage_blob_cap = 0;
-
-  // user proposals (eb_move_set_proposal), indexed by slot
-  struct ProposalSlot {
-    eb_proposal_fn fn = nullptr;
-    void* user = nullptr;
-    int where = EB_CALLBACK_HOST;
-  };
-  std::vector<ProposalSlot> props;
-  bool in_proposal = false;   // every other call on the context is refused while a proposal runs
-  int up_where = EB_CALLBACK_HOST;  // mode of the running proposal
-  int64_t up_m = 0;           // rows the running proposal returns
-  DevPtr<double> up_x;        // device [N, D] rows handed to the proposal (s | c, or the ensemble)
-  DevPtr<double> up_f;        // device [N] its Hastings factors
-  HostPtr<double> up_hx;      // host mode: pinned [N, D] copy of up_x's rows
-  HostPtr<double> up_hq;      // host mode: pinned [N, D] proposals
-  HostPtr<double> up_hf;      // host mode: pinned [N] factors
-
-  std::string err;
-};
+#include "context.h"
 
 static thread_local std::string g_create_err;
-
-// what a running log-probability callback evaluates: a half-step's proposals, the state of eb_set_state(coords,
-// NULL), or the rows of eb_compute_log_prob -- it decides where eb_callback_blobs puts the records
-enum { CB_STEP = 0, CB_SET_STATE = 1, CB_COMPUTE = 2 };
 
 static const char* const MSG_BLOBS_WITH_LOG_PROB =  // moves/move.py:38-42
     "If you start sampling with a given log_prob, you also need to provide the current list of blobs at that "
     "position.";
 
-#define NOT_IN_CALLBACK(ctx)                                                      \
-  do {                                                                            \
-    if ((ctx)->in_callback || (ctx)->in_proposal) {                               \
-      (ctx)->err = (ctx)->in_callback ? "engine is inside a log-probability callback" \
-                                      : "engine is inside a user proposal";       \
-      return EB_ERR_STATE;                                                        \
-    }                                                                             \
-  } while (0)
-
-#define FAIL(ctx, code, ...)                      \
-  do {                                            \
-    char _b[512];                                 \
-    snprintf(_b, sizeof(_b), __VA_ARGS__);        \
-    (ctx)->err = _b;                              \
-    return (code);                                \
-  } while (0)
-
-#define CK(ctx, call)                                                                      \
-  do {                                                                                     \
-    cudaError_t _e = (call);                                                               \
-    if (_e != cudaSuccess) {                                                               \
-      cudaGetLastError();                                                                  \
-      FAIL(ctx, EB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, \
-           __LINE__);                                                                      \
-    }                                                                                      \
-  } while (0)
-
-// an allocation into an owner (dev_alloc / host_alloc) that fails makes the call fail with EB_ERR_NOMEM; the
-// message may name the CUDA error as cudaGetErrorString(alloc_err)
-#define CK_NOMEM(ctx, call, ...)            \
-  do {                                      \
-    const cudaError_t alloc_err = (call);   \
-    if (alloc_err != cudaSuccess) {         \
-      cudaGetLastError();                   \
-      FAIL(ctx, EB_ERR_NOMEM, __VA_ARGS__); \
-    }                                       \
-  } while (0)
-
 // map (and clear) the device status word to the reference's exceptions, in the
 // order compute_log_prob raises them (ensemble.py:476-479, 550-551)
-static int check_status(eb_ctx* c) {
+int check_status(eb_ctx* c) {
   const int f = *c->status_host;
   if (f == 0) return EB_OK;
   *c->status_host = 0;
@@ -267,7 +35,7 @@ static int check_status(eb_ctx* c) {
   FAIL(c, EB_ERR_NAN_LOGPROB, "Probability function returned NaN");
 }
 
-static int fetch_status(eb_ctx* c) {
+int fetch_status(eb_ctx* c) {
   CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
   CK(c, cudaStreamSynchronize(c->st.get()));
   return check_status(c);
@@ -479,7 +247,6 @@ int eb_model_set_callback(eb_ctx* c, eb_logprob_fn fn, void* user, int where) {
   c->cb_fn = fn;
   c->cb_user = user;
   c->cb_where = where;
-  c->chain_ok = false;
   c->have_model = true;
   c->blob_bytes = 0;
   c->blobs_live = false;
@@ -702,7 +469,6 @@ int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
   }
   CK(c, cudaSetDevice(c->device));
   CK(c, cudaStreamSynchronize(c->st.get()));
-  c->chain_ok = false;
   DevPtr<double> box;
   if (lower) {
     CK(c, dev_alloc(box, 2 * D * sizeof(double)));
@@ -714,6 +480,8 @@ int eb_model_set_bounds(eb_ctx* c, const double* lower, const double* upper) {
   c->model_box = std::move(box);
   return EB_OK;
 }
+
+}  // extern "C"
 
 // ---- log-prob ----------------------------------------------------------------
 // the rows handed to the function for `rows` rows: pinned staging (host mode) or a device copy (device mode)
@@ -740,7 +508,7 @@ static int ensure_callback_staging(eb_ctx* c, size_t rows) {
 // steps 2-7 of a callback half-step (include/emcee_b200.h): the device rows x[m, D] have been enqueued;
 // lp[m] (device) gets the callback's values.  scan_x: the rows were not written by a kernel that raises the
 // non-finite flags (WalkMove / GaussianMove proposals, the caller's coordinates)
-static int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x) {
+int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x) {
   const size_t D = (size_t)c->D;
   if (scan_x) CK(c, launch_scan_nonfinite(x, (size_t)m * D, 0, c->status_dev.get(), c->st.get()));
   int rc = fetch_status(c);  // synchronises; ensemble.py:476-479: the function never sees a non-finite row
@@ -810,6 +578,8 @@ static int evaluate_scratch(eb_ctx* c, size_t m) {
   return EB_OK;
 }
 
+extern "C" {
+
 int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -872,9 +642,11 @@ int eb_compute_log_prob_blobs(eb_ctx* c, const double* coords, size_t m, double*
   return rc;
 }
 
+}  // extern "C"
+
 // ---- state -------------------------------------------------------------------
 // rows [r0, r1) this context owns (the whole ensemble on one GPU)
-static void owned_rows(const eb_ctx* c, int64_t& r0, int64_t& r1) {
+void owned_rows(const eb_ctx* c, int64_t& r0, int64_t& r1) {
   r0 = 0;
   r1 = c->N;
   if (c->comm.nranks > 1) {
@@ -885,10 +657,9 @@ static void owned_rows(const eb_ctx* c, int64_t& r0, int64_t& r1) {
 
 // multi-GPU: make log_prob / accept mask / counters (and coords in P2P mode) of every rank's rows
 // valid on this rank.  COLLECTIVE: every rank calls it at the same point (the Python layer does).
-static int sync_replicas(eb_ctx* c) {
+int sync_replicas(eb_ctx* c) {
   if (c->comm.nranks == 1 || !c->replicas_dirty) return EB_OK;
   uint64_t launches = 0;
-  c->chain_ok = false;
   if (comm_sync_state(c->comm, c->st.get(), c->status_dev.get(), c->logp.get(), c->accepted.get(), c->nacc.get(),
                       launches))
     FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
@@ -915,6 +686,8 @@ static int evaluate_initial(eb_ctx* c, int64_t r0, size_t rows) {
   return EB_OK;
 }
 
+extern "C" {
+
 int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -923,7 +696,6 @@ int eb_set_state(eb_ctx* c, const double* coords, const double* log_prob) {
   CK(c, cudaSetDevice(c->device));
   const size_t D = (size_t)c->D;
   c->have_state = false;
-  c->chain_ok = false;
   c->blobs_live = false;  // a given log_prob comes without blobs (eb_set_state_blobs adds them)
   c->blob_bytes = 0;
   if (log_prob) {
@@ -973,7 +745,6 @@ int eb_get_state(eb_ctx* c, double* coords, double* log_prob) {
   CK(c, cudaSetDevice(c->device));
   int rc = sync_replicas(c);  // multi-GPU: the GLOBAL state (collective)
   if (rc) return rc;
-  c->chain_ok = false;
   if (coords)
     CK(c, cudaMemcpyAsync(coords, c->coords.get(), (size_t)c->N * c->D * sizeof(double), cudaMemcpyDeviceToHost,
                           c->st.get()));
@@ -1004,7 +775,6 @@ int eb_set_state_from(eb_ctx* c, const void* coords, int64_t coords_row_stride_b
   if (rc) return rc;
   const size_t N = (size_t)c->N;
   c->have_state = false;
-  c->chain_ok = false;
   c->blobs_live = false;  // as eb_set_state: a given log_prob comes without blobs
   c->blob_bytes = 0;
   rc = copy_records(c, c->coords.get(), coords, (size_t)row, (size_t)coords_row_stride_bytes, N, src_stream);
@@ -1034,7 +804,6 @@ int eb_get_state_to(eb_ctx* c, double* coords_dst, double* log_prob_dst) {
   int rc = coords_dst ? check_device_ptr(c, c->device, coords_dst, "eb_get_state_to", "coords_dst") : EB_OK;
   if (!rc && log_prob_dst) rc = check_device_ptr(c, c->device, log_prob_dst, "eb_get_state_to", "log_prob_dst");
   if (rc) return rc;
-  c->chain_ok = false;
   if (coords_dst)
     CK(c, cudaMemcpyAsync(coords_dst, c->coords.get(), (size_t)c->N * c->D * sizeof(double), cudaMemcpyDefault,
                           c->st.get()));
@@ -1097,7 +866,6 @@ int eb_get_state_rows(eb_ctx* c, int64_t row0, int64_t nrows, double* coords, do
          "read the owned block [%lld, %lld) or call eb_get_state (collective) first",
          (long long)row0, (long long)(row0 + nrows), (long long)r0, (long long)r1);
   CK(c, cudaSetDevice(c->device));
-  c->chain_ok = false;
   if (coords && nrows)
     CK(c, cudaMemcpyAsync(coords, c->coords.get() + (size_t)row0 * c->D, (size_t)nrows * c->D * sizeof(double),
                           cudaMemcpyDeviceToHost, c->st.get()));
@@ -1125,1037 +893,6 @@ int eb_get_rng(const eb_ctx* c, uint64_t* seed, uint64_t* step) {
 
 }  // extern "C"
 
-// ---- the hot path --------------------------------------------------------------
-namespace {
-
-struct Schedule {
-  std::vector<eb_move> moves;
-  std::vector<double> cdf;
-  // GaussianMove: form (0 scalar, 1 diagonal, 2 full) and where its scale / Cholesky factor sits in gauss_dev
-  std::vector<int> gform;
-  std::vector<size_t> goff;
-};
-
-// thresholded lower Cholesky factor (the draw specification's multivariate_normal; oracle/philox.py chol_psd)
-void chol_psd_host(const double* A, int D, std::vector<double>& L) {
-  L.assign((size_t)D * D, 0.0);
-  double m = 0.0;
-  for (int j = 0; j < D; ++j) m = std::max(m, A[(size_t)j * D + j]);
-  const double tol = 1e-12 * m;
-  for (int j = 0; j < D; ++j) {
-    double d = A[(size_t)j * D + j];
-    for (int k = 0; k < j; ++k) d -= L[(size_t)j * D + k] * L[(size_t)j * D + k];
-    if (!(d > tol)) continue;
-    const double piv = sqrt(d);
-    L[(size_t)j * D + j] = piv;
-    for (int i = j + 1; i < D; ++i) {
-      double v = A[(size_t)i * D + j];
-      for (int k = 0; k < j; ++k) v -= L[(size_t)i * D + k] * L[(size_t)j * D + k];
-      L[(size_t)i * D + j] = v / piv;
-    }
-  }
-}
-
-int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) {
-  if (!moves || nmoves == 0) FAIL(c, EB_ERR_INVALID, "eb_step: empty move schedule");
-  s.moves.assign(moves, moves + nmoves);
-  double tot = 0.0;
-  s.gform.assign(nmoves, 0);
-  s.goff.assign(nmoves, 0);
-  std::vector<double> ghost;  // host image of gauss_dev
-  for (size_t mi = 0; mi < nmoves; ++mi) {
-    eb_move& m = s.moves[mi];
-    if (m.kind == EB_MOVE_USER || m.kind == EB_MOVE_USER_MH) {
-      if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "user proposals are not sharded across GPUs");
-      if (c->debug) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: debug taps do not cover user proposals");
-      if (!(m.p0 >= 0.0 && m.p0 < (double)c->props.size()) || m.p0 != floor(m.p0) || !c->props[(size_t)m.p0].fn)
-        FAIL(c, EB_ERR_INVALID, "eb_step: proposal slot %g is not set (eb_move_set_proposal)", m.p0);
-      if (!(m.weight >= 0.0) || !isfinite(m.weight)) FAIL(c, EB_ERR_INVALID, "eb_step: bad move weight");
-      if (m.kind == EB_MOVE_USER_MH) {
-        m.nsplits = 1;  // the split table of such a step is never read
-        m.randomize_split = 0;
-        tot += m.weight;
-        continue;
-      }
-      if (m.mode != 0 && m.mode != EB_USER_SETUP) FAIL(c, EB_ERR_INVALID, "eb_step: unknown user-move mode %d", m.mode);
-    } else if (m.kind < EB_MOVE_STRETCH || m.kind > EB_MOVE_GAUSSIAN) {
-      FAIL(c, EB_ERR_INVALID, "eb_step: unknown move kind %d", m.kind);
-    }
-    if ((m.kind == EB_MOVE_WALK || m.kind == EB_MOVE_GAUSSIAN) && c->comm.nranks > 1)
-      FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove / GaussianMove are not sharded across GPUs yet");
-    if ((m.kind == EB_MOVE_WALK || m.kind == EB_MOVE_GAUSSIAN) && c->debug)
-      FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: debug taps do not cover WalkMove / GaussianMove");
-    if (m.kind == EB_MOVE_GAUSSIAN) {
-      const size_t D = (size_t)c->D;
-      if (!m.cov || (m.ncov != 1 && m.ncov != D && m.ncov != D * D) || (D == 1 && m.ncov != 1))
-        FAIL(c, EB_ERR_INVALID, "Invalid proposal scale dimensions");  // gaussian.py:53-54
-      if (m.mode < EB_GAUSS_VECTOR || m.mode > EB_GAUSS_SEQUENTIAL)
-        FAIL(c, EB_ERR_INVALID, "eb_step: unknown GaussianMove mode %d", m.mode);
-      if (!isnan(m.p1) && m.p1 < 1.0) FAIL(c, EB_ERR_INVALID, "'factor' must be >= 1.0");  // gaussian.py:69-70
-      if (!(m.weight >= 0.0) || !isfinite(m.weight)) FAIL(c, EB_ERR_INVALID, "eb_step: bad move weight");
-      s.goff[mi] = ghost.size();
-      if (m.ncov == D * D && D > 1) {
-        if (m.mode != EB_GAUSS_VECTOR)
-          FAIL(c, EB_ERR_INVALID, "a full proposal covariance only supports mode 'vector'");  // gaussian.py:110-111
-        s.gform[mi] = 2;
-        std::vector<double> L;
-        chol_psd_host(m.cov, c->D, L);
-        ghost.insert(ghost.end(), L.begin(), L.end());
-        ghost.resize(ghost.size() + D);  // the shared shift v[D] of a step lives behind its factor
-      } else {
-        s.gform[mi] = m.ncov == 1 ? 0 : 1;
-        for (size_t k = 0; k < m.ncov; ++k) {
-          if (!(m.cov[k] >= 0.0)) FAIL(c, EB_ERR_INVALID, "GaussianMove: variances must be >= 0");
-          ghost.push_back(sqrt(m.cov[k]));  // gaussian.py:45,58
-        }
-      }
-      m.nsplits = 1;  // the split table of such a step is never read
-      m.randomize_split = 0;
-      tot += m.weight;
-      continue;
-    }
-    if (m.kind == EB_MOVE_WALK && !isnan(m.p0)) {
-      const int64_t nc_min = c->N - (c->N + m.nsplits - 1) / std::max(m.nsplits, 1);
-      if (m.p0 != floor(m.p0) || m.p0 < 2 || (m.nsplits >= 2 && m.p0 > (double)nc_min))
-        FAIL(c, EB_ERR_INVALID, "eb_step: WalkMove needs 2 <= s <= size of the smallest complement (got %g)", m.p0);
-      // launch_step_walk picks the kernel per split: a split whose own complement is larger than s runs the
-      // helper-subset kernel, even when s equals the smallest complement (nwalkers not divisible by nsplits).
-      // Complements grow with the split index, so the first and the last split cover every size.
-      const int P = std::max(m.nsplits, 1);
-      const int64_t nc_max = c->N - c->N / P;
-      const bool subset = (int64_t)m.p0 != nc_min || (int64_t)m.p0 != nc_max;
-      if (subset && !walk_subset_supported(c->D, (int)m.p0))
-        FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove with a helper subset is limited to ndim <= 64 and s <= 4096");
-    }
-    if (m.kind == EB_MOVE_WALK && c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove is limited to ndim <= 1024");
-    if (m.nsplits < 2 || m.nsplits > MAX_SPLITS || m.nsplits > c->N)
-      FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: nsplits must be in [2, min(%d, nwalkers)] (got %d)", MAX_SPLITS,
-           m.nsplits);
-    if (m.kind == EB_MOVE_SNOOKER && m.nsplits != 4)
-      FAIL(c, EB_ERR_INVALID, "eb_step: DESnookerMove uses nsplits = 4 (de_snooker.py:28)");
-    if (m.kind == EB_MOVE_DE && c->N - (c->N + m.nsplits - 1) / m.nsplits < 2)
-      FAIL(c, EB_ERR_INVALID, "eb_step: DEMove needs at least 2 complement walkers");
-    if (!(m.weight >= 0.0) || !isfinite(m.weight)) FAIL(c, EB_ERR_INVALID, "eb_step: bad move weight");
-    if (m.kind == EB_MOVE_STRETCH && !(m.p0 > 0.0)) FAIL(c, EB_ERR_INVALID, "eb_step: stretch scale a must be > 0");
-    tot += m.weight;
-  }
-  if (!(tot > 0.0)) FAIL(c, EB_ERR_INVALID, "eb_step: move weights sum to zero");
-  if (!ghost.empty()) {
-    if (ghost.size() > c->gauss_cap) {
-      CK(c, cudaStreamSynchronize(c->st.get()));
-      CK(c, dev_alloc(c->gauss_dev, ghost.size() * sizeof(double)));
-      c->gauss_cap = ghost.size();
-    }
-    CK(c, cudaMemcpyAsync(c->gauss_dev.get(), ghost.data(), ghost.size() * sizeof(double), cudaMemcpyHostToDevice,
-                          c->st.get()));
-    CK(c, cudaStreamSynchronize(c->st.get()));  // ghost is a local
-  }
-  c->picks.assign(nmoves, 0);
-  // ensemble.py:128-129 then RandomState.choice(p=...): cdf = cumsum(p); cdf /= cdf[-1]
-  s.cdf.resize(nmoves);
-  double run = 0.0;
-  for (size_t k = 0; k < nmoves; ++k) {
-    run += s.moves[k].weight / tot;
-    s.cdf[k] = run;
-  }
-  for (size_t k = 0; k < nmoves; ++k) s.cdf[k] /= run;
-  return EB_OK;
-}
-
-// ensemble.py:406 -- one move per step for the whole ensemble
-size_t choose_move(const eb_ctx* c, const Schedule& s, uint64_t step) {
-  if (s.moves.size() == 1) return 0;
-  const u32x4 w = draw_words(c->seed, step, 0, TAG_MOVE, 0);
-  const double u = u53(w.x, w.y);
-  size_t idx = 0;
-  while (idx + 1 < s.cdf.size() && !(s.cdf[idx] > u)) ++idx;  // searchsorted(side="right")
-  return idx;
-}
-
-void split_starts(int64_t N, int P, int* start) {
-  start[0] = 0;
-  for (int j = 0; j < P; ++j) start[j + 1] = start[j] + (int)((N - j + P - 1) / P);
-}
-
-void fill_base_args(eb_ctx* c, const eb_move& mv, HalfStepArgs& a) {
-  a = HalfStepArgs{};
-  a.coords = c->coords.get();
-  a.logp = c->logp.get();
-  a.accepted = c->accepted.get();
-  a.nacc = c->nacc.get();
-  a.status = c->status_dev.get();
-  a.N = c->N;
-  a.D = c->D;
-  a.seed = c->seed;
-  a.model = c->model;
-  if (c->debug) {
-    a.tap_partners = c->tap_partners.get();
-    a.tap_scalar = c->tap_scalar.get();
-    a.tap_u = c->tap_u.get();
-    a.tap_active = c->tap_active.get();
-  }
-  switch (mv.kind) {
-    case EB_MOVE_STRETCH:
-      a.p0 = mv.p0;
-      break;
-    case EB_MOVE_DE:
-      a.p0 = isnan(mv.p1) ? 2.38 / sqrt(2.0 * (double)c->D) : mv.p1;  // de.py:33-38
-      a.p1 = mv.p0;                                                    // sigma
-      break;
-    default:
-      a.p0 = mv.p0;  // gammas
-  }
-  a.timeline = c->timeline.get();
-  a.dmma_stagger = c->dmma_stagger;
-  comm_fill_args(c->comm, a);
-}
-
-bool dmma_eligible(const eb_ctx* c, const eb_move& mv) {
-  return c->allow_dmma && mv.kind == EB_MOVE_STRETCH && c->model.kind == EB_MODEL_GAUSS_DENSE &&
-         c->model.chol != nullptr && !c->debug;
-}
-
-int check_walker_count(eb_ctx* c, const eb_move& mv) {
-  if (c->N < 2 * (int64_t)c->D && !mv.live_dangerously)  // red_blue.py:64-70
-    FAIL(c, EB_ERR_FEW_WALKERS,
-         "It is unadvisable to use a red-blue move with fewer walkers than twice the number of dimensions.");
-  return EB_OK;
-}
-
-// one half-step of a callback model (eb_model_set_callback): the propose phase of the fused kernel (STRETCH / DE /
-// SNOOKER) -- or the proposals a move's own kernels left in qbuf (MOVE_PRECOMPUTED) --, the callback, then the
-// accept phase.  The proposal rows are the fused kernel's by construction: the same code stages them.
-int callback_half_step(eb_ctx* c, int move_kind, HalfStepArgs a, uint64_t& launches) {
-  ExternalBufs ext{c->qbuf.get(), nullptr, c->ext_lp.get()};
-  if (move_kind != MOVE_PRECOMPUTED) {
-    ext.f = c->ext_f.get();
-    CK(c, launch_half_step_external(move_kind, a, ext, c->st.get()));
-    ++launches;
-  }
-  c->cb_phase = CB_STEP;
-  int rc = run_callback(c, c->qbuf.get(), (int64_t)a.i_hi - a.i_lo, c->ext_lp.get(), move_kind == MOVE_PRECOMPUTED);
-  if (rc) return rc;
-  a.qbuf = c->qbuf.get();
-  CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st.get()));
-  ++launches;
-  if (c->blobs_live) {  // accepted walkers take their proposal's record (moves/move.py:36-43)
-    CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop.get(), c->blob_live.get(),
-                             c->blob_bytes, c->st.get()));
-    ++launches;
-  }
-  c->last_kernel = "callback";
-  snprintf(c->last_variant, sizeof(c->last_variant), "callback G=%d where=%s", lanes_per_walker(c->D),
-           c->cb_where == EB_CALLBACK_HOST ? "host" : "device");
-  return EB_OK;
-}
-
-// launch the P half-steps of one step with the generic kernels (one launch per split)
-int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t* order, size_t step_in_chunk,
-                        uint64_t& launches) {
-  const int P = mv.nsplits;
-  int rc = check_walker_count(c, mv);
-  if (rc) return rc;
-  int start[MAX_SPLITS + 1];
-  split_starts(c->N, P, start);
-  HalfStepArgs a;
-  fill_base_args(c, mv, a);
-  a.order = order;
-  a.step = step;
-  for (int split = 0; split < P; ++split) {
-    a.split = split;
-    a.a_start = start[split];
-    a.a_count = start[split + 1] - start[split];
-    int k = 0;
-    for (int j = 0; j < P && k < 3; ++j) {
-      if (j == split) continue;
-      a.c_start[k] = start[j];
-      a.c_count[k] = start[j + 1] - start[j];
-      ++k;
-    }
-    comm_active_range(c->comm, a, step_in_chunk);  // i_lo / i_hi for this rank
-    if (c->fused_last) {
-      // the previous launch was a dense_dmma kernel that carried the peer barrier itself (signal at its end);
-      // this kernel does not wait on its own, so the ranks meet explicitly before it reads peer rows
-      if (comm_barrier(c->comm, c->st.get(), c->status_dev.get(), launches))
-        FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
-      c->fused_last = false;
-    }
-    c->chain_ok = false;
-    if (c->model.kind == MODEL_EXTERNAL) {
-      rc = callback_half_step(c, mv.kind, a, launches);
-      if (rc) return rc;
-      c->tap_count = a.a_count;
-      continue;
-    }
-    bool used_tma = false;
-    TmaVariant tv{};
-    if (c->allow_tma && !c->debug)
-      CK(c, launch_half_step_tma(mv.kind, a, c->sm_count, c->allow_tma >= 2, c->tma_own_reg, c->st.get(), &used_tma,
-                                 &tv));
-    if (used_tma) {
-      c->last_kernel = "tma_rows";
-      snprintf(c->last_variant, sizeof(c->last_variant), "tma_rows R=%d epl=%d own_reg=%d warps=%d", tv.R, tv.epl,
-               tv.own_reg, tv.warps);
-    } else {
-      CK(c, launch_half_step_generic(mv.kind, a, c->st.get()));
-      c->last_kernel = "generic";
-      snprintf(c->last_variant, sizeof(c->last_variant), "generic G=%d", lanes_per_walker(c->D));
-    }
-    ++launches;
-    c->tap_count = a.a_count;
-    if (comm_after_split(c->comm, c->st.get(), c->status_dev.get(), launches))
-      FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
-  }
-  return EB_OK;
-}
-
-int ensure_move_scratch(eb_ctx* c) {
-  const size_t D = (size_t)c->D;
-  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, (size_t)c->N * D * sizeof(double)));
-  if (!c->walk_work && D <= 1024) CK(c, dev_alloc(c->walk_work, (2 * D + 3 * D * D) * sizeof(double)));
-  if (!c->mom_partial && D <= 1024) CK(c, dev_alloc(c->mom_partial, moments_partial_bytes(c->D, c->sm_count)));
-  return EB_OK;
-}
-
-// WalkMove (walk.py:27-37): per split a proposal kernel writes q[a_count, D], then the fused
-// log-prob + accept + update kernel consumes it
-int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t* order, uint64_t& launches) {
-  const int P = mv.nsplits;
-  int rc = check_walker_count(c, mv);
-  if (rc) return rc;
-  rc = ensure_move_scratch(c);
-  if (rc) return rc;
-  int start[MAX_SPLITS + 1];
-  split_starts(c->N, P, start);
-  HalfStepArgs a;
-  fill_base_args(c, mv, a);
-  a.order = order;
-  a.step = step;
-  a.qbuf = c->qbuf.get();
-  c->chain_ok = false;
-  const size_t D = (size_t)c->D;
-  double* shift = c->walk_work.get();
-  double* acc = shift + D;
-  double* cov = acc + D + D * D;
-  double* L = cov + D * D;
-  for (int split = 0; split < P; ++split) {
-    a.split = split;
-    a.a_start = start[split];
-    a.a_count = start[split + 1] - start[split];
-    a.i_lo = 0;
-    a.i_hi = a.a_count;
-    a.range = nullptr;
-    const int64_t Nc = c->N - a.a_count;
-    const int64_t s0 = isnan(mv.p0) ? Nc : (int64_t)mv.p0;  // walk.py:32
-    if (s0 == Nc) {
-      // every walker of the split draws from the covariance of the WHOLE complement (walk.py:34-35 with a
-      // permutation of all Nc rows): computed once -- moment sums on the tensor pipe, then a D x D factorisation
-      // any shift will do: the ensemble mean
-      CK(c, launch_colmean(c->coords.get(), c->N, c->D, shift, nullptr, c->st.get()));
-      CK(c, cudaMemsetAsync(acc, 0, (D + D * D) * sizeof(double), c->st.get()));
-      CK(c, launch_moments(c->coords.get(), Nc, c->D, shift, c->mom_partial.get(), acc, c->sm_count, c->st.get(), order,
-                           a.a_start, a.a_count));
-      CK(c, launch_cov_chol(acc, (double)Nc, c->D, cov, L, c->st.get()));
-      CK(c, launch_walk_shared_propose(a, L, c->qbuf.get(), c->st.get()));
-      launches += 5;
-    } else {
-      CK(c, launch_walk_subset_propose(a, (int)s0, c->qbuf.get(), c->st.get()));
-      ++launches;
-    }
-    if (c->model.kind == MODEL_EXTERNAL) {
-      rc = callback_half_step(c, MOVE_PRECOMPUTED, a, launches);
-      if (rc) return rc;
-      continue;
-    }
-    CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st.get()));
-    ++launches;
-  }
-  if (c->model.kind == MODEL_EXTERNAL) return EB_OK;
-  c->last_kernel = "walk";
-  snprintf(c->last_variant, sizeof(c->last_variant), "walk");
-  return EB_OK;
-}
-
-// MHMove with the Gaussian proposal (mh.py:35-65, gaussian.py:72-119): every walker is proposed at once
-int launch_step_gaussian(eb_ctx* c, const Schedule& s, size_t mi, uint64_t step, uint64_t& launches) {
-  const eb_move& mv = s.moves[mi];
-  int rc = ensure_move_scratch(c);
-  if (rc) return rc;
-  const int D = c->D;
-  double f = 1.0;
-  if (!isnan(mv.p1)) {  // gaussian.py:88-91  exp(uniform(-log f, log f))
-    const u32x4 w = draw_words(c->seed, step, 0, TAG_MOVE, 1);
-    const double lf = log(mv.p1);
-    f = exp(-lf + (lf - (-lf)) * u53(w.x, w.y));
-  }
-  const int seq_dim = (int)(((uint64_t)mv.seq_index + c->picks[mi]) % (uint64_t)D);  // gaussian.py:102-103
-  const double* dev = c->gauss_dev.get() + s.goff[mi];
-  const int form = s.gform[mi];
-  const double* scale = dev;
-  c->chain_ok = false;
-  if (form == 2) {
-    double* v = c->gauss_dev.get() + s.goff[mi] + (size_t)D * D;
-    CK(c, launch_gaussian_shift(dev, D, f, c->seed, step, v, c->st.get()));
-    scale = v;
-    ++launches;
-  }
-  CK(c, launch_gaussian_propose(c->coords.get(), 0, c->N, D, form, scale, f, mv.mode, seq_dim, c->seed, step,
-                                c->qbuf.get(), c->st.get()));
-  HalfStepArgs a;
-  fill_base_args(c, mv, a);
-  a.order = nullptr;  // the active set is every walker, in walker order
-  a.step = step;
-  a.split = 0;
-  a.a_start = 0;
-  a.a_count = (int)c->N;
-  a.i_lo = 0;
-  a.i_hi = (int)c->N;
-  a.range = nullptr;
-  a.qbuf = c->qbuf.get();
-  if (c->model.kind == MODEL_EXTERNAL) {
-    ++launches;
-    return callback_half_step(c, MOVE_PRECOMPUTED, a, launches);
-  }
-  CK(c, launch_half_step_generic(MOVE_PRECOMPUTED, a, c->st.get()));
-  launches += 2;
-  c->last_kernel = "gaussian";
-  snprintf(c->last_variant, sizeof(c->last_variant), "gaussian");
-  return EB_OK;
-}
-
-// ---- user proposals (eb_move_set_proposal) ----------------------------------------------------------
-int ensure_user_scratch(eb_ctx* c, bool host) {
-  const size_t N = (size_t)c->N, D = (size_t)c->D;
-  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, N * D * sizeof(double)));
-  if (!c->up_x) CK(c, dev_alloc(c->up_x, N * D * sizeof(double)));
-  if (!c->up_f) CK(c, dev_alloc(c->up_f, N * sizeof(double)));
-  if (host && !c->up_hf) {
-    HostPtr<double> hx, hq, hf;
-    CK(c, host_alloc(hx, N * D * sizeof(double)));
-    CK(c, host_alloc(hq, N * D * sizeof(double)));
-    CK(c, host_alloc(hf, N * sizeof(double)));
-    c->up_hx = std::move(hx);
-    c->up_hq = std::move(hq);
-    c->up_hf = std::move(hf);
-  }
-  return EB_OK;
-}
-
-// steps 2-5 of a user half-step (include/emcee_b200.h): rows[N, D] (device; s then c, or the ensemble) are
-// enqueued.  ns > 0: the proposal of ns rows lands in qbuf / up_f; ns == 0: the setup call, which returns nothing
-int user_proposal_call(eb_ctx* c, const eb_ctx::ProposalSlot& p, uint64_t step, int split, const double* rows,
-                       int64_t ns, const int64_t* counts, int nsets) {
-  const size_t N = (size_t)c->N, D = (size_t)c->D;
-  const bool host = p.where == EB_CALLBACK_HOST;
-  // the function gets its own copy of the rows
-  if (host)
-    CK(c, cudaMemcpyAsync(c->up_hx.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
-  else if (rows != c->up_x.get())
-    CK(c, cudaMemcpyAsync(c->up_x.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st.get()));
-  // complete before fn runs (a device consumer may ignore the stream it is given)
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  const double* s = host ? c->up_hx.get() : c->up_x.get();
-  const double* cset = nsets > 0 ? s + (size_t)ns * D : nullptr;
-  double* q = ns > 0 ? (host ? c->up_hq.get() : c->qbuf.get()) : nullptr;
-  double* f = ns > 0 ? (host ? c->up_hf.get() : c->up_f.get()) : nullptr;
-  c->up_m = ns;
-  c->up_where = p.where;
-  c->in_proposal = true;
-  const int r = p.fn(p.user, step, (int32_t)split, s, ns > 0 ? ns : (int64_t)N, cset, nsets > 0 ? counts : nullptr,
-                     nsets, (int64_t)D, q, f, host ? nullptr : (void*)c->st.get());
-  c->in_proposal = false;
-  c->up_m = 0;
-  if (r != 0) {
-    cudaStreamSynchronize(c->st.get());  // whatever the function enqueued before it failed
-    FAIL(c, EB_ERR_CALLBACK, "the user proposal failed (returned %d)", r);
-  }
-  if (ns == 0) return EB_OK;
-  if (host) {
-    CK(c, cudaMemcpyAsync(c->qbuf.get(), c->up_hq.get(), (size_t)ns * D * sizeof(double), cudaMemcpyHostToDevice,
-                          c->st.get()));
-    CK(c, cudaMemcpyAsync(c->up_f.get(), c->up_hf.get(), (size_t)ns * sizeof(double), cudaMemcpyHostToDevice,
-                          c->st.get()));
-  }
-  if (c->model.kind == MODEL_EXTERNAL) return EB_OK;  // run_callback scans the rows before the function sees them
-  // ensemble.py:476-479: a non-finite proposal stops the call before any log-probability is evaluated
-  CK(c, launch_scan_nonfinite(c->qbuf.get(), (size_t)ns * D, 0, c->status_dev.get(), c->st.get()));
-  return fetch_status(c);
-}
-
-// step 6: the log-probability of qbuf's rows and the accept + update (kind EB_MOVE_USER / EB_MOVE_USER_MH)
-int user_accept(eb_ctx* c, int kind, const HalfStepArgs& a, uint64_t& launches) {
-  const ExternalBufs ext{c->qbuf.get(), c->up_f.get(), c->ext_lp.get()};
-  if (c->model.kind == MODEL_EXTERNAL) {
-    c->cb_phase = CB_STEP;
-    int rc = run_callback(c, c->qbuf.get(), (int64_t)a.i_hi - a.i_lo, c->ext_lp.get(), true);
-    if (rc) return rc;
-    if (kind == EB_MOVE_USER)
-      CK(c, launch_half_step_external(MOVE_PRECOMPUTED, a, ext, c->st.get()));
-    else
-      CK(c, launch_half_step_user(EB_MOVE_USER_MH, a, ext, c->st.get()));
-    ++launches;
-    if (c->blobs_live) {
-      CK(c, launch_blob_select(a.order, a.a_start, a.i_lo, a.i_hi, a.accepted, c->blob_prop.get(), c->blob_live.get(),
-                               c->blob_bytes, c->st.get()));
-      ++launches;
-    }
-  } else {
-    CK(c, launch_half_step_user(kind, a, ext, c->st.get()));
-    ++launches;
-  }
-  return EB_OK;
-}
-
-void note_user_kernel(eb_ctx* c, const eb_ctx::ProposalSlot& p) {
-  c->last_kernel = "user_move";
-  snprintf(c->last_variant, sizeof(c->last_variant), "user_move where=%s",
-           p.where == EB_CALLBACK_HOST ? "host" : "device");
-}
-
-// a RedBlueMove with a user get_proposal (red_blue.py:52-106): per split the gather, the function, the accept
-int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, const int32_t* order, uint64_t& launches) {
-  int rc = check_walker_count(c, mv);
-  if (rc) return rc;
-  const eb_ctx::ProposalSlot p = c->props[(size_t)mv.p0];
-  rc = ensure_user_scratch(c, p.where == EB_CALLBACK_HOST);
-  if (rc) return rc;
-  c->chain_ok = false;
-  if (mv.mode == EB_USER_SETUP) {  // red_blue.py:73 setup(state.coords), once per step before the splits
-    rc = user_proposal_call(c, p, step, -1, c->coords.get(), 0, nullptr, 0);
-    if (rc) return rc;
-  }
-  const int P = mv.nsplits;
-  int start[MAX_SPLITS + 1];
-  split_starts(c->N, P, start);
-  HalfStepArgs a;
-  fill_base_args(c, mv, a);
-  a.order = order;
-  a.step = step;
-  a.qbuf = c->qbuf.get();
-  int64_t counts[MAX_SPLITS];
-  for (int split = 0; split < P; ++split) {
-    a.split = split;
-    a.a_start = start[split];
-    a.a_count = start[split + 1] - start[split];
-    a.i_lo = 0;
-    a.i_hi = a.a_count;
-    a.range = nullptr;
-    int k = 0;
-    for (int j = 0; j < P; ++j)
-      if (j != split) counts[k++] = start[j + 1] - start[j];
-    CK(c, launch_split_gather(c->coords.get(), order, c->N, c->D, a.a_start, a.a_count, c->up_x.get(), c->st.get()));
-    ++launches;
-    rc = user_proposal_call(c, p, step, split, c->up_x.get(), a.a_count, counts, P - 1);
-    if (rc) return rc;
-    rc = user_accept(c, EB_MOVE_USER, a, launches);
-    if (rc) return rc;
-  }
-  note_user_kernel(c, p);
-  return EB_OK;
-}
-
-// MHMove with a user proposal_function (mh.py:35-65): the whole ensemble in walker order, one accept launch
-int launch_step_user_mh(eb_ctx* c, const eb_move& mv, uint64_t step, uint64_t& launches) {
-  const eb_ctx::ProposalSlot p = c->props[(size_t)mv.p0];
-  int rc = ensure_user_scratch(c, p.where == EB_CALLBACK_HOST);
-  if (rc) return rc;
-  c->chain_ok = false;
-  HalfStepArgs a;
-  fill_base_args(c, mv, a);
-  a.order = nullptr;  // the active set is every walker, in walker order
-  a.step = step;
-  a.split = 0;
-  a.a_start = 0;
-  a.a_count = (int)c->N;
-  a.i_lo = 0;
-  a.i_hi = (int)c->N;
-  a.range = nullptr;
-  a.qbuf = c->qbuf.get();
-  rc = user_proposal_call(c, p, step, 0, c->coords.get(), c->N, nullptr, 0);
-  if (rc) return rc;
-  rc = user_accept(c, EB_MOVE_USER_MH, a, launches);
-  if (rc) return rc;
-  note_user_kernel(c, p);
-  return EB_OK;
-}
-
-constexpr int DMMA_TILE_SLOTS = 8;  // consumer warps per SM of the dense_dmma kernel
-
-// a run of consecutive half-steps handed to ONE persistent dense_dmma launch
-struct DmmaGroup {
-  size_t first = 0;  // index into the chunk's HalfDesc array
-  int nhalf = 0;
-  int max_count = 0;
-};
-
-int flush_dmma(eb_ctx* c, const eb_move& mv, DmmaGroup& grp, uint64_t& launches) {
-  if (grp.nhalf == 0) return EB_OK;
-  HalfStepArgs a;
-  fill_base_args(c, mv, a);
-  a.order = c->order.get();  // chunk base; HalfDesc::order_step selects the table
-  a.range = c->comm.nranks > 1 ? c->comm.ranges : nullptr;
-  int bound = grp.max_count;
-  if (c->comm.nranks > 1 && c->comm.rows_per_rank < bound) bound = (int)c->comm.rows_per_rank;
-  // Locality-sorted tiles hide the peer barrier and the first remote fetch behind local work, but move the
-  // remote burst to the second round: the gain or loss depends on the GPU count -- hence off by default; "auto"
-  // (option value 1) enables it when a consumer warp has at most ~2 tiles per half-step.
-  const bool few_tiles = (bound + 7) / 8 <= 2 * DMMA_TILE_SLOTS * c->sm_count;
-  a.aperm = (c->comm.nranks > 1 && (c->local_first == 2 || (c->local_first == 1 && few_tiles))) ? c->comm.aperm : nullptr;
-  // P2P: the peer barrier rides inside the kernel (wait at its start, between its half-steps, signal at its end)
-  const bool fused = comm_fuse_barrier(c->comm, a, grp.nhalf);
-  c->fused_last = fused;
-  // (sharded ensembles: measured slower with the dependent launch -- the early CTAs only add pollers on the
-  // peer flags -- so it is opt-in there: option "pdl" = 2)
-  const bool pdl = c->chain_ok && grp.nhalf == 1 && (c->comm.nranks > 1 ? c->pdl >= 2 : c->pdl >= 1);
-  // The predecessor ran only earlier splits of the same step, the last one being split - 1: they write only
-  // their own active walkers, so this split's rows may be requested before the predecessor has finished.
-  // Not across a step boundary (a randomised split can write any row), not sharded (peer GPUs write rows too).
-  const HalfDesc& d0 = c->descs_host.get()[grp.first];
-  a.dmma_early_own = pdl && c->comm.nranks == 1 && d0.split > 0 && c->dmma_first.step == d0.step &&
-                     c->dmma_first.order_step == d0.order_step && c->dmma_last.step == d0.step &&
-                     c->dmma_last.split == d0.split - 1;
-  // "dmma_timeline" = 2: the other launches run uninstrumented, so the stamps left are those of a first split
-  if (c->timeline_first_split && d0.split != 0) a.timeline = nullptr;
-  int grid = 0;
-  CK(c, launch_dense_dmma(a, c->descs_host.get()[grp.first], c->descs_dev.get() + grp.first, grp.nhalf, bound,
-                          c->gbar.get(), c->gbar_count, c->sm_count, pdl, &grid, c->st.get()));
-  c->gbar_count += (unsigned long long)(grp.nhalf - 1) * (unsigned long long)grid;
-  c->last_kernel = "dense_dmma";
-  c->dmma_nhalf_max = std::max(c->dmma_nhalf_max, grp.nhalf);
-  snprintf(c->last_variant, sizeof(c->last_variant), "dense_dmma nhalf_max=%d grid=%d", c->dmma_nhalf_max, grid);
-  c->chain_ok = grid > 0;
-  c->dmma_first = c->descs_host.get()[grp.first];
-  c->dmma_last = c->descs_host.get()[grp.first + grp.nhalf - 1];
-  ++launches;
-  grp = DmmaGroup{};
-  return EB_OK;
-}
-
-// run nsteps steps.  `after_step(k)` is called with the work of step k enqueued and may
-// enqueue copies on the stream; `sync_every` > 0 tells how often it actually does (every
-// sync_every-th step), so that steps in between can share one persistent launch.
-int accumulate_moments(eb_ctx* c, uint64_t& launches);  // below
-int accumulate_histograms(eb_ctx* c, uint64_t& launches);  // below
-int reserve_trace(eb_ctx* c, uint64_t nsteps);             // below
-int accumulate_trace(eb_ctx* c, uint64_t& launches);       // below
-
-template <class F>
-int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every, F&& after_step) {
-  uint64_t launches = 0;
-  const bool perstep = c->l2_flush;  // flush L2 before every step, time each step on its own
-  if (perstep) {
-    if (nsteps > 16384) FAIL(c, EB_ERR_INVALID, "l2_flush mode times each step separately; use nsteps <= 16384");
-    if (!c->flush_buf) CK(c, dev_alloc(c->flush_buf, c->flush_bytes));
-    while (c->ev_pool.size() < 2 * nsteps) {
-      EventPtr e;
-      CK(c, event_create(e));
-      c->ev_pool.push_back(std::move(e));
-    }
-  }
-  if (c->trace_every > 0) {
-    const int rc = reserve_trace(c, nsteps);
-    if (rc) return rc;
-  }
-  c->chain_ok = false;
-  c->dmma_nhalf_max = 0;
-  CK(c, cudaEventRecord(c->ev0.get(), c->st.get()));
-  if (comm_begin(c->comm, c->st.get(), c->status_dev.get(), launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
-  c->fused_last = false;
-  const bool multi = c->comm.nranks > 1;
-  // sharded ensembles run one half-step per launch: NCCL exchanges whole row blocks after every split, and the
-  // P2P peer barrier rides on the kernel boundary (a persistent launch with the peer barrier between its
-  // half-steps measured no faster and was dropped)
-  const bool one_per_launch = multi;
-  const bool exchange_each = multi && c->comm.mode == EB_COMM_ALLGATHER;
-  std::vector<size_t> pick;
-  uint64_t done = 0;
-  while (done < nsteps) {
-    const size_t chunk = (size_t)std::min<uint64_t>(nsteps - done, c->table_cap);
-    pick.resize(chunk);
-    CK(c, cudaStreamSynchronize(c->st.get()));  // info_host / descs_host are reused per chunk
-    size_t ndesc = 0;
-    for (size_t k = 0; k < chunk; ++k) {
-      pick[k] = choose_move(c, s, c->step + k);
-      const eb_move& mv = s.moves[pick[k]];
-      c->info_host.get()[k].nsplits = mv.nsplits;
-      c->info_host.get()[k].randomize = mv.randomize_split;
-    }
-    // Split tables depend only on (seed, step, nsplits, randomize): reuse the ones already on the
-    // device when they cover this chunk, else build them -- looking ahead with the same schedule, so
-    // a caller that steps one iteration per call pays for one table launch every 64 calls, not one each.
-    size_t off = 0, build = 0;
-    bool hit = c->tbl_n > 0 && c->tbl_seed == c->seed && c->step >= c->tbl_step0 &&
-               c->step + chunk <= c->tbl_step0 + c->tbl_n;
-    if (hit) {
-      off = (size_t)(c->step - c->tbl_step0);
-      for (size_t k = 0; k < chunk && hit; ++k)
-        hit = c->tbl_info[off + k].nsplits == c->info_host.get()[k].nsplits &&
-              c->tbl_info[off + k].randomize == c->info_host.get()[k].randomize;
-    }
-    if (!hit) {
-      off = 0;
-      build = std::min<size_t>(c->table_cap, std::max<size_t>(chunk, 64));
-      for (size_t k = chunk; k < build; ++k) {
-        const eb_move& mv = s.moves[choose_move(c, s, c->step + k)];
-        c->info_host.get()[k].nsplits = mv.nsplits;
-        c->info_host.get()[k].randomize = mv.randomize_split;
-      }
-      c->tbl_seed = c->seed;
-      c->tbl_step0 = c->step;
-      c->tbl_n = build;
-      c->tbl_info.assign(c->info_host.get(), c->info_host.get() + build);
-    }
-    for (size_t k = 0; k < chunk; ++k) {
-      const eb_move& mv = s.moves[pick[k]];
-      if (dmma_eligible(c, mv)) {
-        int start[MAX_SPLITS + 1];
-        split_starts(c->N, mv.nsplits, start);
-        for (int split = 0; split < mv.nsplits; ++split) {
-          HalfDesc& d = c->descs_host.get()[ndesc++];
-          d.step = c->step + k;
-          d.order_step = (int32_t)(off + k);
-          d.split = split;
-          d.a_start = start[split];
-          d.a_count = start[split + 1] - start[split];
-        }
-      }
-    }
-    DmmaGroup grp;
-    size_t desc_cursor = 0;
-    const eb_move* grp_move = nullptr;
-    for (size_t k = 0; k < chunk; ++k) {
-      const eb_move& mv = s.moves[pick[k]];
-      if (perstep) {
-        CK(c, cudaMemsetAsync(c->flush_buf.get(), (int)(k & 0xff), c->flush_bytes, c->st.get()));
-        CK(c, cudaEventRecord(c->ev_pool[2 * (done + k)].get(), c->st.get()));
-        c->chain_ok = false;
-      }
-      if (k == 0) {
-        // dense_dmma descriptors of the chunk and, when needed, the split tables (charged to this step)
-        if (ndesc) {
-          CK(c, cudaMemcpyAsync(c->descs_dev.get(), c->descs_host.get(), ndesc * sizeof(HalfDesc),
-                                cudaMemcpyHostToDevice, c->st.get()));
-          c->chain_ok = false;
-        }
-        if (build) {
-          CK(c, cudaMemcpyAsync(c->info_dev.get(), c->info_host.get(), build * sizeof(StepInfo), cudaMemcpyHostToDevice,
-                                c->st.get()));
-          const Comm& cm = c->comm;
-          CK(c, launch_split_tables(c->order.get(), c->info_dev.get(), (int)build, c->N, c->seed, c->step,
-                                    cm.rows_per_rank * cm.rank, cm.rows_per_rank * (cm.rank + 1),
-                                    cm.nranks > 1 ? cm.ranges : nullptr, c->st.get()));
-          ++launches;
-          if (cm.nranks > 1 && cm.aperm) {
-            // front group = one tile (8 walkers) for each of the 8 consumer warps of every SM: the first round
-            CK(c, launch_locality_tables(c->order.get(), c->info_dev.get(), cm.ranges, (int)build, c->N, c->seed,
-                                         c->step, cm.rows_per_rank, cm.rank, 64 * c->sm_count, cm.aperm, c->st.get()));
-            ++launches;
-          }
-          c->chain_ok = false;
-        }
-      }
-      int rc;
-      if (dmma_eligible(c, mv)) {
-        rc = check_walker_count(c, mv);
-        if (rc) return rc;
-        if (grp_move && grp_move != &mv) {  // a different move object: its parameters differ
-          rc = flush_dmma(c, *grp_move, grp, launches);
-          if (rc) return rc;
-        }
-        grp_move = &mv;
-        for (int split = 0; split < mv.nsplits; ++split) {
-          const HalfDesc& d = c->descs_host.get()[desc_cursor];
-          if (grp.nhalf == 0) grp.first = desc_cursor;
-          grp.nhalf += 1;
-          grp.max_count = std::max(grp.max_count, (int)d.a_count);
-          ++desc_cursor;
-          if (one_per_launch || (grp.nhalf >= c->dmma_group && split + 1 < mv.nsplits)) {
-            rc = flush_dmma(c, mv, grp, launches);
-            if (rc) return rc;
-            if (exchange_each) {
-              c->chain_ok = false;
-              if (comm_after_split(c->comm, c->st.get(), c->status_dev.get(), launches))
-                FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
-            }
-          }
-        }
-        const bool moments_now = c->moments_every > 0 && (c->step + 1) % c->moments_every == 0;
-        const bool hist_now = c->hist_every > 0 && (c->step + 1) % c->hist_every == 0;
-        const bool trace_now = c->trace_every > 0 && (c->step + 1) % c->trace_every == 0;
-        const bool host_event =
-            perstep || moments_now || hist_now || trace_now || (sync_every > 0 && (done + k + 1) % sync_every == 0);
-        if (host_event || k + 1 == chunk || grp.nhalf >= c->dmma_group) {
-          rc = flush_dmma(c, mv, grp, launches);
-          if (rc) return rc;
-        }
-      } else {
-        if (grp_move) {
-          rc = flush_dmma(c, *grp_move, grp, launches);
-          if (rc) return rc;
-        }
-        if (mv.kind == EB_MOVE_WALK)
-          rc = launch_step_walk(c, mv, c->step, c->order.get() + (off + k) * (size_t)c->N, launches);
-        else if (mv.kind == EB_MOVE_GAUSSIAN)
-          rc = launch_step_gaussian(c, s, pick[k], c->step, launches);
-        else if (mv.kind == EB_MOVE_USER)
-          rc = launch_step_user(c, mv, c->step, c->order.get() + (off + k) * (size_t)c->N, launches);
-        else if (mv.kind == EB_MOVE_USER_MH)
-          rc = launch_step_user_mh(c, mv, c->step, launches);
-        else
-          rc = launch_step_generic(c, mv, c->step, c->order.get() + (off + k) * (size_t)c->N, off + k, launches);
-        if (rc) return rc;
-      }
-      c->picks[pick[k]] += 1;
-      c->step += 1;
-      if (c->moments_every > 0 && c->step % c->moments_every == 0) {
-        rc = accumulate_moments(c, launches);
-        if (rc) return rc;
-      }
-      if (c->hist_every > 0 && c->step % c->hist_every == 0) {
-        rc = accumulate_histograms(c, launches);
-        if (rc) return rc;
-      }
-      if (c->trace_every > 0 && c->step % c->trace_every == 0) {
-        rc = accumulate_trace(c, launches);
-        if (rc) return rc;
-      }
-      if (perstep) {
-        CK(c, cudaEventRecord(c->ev_pool[2 * (done + k) + 1].get(), c->st.get()));
-        c->chain_ok = false;
-      }
-      rc = after_step(done + k);
-      if (rc) return rc;
-    }
-    done += chunk;
-  }
-  CK(c, cudaEventRecord(c->ev1.get(), c->st.get()));
-  c->chain_ok = false;
-  // multi-GPU: the rows of other ranks are NOT replicated here; collective readers (eb_get_state,
-  // eb_get_naccepted, the accept mask of eb_step) do that on demand, sharded readers never need it
-  if (multi) c->replicas_dirty = true;
-  CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  float ms = 0.f;
-  if (perstep) {
-    double tot = 0.0;
-    for (uint64_t k = 0; k < nsteps; ++k) {
-      CK(c, cudaEventElapsedTime(&ms, c->ev_pool[2 * k].get(), c->ev_pool[2 * k + 1].get()));
-      tot += ms;
-    }
-    c->last_ms = tot;
-  } else {
-    CK(c, cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
-    c->last_ms = ms;
-  }
-  c->last_launches = launches;
-  return check_status(c);
-}
-
-// ---- running chain moments ---------------------------------------------------------------------
-int moments_config(eb_ctx* c, uint64_t every) {
-  CK(c, cudaSetDevice(c->device));
-  if (every > 0 && c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "chain moments are limited to ndim <= 1024");
-  const size_t n = (size_t)c->D + (size_t)c->D * c->D;
-  if (every > 0 && !c->mom_acc) {
-    DevPtr<double> acc, shift, partial;
-    CK(c, dev_alloc(acc, n * sizeof(double)));
-    CK(c, dev_alloc(shift, (size_t)c->D * sizeof(double)));
-    if (!c->mom_partial) CK(c, dev_alloc(partial, moments_partial_bytes(c->D, c->sm_count)));
-    c->mom_acc = std::move(acc);
-    c->mom_shift = std::move(shift);
-    if (partial) c->mom_partial = std::move(partial);
-  }
-  if (c->mom_acc) CK(c, cudaMemsetAsync(c->mom_acc.get(), 0, n * sizeof(double), c->st.get()));
-  c->mom_count = 0;
-  c->mom_have_shift = false;
-  c->moments_every = every;
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  return EB_OK;
-}
-
-// fold the rows this rank owns of the CURRENT state into the accumulators (enqueued on the stream)
-int accumulate_moments(eb_ctx* c, uint64_t& launches) {
-  int64_t r0, r1;
-  owned_rows(c, r0, r1);
-  const double* X = c->coords.get() + (size_t)r0 * c->D;
-  c->chain_ok = false;
-  if (!c->mom_have_shift) {
-    // shift = the ensemble mean at the first accumulation: keeps the raw second moments well conditioned
-    CK(c, launch_colmean(X, r1 - r0, c->D, c->mom_shift.get(), nullptr, c->st.get()));
-    c->mom_have_shift = true;
-    ++launches;
-  }
-  CK(c, launch_moments(X, r1 - r0, c->D, c->mom_shift.get(), c->mom_partial.get(), c->mom_acc.get(), c->sm_count,
-                       c->st.get()));
-  launches += 2;
-  c->mom_count += (unsigned long long)(r1 - r0);
-  return EB_OK;
-}
-
-// count the CURRENT state into the running histograms (kernels only, enqueued on the stream)
-int accumulate_histograms(eb_ctx* c, uint64_t& launches) {
-  c->chain_ok = false;
-  CK(c, live_hist_launch(c->hist, c->st.get(), launches));
-  c->hist_count += (unsigned long long)c->N;
-  return EB_OK;
-}
-
-// Room for the rows the next `nsteps` steps record, made before the first launch: the rows already recorded move
-// into a larger allocation (half as large again when that fits, so that a run of many short calls grows a few times).
-int reserve_trace(eb_ctx* c, uint64_t nsteps) {
-  const uint64_t add = (c->step + nsteps) / c->trace_every - c->step / c->trace_every;
-  const uint64_t have = c->trace_steps.size(), need = have + add;
-  if (need <= c->trace_cap) return EB_OK;
-  const size_t row = (2 * (size_t)c->D + TRACE_EXTRA) * sizeof(double);
-  size_t free_b = 0, total_b = 0;
-  CK(c, cudaMemGetInfo(&free_b, &total_b));
-  uint64_t cap = std::max(need, c->trace_cap + c->trace_cap / 2);
-  if (cap > free_b / row) cap = need;
-  if (cap > free_b / row)
-    FAIL(c, EB_ERR_NOMEM, "the trace needs room for %llu rows of %zu bytes, %zu bytes free", (unsigned long long)need,
-         row, free_b);
-  DevPtr<double> rows;
-  CK_NOMEM(c, dev_alloc(rows, (size_t)cap * row), "the trace: allocating %llu rows of %zu bytes failed (%s)",
-           (unsigned long long)cap, row, cudaGetErrorString(alloc_err));
-  if (have)
-    CK(c, cudaMemcpyAsync(rows.get(), c->trace_rows.get(), (size_t)have * row, cudaMemcpyDeviceToDevice, c->st.get()));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  c->trace_rows = std::move(rows);
-  c->trace_cap = cap;
-  c->trace_steps.reserve((size_t)cap);
-  return EB_OK;
-}
-
-// record the CURRENT state as one row of the trace (kernels only, enqueued on the stream)
-int accumulate_trace(eb_ctx* c, uint64_t& launches) {
-  c->chain_ok = false;
-  double* row = c->trace_rows.get() + c->trace_steps.size() * (2 * (size_t)c->D + TRACE_EXTRA);
-  CK(c, live_trace_launch(c->trace, row, c->step, c->st.get(), launches));
-  c->trace_steps.push_back(c->step);
-  return EB_OK;
-}
-
-int step_preflight(eb_ctx* c) {
-  if (!c->have_model) FAIL(c, EB_ERR_STATE, "eb_step: no model set");
-  if (!c->have_state) FAIL(c, EB_ERR_STATE, "eb_step: no state set");
-  CK(c, cudaSetDevice(c->device));
-  return EB_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-int eb_step(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint8_t* accepted_last) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  int rc = step_preflight(c);
-  if (rc) return rc;
-  Schedule s;
-  rc = build_schedule(c, moves, nmoves, s);
-  if (rc) return rc;
-  if (nsteps > 0) {
-    rc = run_steps(c, s, nsteps, 0, [](uint64_t) { return EB_OK; });
-    if (rc) return rc;
-  }
-  if (accepted_last) {
-    rc = sync_replicas(c);  // multi-GPU: the mask of every rank's rows (collective)
-    if (rc) return rc;
-    CK(c, cudaMemcpyAsync(accepted_last, c->accepted.get(), (size_t)c->N, cudaMemcpyDeviceToHost, c->st.get()));
-    CK(c, cudaStreamSynchronize(c->st.get()));
-  }
-  return EB_OK;
-}
-
-int eb_step_store(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
-                  double* chain, double* log_prob, double* accepted) {
-  return eb_step_store_blobs(c, moves, nmoves, nsteps, thin_by, chain, log_prob, accepted, nullptr);
-}
-
-int eb_step_store_blobs(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
-                        double* chain, double* log_prob, double* accepted, void* blobs) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
-  if (!chain || !log_prob) FAIL(c, EB_ERR_INVALID, "eb_step_store: null output buffer");
-  if (blobs && !c->blobs_live) FAIL(c, EB_ERR_STATE, "eb_step_store_blobs: the state has no blobs");
-  int rc = step_preflight(c);
-  if (rc) return rc;
-  Schedule s;
-  rc = build_schedule(c, moves, nmoves, s);
-  if (rc) return rc;
-  const size_t N = (size_t)c->N, D = (size_t)c->D;
-  const size_t row = N * D + N;  // coords then log_prob, staged together
-  for (int k = 0; k < 2; ++k) {
-    if (c->stage[k]) continue;
-    HostPtr<double> x;
-    HostPtr<uint8_t> acc;
-    EventPtr ev;
-    CK(c, host_alloc(x, row * sizeof(double)));
-    CK(c, host_alloc(acc, N));
-    CK(c, event_create(ev, cudaEventDisableTiming));
-    c->stage[k] = std::move(x);
-    c->stage_acc[k] = std::move(acc);
-    c->stage_ev[k] = std::move(ev);
-  }
-  const size_t blob_row = blobs ? N * c->blob_bytes : 0;  // the blob records of a stored step, staged beside them
-  if (blob_row > c->stage_blob_cap) {
-    for (HostPtr<uint8_t>& b : c->stage_blob) b.reset();
-    c->stage_blob_cap = 0;
-    for (HostPtr<uint8_t>& b : c->stage_blob) CK(c, host_alloc(b, blob_row));
-    c->stage_blob_cap = blob_row;
-  }
-  uint8_t* blob_out = static_cast<uint8_t*>(blobs);
-  // double-buffered pinned staging: the D2H of stored step k overlaps the
-  // kernels of the following steps; the host drains slot k-1 while k is in flight
-  uint64_t stored = 0;
-  int64_t pending[2] = {-1, -1};
-  auto drain = [&](int slot) -> int {
-    if (pending[slot] < 0) return EB_OK;
-    CK(c, cudaEventSynchronize(c->stage_ev[slot].get()));
-    const size_t k = (size_t)pending[slot];
-    memcpy(chain + k * N * D, c->stage[slot].get(), N * D * sizeof(double));          // backend.py:224
-    memcpy(log_prob + k * N, c->stage[slot].get() + N * D, N * sizeof(double));        // backend.py:225
-    if (blob_out) memcpy(blob_out + k * blob_row, c->stage_blob[slot].get(), blob_row);  // backend.py:226-227
-    if (accepted)
-      for (size_t w = 0; w < N; ++w) accepted[w] += (double)c->stage_acc[slot].get()[w];  // backend.py:229
-    pending[slot] = -1;
-    return EB_OK;
-  };
-  rc = run_steps(c, s, nsteps, thin_by, [&](uint64_t k) -> int {
-    if ((k + 1) % thin_by != 0) return EB_OK;  // ensemble.py:416
-    const int slot = (int)(stored & 1);
-    int r = drain(slot);
-    if (r) return r;
-    c->chain_ok = false;
-    if (c->comm.nranks > 1) {
-      // a stored step holds EVERY walker: replicate the other ranks' rows (log_prob, accept mask and, in
-      // P2P mode, coords) before the copy -- the in-run exchange only moves what the kernels need
-      uint64_t l = 0;
-      if (comm_sync_state(c->comm, c->st.get(), c->status_dev.get(), c->logp.get(), c->accepted.get(), nullptr, l))
-        FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
-      c->fused_last = false;
-    }
-    CK(c, cudaMemcpyAsync(c->stage[slot].get(), c->coords.get(), N * D * sizeof(double), cudaMemcpyDeviceToHost,
-                          c->st.get()));
-    CK(c, cudaMemcpyAsync(c->stage[slot].get() + N * D, c->logp.get(), N * sizeof(double), cudaMemcpyDeviceToHost,
-                          c->st.get()));
-    CK(c, cudaMemcpyAsync(c->stage_acc[slot].get(), c->accepted.get(), N, cudaMemcpyDeviceToHost, c->st.get()));
-    if (blob_out) CK(c, cudaMemcpyAsync(c->stage_blob[slot].get(), c->blob_live.get(), blob_row, cudaMemcpyDeviceToHost,
-                                        c->st.get()));
-    CK(c, cudaEventRecord(c->stage_ev[slot].get(), c->st.get()));
-    pending[slot] = (int64_t)stored;
-    ++stored;
-    return EB_OK;
-  });
-  int r0 = drain((int)(stored & 1));
-  int r1 = drain((int)((stored + 1) & 1));
-  if (rc) return rc;
-  if (r0) return r0;
-  return r1;
-}
-
-}  // extern "C"
 
 namespace {
 
@@ -2251,49 +988,32 @@ int chain_scratch(eb_chain* ch, const char* who, size_t bytes, DevPtr<void>& out
   return EB_OK;
 }
 
+// running chain moments (option "moments_every"): allocate and zero the accumulators
+int moments_config(eb_ctx* c, uint64_t every) {
+  CK(c, cudaSetDevice(c->device));
+  if (every > 0 && c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "chain moments are limited to ndim <= 1024");
+  const size_t n = (size_t)c->D + (size_t)c->D * c->D;
+  if (every > 0 && !c->mom_acc) {
+    DevPtr<double> acc, shift, partial;
+    CK(c, dev_alloc(acc, n * sizeof(double)));
+    CK(c, dev_alloc(shift, (size_t)c->D * sizeof(double)));
+    if (!c->mom_partial) CK(c, dev_alloc(partial, moments_partial_bytes(c->D, c->sm_count)));
+    c->mom_acc = std::move(acc);
+    c->mom_shift = std::move(shift);
+    if (partial) c->mom_partial = std::move(partial);
+  }
+  if (c->mom_acc) CK(c, cudaMemsetAsync(c->mom_acc.get(), 0, n * sizeof(double), c->st.get()));
+  c->mom_count = 0;
+  c->mom_have_shift = false;
+  c->moments_every = every;
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  return EB_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
-int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t nsteps, uint64_t thin_by,
-                        eb_chain* ch, uint64_t slot0) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
-  if (!ch) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: null chain");
-  if (ch->device != c->device || ch->N != c->N || ch->D != c->D)
-    FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: the chain is [%lld, %d] on device %d, the engine [%lld, %d] on device %d",
-         (long long)ch->N, ch->D, ch->device, (long long)c->N, c->D, c->device);
-  if (c->comm.nranks > 1)
-    FAIL(c, EB_ERR_UNSUPPORTED,
-         "eb_step_store_chain: a stored step holds every walker, and sharded ensembles replicate the other ranks' "
-         "rows before each stored step only for host chains (eb_step_store); device chains are not sharded");
-  const uint64_t nstore = nsteps / thin_by;
-  if (nstore > 0 && (slot0 >= ch->start.back() || nstore > ch->start.back() - slot0))
-    FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: slots [%llu, %llu) out of range (capacity %llu slots)",
-         (unsigned long long)slot0, (unsigned long long)(slot0 + nstore), (unsigned long long)ch->start.back());
-  int rc = step_preflight(c);
-  if (rc) return rc;
-  Schedule s;
-  rc = build_schedule(c, moves, nmoves, s);
-  if (rc) return rc;
-  const size_t nx = (size_t)c->N * c->D;
-  uint64_t slot = slot0;
-  size_t seg = 0;
-  // no host synchronisation per stored step: the store kernel is enqueued behind the step on the engine's
-  // stream, and run_steps synchronises once at its end
-  return run_steps(c, s, nsteps, thin_by, [&](uint64_t k) -> int {
-    if ((k + 1) % thin_by != 0) return EB_OK;  // ensemble.py:416
-    while (slot >= ch->start[seg + 1]) ++seg;
-    const uint64_t off = slot - ch->start[seg];
-    c->chain_ok = false;
-    CK(c, launch_chain_store(c->coords.get(), c->logp.get(), c->accepted.get(), ch->segs[seg].x.get() + off * ch->xs,
-                             ch->segs[seg].lp.get() + off * ch->ls, ch->accepted.get(), nx, (size_t)c->N, c->N,
-                             c->sm_count, c->st.get()));
-    ++slot;
-    return EB_OK;
-  });
-}
 
 const char* eb_chain_last_error(const eb_chain* ch) { return ch ? ch->err.c_str() : g_create_err.c_str(); }
 
@@ -2656,7 +1376,6 @@ int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* 
                           cudaMemcpyDeviceToHost, c->st.get()));
   }
   CK(c, cudaStreamSynchronize(c->st.get()));
-  c->chain_ok = false;
   if (count) *count = c->mom_count;
   if (naccepted_total) {
     unsigned long long tot = 0;
@@ -2731,7 +1450,6 @@ int eb_histograms(eb_ctx* c, uint64_t* hist, uint64_t* hist2d, uint64_t* count) 
   CK(c, cudaSetDevice(c->device));
   bool bad = false;
   CK(c, live_hist_read(c->hist, hist, hist2d, &bad, c->st.get()));
-  c->chain_ok = false;
   if (count) *count = c->hist_count;
   if (bad)
     FAIL(c, EB_ERR_INVALID, "eb_histograms: a value's truncated bin index is above bins (np.histogram raises "
@@ -2792,7 +1510,6 @@ int eb_trace_read(eb_ctx* c, uint64_t first, uint64_t count, uint64_t* step, dou
     CK(c, cudaMemcpyAsync(rows_out, c->trace_rows.get() + first * W, (size_t)count * W * sizeof(double),
                           cudaMemcpyDeviceToHost, c->st.get()));
     CK(c, cudaStreamSynchronize(c->st.get()));
-    c->chain_ok = false;
   }
   return EB_OK;
 }
@@ -2805,7 +1522,6 @@ int eb_trace_best(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, u
   CK(c, cudaSetDevice(c->device));
   TraceBest b;
   CK(c, live_trace_best(c->trace, &b, coords, c->st.get()));
-  c->chain_ok = false;
   if (log_prob) *log_prob = b.log_prob;
   if (step) *step = b.step;
   if (walker) *walker = b.walker;
@@ -2824,7 +1540,6 @@ int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, 
   DevPtr<double> dwork;  // [D mean | D + D*D accumulators]
   CK(c, dev_alloc(dwork, (D + n) * sizeof(double)));
   if (!c->mom_partial) CK(c, dev_alloc(c->mom_partial, moments_partial_bytes(c->D, c->sm_count)));
-  c->chain_ok = false;
   std::vector<double> acc(n);
   int f = 0;
   double* work = dwork.get();
@@ -2875,7 +1590,6 @@ int eb_autocorr(eb_ctx* c, const double* chain, size_t n_t, size_t nw, size_t nd
   NOT_IN_CALLBACK(c);
   if (!chain || !acf || n_t == 0 || nw == 0 || nd == 0) FAIL(c, EB_ERR_INVALID, "eb_autocorr: empty chain or null buffer");
   CK(c, cudaSetDevice(c->device));
-  c->chain_ok = false;
   return acf_slabs(c, "eb_autocorr", c->st.get(), n_t, nw, nd, acf, [&](double* xin, size_t w0, size_t wn) {
     // chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd]: one strided copy (rows of the slab are contiguous in a step)
     return cudaMemcpy2DAsync(xin, wn * nd * sizeof(double), chain + w0 * nd, nw * nd * sizeof(double),

@@ -1,4 +1,4 @@
-// Stored index -> (segment, offset) of a device chain kept as a list of segments (eb_chain, capi.cu).  Host code
+// Stored index -> (segment, offset) of a device chain kept as a list of segments (eb_chain, context.h).  Host code
 // only, without CUDA, so that tests/helpers/chain_map_host.cpp can build it for the CPU tests.
 #pragma once
 #include <stddef.h>

@@ -230,7 +230,7 @@ def test_dense_cuda_core(N, D, mean, options, icov):
 
 # ---- grouped dense_dmma ----------------------------------------------------------------------------------------
 class LaunchModel(object):
-    """Host-side mirror of run_steps (capi.cu) for one single-GPU engine with a dense-Gaussian model: predicts the
+    """Host-side mirror of run_steps (step.cu) for one single-GPU engine with a dense-Gaussian model: predicts the
     launch count of a stepping call (eb_last_step_timing) and the largest / last dense_dmma group.  Keeps the
     engine's split-table cache (64-step look-ahead, tables of at most 512 steps) across calls."""
 
