@@ -30,6 +30,7 @@ EB_ERR_INF_PARAM = -11
 EB_ERR_NAN_PARAM = -12
 EB_ERR_FEW_WALKERS = -13
 EB_ERR_NAN_INITIAL = -14
+EB_ERR_SINGULAR = -15
 
 EB_COMM_ID_BYTES = 128
 EB_IPC_BLOB_BYTES = 256
@@ -43,7 +44,7 @@ EB_MAX_PROPOSAL_SLOTS = 64  # user proposals one engine can hold (eb_move_set_pr
 EB_STREAM_UNKNOWN = 2**64 - 1  # eb_callback_result: the producer named no stream -> wait for the whole device
 
 MODEL_KINDS = {"gauss_iso": 0, "gauss_dense": 1, "rosenbrock": 2, "ring": 3}
-MOVE_KINDS = {"stretch": 0, "de": 1, "snooker": 2, "walk": 3, "gaussian": 4, "user": 5, "user_mh": 6}
+MOVE_KINDS = {"stretch": 0, "de": 1, "snooker": 2, "walk": 3, "gaussian": 4, "user": 5, "user_mh": 6, "kde": 7}
 
 
 class EbMove(C.Structure):
@@ -262,6 +263,8 @@ def _raise(rc, msg):
         raise RuntimeError(msg)
     if rc == EB_ERR_NOMEM:
         raise MemoryError(msg)
+    if rc == EB_ERR_SINGULAR:
+        raise np.linalg.LinAlgError(msg)
     raise EngineError("%s (eb_status %d)" % (msg, rc))
 
 

@@ -29,6 +29,12 @@ int check_status(eb_ctx* c) {
   cudaStreamSynchronize(c->st.get());
   if (f & FLAG_COMM_TIMEOUT) FAIL(c, EB_ERR_COMM, "peer-memory barrier timed out: another rank did not arrive");
   if (f & FLAG_WAIT_TIMEOUT) FAIL(c, EB_ERR_CUDA, "kernel stalled: a warp waited ~2 minutes for a hand-off in its block");
+  if (f & FLAG_KDE_SINGULAR)  // scipy/stats/_kde.py, gaussian_kde.__init__'s LinAlgError
+    FAIL(c, EB_ERR_SINGULAR,
+         "The data appears to lie in a lower-dimensional subspace of the space in which it is expressed. This has "
+         "resulted in a singular data covariance matrix, which cannot be treated using the algorithms implemented in "
+         "`gaussian_kde`. Consider performing principal component analysis / dimensionality reduction and using "
+         "`gaussian_kde` with the transformed data.");
   if (f & FLAG_NAN_INITIAL) FAIL(c, EB_ERR_NAN_INITIAL, "The initial log_prob was NaN");  // ensemble.py:357-358
   if (f & FLAG_INF_PARAM) FAIL(c, EB_ERR_INF_PARAM, "At least one parameter value was infinite");
   if (f & FLAG_NAN_PARAM) FAIL(c, EB_ERR_NAN_PARAM, "At least one parameter value was NaN");

@@ -147,6 +147,12 @@ struct eb_ctx {
   DevPtr<double> gauss_dev;  // per schedule entry: scale / factor L of GaussianMove
   size_t gauss_cap = 0;
   std::vector<uint64_t> picks;  // per schedule entry: steps of the last call that ran it
+  // KDEMove scratch (kde.cu), allocated together on its first half-step
+  DevPtr<double> kde_y;     // [ns + ns + nc <= N + N / 2 + 1, D] whitened s | q rows, then complement rows
+  DevPtr<double> kde_f;     // [N] Hastings factors
+  DevPtr<int64_t> kde_j;    // [N] walker id of each proposal's kernel centre (debug taps)
+  DevPtr<double> kde_part;  // kde_partial_doubles: partial (max, sum) pairs of the log-sum-exps
+  DevPtr<double> kde_mat;   // [D * D] (bw L)^-1, then [D] the complement mean
 
   Comm comm;  // multi-GPU (comm.h)
 

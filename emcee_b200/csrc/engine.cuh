@@ -24,6 +24,7 @@ enum : int {
   FLAG_COMM_TIMEOUT = 8,
   FLAG_WAIT_TIMEOUT = 16,  // a warp gave up on an in-kernel hand-off (shared-memory barrier) of its own CTA
   FLAG_NAN_INITIAL = 32,   // a NaN in an initial log_prob given in device memory (eb_set_state_from)
+  FLAG_KDE_SINGULAR = 64,  // KDEMove: the complement covariance of a split has a zero pivot (kde.cu)
 };
 
 struct ModelDev {
@@ -187,6 +188,28 @@ cudaError_t launch_gaussian_shift(const double* L, int D, double f, uint64_t see
 cudaError_t launch_gaussian_propose(const double* x0, int64_t row0, int64_t nrows, int D, int form, const double* scale,
                                     double f, int mode, int seq_dim, uint64_t seed, uint64_t step, double* qbuf,
                                     cudaStream_t st);
+
+// ---- KDEMove (kde.cu) ---------------------------------------------------------------------------
+// launch geometry of the log-density kernel: ptiles point tiles of 64 (2 ns points: the s rows, then the q rows) x
+// nchunks chunks of tpc centre tiles of 64
+struct KdePlan {
+  int64_t ptiles;
+  int tpc, nchunks;
+};
+KdePlan kde_plan(int64_t ns, int64_t nc, int sm_count);
+// doubles of the partial (max, sum) buffer every plan of an N-walker engine fits in
+size_t kde_partial_doubles(int64_t N, int sm_count);
+// L of cov_chol over nc complement rows with moment sums acc about shift -> minv = (bw L)^-1, mean = the complement
+// mean; a zero pivot of L sets FLAG_KDE_SINGULAR in status and writes nothing
+cudaError_t launch_kde_factor(const double* L, const double* acc, const double* shift, double nc, int D, double bw,
+                              double* minv, double* mean, int* status, cudaStream_t st);
+// the proposals qbuf[ns, D], whitened points yp[2 ns, D] (s rows, then q rows), whitened complement yc[nc, D] and
+// the walker id of each proposal's kernel centre jw[ns] of half-step a
+cudaError_t launch_kde_prepare(const HalfStepArgs& a, const double* L, const double* minv, const double* mean,
+                               double bw, double* qbuf, double* yp, double* yc, int64_t* jw, cudaStream_t st);
+// f[ns] = LSE_c(-|y_s - y_c|^2 / 2) - LSE_c(-|y_q - y_c|^2 / 2); part: kde_partial_doubles scratch
+cudaError_t launch_kde_factors(const double* yp, const double* yc, int64_t ns, int64_t nc, int D, const KdePlan& p,
+                               double* part, double* f, cudaStream_t st);
 
 // ---- chain analysis (analysis.cu) ------------------------------------------------------------
 // column means of X[nrows, D] (fixed summation order); status (nullable) gets the non-finite flags

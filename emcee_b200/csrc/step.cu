@@ -65,8 +65,24 @@ int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) 
         continue;
       }
       if (m.mode != 0 && m.mode != EB_USER_SETUP) FAIL(c, EB_ERR_INVALID, "eb_step: unknown user-move mode %d", m.mode);
-    } else if (m.kind < EB_MOVE_STRETCH || m.kind > EB_MOVE_GAUSSIAN) {
+    } else if ((m.kind < EB_MOVE_STRETCH || m.kind > EB_MOVE_GAUSSIAN) && m.kind != EB_MOVE_KDE) {
       FAIL(c, EB_ERR_INVALID, "eb_step: unknown move kind %d", m.kind);
+    }
+    if (m.kind == EB_MOVE_KDE) {
+      if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: KDEMove is not sharded across GPUs");
+      if (c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: KDEMove is limited to ndim <= 1024");
+      if (!isnan(m.p0) && m.p0 != EB_KDE_SILVERMAN && m.p0 != EB_KDE_SCALAR)
+        FAIL(c, EB_ERR_INVALID, "eb_step: unknown KDEMove bandwidth rule %g", m.p0);
+      if (m.p0 == EB_KDE_SCALAR && !(m.p1 > 0.0 && isfinite(m.p1)))
+        FAIL(c, EB_ERR_INVALID, "eb_step: a KDEMove bandwidth must be finite and > 0 (got %g)", m.p1);
+      // the smallest complement, that of the first split (scipy/stats/_kde.py gaussian_kde.__init__)
+      if (m.nsplits >= 2 && m.nsplits <= MAX_SPLITS && m.nsplits <= c->N &&
+          (int64_t)c->D > c->N - (c->N + m.nsplits - 1) / m.nsplits)
+        FAIL(c, EB_ERR_INVALID,
+             "Number of dimensions is greater than number of samples. This results in a singular data covariance "
+             "matrix, which cannot be treated using the algorithms implemented in `gaussian_kde`. Note that "
+             "`gaussian_kde` interprets each *column* of `dataset` to be a point; consider transposing the input to "
+             "`dataset`.");
     }
     if ((m.kind == EB_MOVE_WALK || m.kind == EB_MOVE_GAUSSIAN) && c->comm.nranks > 1)
       FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: WalkMove / GaussianMove are not sharded across GPUs yet");
@@ -381,6 +397,93 @@ int launch_step_walk(eb_ctx* c, const eb_move& mv, uint64_t step, size_t tbl, ui
     if (rc) return rc;
   }
   if (c->model.kind != MODEL_EXTERNAL) note_kernel(c, "walk", "walk");
+  return EB_OK;
+}
+
+// scipy's bandwidth factor of a KDE of n uniformly weighted points (gaussian_kde.scotts_factor / silverman_factor;
+// neff = n)
+double kde_bandwidth(const eb_move& mv, int64_t n, int D) {
+  if (mv.p0 == EB_KDE_SCALAR) return mv.p1;
+  const double neff = (double)n;
+  if (mv.p0 == EB_KDE_SILVERMAN) return pow(neff * (D + 2.0) / 4.0, -1.0 / (D + 4));
+  return pow(neff, -1.0 / (D + 4));
+}
+
+int ensure_kde_scratch(eb_ctx* c) {
+  if (c->kde_y) return EB_OK;
+  const size_t N = (size_t)c->N, D = (size_t)c->D;
+  DevPtr<double> y, f, part, mat;
+  DevPtr<int64_t> j;
+  CK(c, dev_alloc(y, (N + N / 2 + 1) * D * sizeof(double)));
+  CK(c, dev_alloc(f, N * sizeof(double)));
+  CK(c, dev_alloc(j, N * sizeof(int64_t)));
+  CK(c, dev_alloc(part, kde_partial_doubles(c->N, c->sm_count) * sizeof(double)));
+  CK(c, dev_alloc(mat, (D * D + D) * sizeof(double)));
+  c->kde_y = std::move(y);
+  c->kde_f = std::move(f);
+  c->kde_j = std::move(j);
+  c->kde_part = std::move(part);
+  c->kde_mat = std::move(mat);
+  return EB_OK;
+}
+
+// KDEMove (kde.py:39-43): per split the complement covariance and factor as the whole-complement WalkMove's, then
+// kde.cu's kernels write the proposals and their Hastings factors, and the accept of precomputed rows takes them.
+// A singular factor stops the call here, before this split's update: the status read synchronises once per split.
+int launch_step_kde(eb_ctx* c, const eb_move& mv, uint64_t step, size_t tbl, uint64_t& launches) {
+  int rc = check_walker_count(c, mv);
+  if (rc) return rc;
+  rc = ensure_move_scratch(c);
+  if (rc) return rc;
+  rc = ensure_kde_scratch(c);
+  if (rc) return rc;
+  int start[MAX_SPLITS + 1];
+  split_starts(c->N, mv.nsplits, start);
+  const size_t D = (size_t)c->D;
+  double* shift = c->walk_work.get();
+  double* acc = shift + D;
+  double* cov = acc + D + D * D;
+  double* L = cov + D * D;
+  double* minv = c->kde_mat.get();
+  double* mean = minv + D * D;
+  KdePlan plan{};
+  for (int split = 0; split < mv.nsplits; ++split) {
+    const HalfStepArgs a = split_args(c, mv, step, tbl, start, split);
+    const int64_t ns = a.a_count, nc = c->N - a.a_count;
+    const double bw = kde_bandwidth(mv, nc, c->D);
+    CK(c, launch_colmean(c->coords.get(), c->N, c->D, shift, nullptr, c->st.get()));
+    CK(c, cudaMemsetAsync(acc, 0, (D + D * D) * sizeof(double), c->st.get()));
+    CK(c, launch_moments(c->coords.get(), nc, c->D, shift, c->mom_partial.get(), acc, c->sm_count, c->st.get(),
+                         a.order, a.a_start, a.a_count));
+    CK(c, launch_cov_chol(acc, (double)nc, c->D, cov, L, c->st.get()));
+    CK(c, launch_kde_factor(L, acc, shift, (double)nc, c->D, bw, minv, mean, c->status_dev.get(), c->st.get()));
+    launches += 5;
+    rc = fetch_status(c);
+    if (rc) return rc;
+    double* yp = c->kde_y.get();
+    double* yc = yp + (size_t)2 * ns * D;
+    CK(c, launch_kde_prepare(a, L, minv, mean, bw, c->qbuf.get(), yp, yc, c->kde_j.get(), c->st.get()));
+    plan = kde_plan(ns, nc, c->sm_count);
+    CK(c, launch_kde_factors(yp, yc, ns, nc, c->D, plan, c->kde_part.get(), c->kde_f.get(), c->st.get()));
+    launches += 3;
+    if (c->model.kind == MODEL_EXTERNAL) {
+      rc = external_accept(c, MOVE_PRECOMPUTED, a, c->kde_f.get(), launches);
+      if (rc) return rc;
+      note_callback(c);
+    } else {
+      CK(c, launch_half_step_user(EB_MOVE_USER, a, ExternalBufs{c->qbuf.get(), c->kde_f.get(), nullptr}, c->st.get()));
+      ++launches;
+    }
+    if (c->debug) {  // the accept wrote the uniforms and walkers; the centres and factors are this move's
+      CK(c, cudaMemcpyAsync(c->tap_partners.get(), c->kde_j.get(), (size_t)ns * sizeof(int64_t),
+                            cudaMemcpyDeviceToDevice, c->st.get()));
+      CK(c, cudaMemcpyAsync(c->tap_scalar.get(), c->kde_f.get(), (size_t)ns * sizeof(double), cudaMemcpyDeviceToDevice,
+                            c->st.get()));
+      c->tap_count = a.a_count;
+    }
+  }
+  if (c->model.kind != MODEL_EXTERNAL)
+    note_kernel(c, "kde", "kde tpc=%d nchunks=%d", plan.tpc, plan.nchunks);
   return EB_OK;
 }
 
@@ -769,6 +872,9 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         switch (mv.kind) {
           case EB_MOVE_WALK:
             rc = launch_step_walk(c, mv, c->step, tbl, launches);
+            break;
+          case EB_MOVE_KDE:
+            rc = launch_step_kde(c, mv, c->step, tbl, launches);
             break;
           case EB_MOVE_GAUSSIAN:
             rc = launch_step_gaussian(c, s, ch.pick[k], c->step, launches);

@@ -308,6 +308,8 @@ class EnsembleSampler(object):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
             raise NotImplementedError("a user proposal runs on one GPU; a schedule with user moves cannot be sharded")
+        if any(getattr(m, "kind", None) == "kde" for m in self._moves):
+            raise NotImplementedError("KDEMove runs on one GPU; a schedule with it cannot be sharded")
         dist.attach(self._engine, rdv, mode)
         self._rdv = rdv
         self._gather_results = bool(gather_results)

@@ -3,12 +3,13 @@
 The red-blue family (``StretchMove``, ``DEMove``, ``DESnookerMove``, ``WalkMove``) and the
 Metropolis family with Gaussian proposals (``MHMove``, ``GaussianMove``), and user-written proposals:
 ``RedBlueMove`` subclasses that override ``get_proposal`` (``CudaArrayRedBlueMove`` for CUDA arrays) and
-``MHMove(HostProposal(fn))`` / ``MHMove(CudaArrayProposal(fn))``; the reference's ``KDEMove`` (SciPy
-kernel-density proposals) is out of scope (DESIGN.md)."""
+``MHMove(HostProposal(fn))`` / ``MHMove(CudaArrayProposal(fn))``, and ``KDEMove`` (the reference's SciPy
+kernel-density proposals, built on the device)."""
 
 from .de import DEMove
 from .de_snooker import DESnookerMove
 from .gaussian import GaussianMove
+from .kde import KDEMove
 from .mh import MHMove
 from .move import Move
 from .red_blue import RedBlueMove
@@ -16,5 +17,5 @@ from .stretch import StretchMove
 from .user import CudaArrayProposal, CudaArrayRedBlueMove, HostProposal, user_random
 from .walk import WalkMove
 
-__all__ = ["Move", "RedBlueMove", "StretchMove", "DEMove", "DESnookerMove", "WalkMove", "MHMove", "GaussianMove",
-           "HostProposal", "CudaArrayProposal", "CudaArrayRedBlueMove", "user_random"]
+__all__ = ["Move", "RedBlueMove", "StretchMove", "DEMove", "DESnookerMove", "WalkMove", "KDEMove", "MHMove",
+           "GaussianMove", "HostProposal", "CudaArrayProposal", "CudaArrayRedBlueMove", "user_random"]

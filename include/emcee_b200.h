@@ -42,7 +42,8 @@ typedef enum eb_status {
   EB_ERR_INF_PARAM = -11,   /* ensemble.py:476-477 "At least one parameter value was infinite" */
   EB_ERR_NAN_PARAM = -12,   /* ensemble.py:478-479 "At least one parameter value was NaN" */
   EB_ERR_FEW_WALKERS = -13, /* moves/red_blue.py:64-70 RuntimeError (nwalkers < 2*ndim) */
-  EB_ERR_NAN_INITIAL = -14  /* ensemble.py:357-358 "The initial log_prob was NaN" */
+  EB_ERR_NAN_INITIAL = -14, /* ensemble.py:357-358 "The initial log_prob was NaN" */
+  EB_ERR_SINGULAR = -15     /* EB_MOVE_KDE: a complement covariance is singular (gaussian_kde's LinAlgError) */
 } eb_status;
 
 /* registered device-side log-probability models (replace the Python callable
@@ -72,6 +73,16 @@ typedef enum eb_move_kind {
 #define EB_MOVE_USER_MH 6 /* MHMove with a user proposal_function (mh.py:31-33,52); p0 = proposal slot;
                              nsplits / randomize_split are ignored */
 #define EB_USER_SETUP 1
+
+/* KDEMove (moves/kde.py: scipy.stats.gaussian_kde of the complement, resample + logpdf ratio); not a member of
+ * eb_move_kind for the same reason.  p0 = the bandwidth rule: NaN Scott (n ** (-1 / (d + 4))), EB_KDE_SILVERMAN
+ * ((n (d + 2) / 4) ** (-1 / (d + 4))), EB_KDE_SCALAR: p1 is the bandwidth (finite, > 0); n = the complement size.
+ * A split whose complement has fewer rows than ndim is refused before any update (EB_ERR_INVALID, scipy's
+ * message); a singular complement covariance (a Cholesky pivot <= 1e-12 max(diag)) stops the call at that
+ * half-step with EB_ERR_SINGULAR, earlier splits applied.  ndim <= 1024; sharded engines: EB_ERR_UNSUPPORTED. */
+#define EB_MOVE_KDE 7
+#define EB_KDE_SILVERMAN 1.0
+#define EB_KDE_SCALAR 2.0
 
 typedef enum eb_gaussian_mode { /* gaussian.py:63,99-104 */
   EB_GAUSS_VECTOR = 0, EB_GAUSS_RANDOM = 1, EB_GAUSS_SEQUENTIAL = 2
