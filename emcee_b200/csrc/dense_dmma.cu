@@ -32,6 +32,7 @@
 //     the 74 KB factor, pipeline refill from cold).
 #include <math.h>
 
+#include "draws.cuh"
 #include "engine.cuh"
 #include "tma.cuh"
 
@@ -285,15 +286,13 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         p.valid = i < i_hi;
         if (!p.valid) i = i_hi - 1;
         if (aperm) i = __ldg(aperm + i);  // sharded: tiles are built partner-local first (locality_table_kernel)
-        const u32x4 A = draw_words(a.seed, d.step, (uint32_t)d.split, TAG_PROP_A, (uint32_t)i);
-        const double tt = __dadd_rn(__dmul_rn(__dsub_rn(a.p0, 1.0), u53(A.x, A.y)), 1.0);  // stretch.py:30
-        p.zz = __ddiv_rn(__dmul_rn(tt, tt), a.p0);
-        const int64_t r = (int64_t)bounded64(A.z, A.w, (uint64_t)Nc);  // stretch.py:32
+        const u32x4 A = prop_a(a.seed, d.step, (uint32_t)d.split, (uint32_t)i);
+        p.zz = stretch_zz(A, a.p0);
+        const int64_t r = stretch_rank(A, Nc);
         p.w = __ldg(order + d.a_start + i);
-        p.wp = __ldg(order + (r < d.a_start ? r : r + d.a_count));
-        const u32x4 U = draw_words(a.seed, d.step, (uint32_t)d.split, TAG_ACCEPT, (uint32_t)i);
-        p.log_u = log(u53(U.x, U.y));
-        p.factor = __dmul_rn(dm1, log(p.zz));  // stretch.py:31
+        p.wp = __ldg(order + complement_slot(r, d.a_start, d.a_count));
+        p.log_u = log(accept_uniform(a.seed, d.step, (uint32_t)d.split, (uint32_t)i));
+        p.factor = stretch_factor(dm1, p.zz);
         p.lp_old = with_lp ? a.logp[p.w] : 0.0;
         p.remote = multi && (p.wp / a.rows_per_rank != a.p2p_rank);
         return p;
@@ -428,9 +427,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
           for (int j = 0; j < KB; ++j) {
             const double2 s2 = *reinterpret_cast<const double2*>(myS + 8 * j);
             const double2 c2 = *reinterpret_cast<const double2*>(myC + 8 * j);
-            double2 q2;  // stretch.py:33, as below
-            q2.x = __dsub_rn(c2.x, __dmul_rn(__dsub_rn(c2.x, s2.x), zz));
-            q2.y = __dsub_rn(c2.y, __dmul_rn(__dsub_rn(c2.y, s2.y), zz));
+            const double2 q2 = make_double2(stretch_q(s2.x, c2.x, zz), stretch_q(s2.y, c2.y, zz));
             *reinterpret_cast<double2*>(myC + 8 * j) = q2;
             const double2 l2 = __ldg(reinterpret_cast<const double2*>(a.model.lo + 8 * j + 2 * t));
             const double2 h2 = __ldg(reinterpret_cast<const double2*>(a.model.hi + 8 * j + 2 * t));
@@ -444,11 +441,8 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
           for (int j = 0; j < KB; ++j) {
             const double2 s2 = *reinterpret_cast<const double2*>(myS + 8 * j);
             const double2 c2 = *reinterpret_cast<const double2*>(myC + 8 * j);
-            // stretch.py:33  q = c - (c - s) * zz, each op rounded once (no FMA contraction)
-            double2 q2;
-            q2.x = __dsub_rn(c2.x, __dmul_rn(__dsub_rn(c2.x, s2.x), zz));
-            q2.y = __dsub_rn(c2.y, __dmul_rn(__dsub_rn(c2.y, s2.y), zz));
-            *reinterpret_cast<double2*>(myC + 8 * j) = q2;
+            *reinterpret_cast<double2*>(myC + 8 * j) =
+                make_double2(stretch_q(s2.x, c2.x, zz), stretch_q(s2.y, c2.y, zz));
           }
         }
         __syncwarp();
@@ -539,7 +533,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       }
 
       // ---- Metropolis accept + in-place update (red_blue.py:96-104, move.py:29-34)
-      const double lnpdiff = __dsub_rn(__dadd_rn(factor, lp_new), lp_old);
+      const double lnpdiff = lnpdiff_red_blue(factor, lp_new, lp_old);
       const bool acc = (w >= 0) && (lnpdiff > log_u);
       if (multi && !peers_passed) {
         // sharded: a slower peer may still be reading this rank's rows for ITS previous half-step; nothing is

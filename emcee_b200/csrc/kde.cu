@@ -16,10 +16,11 @@
 //                       gridDim.y CTAs, whose partial (max, sum) pairs kde_merge_kernel folds into the factors
 // and the accept of precomputed rows with a Hastings factor buffer (half_step_generic_kernel<EB_MOVE_USER>).
 //
-// Draw specification (DESIGN.md §2, oracle/philox.py): j_i = mulhi64(w1:w0, nc) of block (index = i, TAG_PROP_A);
-// z_i = the TAG_NORMAL normals of row i (as WalkMove).
+// Draws (DESIGN.md §2, draws.cuh): the kernel centre j_i from block (index = i, TAG_PROP_A), z_i = the TAG_NORMAL
+// normals of row i (as WalkMove).
 #include <math.h>
 
+#include "draws.cuh"
 #include "engine.cuh"
 
 namespace eb {
@@ -30,17 +31,6 @@ constexpr int KT = 64;          // points and centres per tile
 constexpr int KD = 32;          // dimensions per staged chunk
 constexpr int KPAD = KT + 1;    // smem row pitch of a transposed chunk: [KD][KT + 1]
 constexpr int LSE_THREADS = 256;  // 16 point lanes x 16 centre lanes, each 4 points x 4 centres
-
-// the pair of standard normals (2k, 2k+1) of row `index` (moves_extra.cu's normal_pair)
-__device__ __forceinline__ void normal_pair(uint64_t seed, uint64_t step, uint32_t split, uint32_t k, uint32_t index,
-                                            double& n0, double& n1) {
-  const u32x4 w = draw_words(seed, step, (split & 0x3Fu) | (k << 6), TAG_NORMAL, index);
-  const double r = sqrt(-2.0 * log(1.0 - u53(w.x, w.y)));
-  double sn, cs;
-  sincos(6.283185307179586 * u53(w.z, w.w), &sn, &cs);
-  n0 = r * cs;
-  n1 = r * sn;
-}
 
 // L (cov_chol_kernel) -> minv = (bw L)^-1 (lower, row-major), mean = shift + S1 / nc.  A zero pivot (at or below
 // chol_psd's 1e-12 max-diag threshold, or past the rank bound nc - 1) sets FLAG_KDE_SINGULAR and writes nothing.
@@ -105,16 +95,14 @@ __global__ void __launch_bounds__(256) kde_prepare_kernel(const HalfStepArgs a, 
   double* y;
   if (r < ns || r >= 2 * ns) {
     const int64_t k = r - 2 * ns;
-    const int64_t w = r < ns ? a.order[a.a_start + r] : a.order[k < a.a_start ? k : k + a.a_count];
+    const int64_t w = r < ns ? a.order[a.a_start + r] : a.order[complement_slot(k, a.a_start, a.a_count)];
     const double* x = a.coords + (size_t)w * D;
     for (int e = g; e < D; e += G) v[e] = x[e] - mean[e];
     y = r < ns ? yp + (size_t)r * D : yc + (size_t)k * D;
   } else {
     const int64_t i = r - ns;
-    // kde.resample: choice(nc, size=ns, p=uniform) -> complement rank -> walker id
-    const u32x4 A = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_A, (uint32_t)i);
-    const int64_t k = (int64_t)bounded64(A.x, A.y, (uint64_t)nc);
-    const int64_t cw = a.order[k < a.a_start ? k : k + a.a_count];
+    const int64_t k = kde_centre_rank(prop_a(a.seed, a.step, (uint32_t)a.split, (uint32_t)i), nc);
+    const int64_t cw = a.order[complement_slot(k, a.a_start, a.a_count)];
     for (int kk = g; 2 * kk < D; kk += G) {
       double n0, n1;
       normal_pair(a.seed, a.step, (uint32_t)a.split, (uint32_t)kk, (uint32_t)i, n0, n1);

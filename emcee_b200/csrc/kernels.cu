@@ -12,6 +12,7 @@
 
 #include <algorithm>
 
+#include "draws.cuh"
 #include "engine.cuh"
 #include "rowops.cuh"
 
@@ -126,9 +127,8 @@ __global__ void __launch_bounds__(TABLE_THREADS) locality_table_kernel(const int
   const int i_lo = rg.x, i_hi = rg.y;
   const int64_t Nc = N - a_count;
   auto is_local = [&](int i) -> bool {
-    const u32x4 A = draw_words(seed, step, (uint32_t)split, TAG_PROP_A, (uint32_t)i);
-    const int64_t r = (int64_t)bounded64(A.z, A.w, (uint64_t)Nc);  // stretch.py:32
-    const int64_t wp = order[r < a_start ? r : r + a_count];
+    const int64_t r = stretch_rank(prop_a(seed, step, (uint32_t)split, (uint32_t)i), Nc);
+    const int64_t wp = order[complement_slot(r, a_start, a_count)];
     return wp / rows_per_rank == rank;
   };
   // pass 1: how many owned active ranks have a local partner; at most `front_cap` of them (one tile per consumer
@@ -224,43 +224,32 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
   const int64_t w = a.order ? (int64_t)a.order[a.a_start + i] : i;  // no table: the active set is every walker (MHMove)
   const double* s_row = a.coords + (size_t)w * D;  // the active walker is always local
 
-  const u32x4 A = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_A, (uint32_t)i);
+  const u32x4 A = prop_a(a.seed, a.step, (uint32_t)a.split, (uint32_t)i);
   double factor = 0.0, tap_scalar = 0.0;
   int64_t pw[3] = {-1, -1, -1};
 
   if (MOVE == EB_MOVE_STRETCH) {
     const int64_t Nc = a.N - a.a_count;
-    // stretch.py:30  zz = ((a - 1) * u + 1) ** 2 / a   (each op rounded once)
-    const double t = __dadd_rn(__dmul_rn(__dsub_rn(a.p0, 1.0), u53(A.x, A.y)), 1.0);
-    const double zz = __ddiv_rn(__dmul_rn(t, t), a.p0);
-    // stretch.py:32  rint ; complement rank -> walker id
-    const int64_t r = (int64_t)bounded64(A.z, A.w, (uint64_t)Nc);
-    pw[0] = a.order[r < a.a_start ? r : r + a.a_count];
+    const double zz = stretch_zz(A, a.p0);
+    pw[0] = a.order[complement_slot(stretch_rank(A, Nc), a.a_start, a.a_count)];
     const double* c_row = row_ptr(a, pw[0]);
     for (int e = g; e < D; e += G) {
-      const double s = s_row[e], c = c_row[e];
-      // stretch.py:33  q = c - (c - s) * zz   (no FMA contraction)
-      const double v = __dsub_rn(c, __dmul_rn(__dsub_rn(c, s), zz));
+      const double v = stretch_q(s_row[e], c_row[e], zz);
       q[e] = v;
       if (!isfinite(v)) flag_nonfinite(v, a.status);
     }
-    factor = __dmul_rn((double)D - 1.0, log(zz));  // stretch.py:31
+    factor = stretch_factor((double)D - 1.0, zz);
     tap_scalar = zz;
   } else if (MOVE == EB_MOVE_DE) {
-    const uint64_t Nc = (uint64_t)(a.N - a.a_count);
-    const uint64_t m = bounded64(A.x, A.y, Nc * (Nc - 1));  // de.py:49
-    uint64_t r0, r1;
-    de_pair_decode(m, Nc, r0, r1);  // de.py:67-77
-    pw[0] = a.order[(int64_t)r0 < a.a_start ? (int64_t)r0 : (int64_t)r0 + a.a_count];
-    pw[1] = a.order[(int64_t)r1 < a.a_start ? (int64_t)r1 : (int64_t)r1 + a.a_count];
-    const u32x4 B = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_B, (uint32_t)i);
-    const double n = sqrt(-2.0 * log(1.0 - u53(B.x, B.y))) * cos(6.283185307179586 * u53(B.z, B.w));
-    const double gamma = __dmul_rn(a.p0, __dadd_rn(1.0, __dmul_rn(a.p1, n)));  // de.py:56
+    int64_t r0, r1;
+    de_pair(A, a.N - a.a_count, r0, r1);
+    pw[0] = a.order[complement_slot(r0, a.a_start, a.a_count)];
+    pw[1] = a.order[complement_slot(r1, a.a_start, a.a_count)];
+    const double gamma = de_gamma(prop_b(a.seed, a.step, (uint32_t)a.split, (uint32_t)i), a.p0, a.p1);
     const double* c0 = row_ptr(a, pw[0]);
     const double* c1 = row_ptr(a, pw[1]);
     for (int e = g; e < D; e += G) {
-      // de.py:53,62  q = s + gamma * (c[p1] - c[p0])
-      const double v = __dadd_rn(s_row[e], __dmul_rn(gamma, __dsub_rn(c1[e], c0[e])));
+      const double v = de_q(s_row[e], c0[e], c1[e], gamma);
       q[e] = v;
       if (!isfinite(v)) flag_nonfinite(v, a.status);
     }
@@ -277,21 +266,8 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     }
     if ((MODEL == MODEL_EXTERNAL || MOVE != MOVE_PRECOMPUTED) && ext.f != nullptr) factor = ext.f[i - i_lo];
   } else {  // EB_MOVE_SNOOKER
-    const u32x4 B = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_B, (uint32_t)i);
-    int64_t cw[3];
-    cw[0] = a.order[a.c_start[0] + (int64_t)bounded64(A.x, A.y, (uint64_t)a.c_count[0])];  // de_snooker.py:38
-    cw[1] = a.order[a.c_start[1] + (int64_t)bounded64(A.z, A.w, (uint64_t)a.c_count[1])];
-    cw[2] = a.order[a.c_start[2] + (int64_t)bounded64(B.x, B.y, (uint64_t)a.c_count[2])];
-    // de_snooker.py:39  shuffle of the three rows -> one of 6 orders
-    const int p = (int)bounded64(B.z, B.w, 6);
-    const int i0 = p >> 1;                                 // 0,0,1,1,2,2
-    const int rest0 = (i0 == 0) ? 1 : 0;                   // smaller of the remaining two
-    const int rest1 = (i0 == 2) ? 1 : 2;                   // larger of the remaining two
-    const int i1 = (p & 1) ? rest1 : rest0;
-    const int i2 = (p & 1) ? rest0 : rest1;
-    pw[0] = cw[i0];
-    pw[1] = cw[i1];
-    pw[2] = cw[i2];
+    const u32x4 B = prop_b(a.seed, a.step, (uint32_t)a.split, (uint32_t)i);
+    snooker_partners(A, B, a.c_start, a.c_count, [&](int64_t slot) -> int64_t { return a.order[slot]; }, pw);
     double* sS = q + (size_t)1 * D;  // rows: q | s | z | (z1 - z2 is streamed)
     double* sZ = q + (size_t)2 * D;
     double* sU = q + (size_t)3 * D;
@@ -301,7 +277,7 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     double n2 = 0.0;
     for (int e = g; e < D; e += G) {
       const double s = s_row[e], zz_ = z[e];
-      const double d = __dsub_rn(s, zz_);  // de_snooker.py:41 delta
+      const double d = snooker_delta(s, zz_);
       sS[e] = s;
       sZ[e] = zz_;
       sU[e] = d;
@@ -310,7 +286,7 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     const double norm = sqrt(group_sum(n2, G, mask));  // de_snooker.py:42
     double d1 = 0.0, d2 = 0.0;
     for (int e = g; e < D; e += G) {
-      const double u = __ddiv_rn(sU[e], norm);  // de_snooker.py:43
+      const double u = snooker_u(sU[e], norm);
       sU[e] = u;
       d1 = fma(u, z1[e], d1);
       d2 = fma(u, z2[e], d2);
@@ -320,15 +296,14 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     const double dd = __dsub_rn(d1, d2);
     double m2 = 0.0;
     for (int e = g; e < D; e += G) {
-      // de_snooker.py:44  q = s + u * gammas * (u.z1 - u.z2)
-      const double v = __dadd_rn(sS[e], __dmul_rn(__dmul_rn(sU[e], a.p0), dd));
+      const double v = snooker_q(sS[e], sU[e], a.p0, dd);
       q[e] = v;
       if (!isfinite(v)) flag_nonfinite(v, a.status);
       const double dq = __dsub_rn(v, sZ[e]);
       m2 = fma(dq, dq, m2);
     }
     const double qn = sqrt(group_sum(m2, G, mask));
-    factor = __dmul_rn((double)D - 1.0, __dsub_rn(log(qn), log(norm)));  // de_snooker.py:45-46
+    factor = snooker_factor((double)D - 1.0, qn, norm);
     tap_scalar = norm;
   }
   __syncwarp(mask);
@@ -359,13 +334,10 @@ __global__ void __launch_bounds__(256) half_step_generic_kernel(const HalfStepAr
     if (isnan(lp_new) && g == 0) atomicOr(a.status, FLAG_NAN_LOGPROB);
   }
 
-  // red_blue.py:96-101
-  const u32x4 U = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_ACCEPT, (uint32_t)i);
-  const double u_acc = u53(U.x, U.y);
-  // red_blue.py:99 (f + lp_new) - lp_old; a user MHMove keeps mh.py:57's order (lp_new - lp_old) + f, which rounds
-  // differently once f != 0
-  const double lnpdiff = MOVE == EB_MOVE_USER_MH ? __dadd_rn(__dsub_rn(lp_new, a.logp[w]), factor)
-                                                 : __dsub_rn(__dadd_rn(factor, lp_new), a.logp[w]);
+  // red_blue.py:96-101; a user MHMove keeps mh.py's order of the difference
+  const double u_acc = accept_uniform(a.seed, a.step, (uint32_t)a.split, (uint32_t)i);
+  const double lnpdiff = MOVE == EB_MOVE_USER_MH ? lnpdiff_mh(factor, lp_new, a.logp[w])
+                                                 : lnpdiff_red_blue(factor, lp_new, a.logp[w]);
   const bool acc = lnpdiff > log(u_acc);
 
   // red_blue.py:103-104 -> move.py:29-34

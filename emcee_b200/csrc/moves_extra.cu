@@ -11,23 +11,13 @@
 // multivariate_normal(mean, cov) := mean + L z with L the thresholded lower Cholesky factor of cov.
 #include <math.h>
 
+#include "draws.cuh"
 #include "engine.cuh"
 #include "rowops.cuh"
 
 namespace eb {
 
 namespace {
-
-// the pair of standard normals (2k, 2k+1) of row `index`
-__device__ __forceinline__ void normal_pair(uint64_t seed, uint64_t step, uint32_t split, uint32_t k, uint32_t index,
-                                            double& n0, double& n1) {
-  const u32x4 w = draw_words(seed, step, (split & 0x3Fu) | (k << 6), TAG_NORMAL, index);
-  const double r = sqrt(-2.0 * log(1.0 - u53(w.x, w.y)));
-  double sn, cs;
-  sincos(6.283185307179586 * u53(w.z, w.w), &sn, &cs);
-  n0 = r * cs;
-  n1 = r * sn;
-}
 
 // ===========================================================================
 // thresholded Cholesky of a covariance held as moment sums (oracle/philox.py chol_psd)
@@ -126,7 +116,7 @@ __global__ void __launch_bounds__(128) walk_subset_propose_kernel(const HalfStep
   FeistelKeys fk;
 #pragma unroll
   for (int b = 0; b < FEISTEL_ROUNDS / 4; ++b) {
-    const u32x4 kw = draw_words(a.seed, a.step, ((uint32_t)a.split & 0x3Fu) | ((uint32_t)b << 6), TAG_SUBSET, (uint32_t)i);
+    const u32x4 kw = draw_words(a.seed, a.step, sub_split((uint32_t)a.split, (uint32_t)b), TAG_SUBSET, (uint32_t)i);
     fk.k[4 * b + 0] = kw.x;
     fk.k[4 * b + 1] = kw.y;
     fk.k[4 * b + 2] = kw.z;
@@ -135,7 +125,7 @@ __global__ void __launch_bounds__(128) walk_subset_propose_kernel(const HalfStep
   const int h = feistel_half_bits((uint64_t)Nc);
   for (int j = tid; j < s0; j += nt) {
     const int64_t r = (int64_t)split_permute((uint64_t)j, (uint64_t)Nc, h, fk);
-    ids[j] = a.order[r < a.a_start ? r : r + a.a_count];
+    ids[j] = a.order[complement_slot(r, a.a_start, a.a_count)];
   }
   for (int k = tid; 2 * k < D; k += nt) {
     double n0, n1;
@@ -234,8 +224,7 @@ __global__ void gaussian_propose_kernel(const double* __restrict__ x0, int64_t r
   const int64_t w = row0 + r;
   int dim = -1;  // "vector": every dimension moves
   if (mode == 1) {
-    const u32x4 B = draw_words(seed, step, 0, TAG_PROP_B, (uint32_t)w);
-    dim = (int)bounded64(B.x, B.y, (uint64_t)D);  // gaussian.py:100
+    dim = gaussian_random_dim(prop_b(seed, step, 0, (uint32_t)w), D);
   } else if (mode == 2) {
     dim = seq_dim;  // gaussian.py:102
   }

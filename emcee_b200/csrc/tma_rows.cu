@@ -22,6 +22,7 @@
 // walkers' rows across the banks so a warp-wide access costs the minimum number of wavefronts.
 #include <math.h>
 
+#include "draws.cuh"
 #include "engine.cuh"
 #include "rowops.cuh"
 #include "tma.cuh"
@@ -97,43 +98,28 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
     int64_t i = (int64_t)i_lo + tile * R + (lane % R);
     const bool valid = tile < ntiles && i < i_hi;
     if (!valid) i = (int64_t)i_hi - 1;
-    const u32x4 A = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_A, (uint32_t)i);
+    const u32x4 A = prop_a(a.seed, a.step, (uint32_t)a.split, (uint32_t)i);
     m.pw[0] = m.pw[1] = m.pw[2] = 0;
     m.scalar = 0.0;
     m.factor = 0.0;
     if (MOVE == EB_MOVE_STRETCH) {
-      const double t = __dadd_rn(__dmul_rn(__dsub_rn(a.p0, 1.0), u53(A.x, A.y)), 1.0);  // stretch.py:30
-      m.scalar = __ddiv_rn(__dmul_rn(t, t), a.p0);
-      m.factor = __dmul_rn((double)D - 1.0, log(m.scalar));  // stretch.py:31
-      const int64_t r = (int64_t)bounded64(A.z, A.w, (uint64_t)Nc);  // stretch.py:32
-      m.pw[0] = __ldg(a.order + (r < a.a_start ? r : r + a.a_count));
+      m.scalar = stretch_zz(A, a.p0);
+      m.factor = stretch_factor((double)D - 1.0, m.scalar);
+      m.pw[0] = __ldg(a.order + complement_slot(stretch_rank(A, Nc), a.a_start, a.a_count));
     } else if (MOVE == EB_MOVE_DE) {
-      const uint64_t mm = bounded64(A.x, A.y, (uint64_t)Nc * (uint64_t)(Nc - 1));  // de.py:49
-      uint64_t r0, r1;
-      de_pair_decode(mm, (uint64_t)Nc, r0, r1);  // de.py:67-77
-      m.pw[0] = __ldg(a.order + ((int64_t)r0 < a.a_start ? (int64_t)r0 : (int64_t)r0 + a.a_count));
-      m.pw[1] = __ldg(a.order + ((int64_t)r1 < a.a_start ? (int64_t)r1 : (int64_t)r1 + a.a_count));
-      const u32x4 B = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_B, (uint32_t)i);
-      const double n = sqrt(-2.0 * log(1.0 - u53(B.x, B.y))) * cos(6.283185307179586 * u53(B.z, B.w));
-      m.scalar = __dmul_rn(a.p0, __dadd_rn(1.0, __dmul_rn(a.p1, n)));  // de.py:56
+      int64_t r0, r1;
+      de_pair(A, Nc, r0, r1);
+      m.pw[0] = __ldg(a.order + complement_slot(r0, a.a_start, a.a_count));
+      m.pw[1] = __ldg(a.order + complement_slot(r1, a.a_start, a.a_count));
+      m.scalar = de_gamma(prop_b(a.seed, a.step, (uint32_t)a.split, (uint32_t)i), a.p0, a.p1);
     } else {
-      const u32x4 B = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_PROP_B, (uint32_t)i);
-      int32_t cw[3];
-      cw[0] = __ldg(a.order + a.c_start[0] + (int64_t)bounded64(A.x, A.y, (uint64_t)a.c_count[0]));  // de_snooker.py:38
-      cw[1] = __ldg(a.order + a.c_start[1] + (int64_t)bounded64(A.z, A.w, (uint64_t)a.c_count[1]));
-      cw[2] = __ldg(a.order + a.c_start[2] + (int64_t)bounded64(B.x, B.y, (uint64_t)a.c_count[2]));
-      const int p = (int)bounded64(B.z, B.w, 6);  // de_snooker.py:39: one of the 6 row orders
-      const int i0 = p >> 1;
-      const int rest0 = (i0 == 0) ? 1 : 0, rest1 = (i0 == 2) ? 1 : 2;
-      const int i1 = (p & 1) ? rest1 : rest0, i2 = (p & 1) ? rest0 : rest1;
-      m.pw[0] = i0 == 0 ? cw[0] : (i0 == 1 ? cw[1] : cw[2]);
-      m.pw[1] = i1 == 0 ? cw[0] : (i1 == 1 ? cw[1] : cw[2]);
-      m.pw[2] = i2 == 0 ? cw[0] : (i2 == 1 ? cw[1] : cw[2]);
+      const u32x4 B = prop_b(a.seed, a.step, (uint32_t)a.split, (uint32_t)i);
+      snooker_partners(A, B, a.c_start, a.c_count, [&](int64_t slot) -> int32_t { return __ldg(a.order + slot); },
+                       m.pw);
     }
     const int32_t w = __ldg(a.order + a.a_start + i);
     m.w = valid ? w : -(w + 1);  // keep the id (its rows are still fetched), flag it as padding
-    const u32x4 U = draw_words(a.seed, a.step, (uint32_t)a.split, TAG_ACCEPT, (uint32_t)i);
-    m.log_u = log(u53(U.x, U.y));
+    m.log_u = log(accept_uniform(a.seed, a.step, (uint32_t)a.split, (uint32_t)i));
     m.lp_old = a.logp[w];
     return m;
   };
@@ -233,19 +219,15 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
           ld8(s, sv);
           ld8(buf + ((size_t)1 * R + grp) * RS, cv);
         }
-        const double zz = cur_scalar;
 #pragma unroll
-        for (int e = 0; e < 8; ++e)  // stretch.py:33  q = c - (c - s) * zz   (each op rounded once)
-          q[e] = __dsub_rn(cv[e], __dmul_rn(__dsub_rn(cv[e], sv[e]), zz));
+        for (int e = 0; e < 8; ++e) q[e] = stretch_q(sv[e], cv[e], cur_scalar);
       } else if (MOVE == EB_MOVE_DE) {
         double sv[8], c0[8], c1[8];
         ld8(s, sv);
         ld8(buf + ((size_t)1 * R + grp) * RS, c0);
         ld8(buf + ((size_t)2 * R + grp) * RS, c1);
-        const double gamma = cur_scalar;
 #pragma unroll
-        for (int e = 0; e < 8; ++e)  // de.py:53,62  q = s + gamma * (c[p1] - c[p0])
-          q[e] = __dadd_rn(sv[e], __dmul_rn(gamma, __dsub_rn(c1[e], c0[e])));
+        for (int e = 0; e < 8; ++e) q[e] = de_q(sv[e], c0[e], c1[e], cur_scalar);
       } else {
         double sv[8], zv[8], u[8];
         ld8(s, sv);
@@ -253,7 +235,7 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
         double n2 = 0.0;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          u[e] = __dsub_rn(sv[e], zv[e]);  // de_snooker.py:41
+          u[e] = snooker_delta(sv[e], zv[e]);
           n2 = fma(u[e], u[e], n2);
         }
         const double norm = sqrt(group_sum(n2, G, mask));  // de_snooker.py:42
@@ -264,7 +246,7 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
           ld8(buf + ((size_t)3 * R + grp) * RS, z2);
 #pragma unroll
           for (int e = 0; e < 8; ++e) {
-            u[e] = __ddiv_rn(u[e], norm);  // de_snooker.py:43
+            u[e] = snooker_u(u[e], norm);
             d1 = fma(u[e], z1[e], d1);
             d2 = fma(u[e], z2[e], d2);
           }
@@ -275,13 +257,11 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
         double m2 = 0.0;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          // de_snooker.py:44  q = s + u * gammas * (u.z1 - u.z2)
-          q[e] = __dadd_rn(sv[e], __dmul_rn(__dmul_rn(u[e], a.p0), dd));
+          q[e] = snooker_q(sv[e], u[e], a.p0, dd);
           const double dq = __dsub_rn(q[e], zv[e]);
           m2 = fma(dq, dq, m2);
         }
-        const double qn = sqrt(group_sum(m2, G, mask));
-        factor = __dmul_rn((double)D - 1.0, __dsub_rn(log(qn), log(norm)));  // de_snooker.py:45-46
+        factor = snooker_factor((double)D - 1.0, sqrt(group_sum(m2, G, mask)), norm);
       }
       if (OWN_REG) {
 #pragma unroll
@@ -347,21 +327,16 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
     } else {
       if (MOVE == EB_MOVE_STRETCH) {
         const double* c = buf + ((size_t)1 * R + grp) * RS;
-        const double zz = cur_scalar;
         for (int e = g; e < D; e += G) {
-          const double sv = s[e], cv = c[e];
-          // stretch.py:33  q = c - (c - s) * zz   (each op rounded once, no FMA contraction)
-          const double v = __dsub_rn(cv, __dmul_rn(__dsub_rn(cv, sv), zz));
+          const double v = stretch_q(s[e], c[e], cur_scalar);
           s[e] = v;
           if (!isfinite(v)) flag_nonfinite(v, a.status);
         }
       } else if (MOVE == EB_MOVE_DE) {
         const double* c0 = buf + ((size_t)1 * R + grp) * RS;
         const double* c1 = buf + ((size_t)2 * R + grp) * RS;
-        const double gamma = cur_scalar;
         for (int e = g; e < D; e += G) {
-          // de.py:53,62  q = s + gamma * (c[p1] - c[p0])
-          const double v = __dadd_rn(s[e], __dmul_rn(gamma, __dsub_rn(c1[e], c0[e])));
+          const double v = de_q(s[e], c0[e], c1[e], cur_scalar);
           s[e] = v;
           if (!isfinite(v)) flag_nonfinite(v, a.status);
         }
@@ -371,13 +346,13 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
         const double* z2 = buf + ((size_t)3 * R + grp) * RS;
         double n2 = 0.0;
         for (int e = g; e < D; e += G) {
-          const double d = __dsub_rn(s[e], z[e]);  // de_snooker.py:41
+          const double d = snooker_delta(s[e], z[e]);
           n2 = fma(d, d, n2);
         }
         const double norm = sqrt(group_sum(n2, G, mask));  // de_snooker.py:42
         double d1 = 0.0, d2 = 0.0;
         for (int e = g; e < D; e += G) {
-          const double u = __ddiv_rn(__dsub_rn(s[e], z[e]), norm);  // de_snooker.py:43
+          const double u = snooker_u(snooker_delta(s[e], z[e]), norm);
           d1 = fma(u, z1[e], d1);
           d2 = fma(u, z2[e], d2);
           z1[e] = u;
@@ -387,15 +362,13 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
         const double dd = __dsub_rn(d1, d2);
         double m2 = 0.0;
         for (int e = g; e < D; e += G) {
-          // de_snooker.py:44  q = s + u * gammas * (u.z1 - u.z2)
-          const double v = __dadd_rn(s[e], __dmul_rn(__dmul_rn(z1[e], a.p0), dd));
+          const double v = snooker_q(s[e], z1[e], a.p0, dd);
           s[e] = v;
           if (!isfinite(v)) flag_nonfinite(v, a.status);
           const double dq = __dsub_rn(v, z[e]);
           m2 = fma(dq, dq, m2);
         }
-        const double qn = sqrt(group_sum(m2, G, mask));
-        factor = __dmul_rn((double)D - 1.0, __dsub_rn(log(qn), log(norm)));  // de_snooker.py:45-46
+        factor = snooker_factor((double)D - 1.0, sqrt(group_sum(m2, G, mask)), norm);
       }
       __syncwarp(mask);
 
@@ -405,7 +378,7 @@ __global__ void __launch_bounds__(TMA_MAX_THREADS, 1) half_step_tma_kernel(const
     }
     if (isnan(lp_new) && g == 0) atomicOr(a.status, FLAG_NAN_LOGPROB);
     // red_blue.py:96-101
-    const double lnpdiff = __dsub_rn(__dadd_rn(factor, lp_new), cur_lp_old);
+    const double lnpdiff = lnpdiff_red_blue(factor, lp_new, cur_lp_old);
     const bool acc = valid && (lnpdiff > cur_log_u);
     if constexpr (OWN_REG) {
       // red_blue.py:103-104 -> move.py:29-34: an accepted row is stored from the registers that hold the proposal
