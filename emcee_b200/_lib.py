@@ -40,6 +40,7 @@ EB_CALLBACK_HOST = 0
 EB_CHAIN_COORDS = 0
 EB_CHAIN_LOG_PROB = 1
 EB_CALLBACK_DEVICE = 1
+EB_CALLBACK_GRAPH = 2
 EB_MAX_PROPOSAL_SLOTS = 64  # user proposals one engine can hold (eb_move_set_proposal)
 EB_STREAM_UNKNOWN = 2**64 - 1  # eb_callback_result: the producer named no stream -> wait for the whole device
 
@@ -65,6 +66,17 @@ class EbMove(C.Structure):
     ]
 
 
+class EbGraph(C.Structure):
+    _fields_ = [
+        ("m", C.c_int64),
+        ("exec", C.c_uint64),
+        ("x", C.c_void_p),
+        ("x_row_stride_bytes", C.c_int64),
+        ("lp", C.c_void_p),
+        ("lp_stride_bytes", C.c_int64),
+    ]
+
+
 class EngineError(RuntimeError):
     """A failing C-ABI call that does not map onto one of the reference's own
     exception types."""
@@ -85,6 +97,7 @@ _SIGNATURES = {
     "eb_model_set": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_size_t]),
     "eb_model_set_bounds": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_model_set_callback": (C.c_int, [C.c_void_p, LOGPROB_FN, C.c_void_p, C.c_int]),
+    "eb_model_set_graphs": (C.c_int, [C.c_void_p, C.POINTER(EbGraph), C.c_size_t]),
     "eb_callback_result": (C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_callback_blobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_move_set_proposal": (C.c_int, [C.c_void_p, C.c_int32, PROPOSAL_FN, C.c_void_p, C.c_int]),
@@ -964,6 +977,20 @@ class Engine(object):
         self._check(lib().eb_model_set_callback(self._h, cb, None, mode))
         self._cb = cb
         self._blob_sink = sink
+        self._blob_layout = None
+
+    def set_graphs(self, specs, keep):
+        """Make captured graphs the model (``eb_model_set_graphs``): ``specs`` holds one
+        ``(m, exec, x_ptr, x_row_stride, lp_ptr, lp_stride)`` per row count; ``keep`` (the graphs' owners) stays
+        referenced while they are the model."""
+        arr = (EbGraph * len(specs))()
+        for k, (m, ex, xp, xs, lpp, lps) in enumerate(specs):
+            arr[k].m, arr[k].exec = int(m), int(ex)
+            arr[k].x, arr[k].x_row_stride_bytes = int(xp), int(xs)
+            arr[k].lp, arr[k].lp_stride_bytes = int(lpp), int(lps)
+        self._check(lib().eb_model_set_graphs(self._h, arr, len(specs)))
+        self._cb = list(keep)
+        self._blob_sink = None
         self._blob_layout = None
 
     def _expect_blobs(self):

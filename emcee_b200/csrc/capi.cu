@@ -22,7 +22,23 @@ static const char* const MSG_BLOBS_WITH_LOG_PROB =  // moves/move.py:38-42
 // map (and clear) the device status word to the reference's exceptions, in the
 // order compute_log_prob raises them (ensemble.py:476-479, 550-551)
 int check_status(eb_ctx* c) {
-  const int f = *c->status_host;
+  int f = *c->status_host;
+  // a graph model: the first error its half-steps recorded, which later ones may have added flags to
+  const unsigned long long g = graph_mode(c) ? *c->graph_err_host : 0ull;
+  if (g != 0) {
+    *c->graph_err_host = 0;
+    cudaMemsetAsync(c->graph_err.get(), 0, sizeof(unsigned long long), c->st.get());
+    f = (int)(g & 0xff);
+    const uint64_t es = g >> 16;
+    // inside a stepping call: back to the step that failed, as if the call had stopped there
+    if (((g >> 8) & 0xff) != GRAPH_NO_SPLIT && c->graph_run && es >= c->graph_step0 && es <= c->step) {
+      for (uint64_t s = es; s < c->step; ++s) c->picks[c->graph_picks[(size_t)(s - c->graph_step0)]] -= 1;
+      c->step = es;
+    }
+  } else if (f == 0 && c->graph_run) {
+    c->graph_step0 = c->step;  // every step enqueued so far completed without an error
+    c->graph_picks.clear();
+  }
   if (f == 0) return EB_OK;
   *c->status_host = 0;
   cudaMemsetAsync(c->status_dev.get(), 0, sizeof(int), c->st.get());
@@ -41,8 +57,17 @@ int check_status(eb_ctx* c) {
   FAIL(c, EB_ERR_NAN_LOGPROB, "Probability function returned NaN");
 }
 
-int fetch_status(eb_ctx* c) {
+int enqueue_status_read(eb_ctx* c) {
   CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
+  if (graph_mode(c))
+    CK(c, cudaMemcpyAsync(c->graph_err_host.get(), c->graph_err.get(), sizeof(unsigned long long),
+                          cudaMemcpyDeviceToHost, c->st.get()));
+  return EB_OK;
+}
+
+int fetch_status(eb_ctx* c) {
+  const int rc = enqueue_status_read(c);
+  if (rc) return rc;
   CK(c, cudaStreamSynchronize(c->st.get()));
   return check_status(c);
 }
@@ -228,6 +253,7 @@ int eb_model_set(eb_ctx* c, int kind, const double* params, size_t nparams) {
   c->have_model = true;
   c->cb_fn = nullptr;
   c->cb_user = nullptr;
+  c->graphs.clear();
   c->blob_bytes = 0;
   c->blobs_live = false;
   return EB_OK;
@@ -253,6 +279,7 @@ int eb_model_set_callback(eb_ctx* c, eb_logprob_fn fn, void* user, int where) {
   c->cb_fn = fn;
   c->cb_user = user;
   c->cb_where = where;
+  c->graphs.clear();
   c->have_model = true;
   c->blob_bytes = 0;
   c->blobs_live = false;
@@ -420,6 +447,69 @@ int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_by
   return copy_records(c, lp, src, sizeof(double), (size_t)stride_bytes, (size_t)m, src_stream);
 }
 
+int eb_model_set_graphs(eb_ctx* c, const eb_graph* graphs, size_t n) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "log-probability graphs are not sharded across GPUs");
+  if (!graphs || n == 0) FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: no graphs");
+  const int64_t row = (int64_t)c->D * (int64_t)sizeof(double);
+  std::vector<eb_ctx::Graph> set;
+  bool have_n = false;
+  CK(c, cudaSetDevice(c->device));
+  for (size_t k = 0; k < n; ++k) {
+    const eb_graph& g = graphs[k];
+    if (g.m < 1 || g.m > c->N)
+      FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: graph %zu has %lld rows; a graph takes 1 to %lld rows", k,
+           (long long)g.m, (long long)c->N);
+    for (const eb_ctx::Graph& h : set)
+      if (h.m == g.m) FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: two graphs for %lld rows", (long long)g.m);
+    if (g.exec == 0) FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: graph %zu has no executable graph", k);
+    if (!g.x || !g.lp) FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: graph %zu has a null buffer", k);
+    if (g.x_row_stride_bytes <= 0 || g.x_row_stride_bytes % 8 != 0 || (g.m > 1 && g.x_row_stride_bytes < row))
+      FAIL(c, EB_ERR_INVALID,
+           "eb_model_set_graphs: the row stride of x must be a multiple of 8 bytes, at least %lld (got %lld)",
+           (long long)row, (long long)g.x_row_stride_bytes);
+    if (g.lp_stride_bytes <= 0 || g.lp_stride_bytes % 8 != 0)
+      FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: the stride of lp must be a positive multiple of 8 bytes (got %lld)",
+           (long long)g.lp_stride_bytes);
+    int rc = check_device_ptr(c, c->device, g.x, "eb_model_set_graphs", "x");
+    if (!rc) rc = check_device_ptr(c, c->device, g.lp, "eb_model_set_graphs", "lp");
+    if (rc) return rc;
+    set.push_back(eb_ctx::Graph{g.m, reinterpret_cast<cudaGraphExec_t>((uintptr_t)g.exec), static_cast<double*>(g.x),
+                                g.x_row_stride_bytes, static_cast<const double*>(g.lp), g.lp_stride_bytes});
+    have_n |= g.m == c->N;
+  }
+  if (!have_n)
+    FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: no graph for nwalkers = %lld rows", (long long)c->N);
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  if (!c->ext_f) CK(c, dev_alloc(c->ext_f, (size_t)c->N * sizeof(double)));
+  if (!c->ext_lp) CK(c, dev_alloc(c->ext_lp, (size_t)c->N * sizeof(double)));
+  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, (size_t)c->N * c->D * sizeof(double)));
+  if (!c->graph_err) {
+    DevPtr<unsigned long long> err;
+    HostPtr<unsigned long long> err_host;
+    CK(c, dev_alloc(err, sizeof(unsigned long long)));
+    CK(c, host_alloc(err_host, sizeof(unsigned long long)));
+    CK(c, cudaMemset(err.get(), 0, sizeof(unsigned long long)));
+    *err_host = 0;
+    c->graph_err = std::move(err);
+    c->graph_err_host = std::move(err_host);
+  }
+  c->model_params.reset();
+  c->model_chol.reset();
+  c->model_box.reset();
+  c->model = ModelDev{};
+  c->model.kind = MODEL_EXTERNAL;
+  c->cb_fn = nullptr;
+  c->cb_user = nullptr;
+  c->cb_where = EB_CALLBACK_GRAPH;
+  c->graphs = std::move(set);
+  c->have_model = true;
+  c->blob_bytes = 0;
+  c->blobs_live = false;
+  return EB_OK;
+}
+
 int eb_move_set_proposal(eb_ctx* c, int32_t slot, eb_proposal_fn fn, void* user, int where) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -514,7 +604,44 @@ static int ensure_callback_staging(eb_ctx* c, size_t rows) {
 // steps 2-7 of a callback half-step (include/emcee_b200.h): the device rows x[m, D] have been enqueued;
 // lp[m] (device) gets the callback's values.  scan_x: the rows were not written by a kernel that raises the
 // non-finite flags (WalkMove / GaussianMove proposals, the caller's coordinates)
+static const eb_ctx::Graph* find_graph(const eb_ctx* c, int64_t m) {
+  for (const eb_ctx::Graph& g : c->graphs)
+    if (g.m == m) return &g;
+  return nullptr;
+}
+
+// rows x[rows, D] -> lp[rows] through graph g (g.m >= rows; the rows past `rows` repeat the last one), all enqueued
+static int launch_graph_eval(eb_ctx* c, const eb_ctx::Graph& g, const double* x, int64_t rows, double* lp,
+                             unsigned long long tag) {
+  CK(c, launch_graph_stage(x, rows, g.m, c->D, g.x, g.x_stride, c->status_dev.get(), c->graph_err.get(), tag,
+                           c->st.get()));
+  CK(c, cudaGraphLaunch(g.exec, c->st.get()));
+  CK(c, launch_graph_result(g.lp, g.lp_stride, rows, lp, c->status_dev.get(), c->graph_err.get(), tag, c->st.get()));
+  return EB_OK;
+}
+
+// run_callback of a graph model (eb_model_set_graphs).  A half-step uses the graph for its m rows and leaves its
+// errors on the device; the initial state and compute_log_prob run the nwalkers-row graph in chunks and report
+// their errors before returning, as run_callback does.
+static int run_graph(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x) {
+  const size_t D = (size_t)c->D;
+  if (scan_x) CK(c, launch_scan_nonfinite(x, (size_t)m * D, 0, c->status_dev.get(), c->st.get()));
+  if (c->cb_phase == CB_STEP) {
+    const eb_ctx::Graph* g = find_graph(c, m);
+    if (!g) FAIL(c, EB_ERR_INVALID, "no captured log-probability graph for %lld rows", (long long)m);
+    return launch_graph_eval(c, *g, x, m, lp, graph_err_word(0, (unsigned)c->cb_split, c->step));
+  }
+  const eb_ctx::Graph* g = find_graph(c, c->N);  // eb_model_set_graphs requires it
+  const unsigned long long tag = graph_err_word(0, GRAPH_NO_SPLIT, c->step);
+  for (int64_t off = 0; off < m; off += c->N) {
+    const int rc = launch_graph_eval(c, *g, x + (size_t)off * D, std::min<int64_t>(c->N, m - off), lp + off, tag);
+    if (rc) return rc;
+  }
+  return fetch_status(c);
+}
+
 int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x) {
+  if (c->cb_where == EB_CALLBACK_GRAPH) return run_graph(c, x, m, lp, scan_x);
   const size_t D = (size_t)c->D;
   if (scan_x) CK(c, launch_scan_nonfinite(x, (size_t)m * D, 0, c->status_dev.get(), c->st.get()));
   int rc = fetch_status(c);  // synchronises; ensemble.py:476-479: the function never sees a non-finite row

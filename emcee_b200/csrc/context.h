@@ -169,6 +169,25 @@ struct eb_ctx {
   DevPtr<double> ext_lp;           // device [N] the callback's log-probabilities
   int cb_phase = 0;                // CB_STEP / CB_SET_STATE / CB_COMPUTE: what the running callback evaluates
   int64_t cb_m = 0;                // rows of the running callback
+  int cb_split = 0;                // CB_STEP: the split of the running half-step
+
+  // captured log-probability graphs (eb_model_set_graphs; cb_where == EB_CALLBACK_GRAPH), one per row count
+  struct Graph {
+    int64_t m;
+    cudaGraphExec_t exec;
+    double* x;
+    int64_t x_stride;  // bytes
+    const double* lp;
+    int64_t lp_stride;  // bytes
+  };
+  std::vector<Graph> graphs;
+  DevPtr<unsigned long long> graph_err;       // the first error since the last check, graph_err_word (engine.cuh)
+  HostPtr<unsigned long long> graph_err_host;  // read back beside the status word
+  // run_steps in graph mode: the steps [graph_step0, step) enqueued since the last clean check, and the schedule
+  // entry of each, so that an error found later can put the step counter and the picks back to its step
+  bool graph_run = false;
+  uint64_t graph_step0 = 0;
+  std::vector<size_t> graph_picks;
 
   // blobs of a callback model (eb_callback_blobs): packed records of blob_bytes bytes, one per walker
   size_t blob_bytes = 0;           // the live layout (0: none)
@@ -245,8 +264,11 @@ enum { CB_STEP = 0, CB_SET_STATE = 1, CB_COMPUTE = 2 };
     }                                       \
   } while (0)
 
+// a graph model (eb_model_set_graphs): its half-steps report errors through graph_err, read by fetch_status
+inline bool graph_mode(const eb_ctx* c) { return c->model.kind == MODEL_EXTERNAL && c->cb_where == EB_CALLBACK_GRAPH; }
 int check_status(eb_ctx* c);  // map (and clear) the status word read back last
 int fetch_status(eb_ctx* c);  // read the status word back, then check_status
+int enqueue_status_read(eb_ctx* c);  // the read-back of fetch_status, without its synchronisation
 int run_callback(eb_ctx* c, const double* x, int64_t m, double* lp, bool scan_x);
 void owned_rows(const eb_ctx* c, int64_t& r0, int64_t& r1);
 int sync_replicas(eb_ctx* c);

@@ -137,6 +137,21 @@ cudaError_t launch_split_gather(const double* coords, const int32_t* order, int6
 cudaError_t launch_scan_nonfinite(const double* x, size_t n, int logprob, int* status, cudaStream_t st);
 // cuda_arrays.cu: status |= flag if any of x[n] is NaN
 cudaError_t launch_flag_nan(const double* x, size_t n, int flag, int* status, cudaStream_t st);
+// graph_fn.cu, around a captured log-probability graph (eb_model_set_graphs).  The first error of a call is recorded
+// once in *err as graph_err_word(flags, split, step); `tag` is graph_err_word(0, split, step) of the running half-step.
+constexpr int GRAPH_RESULT_THREADS = 512;
+constexpr unsigned GRAPH_NO_SPLIT = 0xff;  // the split field of an evaluation outside a step (initial state, compute)
+inline unsigned long long graph_err_word(int flags, unsigned split, uint64_t step) {
+  return (unsigned long long)(flags & 0xff) | ((unsigned long long)(split & 0xff) << 8) | ((unsigned long long)step << 16);
+}
+// x[r, :] (row stride x_stride_bytes) = src[min(r, rows - 1), :] for r < m, unless *status holds an error: then
+// nothing is copied and the error is recorded
+cudaError_t launch_graph_stage(const double* src, int64_t rows, int64_t m, int D, double* x, int64_t x_stride_bytes,
+                               const int* status, unsigned long long* err, unsigned long long tag, cudaStream_t st);
+// out[i] = lp[i] (stride lp_stride_bytes) for i < rows; a NaN raises and records FLAG_NAN_LOGPROB; after a NaN, or
+// when *status held an error already, every out[i] is NaN
+cudaError_t launch_graph_result(const double* lp, int64_t lp_stride_bytes, int64_t rows, double* out, int* status,
+                                unsigned long long* err, unsigned long long tag, cudaStream_t st);
 // the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)
 struct TmaVariant {
   int R;        // walkers per tile (G = 32 / R lanes per walker)

@@ -257,7 +257,7 @@ __attribute__((format(printf, 3, 4))) void note_kernel(eb_ctx* c, const char* na
 
 void note_callback(eb_ctx* c) {
   note_kernel(c, "callback", "callback G=%d where=%s", lanes_per_walker(c->D),
-              c->cb_where == EB_CALLBACK_HOST ? "host" : "device");
+              c->cb_where == EB_CALLBACK_HOST ? "host" : c->cb_where == EB_CALLBACK_GRAPH ? "graph" : "device");
 }
 
 bool dmma_eligible(const eb_ctx* c, const eb_move& mv) {
@@ -279,6 +279,7 @@ int check_walker_count(eb_ctx* c, const eb_move& mv) {
 int external_accept(eb_ctx* c, int kind, const HalfStepArgs& a, double* f, uint64_t& launches) {
   const ExternalBufs ext{c->qbuf.get(), f, c->ext_lp.get()};
   c->cb_phase = CB_STEP;
+  c->cb_split = a.split;
   const int rc = run_callback(c, c->qbuf.get(), (int64_t)a.i_hi - a.i_lo, c->ext_lp.get(), f != c->ext_f.get());
   if (rc) return rc;
   if (kind == EB_MOVE_USER_MH)
@@ -547,8 +548,14 @@ int user_proposal_call(eb_ctx* c, const eb_ctx::ProposalSlot& p, uint64_t step, 
     CK(c, cudaMemcpyAsync(c->up_hx.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
   else if (rows != c->up_x.get())
     CK(c, cudaMemcpyAsync(c->up_x.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st.get()));
-  // complete before fn runs (a device consumer may ignore the stream it is given)
-  CK(c, cudaStreamSynchronize(c->st.get()));
+  // complete before fn runs (a device consumer may ignore the stream it is given); a graph model's errors so far
+  // stop the call here, so that the function never sees the state past one
+  if (graph_mode(c)) {
+    const int rc = fetch_status(c);
+    if (rc) return rc;
+  } else {
+    CK(c, cudaStreamSynchronize(c->st.get()));
+  }
   const double* s = host ? c->up_hx.get() : c->up_x.get();
   const double* cset = nsets > 0 ? s + (size_t)ns * D : nullptr;
   double* q = ns > 0 ? (host ? c->up_hq.get() : c->qbuf.get()) : nullptr;
@@ -782,9 +789,21 @@ int reserve_trace(eb_ctx* c, uint64_t nsteps);                    // below
 unsigned stats_due(const eb_ctx* c, uint64_t n);                  // below
 int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches);  // below
 
+// graph mode (eb_model_set_graphs): run_steps logs the steps it enqueues for check_status while it runs
+struct GraphRun {
+  eb_ctx* c;
+  explicit GraphRun(eb_ctx* ctx) : c(ctx) {
+    c->graph_run = graph_mode(c);
+    c->graph_step0 = c->step;
+    c->graph_picks.clear();
+  }
+  ~GraphRun() { c->graph_run = false; }
+};
+
 template <class F>
 int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every, F&& after_step) {
   uint64_t launches = 0;
+  const GraphRun graph_run(c);
   const bool perstep = c->l2_flush;  // flush L2 before every step, time each step on its own
   if (perstep) {
     if (nsteps > 16384) FAIL(c, EB_ERR_INVALID, "l2_flush mode times each step separately; use nsteps <= 16384");
@@ -814,7 +833,9 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
   uint64_t done = 0;
   while (done < nsteps) {
     const size_t chunk = (size_t)std::min<uint64_t>(nsteps - done, c->table_cap);
-    int rc = prepare_chunk(c, s, chunk, ch);
+    int rc = EB_OK;
+    if (c->graph_run && done > 0) rc = fetch_status(c);  // prepare_chunk waits for the stream anyway
+    if (!rc) rc = prepare_chunk(c, s, chunk, ch);
     if (rc) return rc;
     DmmaGroup grp;
     size_t desc_cursor = 0;
@@ -892,6 +913,14 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
       }
       c->picks[ch.pick[k]] += 1;
       c->step += 1;
+      if (c->graph_run) {
+        c->graph_picks.push_back(ch.pick[k]);
+        // a graph model's error stops the call before a statistic or a stored step records a state past it
+        if (due || stored) {
+          rc = fetch_status(c);
+          if (rc) return rc;
+        }
+      }
       if (due) {
         rc = accumulate_due(c, due, launches);
         if (rc) return rc;
@@ -911,7 +940,8 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
   // multi-GPU: the rows of other ranks are NOT replicated here; collective readers (eb_get_state,
   // eb_get_naccepted, the accept mask of eb_step) do that on demand, sharded readers never need it
   if (multi) c->replicas_dirty = true;
-  CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
+  int rc = enqueue_status_read(c);
+  if (rc) return rc;
   CK(c, cudaStreamSynchronize(c->st.get()));
   float ms = 0.f;
   if (perstep) {

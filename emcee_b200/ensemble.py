@@ -20,7 +20,7 @@ import numpy as np
 from . import _lib
 from .backend import Backend, DeviceBackend
 from .model import Model
-from .models import CallbackFunction, DeviceModel
+from .models import CallbackFunction, CudaGraphFunction, DeviceModel, graph_row_counts
 from .moves import StretchMove
 from .moves.user import user_move_spec
 from .rng import DeviceRandom
@@ -205,6 +205,12 @@ class EnsembleSampler(object):
         # so a rebuilt engine (__setstate__) gets it back too; a user function is registered as the
         # engine's callback
         m = self.log_prob_fn
+        if isinstance(m, CudaGraphFunction):
+            # one capture per row count the schedule evaluates, all checked before the engine sees any
+            rows = graph_row_counts(self.nwalkers, [mv.descriptor() for mv in self._moves])
+            captured = [m.captured(r, self.ndim, self._device) for r in rows]
+            self._engine.set_graphs([spec for _, spec in captured], [g for g, _ in captured])
+            return
         if isinstance(m, CallbackFunction):
             self._engine.set_callback(m.evaluate, m.where, self.blobs_dtype)
             return

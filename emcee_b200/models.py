@@ -10,7 +10,8 @@ The reference takes an arbitrary Python callable ``log_prob_fn``
   whole half-step -- proposal, log-probability, accept -- is one kernel.
   These classes only carry parameters and are deliberately not callable.
 * a *user function*, wrapped explicitly in ``HostFunction`` (numpy on the
-  host) or ``CudaArrayFunction`` (any CUDA-array library).  The engine calls
+  host), ``CudaArrayFunction`` (any CUDA-array library) or
+  ``CudaGraphFunction`` (the function captured as CUDA graphs).  The engine calls
   it once per half-step with the whole ``[M, ndim]`` block of proposals of
   one split, never once per walker; split assignment, proposals, the accept
   decision and the update stay on the GPU.  The explicit wrapper keeps the
@@ -19,12 +20,13 @@ The reference takes an arbitrary Python callable ``log_prob_fn``
 
 import numpy as np
 
+from . import _lib
 from ._lib import FIXED_WIDTH as _FIXED_WIDTH
 from ._lib import fixed_width_dtype
 
 __all__ = [
     "DeviceModel", "GaussianIso", "GaussianDense", "Rosenbrock", "Ring", "Bounded",
-    "CallbackFunction", "HostFunction", "CudaArrayFunction",
+    "CallbackFunction", "HostFunction", "CudaArrayFunction", "CapturedGraph", "CudaGraphFunction",
 ]
 
 
@@ -306,3 +308,129 @@ class CudaArrayFunction(CallbackFunction):
 
     def evaluate(self, x):
         return self._call(x)
+
+
+class CapturedGraph(object):
+    """One captured evaluation of ``m`` rows, what ``CudaGraphFunction``'s ``capture(m)`` returns.
+
+    * ``exec``: the executable graph, a ``cudaGraphExec_t`` as an int (torch:
+      ``torch.cuda.CUDAGraph().raw_cuda_graph_exec()``), instantiated on the sampler's device;
+    * ``x``: its static input, a CUDA-array-interface object of shape ``(m, ndim)`` and dtype ``<f8`` whose rows
+      are contiguous (the first axis may be strided);
+    * ``lp``: its static output, shape ``(m,)``, ``<f8``, strided or not;
+    * ``owner``: anything that must stay alive while the graph is used (torch: the ``CUDAGraph``, which owns the
+      executable graph and its memory pool).
+
+    The sampler keeps the object, and so ``x``, ``lp`` and ``owner``, alive while the model is loaded."""
+
+    __slots__ = ("exec", "x", "lp", "owner")
+
+    def __init__(self, exec, x, lp, owner=None):
+        self.exec = exec
+        self.x = x
+        self.lp = lp
+        self.owner = owner
+
+    def __repr__(self):
+        return "CapturedGraph(exec=%r, x=%r, lp=%r)" % (self.exec, self.x, self.lp)
+
+
+class CudaGraphFunction(CallbackFunction):
+    """A log-probability function that the engine runs as CUDA graphs, without the host.
+
+    ``capture(m)`` returns a :class:`CapturedGraph` that evaluates ``m`` rows: launched, it reads the rows from
+    its static ``x`` and writes their log-probabilities to its static ``lp``.  The sampler calls ``capture`` once
+    per row count it needs when it loads the model -- in its constructor, and again after unpickling, since graphs
+    do not travel: ``nwalkers``, and the split sizes ``ceil((nwalkers - j) / nsplits)`` of every red-blue move of
+    the schedule.  From then on every log-probability the sampler evaluates comes from these graphs: each
+    half-step copies its proposals into ``x``, launches the graph and reads ``lp`` on the engine's stream, with no
+    Python call and no host synchronisation in between; the initial state and ``compute_log_prob`` run the
+    ``nwalkers``-row graph in chunks, the last padded with copies of its last row.  Non-finite proposals and NaN
+    log-probabilities raise the same exceptions as under :class:`CudaArrayFunction`, and leave the chain, the
+    state and the random state where it leaves them; a stepping call reports them where it synchronises anyway, so
+    a run with ``store=False`` and no running statistics synchronises once per chunk of up to 512 steps.
+
+    The contract:
+
+    * the graph must be deterministic and draw no random numbers: the engine launches it as captured, and torch's
+      ``replay()`` bookkeeping (the random generator's offsets) does not run;
+    * the graph may overwrite ``x``, so ``x`` must be writable; it never sees a non-finite row from the caller or a
+      move.  After an error the engine copies no more rows into ``x``, and the launches that follow read what ``x``
+      last held, possibly the graph's own writes, and their output is discarded;
+    * one executable graph must not be shared by two samplers that run at the same time, since both would write
+      the same ``x``;
+    * no blobs (``blobs_dtype`` raises ``NotImplementedError``), and one GPU only (``attach`` is refused).
+
+    The torch recipe (this package imports no torch)::
+
+        def capture(m):
+            x = torch.zeros(m, ndim, dtype=torch.float64, device="cuda")
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):  # warm up outside the capture
+                for _ in range(3):
+                    f(x)
+            torch.cuda.current_stream().wait_stream(side)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                lp = f(x)
+            return models.CapturedGraph(g.raw_cuda_graph_exec(), x, lp, owner=g)
+
+        sampler = EnsembleSampler(nwalkers, ndim, models.CudaGraphFunction(capture))
+
+    ``capture`` is pickled with the sampler, so for a picklable sampler it must be a module-level function."""
+
+    where = "graph"
+
+    def __init__(self, capture, blobs_dtype=None):
+        if blobs_dtype is not None:
+            raise NotImplementedError("CudaGraphFunction returns no blobs: a captured graph writes log-probabilities "
+                                      "only; use CudaArrayFunction(fn, blobs_dtype=...) for blobs")
+        super().__init__(capture)
+        self.capture = capture
+
+    def evaluate(self, x):
+        raise TypeError("a CudaGraphFunction is evaluated by launching its captured graphs "
+                        "(EnsembleSampler.compute_log_prob)")
+
+    def captured(self, m, ndim, device):
+        """``(graph, (m, exec, x_ptr, x_row_stride, lp_ptr, lp_stride))``: ``capture(m)`` and its checked
+        description.  A result of the wrong type, shape, dtype or strides, or with ``exec = 0``, raises here."""
+        g = self.capture(m)
+        what = "capture(%d) returned" % m
+        if not isinstance(g, CapturedGraph):
+            raise TypeError("%s %r; it must return a models.CapturedGraph" % (what, type(g).__name__))
+        ex = g.exec
+        if isinstance(ex, bool) or not isinstance(ex, (int, np.integer)) or not 0 < int(ex) < 2**64:
+            raise ValueError("%s a graph whose exec is %r; it must be a non-zero cudaGraphExec_t handle as an int "
+                             "(torch: CUDAGraph.raw_cuda_graph_exec())" % (what, ex))
+        bufs = []
+        for name, obj, shape in (("x", g.x, (m, ndim)), ("lp", g.lp, (m,))):
+            if not _lib.is_cuda_array(obj):
+                raise TypeError("%s a graph whose %s is not a CUDA array (it has no __cuda_array_interface__)"
+                                % (what, name))
+            cai = obj.__cuda_array_interface__
+            got = tuple(int(n) for n in cai["shape"])
+            if got != shape:
+                raise ValueError("%s a graph whose %s has shape %s; it must be %s" % (what, name, got, shape))
+            if name == "x" and cai["data"][1]:
+                raise ValueError("%s a graph whose x is exported read-only; the engine writes the rows into x, so "
+                                 "it must be writable" % what)
+            rows = _lib.CudaRows(obj, shape, device, "the graph's " + name)
+            if rows.ptr == 0:
+                raise ValueError("%s a graph whose %s has a null data pointer" % (what, name))
+            bufs.append(rows)
+        x, lp = bufs
+        return g, (m, int(ex), x.ptr, x.stride, lp.ptr, lp.stride)
+
+
+def graph_row_counts(nwalkers, descriptors):
+    """The row counts a ``CudaGraphFunction`` is captured for: ``nwalkers`` (the initial state, compute_log_prob,
+    and the moves that propose every walker at once) and each split size ``ceil((nwalkers - j) / nsplits)`` of the
+    moves' descriptors, in ascending order."""
+    n = int(nwalkers)
+    rows = {n}
+    for d in descriptors:
+        p = int(d["nsplits"])
+        rows.update((n - j + p - 1) // p for j in range(p))
+    return sorted(rows)

@@ -187,6 +187,35 @@ int eb_callback_result(eb_ctx* ctx, double* lp, const void* src, int64_t stride_
 int eb_callback_blobs(eb_ctx* ctx, const void* src, int64_t record_bytes, int64_t stride_bytes, int64_t m,
                       uint64_t src_stream);
 
+/* A user log-probability function captured as CUDA graphs, one per row count m: the graph reads m rows from its
+ * static input x[m, ndim] (float64, rows contiguous, x_row_stride_bytes apart) and writes m values to its static
+ * output lp[m] (lp_stride_bytes apart).  exec is a cudaGraphExec_t instantiated on the engine's device. */
+#define EB_CALLBACK_GRAPH 2
+typedef struct {
+  int64_t m;
+  uint64_t exec;
+  void* x;
+  int64_t x_row_stride_bytes;
+  void* lp;
+  int64_t lp_stride_bytes;
+} eb_graph;
+/* replaces the model, like eb_model_set_callback, by n captured graphs (callback mode EB_CALLBACK_GRAPH).  Every
+ * log-probability is then evaluated on the engine's stream without the host: a half-step of m rows enqueues the
+ * non-finite scan of the rows when the move's kernels do not raise it themselves, a copy of the rows into the x of
+ * the graph for m, cudaGraphLaunch, and a copy of its lp into the engine with the NaN scan.  The initial state and
+ * eb_compute_log_prob run the graph for nwalkers rows in chunks, the last chunk padded with copies of its last row.
+ * Errors (EB_ERR_INF_PARAM, EB_ERR_NAN_PARAM, EB_ERR_NAN_LOGPROB) are found on the device: from the first one on,
+ * nothing is copied into x and every proposal is rejected.  The host reads them where a stepping call synchronises
+ * anyway (the start of each chunk of steps, KDEMove's per-half-step check, user proposals), before each stored step
+ * and each step a running statistic records, and at the end of the call; it then reports the first error, with the
+ * step counter, the stored steps and the statistics where eb_model_set_callback leaves them.  Refused
+ * (EB_ERR_INVALID): no graph for m = nwalkers, m outside [1, nwalkers], a repeated m, exec = 0, null buffers, strides
+ * that are not positive multiples of 8 (x: at least a row), and buffers that are not device memory of the engine's
+ * device.  Sharded engines are refused with EB_ERR_UNSUPPORTED.  The engine does not own the graphs or the
+ * buffers: they must stay valid, and unused by anything else, while the model is set.  eb_model_set and
+ * eb_model_set_callback clear the set. */
+int eb_model_set_graphs(eb_ctx* ctx, const eb_graph* graphs, size_t n);
+
 /* ---- user proposals (moves/red_blue.py:47,82-93; moves/mh.py:31-33,52) ------------------------------------ */
 /* A user proposal, called once per half-step of a schedule entry of kind EB_MOVE_USER / EB_MOVE_USER_MH:
  *   EB_MOVE_USER (RedBlueMove.get_proposal(s, c, random), red_blue.py:85-90): split = the active set; s[ns, ndim]
@@ -575,7 +604,7 @@ const char* eb_last_kernel_name(const eb_ctx* ctx);
 /* the cell of that kernel the last half-step launch ran, with the parameters its launcher chose:
  * "tma_rows R=<walkers per tile> epl=<8 register path | 0 strided> own_reg=<0|1> warps=<per CTA>",
  * "dense_dmma nhalf_max=<most half-steps of one launch in the call> grid=<CTAs>", "generic G=<lanes per
- * walker>", "walk", "gaussian", "callback G=<lanes per walker> where=host|device" (eb_last_kernel_name
+ * walker>", "walk", "gaussian", "callback G=<lanes per walker> where=host|device|graph" (eb_last_kernel_name
  * "callback": any move with a callback model), "user_move where=host|device" (eb_last_kernel_name "user_move": a
  * user proposal, with any model) or "none". */
 const char* eb_last_kernel_variant(const eb_ctx* ctx);
