@@ -42,6 +42,8 @@ EB_CHAIN_LOG_PROB = 1
 EB_CALLBACK_DEVICE = 1
 EB_CALLBACK_GRAPH = 2
 EB_MAX_PROPOSAL_SLOTS = 64  # user proposals one engine can hold (eb_move_set_proposal)
+EB_DRAW_KINDS = {"uniform": 0, "normal": 1}  # eb_move_set_proposal_graphs: EB_DRAW_UNIFORM, EB_DRAW_NORMAL
+EB_MAX_GRAPH_DRAWS = 2**19  # draws per row of a captured proposal: the counter's 18-bit sub-index holds k < 2**18
 EB_STREAM_UNKNOWN = 2**64 - 1  # eb_callback_result: the producer named no stream -> wait for the whole device
 
 MODEL_KINDS = {"gauss_iso": 0, "gauss_dense": 1, "rosenbrock": 2, "ring": 3}
@@ -77,6 +79,24 @@ class EbGraph(C.Structure):
     ]
 
 
+class EbProposalGraph(C.Structure):
+    _fields_ = [
+        ("split", C.c_int32),
+        ("ns", C.c_int64),
+        ("exec", C.c_uint64),
+        ("s", C.c_void_p),
+        ("s_row_stride_bytes", C.c_int64),
+        ("c", C.c_void_p),
+        ("c_row_stride_bytes", C.c_int64),
+        ("draws", C.c_void_p),
+        ("draws_row_stride_bytes", C.c_int64),
+        ("q", C.c_void_p),
+        ("q_row_stride_bytes", C.c_int64),
+        ("factors", C.c_void_p),
+        ("factors_stride_bytes", C.c_int64),
+    ]
+
+
 class EngineError(RuntimeError):
     """A failing C-ABI call that does not map onto one of the reference's own
     exception types."""
@@ -101,6 +121,8 @@ _SIGNATURES = {
     "eb_callback_result": (C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_callback_blobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_move_set_proposal": (C.c_int, [C.c_void_p, C.c_int32, PROPOSAL_FN, C.c_void_p, C.c_int]),
+    "eb_move_set_proposal_graphs": (C.c_int, [C.c_void_p, C.c_int32, C.c_int, C.c_int64, C.POINTER(EbProposalGraph),
+                                              C.c_size_t]),
     "eb_proposal_result": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_uint64]),
     "eb_set_state": (C.c_int, [C.c_void_p, _dp, _dp]),
     "eb_get_state": (C.c_int, [C.c_void_p, _dp, _dp]),
@@ -1226,6 +1248,19 @@ class Engine(object):
         fn = make_proposal_trampoline(self._h, propose, setup, mode, self._cb_failure, self._seed_box)
         self._check(lib().eb_move_set_proposal(self._h, int(slot), fn, None, mode))
         self._props[int(slot)] = fn
+
+    def set_proposal_graphs(self, slot, draw, ndraws, specs, keep):
+        """Make captured graphs proposal slot ``slot`` (``eb_move_set_proposal_graphs``): ``specs`` holds one
+        ``(split, ns, exec, s, s_stride, c, c_stride, draws, draws_stride, q, q_stride, factors, factors_stride)`` per
+        split, pointers and byte strides; ``draw`` is ``"uniform"`` or ``"normal"``; ``keep`` (the captures' owners)
+        stays referenced while the slot is set."""
+        arr = (EbProposalGraph * len(specs))()
+        for k, spec in enumerate(specs):
+            for name, v in zip([f[0] for f in EbProposalGraph._fields_], spec):
+                setattr(arr[k], name, int(v))
+        self._check(lib().eb_move_set_proposal_graphs(self._h, int(slot), EB_DRAW_KINDS[draw], int(ndraws), arr,
+                                                      len(specs)))
+        self._props[int(slot)] = list(keep)
 
     def get_rng(self):
         seed, step = C.c_uint64(), C.c_uint64()

@@ -23,8 +23,10 @@ static const char* const MSG_BLOBS_WITH_LOG_PROB =  // moves/move.py:38-42
 // order compute_log_prob raises them (ensemble.py:476-479, 550-551)
 int check_status(eb_ctx* c) {
   int f = *c->status_host;
-  // a graph model: the first error its half-steps recorded, which later ones may have added flags to
-  const unsigned long long g = graph_mode(c) ? *c->graph_err_host : 0ull;
+  c->gm_unchecked = false;
+  // a graph model or a captured proposal: the first error its half-steps recorded, which later ones may have added
+  // flags to
+  const unsigned long long g = graph_errors(c) ? *c->graph_err_host : 0ull;
   if (g != 0) {
     *c->graph_err_host = 0;
     cudaMemsetAsync(c->graph_err.get(), 0, sizeof(unsigned long long), c->st.get());
@@ -59,7 +61,7 @@ int check_status(eb_ctx* c) {
 
 int enqueue_status_read(eb_ctx* c) {
   CK(c, cudaMemcpyAsync(c->status_host.get(), c->status_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->st.get()));
-  if (graph_mode(c))
+  if (graph_errors(c))
     CK(c, cudaMemcpyAsync(c->graph_err_host.get(), c->graph_err.get(), sizeof(unsigned long long),
                           cudaMemcpyDeviceToHost, c->st.get()));
   return EB_OK;
@@ -447,6 +449,20 @@ int eb_callback_result(eb_ctx* c, double* lp, const void* src, int64_t stride_by
   return copy_records(c, lp, src, sizeof(double), (size_t)stride_bytes, (size_t)m, src_stream);
 }
 
+// the device word of the first error of a graph model's or a captured proposal's half-steps (graph_err_word)
+static int ensure_graph_err(eb_ctx* c) {
+  if (c->graph_err) return EB_OK;
+  DevPtr<unsigned long long> err;
+  HostPtr<unsigned long long> err_host;
+  CK(c, dev_alloc(err, sizeof(unsigned long long)));
+  CK(c, host_alloc(err_host, sizeof(unsigned long long)));
+  CK(c, cudaMemset(err.get(), 0, sizeof(unsigned long long)));
+  *err_host = 0;
+  c->graph_err = std::move(err);
+  c->graph_err_host = std::move(err_host);
+  return EB_OK;
+}
+
 int eb_model_set_graphs(eb_ctx* c, const eb_graph* graphs, size_t n) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -485,16 +501,8 @@ int eb_model_set_graphs(eb_ctx* c, const eb_graph* graphs, size_t n) {
   if (!c->ext_f) CK(c, dev_alloc(c->ext_f, (size_t)c->N * sizeof(double)));
   if (!c->ext_lp) CK(c, dev_alloc(c->ext_lp, (size_t)c->N * sizeof(double)));
   if (!c->qbuf) CK(c, dev_alloc(c->qbuf, (size_t)c->N * c->D * sizeof(double)));
-  if (!c->graph_err) {
-    DevPtr<unsigned long long> err;
-    HostPtr<unsigned long long> err_host;
-    CK(c, dev_alloc(err, sizeof(unsigned long long)));
-    CK(c, host_alloc(err_host, sizeof(unsigned long long)));
-    CK(c, cudaMemset(err.get(), 0, sizeof(unsigned long long)));
-    *err_host = 0;
-    c->graph_err = std::move(err);
-    c->graph_err_host = std::move(err_host);
-  }
+  const int rc = ensure_graph_err(c);
+  if (rc) return rc;
   c->model_params.reset();
   c->model_chol.reset();
   c->model_box.reset();
@@ -522,6 +530,91 @@ int eb_move_set_proposal(eb_ctx* c, int32_t slot, eb_proposal_fn fn, void* user,
   c->props[(size_t)slot].fn = fn;
   c->props[(size_t)slot].user = fn ? user : nullptr;
   c->props[(size_t)slot].where = where;
+  if ((size_t)slot < c->prop_graphs.size()) c->prop_graphs[(size_t)slot] = eb_ctx::ProposalGraphs{};
+  return EB_OK;
+}
+
+// a buffer of rows `rows` long of `width` doubles each, row_stride bytes apart
+static int check_graph_rows(eb_ctx* c, size_t k, const char* what, const void* p, int64_t row_stride, int64_t rows,
+                            int64_t width) {
+  if (!p) FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: graph %zu has a null %s", k, what);
+  const int64_t row = width * (int64_t)sizeof(double);
+  if (row_stride <= 0 || row_stride % 8 != 0 || (rows > 1 && row_stride < row))
+    FAIL(c, EB_ERR_INVALID,
+         "eb_move_set_proposal_graphs: the row stride of %s must be a positive multiple of 8 bytes, at least %lld "
+         "(got %lld)",
+         what, (long long)row, (long long)row_stride);
+  return check_device_ptr(c, c->device, p, "eb_move_set_proposal_graphs", what);
+}
+
+int eb_move_set_proposal_graphs(eb_ctx* c, int32_t slot, int draw_kind, int64_t ndraws, const eb_proposal_graph* graphs,
+                                size_t n) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (slot < 0 || slot >= EB_MAX_PROPOSAL_SLOTS)
+    FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: slot must be in [0, %d) (got %d)", EB_MAX_PROPOSAL_SLOTS,
+         slot);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "user proposals are not sharded across GPUs");
+  if (draw_kind != EB_DRAW_UNIFORM && draw_kind != EB_DRAW_NORMAL)
+    FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: draw_kind must be EB_DRAW_UNIFORM or EB_DRAW_NORMAL (got %d)",
+         draw_kind);
+  if (ndraws < 0) FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: ndraws must be >= 0 (got %lld)", (long long)ndraws);
+  if (ndraws > EB_MAX_GRAPH_DRAWS)
+    FAIL(c, EB_ERR_UNSUPPORTED, "a captured proposal takes at most %d draws per row (got %lld)", EB_MAX_GRAPH_DRAWS,
+         (long long)ndraws);
+  if (!graphs || n == 0) FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: no graphs");
+  std::vector<eb_ctx::ProposalGraph> set;
+  CK(c, cudaSetDevice(c->device));
+  for (size_t k = 0; k < n; ++k) {
+    const eb_proposal_graph& g = graphs[k];
+    if (g.split < 0 || g.split >= MAX_SPLITS)
+      FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: graph %zu has split %d; a split is in [0, %d)", k,
+           (int)g.split, MAX_SPLITS);
+    for (const eb_ctx::ProposalGraph& h : set)
+      if (h.split == g.split)
+        FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: two graphs for split %d", (int)g.split);
+    if (g.ns < 1 || g.ns > c->N)
+      FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: graph %zu has %lld rows; a graph takes 1 to %lld rows", k,
+           (long long)g.ns, (long long)c->N);
+    if (g.exec == 0) FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: graph %zu has no executable graph", k);
+    const int64_t nc = c->N - g.ns;
+    int rc = check_graph_rows(c, k, "s", g.s, g.s_row_stride_bytes, g.ns, c->D);
+    if (!rc && nc > 0) rc = check_graph_rows(c, k, "c", g.c, g.c_row_stride_bytes, nc, c->D);
+    if (!rc && ndraws > 0) rc = check_graph_rows(c, k, "draws", g.draws, g.draws_row_stride_bytes, g.ns, ndraws);
+    if (!rc) rc = check_graph_rows(c, k, "q", g.q, g.q_row_stride_bytes, g.ns, c->D);
+    if (!rc) rc = check_graph_rows(c, k, "factors", g.factors, g.factors_stride_bytes, 1, 1);
+    if (rc) return rc;
+    GraphMoveBufs b{};
+    b.s = static_cast<double*>(g.s);
+    b.s_stride = g.s_row_stride_bytes / 8;
+    b.c = nc > 0 ? static_cast<double*>(g.c) : nullptr;
+    b.c_stride = nc > 0 ? g.c_row_stride_bytes / 8 : 0;
+    b.draws = ndraws > 0 ? static_cast<double*>(g.draws) : nullptr;
+    b.draws_stride = ndraws > 0 ? g.draws_row_stride_bytes / 8 : 0;
+    b.q = static_cast<const double*>(g.q);
+    b.q_stride = g.q_row_stride_bytes / 8;
+    b.f = static_cast<const double*>(g.factors);
+    b.f_stride = g.factors_stride_bytes / 8;
+    set.push_back(eb_ctx::ProposalGraph{g.split, g.ns, reinterpret_cast<cudaGraphExec_t>((uintptr_t)g.exec), b});
+  }
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  if (!c->qbuf) CK(c, dev_alloc(c->qbuf, (size_t)c->N * c->D * sizeof(double)));
+  if (!c->up_f) CK(c, dev_alloc(c->up_f, (size_t)c->N * sizeof(double)));
+  if (!c->gm_ticket) {
+    DevPtr<unsigned> t;
+    CK(c, dev_alloc(t, sizeof(unsigned)));
+    CK(c, cudaMemset(t.get(), 0, sizeof(unsigned)));
+    c->gm_ticket = std::move(t);
+  }
+  const int rc = ensure_graph_err(c);
+  if (rc) return rc;
+  if ((size_t)slot >= c->props.size()) c->props.resize((size_t)slot + 1);
+  if ((size_t)slot >= c->prop_graphs.size()) c->prop_graphs.resize((size_t)slot + 1);
+  c->props[(size_t)slot] = eb_ctx::ProposalSlot{nullptr, nullptr, EB_CALLBACK_GRAPH};
+  eb_ctx::ProposalGraphs& p = c->prop_graphs[(size_t)slot];
+  p.graphs = std::move(set);
+  p.draw_kind = draw_kind;
+  p.ndraws = ndraws;
   return EB_OK;
 }
 

@@ -210,6 +210,20 @@ struct eb_ctx {
     int where = EB_CALLBACK_HOST;
   };
   std::vector<ProposalSlot> props;
+  // captured proposal graphs (eb_move_set_proposal_graphs; props[slot].where == EB_CALLBACK_GRAPH), indexed by slot,
+  // one graph per split; empty for the other slots
+  struct ProposalGraph {
+    int split;
+    int64_t ns;
+    cudaGraphExec_t exec;
+    GraphMoveBufs b;
+  };
+  struct ProposalGraphs {
+    std::vector<ProposalGraph> graphs;
+    int draw_kind = EB_DRAW_UNIFORM;
+    int64_t ndraws = 0;
+  };
+  std::vector<ProposalGraphs> prop_graphs;
   bool in_proposal = false;   // every other call on the context is refused while a proposal runs
   int up_where = EB_CALLBACK_HOST;  // mode of the running proposal
   int64_t up_m = 0;           // rows the running proposal returns
@@ -218,6 +232,10 @@ struct eb_ctx {
   HostPtr<double> up_hx;      // host mode: pinned [N, D] copy of up_x's rows
   HostPtr<double> up_hq;      // host mode: pinned [N, D] proposals
   HostPtr<double> up_hf;      // host mode: pinned [N] factors
+  DevPtr<unsigned> gm_ticket;  // captured proposals: the block counter of graph_move_result (zero between launches)
+  // a captured proposal's half-step was enqueued since the status was last read: its error freezes only the captured
+  // moves (and a graph model's evaluations), so run_steps reads the status before it enqueues any other move
+  bool gm_unchecked = false;
 
   std::string err;
 };
@@ -266,6 +284,18 @@ enum { CB_STEP = 0, CB_SET_STATE = 1, CB_COMPUTE = 2 };
 
 // a graph model (eb_model_set_graphs): its half-steps report errors through graph_err, read by fetch_status
 inline bool graph_mode(const eb_ctx* c) { return c->model.kind == MODEL_EXTERNAL && c->cb_where == EB_CALLBACK_GRAPH; }
+// a proposal slot holds captured graphs (eb_move_set_proposal_graphs)
+inline bool proposal_graphs(const eb_ctx* c) {
+  for (const eb_ctx::ProposalGraphs& p : c->prop_graphs)
+    if (!p.graphs.empty()) return true;
+  return false;
+}
+// the captured graphs of proposal slot `slot`, or null
+inline const eb_ctx::ProposalGraphs* slot_graphs(const eb_ctx* c, size_t slot) {
+  return slot < c->prop_graphs.size() && !c->prop_graphs[slot].graphs.empty() ? &c->prop_graphs[slot] : nullptr;
+}
+// half-steps report errors through graph_err: a graph model, or a captured proposal
+inline bool graph_errors(const eb_ctx* c) { return graph_mode(c) || proposal_graphs(c); }
 int check_status(eb_ctx* c);  // map (and clear) the status word read back last
 int fetch_status(eb_ctx* c);  // read the status word back, then check_status
 int enqueue_status_read(eb_ctx* c);  // the read-back of fetch_status, without its synchronisation

@@ -121,12 +121,7 @@ __device__ __forceinline__ int gaussian_random_dim(const u32x4& B, int D) {
 // the pair of standard normals (2k, 2k+1) of row `index` (walk.py:36, gaussian.py:97,116, kde.py:41): Box-Muller
 __device__ __forceinline__ void normal_pair(uint64_t seed, uint64_t step, uint32_t split, uint32_t k, uint32_t index,
                                             double& n0, double& n1) {
-  const u32x4 w = draw_words(seed, step, sub_split(split, k), TAG_NORMAL, index);
-  const double r = sqrt(-2.0 * log(1.0 - u53(w.x, w.y)));
-  double sn, cs;
-  sincos(6.283185307179586 * u53(w.z, w.w), &sn, &cs);
-  n0 = r * cs;
-  n1 = r * sn;
+  box_muller_pair(draw_words(seed, step, sub_split(split, k), TAG_NORMAL, index), n0, n1);
 }
 
 // red_blue.py:100, mh.py:58  the accept uniform of active rank (or MHMove walker) i

@@ -152,6 +152,33 @@ cudaError_t launch_graph_stage(const double* src, int64_t rows, int64_t m, int D
 // when *status held an error already, every out[i] is NaN
 cudaError_t launch_graph_result(const double* lp, int64_t lp_stride_bytes, int64_t rows, double* out, int* status,
                                 unsigned long long* err, unsigned long long tag, cudaStream_t st);
+// graph_moves.cu, around a captured proposal graph (eb_move_set_proposal_graphs).  Strides are in doubles.
+struct GraphMoveBufs {
+  double* s;
+  int64_t s_stride;
+  double* c;  // null: an MHMove, whose s is every walker
+  int64_t c_stride;
+  double* draws;
+  int64_t draws_stride;
+  const double* q;
+  int64_t q_stride;
+  const double* f;
+  int64_t f_stride;
+};
+// rows r < N of the live state into s (r < a_count) and c, walker order[a_start + r] / order[r - a_count] /
+// order[r] as launch_split_gather (order null: walker r, a_count = N), and draws[i, 0 .. ndraws) for i < a_count from
+// TAG_GRAPH blocks (index i, sub-index k) at (seed, step, split); unless *status holds an error: then nothing is
+// written and the error is recorded in *err as `tag` | flags
+cudaError_t launch_graph_move_stage(const double* coords, const int32_t* order, int64_t N, int D, int a_start,
+                                    int a_count, const GraphMoveBufs& b, int normal, int64_t ndraws, uint64_t seed,
+                                    uint64_t step, uint32_t split, const int* status, unsigned long long* err,
+                                    unsigned long long tag, cudaStream_t st);
+// qbuf[ns, D] = q, f[ns] = factors; a non-finite q raises FLAG_INF_PARAM / FLAG_NAN_PARAM (ensemble.py:476-479).
+// After the launch's last block sees an error in *status (raised now or earlier) it records it and sets every f[i]
+// to NaN.  `ticket` is a zeroed counter the launch leaves zeroed.
+cudaError_t launch_graph_move_result(const GraphMoveBufs& b, int64_t ns, int D, double* qbuf, double* f, int* status,
+                                     unsigned* ticket, unsigned long long* err, unsigned long long tag,
+                                     cudaStream_t st);
 // the cell of the tma_rows kernel a launch chose (eb_last_kernel_variant)
 struct TmaVariant {
   int R;        // walkers per tile (G = 32 / R lanes per walker)

@@ -4,6 +4,7 @@
 //
 // counter = (index, step_lo, step_hi, (split << 8) | tag), key = (seed_lo, seed_hi)
 #pragma once
+#include <math.h>
 #include <stdint.h>
 
 #ifdef __CUDACC__
@@ -26,7 +27,8 @@ enum : uint32_t {
   TAG_PROP_B = 4,   // proposal draw block B of active rank i
   TAG_ACCEPT = 5,   // Metropolis uniform of active rank i (red_blue.py:100)
   TAG_NORMAL = 6,   // bulk standard normals of row i: block k = normals 2k, 2k+1 (walk.py:36, gaussian.py:97)
-  TAG_SUBSET = 7    // round keys of the helper-subset permutation of active rank i (walk.py:34)
+  TAG_SUBSET = 7,   // round keys of the helper-subset permutation of active rank i (walk.py:34)
+  TAG_GRAPH = 9     // draws of a captured proposal's row i: block k = draws 2k, 2k+1 (eb_move_set_proposal_graphs)
 };
 
 constexpr int FEISTEL_ROUNDS = 8;
@@ -77,6 +79,33 @@ EB_HD u32x4 draw_words(uint64_t seed, uint64_t step, uint32_t split, uint32_t ta
 EB_HD double u53(uint32_t lo, uint32_t hi) {
   uint64_t x = ((uint64_t)hi << 32) | (uint64_t)lo;
   return (double)(x >> 11) * (1.0 / 9007199254740992.0);
+}
+
+// the Box-Muller pair of a block's words (draw specification, tag 6): r cos t, r sin t with r = sqrt(-2 log(1 -
+// u53(w0, w1))), t = 2 pi u53(w2, w3).  Tag 6 (normal_pair, draws.cuh) and tag 9 ("normal") both decode with it.
+EB_HD void box_muller_pair(const u32x4& w, double& n0, double& n1) {
+  const double r = sqrt(-2.0 * log(1.0 - u53(w.x, w.y)));
+  double sn, cs;
+#ifdef __CUDA_ARCH__
+  sincos(6.283185307179586 * u53(w.z, w.w), &sn, &cs);
+#else
+  const double th = 6.283185307179586 * u53(w.z, w.w);
+  sn = sin(th);
+  cs = cos(th);
+#endif
+  n0 = r * cs;
+  n1 = r * sn;
+}
+
+// draws 2k and 2k + 1 of a captured proposal's row from the words w of its TAG_GRAPH block k: two uniforms, or
+// (normal != 0) the Box-Muller pair of these words
+EB_HD void graph_draw_pair(const u32x4& w, int normal, double& d0, double& d1) {
+  if (normal) {
+    box_muller_pair(w, d0, d1);
+    return;
+  }
+  d0 = u53(w.x, w.y);
+  d1 = u53(w.z, w.w);
 }
 
 // integer on [0,n): high 64 bits of (hi:lo) * n

@@ -43,6 +43,45 @@ void chol_psd_host(const double* A, int D, std::vector<double>& L) {
   }
 }
 
+void split_starts(int64_t N, int P, int* start);  // below
+
+// the captured graph of split `split` of a proposal slot, or null
+const eb_ctx::ProposalGraph* find_proposal_graph(const eb_ctx::ProposalGraphs& p, int split) {
+  for (const eb_ctx::ProposalGraph& g : p.graphs)
+    if (g.split == split) return &g;
+  return nullptr;
+}
+
+// a schedule entry whose proposal runs as captured graphs (eb_move_set_proposal_graphs)
+bool captured_proposal(const eb_ctx* c, const eb_move& m) {
+  return (m.kind == EB_MOVE_USER || m.kind == EB_MOVE_USER_MH) && slot_graphs(c, (size_t)m.p0) != nullptr;
+}
+
+// a schedule entry whose slot holds captured graphs (eb_move_set_proposal_graphs): a graph of the right size for
+// every half-step it runs, and no setup call
+int check_proposal_graphs(eb_ctx* c, const eb_move& m) {
+  const eb_ctx::ProposalGraphs& p = *slot_graphs(c, (size_t)m.p0);
+  if (m.kind == EB_MOVE_USER_MH) {
+    const eb_ctx::ProposalGraph* g = find_proposal_graph(p, 0);
+    if (!g || g->ns != c->N)
+      FAIL(c, EB_ERR_INVALID, "eb_step: proposal slot %g has no captured graph of split 0 for all %lld walkers", m.p0,
+           (long long)c->N);
+    return EB_OK;
+  }
+  if (m.mode == EB_USER_SETUP) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: a captured proposal has no setup call");
+  if (m.nsplits < 2 || m.nsplits > MAX_SPLITS || m.nsplits > c->N) return EB_OK;  // refused below
+  int start[MAX_SPLITS + 1];
+  split_starts(c->N, m.nsplits, start);
+  for (int j = 0; j < m.nsplits; ++j) {
+    const eb_ctx::ProposalGraph* g = find_proposal_graph(p, j);
+    const int64_t ns = start[j + 1] - start[j];
+    if (!g || g->ns != ns || !g->b.c)
+      FAIL(c, EB_ERR_INVALID, "eb_step: proposal slot %g has no captured graph of split %d for %lld rows", m.p0, j,
+           (long long)ns);
+  }
+  return EB_OK;
+}
+
 int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) {
   if (!moves || nmoves == 0) FAIL(c, EB_ERR_INVALID, "eb_step: empty move schedule");
   s.moves.assign(moves, moves + nmoves);
@@ -55,9 +94,14 @@ int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) 
     if (m.kind == EB_MOVE_USER || m.kind == EB_MOVE_USER_MH) {
       if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "user proposals are not sharded across GPUs");
       if (c->debug) FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: debug taps do not cover user proposals");
-      if (!(m.p0 >= 0.0 && m.p0 < (double)c->props.size()) || m.p0 != floor(m.p0) || !c->props[(size_t)m.p0].fn)
+      if (!(m.p0 >= 0.0 && m.p0 < (double)c->props.size()) || m.p0 != floor(m.p0) ||
+          (!c->props[(size_t)m.p0].fn && !slot_graphs(c, (size_t)m.p0)))
         FAIL(c, EB_ERR_INVALID, "eb_step: proposal slot %g is not set (eb_move_set_proposal)", m.p0);
       if (!(m.weight >= 0.0) || !isfinite(m.weight)) FAIL(c, EB_ERR_INVALID, "eb_step: bad move weight");
+      if (slot_graphs(c, (size_t)m.p0)) {
+        const int rc = check_proposal_graphs(c, m);
+        if (rc) return rc;
+      }
       if (m.kind == EB_MOVE_USER_MH) {
         m.nsplits = 1;  // the split table of such a step is never read
         m.randomize_split = 0;
@@ -548,9 +592,9 @@ int user_proposal_call(eb_ctx* c, const eb_ctx::ProposalSlot& p, uint64_t step, 
     CK(c, cudaMemcpyAsync(c->up_hx.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
   else if (rows != c->up_x.get())
     CK(c, cudaMemcpyAsync(c->up_x.get(), rows, N * D * sizeof(double), cudaMemcpyDeviceToDevice, c->st.get()));
-  // complete before fn runs (a device consumer may ignore the stream it is given); a graph model's errors so far
-  // stop the call here, so that the function never sees the state past one
-  if (graph_mode(c)) {
+  // complete before fn runs (a device consumer may ignore the stream it is given); the errors of a graph model or a
+  // captured proposal so far stop the call here, so that the function never sees the state past one
+  if (graph_errors(c)) {
     const int rc = fetch_status(c);
     if (rc) return rc;
   } else {
@@ -593,7 +637,26 @@ int user_accept(eb_ctx* c, const eb_ctx::ProposalSlot& p, int kind, const HalfSt
     CK(c, launch_half_step_user(kind, a, ExternalBufs{c->qbuf.get(), c->up_f.get(), c->ext_lp.get()}, c->st.get()));
     ++launches;
   }
-  note_kernel(c, "user_move", "user_move where=%s", p.where == EB_CALLBACK_HOST ? "host" : "device");
+  note_kernel(c, "user_move", "user_move where=%s",
+              p.where == EB_CALLBACK_HOST ? "host" : p.where == EB_CALLBACK_GRAPH ? "graph" : "device");
+  return EB_OK;
+}
+
+// steps 1-3 of a captured proposal's half-step (eb_move_set_proposal_graphs), all enqueued: the gather of s and c
+// (split table `order`; null: an MHMove, every walker in walker order) with the draws, the graph, the read of q and
+// the factors into qbuf / up_f
+int graph_proposal(eb_ctx* c, const eb_ctx::ProposalGraphs& p, const HalfStepArgs& a, const int32_t* order,
+                   uint64_t& launches) {
+  const eb_ctx::ProposalGraph& g = *find_proposal_graph(p, a.split);  // build_schedule checked it is there
+  const unsigned long long tag = graph_err_word(0, (unsigned)a.split, a.step);
+  CK(c, launch_graph_move_stage(c->coords.get(), order, c->N, c->D, a.a_start, a.a_count, g.b,
+                                p.draw_kind == EB_DRAW_NORMAL, p.ndraws, c->seed, a.step, (uint32_t)a.split,
+                                c->status_dev.get(), c->graph_err.get(), tag, c->st.get()));
+  CK(c, cudaGraphLaunch(g.exec, c->st.get()));
+  CK(c, launch_graph_move_result(g.b, a.a_count, c->D, c->qbuf.get(), c->up_f.get(), c->status_dev.get(),
+                                 c->gm_ticket.get(), c->graph_err.get(), tag, c->st.get()));
+  launches += 3;
+  c->gm_unchecked = true;
   return EB_OK;
 }
 
@@ -601,6 +664,17 @@ int user_accept(eb_ctx* c, const eb_ctx::ProposalSlot& p, int kind, const HalfSt
 int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, size_t tbl, uint64_t& launches) {
   int rc = check_walker_count(c, mv);
   if (rc) return rc;
+  if (const eb_ctx::ProposalGraphs* g = slot_graphs(c, (size_t)mv.p0)) {  // captured graphs: no host work per half-step
+    int start[MAX_SPLITS + 1];
+    split_starts(c->N, mv.nsplits, start);
+    for (int split = 0; split < mv.nsplits; ++split) {
+      const HalfStepArgs a = split_args(c, mv, step, tbl, start, split);
+      rc = graph_proposal(c, *g, a, a.order, launches);
+      if (!rc) rc = user_accept(c, c->props[(size_t)mv.p0], EB_MOVE_USER, a, launches);
+      if (rc) return rc;
+    }
+    return EB_OK;
+  }
   const eb_ctx::ProposalSlot p = c->props[(size_t)mv.p0];
   rc = ensure_user_scratch(c, p.where == EB_CALLBACK_HOST);
   if (rc) return rc;
@@ -630,6 +704,11 @@ int launch_step_user(eb_ctx* c, const eb_move& mv, uint64_t step, size_t tbl, ui
 
 // MHMove with a user proposal_function (mh.py:35-65): the whole ensemble in walker order, one accept launch
 int launch_step_user_mh(eb_ctx* c, const eb_move& mv, uint64_t step, uint64_t& launches) {
+  if (const eb_ctx::ProposalGraphs* g = slot_graphs(c, (size_t)mv.p0)) {  // a captured graph
+    const HalfStepArgs a = ensemble_args(c, mv, step);
+    const int rc = graph_proposal(c, *g, a, nullptr, launches);
+    return rc ? rc : user_accept(c, c->props[(size_t)mv.p0], EB_MOVE_USER_MH, a, launches);
+  }
   const eb_ctx::ProposalSlot p = c->props[(size_t)mv.p0];
   int rc = ensure_user_scratch(c, p.where == EB_CALLBACK_HOST);
   if (rc) return rc;
@@ -789,11 +868,12 @@ int reserve_trace(eb_ctx* c, uint64_t nsteps);                    // below
 unsigned stats_due(const eb_ctx* c, uint64_t n);                  // below
 int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches);  // below
 
-// graph mode (eb_model_set_graphs): run_steps logs the steps it enqueues for check_status while it runs
+// graph mode (eb_model_set_graphs, eb_move_set_proposal_graphs): run_steps logs the steps it enqueues for
+// check_status while it runs
 struct GraphRun {
   eb_ctx* c;
   explicit GraphRun(eb_ctx* ctx) : c(ctx) {
-    c->graph_run = graph_mode(c);
+    c->graph_run = graph_errors(c);
     c->graph_step0 = c->step;
     c->graph_picks.clear();
   }
@@ -842,6 +922,13 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
     const eb_move* grp_move = nullptr;
     for (size_t k = 0; k < chunk; ++k) {
       const eb_move& mv = s.moves[ch.pick[k]];
+      // Only a captured proposal's own kernels, and a graph model's, stop at an error the device has recorded; every
+      // other move would go on updating the state.  So after a captured proposal has run, the status is read before
+      // any other move is enqueued (a graph model freezes every move itself).
+      if (c->gm_unchecked && !graph_mode(c) && !captured_proposal(c, mv)) {
+        rc = fetch_status(c);
+        if (rc) return rc;
+      }
       const unsigned due = stats_due(c, c->step + 1);
       const bool stored = sync_every > 0 && (done + k + 1) % sync_every == 0;  // after_step enqueues copies
       if (perstep) {

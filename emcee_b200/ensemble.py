@@ -229,9 +229,16 @@ class EnsembleSampler(object):
         if len(slots) > _lib.EB_MAX_PROPOSAL_SLOTS:
             raise NotImplementedError("a move schedule holds at most %d user moves (got %d)"
                                       % (_lib.EB_MAX_PROPOSAL_SLOTS, len(slots)))
+        specs = {k: user_move_spec(self._moves[k]) for k in slots}
+        # captured proposals: every capture of every move checked before the engine sees any
+        graphs = {k: sp[2]._graph_specs(self.nwalkers, self.ndim, self._device)
+                  for k, sp in specs.items() if sp[1] == "graph"}
         for k, slot in slots.items():
-            _, where, propose, setup = user_move_spec(self._moves[k])
-            self._engine.set_proposal(slot, propose, where, setup)
+            _, where, propose, setup = specs[k]
+            if where == "graph":
+                self._engine.set_proposal_graphs(slot, propose.draw, propose.ndraws, *graphs[k])
+            else:
+                self._engine.set_proposal(slot, propose, where, setup)
 
     # ------------------------------------------------------------------ state
     @property

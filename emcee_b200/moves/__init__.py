@@ -3,7 +3,8 @@
 The red-blue family (``StretchMove``, ``DEMove``, ``DESnookerMove``, ``WalkMove``) and the
 Metropolis family with Gaussian proposals (``MHMove``, ``GaussianMove``), and user-written proposals:
 ``RedBlueMove`` subclasses that override ``get_proposal`` (``CudaArrayRedBlueMove`` for CUDA arrays) and
-``MHMove(HostProposal(fn))`` / ``MHMove(CudaArrayProposal(fn))``, and ``KDEMove`` (the reference's SciPy
+``MHMove(HostProposal(fn))`` / ``MHMove(CudaArrayProposal(fn))``, their captured-graph forms
+``CudaGraphRedBlueMove`` / ``MHMove(CudaGraphProposal(capture))``, and ``KDEMove`` (the reference's SciPy
 kernel-density proposals, built on the device)."""
 
 from .de import DEMove
@@ -14,8 +15,10 @@ from .mh import MHMove
 from .move import Move
 from .red_blue import RedBlueMove
 from .stretch import StretchMove
-from .user import CudaArrayProposal, CudaArrayRedBlueMove, HostProposal, user_random
+from .user import (CapturedProposal, CudaArrayProposal, CudaArrayRedBlueMove, CudaGraphProposal, CudaGraphRedBlueMove,
+                   HostProposal, user_random)
 from .walk import WalkMove
 
 __all__ = ["Move", "RedBlueMove", "StretchMove", "DEMove", "DESnookerMove", "WalkMove", "KDEMove", "MHMove",
-           "GaussianMove", "HostProposal", "CudaArrayProposal", "CudaArrayRedBlueMove", "user_random"]
+           "GaussianMove", "HostProposal", "CudaArrayProposal", "CudaArrayRedBlueMove", "user_random",
+           "CapturedProposal", "CudaGraphRedBlueMove", "CudaGraphProposal"]

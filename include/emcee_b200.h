@@ -255,6 +255,52 @@ int eb_move_set_proposal(eb_ctx* ctx, int32_t slot, eb_proposal_fn fn, void* use
 int eb_proposal_result(eb_ctx* ctx, const void* q, int64_t q_row_stride_bytes, const void* factors,
                        int64_t f_stride_bytes, int64_t m, uint64_t src_stream);
 
+/* A user proposal captured as CUDA graphs, one per split of the moves that use its slot: launched, the graph reads
+ * the active set s[ns, ndim], the other sets c[N - ns, ndim] back to back in set order (NULL for an MHMove, whose
+ * s is the whole ensemble in walker order and whose split is 0) and ndraws draws per row draws[ns, ndraws], and
+ * writes q[ns, ndim] and factors[ns].  Every buffer is float64 device memory of the engine's device with contiguous
+ * rows; the *_stride_bytes are the distances between rows (factors: between entries).  Splits that see the same
+ * shapes may share one graph and its buffers.  exec is a cudaGraphExec_t instantiated on the engine's device. */
+typedef struct {
+  int32_t split;
+  int64_t ns;
+  uint64_t exec;
+  void* s;
+  int64_t s_row_stride_bytes;
+  void* c;
+  int64_t c_row_stride_bytes;
+  void* draws;
+  int64_t draws_row_stride_bytes;
+  void* q;
+  int64_t q_row_stride_bytes;
+  void* factors;
+  int64_t factors_stride_bytes;
+} eb_proposal_graph;
+#define EB_DRAW_UNIFORM 0 /* draws 2k, 2k+1 of row i: u53(w0, w1), u53(w2, w3) of block (i, sub-index k, purpose 9) */
+#define EB_DRAW_NORMAL 1  /* the same words through purpose 6's Box-Muller pair */
+#define EB_MAX_GRAPH_DRAWS (1 << 19) /* the 18-bit sub-index field of the counter holds k < 2^18 */
+/* make n captured graphs proposal slot `slot` (callback mode EB_CALLBACK_GRAPH); eb_move_set_proposal on the same
+ * slot clears them.  A half-step of a schedule entry of kind EB_MOVE_USER / EB_MOVE_USER_MH naming the slot enqueues,
+ * with no host synchronisation:
+ *   1. one kernel that gathers s and c from the live state into the graph's buffers (red_blue.py:85-87) and fills
+ *      draws from purpose 9 of the draw specification (DESIGN.md §2) at the sampler's (seed, step, split);
+ *   2. cudaGraphLaunch;
+ *   3. one kernel that copies q and factors into the engine and raises EB_ERR_INF_PARAM / EB_ERR_NAN_PARAM for a
+ *      non-finite q (ensemble.py:476-479); NaN factors are no error;
+ *   4. step 6 of eb_move_set_proposal: the log-probability and the accept + update.
+ * Errors stay on the device as under eb_model_set_graphs: from the first one on, nothing is copied into the graphs'
+ * inputs and every factor is NaN, so every later proposal is rejected; the host reports the first error where a
+ * stepping call synchronises, with the step counter, the stored steps and the statistics where eb_move_set_proposal
+ * leaves them.  Refused (EB_ERR_INVALID): draw_kind other than EB_DRAW_UNIFORM / EB_DRAW_NORMAL, ndraws < 0, a split
+ * outside [0, 32) or given twice, ns outside [1, nwalkers], exec = 0, null buffers (c: an MHMove passes none; draws:
+ * none when ndraws = 0), strides that are not positive multiples of 8 or shorter than a row, buffers that are not
+ * device memory of the engine's device; ndraws > EB_MAX_GRAPH_DRAWS and sharded engines: EB_ERR_UNSUPPORTED.  A
+ * schedule whose entry needs a split the slot lacks, or a split of another size, or EB_USER_SETUP, is refused by
+ * eb_step.  The engine does not own the graphs or the buffers: they must stay valid, and unused by anything else,
+ * while the slot is set. */
+int eb_move_set_proposal_graphs(eb_ctx* ctx, int32_t slot, int draw_kind, int64_t ndraws,
+                                const eb_proposal_graph* graphs, size_t n);
+
 /* ---- state (state.py:10-45) ------------------------------------------- */
 /* State(initial_state, copy=True) + the initial compute_log_prob
  * (ensemble.py:312,350-358): copies coords[nwalkers*ndim] to the device;
@@ -605,7 +651,7 @@ const char* eb_last_kernel_name(const eb_ctx* ctx);
  * "tma_rows R=<walkers per tile> epl=<8 register path | 0 strided> own_reg=<0|1> warps=<per CTA>",
  * "dense_dmma nhalf_max=<most half-steps of one launch in the call> grid=<CTAs>", "generic G=<lanes per
  * walker>", "walk", "gaussian", "callback G=<lanes per walker> where=host|device|graph" (eb_last_kernel_name
- * "callback": any move with a callback model), "user_move where=host|device" (eb_last_kernel_name "user_move": a
+ * "callback": any move with a callback model), "user_move where=host|device|graph" (eb_last_kernel_name "user_move": a
  * user proposal, with any model) or "none". */
 const char* eb_last_kernel_variant(const eb_ctx* ctx);
 
