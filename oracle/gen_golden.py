@@ -85,6 +85,25 @@ def case_list(emcee):
         ("mix_walk_stretch_gauss_ring_64x4", 64, 4, T.Ring(4),
          [(mv.WalkMove(s=8), 0.4), (mv.StretchMove(), 0.3), (mv.GaussianMove(0.1), 0.2), (mv.WalkMove(), 0.1)],
          p0(64, 4, 2.5), 50),
+        # ---- split counts above 5: one warp per set of the split table up to 32 sets, sets of one walker,
+        # fixed splits, dense_dmma sets smaller than one 8-walker tile, split indices >= 8 in the per-walker draws
+        ("stretch_iso_nsplits7_61x5", 61, 5, iso5, mv.StretchMove(nsplits=7), p0(61, 5), 30),
+        ("stretch_iso_nsplits32_32x3", 32, 3, T.GaussIso(3), mv.StretchMove(nsplits=32), p0(32, 3), 30),
+        ("stretch_ring_fixed_nsplits32_100x4", 100, 4, T.Ring(4),
+         mv.StretchMove(nsplits=32, randomize_split=False), p0(100, 4, 2.5), 30),
+        ("stretch_dense_mean_nsplits32_75x16", 75, 16, d16m, mv.StretchMove(nsplits=32), p0(75, 16), 25),
+        ("de_rosen_nsplits9_29x4", 29, 4, T.Rosenbrock(4), mv.DEMove(nsplits=9), p0(29, 4, 0.1, 1.0), 30),
+        ("de_iso_nsplits3_3x1", 3, 1, T.GaussIso(1), mv.DEMove(nsplits=3), p0(3, 1), 30),
+        ("walk_all_nsplits6_ring_50x4", 50, 4, T.Ring(4), mv.WalkMove(nsplits=6), p0(50, 4, 2.5), 30),
+        # complements of 6 and 7 walkers in 8 dimensions: rank-deficient helper covariances (live_dangerously)
+        ("walk_all_nsplits3_rankcap_iso_10x8", 10, 8, T.GaussIso(8),
+         mv.WalkMove(nsplits=3, live_dangerously=True), p0(10, 8), 25),
+        # complements of 38 and 39 walkers with s = 38: both Walk kernels in every step
+        ("walk_s38_nsplits32_iso_40x4", 40, 4, T.GaussIso(4), mv.WalkMove(s=38, nsplits=32), p0(40, 4), 20),
+        ("mix_nsplits_2_7_32_5_ring_64x4", 64, 4, T.Ring(4),
+         [(mv.StretchMove(), 0.3), (mv.StretchMove(nsplits=7, randomize_split=False), 0.3),
+          (mv.DEMove(nsplits=32), 0.2), (mv.WalkMove(s=3, nsplits=5), 0.2)],
+         p0(64, 4, 2.5), 40),
     ]
 
 
@@ -173,6 +192,8 @@ def run_case(emcee, name, nwalkers, ndim, target, moves, p0, nsteps, seed):
     }
     arrays.update(describe_moves(moves)[1])
     arrays.update(model_arrays(target))
+    if any(getattr(m, "live_dangerously", False) for m, _ in (moves if isinstance(moves, list) else [(moves, 1)])):
+        arrays["live_dangerously"] = np.array(True)  # red_blue.py:64-70 refuses nwalkers < 2 * ndim without it
     for kind, parts in tr.items():
         arrays["trace_" + kind] = np.concatenate(parts)
     np.savez_compressed(os.path.join(OUT, name + ".npz"), **arrays)

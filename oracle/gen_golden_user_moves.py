@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate ``tests/golden/user_moves/*.npz`` from the UNMODIFIED reference (TEST INFRASTRUCTURE).
 
-    python -m oracle.gen_golden_user_moves            # needs oracle/_ref/emcee_reference.zip (make_ref.py)
+    python -m oracle.gen_golden_user_moves [names]    # needs oracle/_ref/emcee_reference.zip (make_ref.py)
 
 Each case runs the reference's own ``EnsembleSampler`` with ``oracle.philox.PhiloxRandom`` as ``sampler._random``
 (``ensemble.py:166``) and user moves written against the reference's plugin boundary: a ``RedBlueMove`` subclass
@@ -60,6 +60,7 @@ CASES = [
     ("mix_dense_64x6", 64, 6, "gauss_dense",
      [("user", "stretch", 0.3, {}), ("stretch", None, 0.3, {}), ("de", None, 0.2, {}), ("user_mh", "mh", 0.2, {})],
      30),
+    ("stretch_nsplits32_ring_70x4", 70, 4, "ring", [("user", "stretch", 1.0, dict(nsplits=32))], 20),
 ]
 SEED = 0x0B200
 
@@ -145,14 +146,16 @@ def run_case(emcee, name, nwalkers, ndim, kind, spec, nsteps):
                 chain=sampler.get_chain(), log_prob=sampler.get_log_prob(), accepted=acc)
 
 
-def generate(out_dir=OUT):
+def generate(out_dir=OUT, only=()):
     emcee = import_reference()
     os.makedirs(out_dir, exist_ok=True)
     for name, nwalkers, ndim, kind, spec, nsteps in CASES:
+        if only and name not in only:
+            continue
         arrays = run_case(emcee, name, nwalkers, ndim, kind, spec, nsteps)
         np.savez_compressed(os.path.join(out_dir, name + ".npz"), **arrays)
         print("%s: %d steps, acceptance %.3f" % (name, nsteps, arrays["accepted"].mean()))
 
 
 if __name__ == "__main__":
-    generate()
+    generate(only=set(sys.argv[1:]))

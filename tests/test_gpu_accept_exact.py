@@ -203,11 +203,12 @@ def _model(kind, D):
     return m, AX.Model("dense", A=A, mu=mu, dmma=dmma), 1.0
 
 
-def _move(spec, D):
+def _move(spec, D, nsplits=2):
     if spec[0] == "stretch":
-        return moves.StretchMove(a=spec[1]), rb.Stretch(a=spec[1])
+        return moves.StretchMove(a=spec[1], nsplits=nsplits), rb.Stretch(a=spec[1], nsplits=nsplits)
     if spec[0] == "de":
-        return moves.DEMove(sigma=spec[1], gamma0=spec[2]), rb.DE(sigma=spec[1], gamma0=spec[2])
+        return (moves.DEMove(sigma=spec[1], gamma0=spec[2], nsplits=nsplits),
+                rb.DE(sigma=spec[1], gamma0=spec[2], nsplits=nsplits))
     if spec[0] == "snooker":
         return moves.DESnookerMove(gammas=spec[1]), rb.Snooker(gammas=spec[1])
     if spec[0] == "walk":
@@ -256,7 +257,8 @@ def _complement_state(X0, X1, sets, k):
 
 
 @pytest.mark.parametrize("model_kind,N,D,mspec,options,variant,skind", [r[1:] for r in ROWS], ids=[r[0] for r in ROWS])
-def test_accept_threshold_exact(model_kind, N, D, mspec, options, variant, skind):
+def test_accept_threshold_exact(model_kind, N, D, mspec, options, variant, skind, nsplits=2):
+    """nsplits (stretch and DE rows only) is left at the default here; test_gpu_splits.py runs rows at 7 splits."""
     if D > AX.MP_MAX_D and mspec[0] in ("de", "snooker") and not AX.PX.longdouble_ok():
         pytest.skip("np.longdouble is not wider than double here (eps %g >= 1e-18)" % np.finfo(np.longdouble).eps)
     t0 = time.time()
@@ -264,7 +266,7 @@ def test_accept_threshold_exact(model_kind, N, D, mspec, options, variant, skind
     if callable(N):
         N = N(sm)
     dmodel, xm, scale = _model(model_kind, D)
-    dmove, omove = _move(mspec, D)
+    dmove, omove = _move(mspec, D, nsplits)
     desc = dmove.descriptor()
     eng = emcee_b200.EnsembleSampler(N, D, dmodel, seed=1)._engine
     for k, v in options:

@@ -38,7 +38,7 @@ GAUSS_MODES = ("vector", "random", "sequential")
 def oracle_moves(g):
     out = []
     for k, (kind, w, nsplits, rand, p0, p1) in enumerate(g["moves"]):
-        kw = dict(nsplits=int(nsplits), randomize_split=bool(rand))
+        kw = dict(nsplits=int(nsplits), randomize_split=bool(rand), live_dangerously=bool(g.get("live_dangerously", False)))
         if kind == 0:
             m = rb.Stretch(a=p0, **kw)
         elif kind == 1:
