@@ -185,6 +185,11 @@ _SIGNATURES = {
     "eb_trace_count": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "eb_trace_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), _dp]),
     "eb_trace_best": (C.c_int, [C.c_void_p, _dp, _dp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_reservoir_config": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64]),
+    "eb_reservoir_count": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_reservoir_read": (C.c_int, [C.c_void_p, _dp, _dp, C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]),
+    "eb_reservoir_read_to": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64),
+                                       C.POINTER(C.c_int64)]),
     "eb_walkers_gram": (C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp, C.POINTER(C.c_int)]),
     "eb_autocorr": (C.c_int, [C.c_void_p, _dp, C.c_size_t, C.c_size_t, C.c_size_t, _dp]),
     "eb_last_step_timing": (C.c_int, [C.c_void_p, _dp, C.POINTER(C.c_uint64)]),
@@ -1167,6 +1172,34 @@ class Engine(object):
         lp, step, walker = C.c_double(), C.c_uint64(), C.c_uint64()
         self._check(lib().eb_trace_best(self._h, _as_dp(coords), C.byref(lp), C.byref(step), C.byref(walker)))
         return coords, float(lp.value), int(step.value), int(walker.value)
+
+    def reservoir_config(self, size, every):
+        """Keep ``size`` of the rows of every ``every``-th step (``eb_reservoir_config``).  Values past uint64 reach the
+        library as its largest value instead of wrapping: a size it refuses, a cadence no run reaches."""
+        top = 2**64 - 1
+        self._check(lib().eb_reservoir_config(self._h, min(int(size), top), min(int(every), top)))
+
+    def reservoir_count(self):
+        """``(offered, kept)`` rows of the reservoir (``eb_reservoir_count``)."""
+        offered, kept = C.c_uint64(), C.c_uint64()
+        self._check(lib().eb_reservoir_count(self._h, C.byref(offered), C.byref(kept)))
+        return int(offered.value), int(kept.value)
+
+    def reservoir_read(self, cuda=False):
+        """``(coords[k, ndim], log_prob[k], step[k] uint64, walker[k] int64)`` of the kept rows in the reservoir's
+        order (``eb_reservoir_read``); ``cuda=True``: coords and log_prob as :class:`DeviceArray` s
+        (``eb_reservoir_read_to``)."""
+        k = self.reservoir_count()[1]
+        step = np.zeros(k, dtype=np.uint64)
+        walker = np.zeros(k, dtype=np.int64)
+        sp, wp = step.ctypes.data_as(C.POINTER(C.c_uint64)), walker.ctypes.data_as(C.POINTER(C.c_int64))
+        if cuda:
+            coords, lp = DeviceArray((k, self.ndim), self.device), DeviceArray((k,), self.device)
+            self._check(lib().eb_reservoir_read_to(self._h, C.c_void_p(coords._ptr), C.c_void_p(lp._ptr), sp, wp))
+        else:
+            coords, lp = np.zeros((k, self.ndim), dtype=np.float64), np.zeros(k, dtype=np.float64)
+            self._check(lib().eb_reservoir_read(self._h, _as_dp(coords), _as_dp(lp), sp, wp))
+        return coords, lp, step, walker
 
     def walkers_gram(self, coords):
         """``(gram[D, D], flags)`` of ``eb_walkers_gram`` for ``coords[rows, D]``."""

@@ -1105,6 +1105,15 @@ int eb_get_state_rows(eb_ctx* c, int64_t row0, int64_t nrows, double* coords, do
 int eb_set_rng(eb_ctx* c, uint64_t seed, uint64_t step) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
+  // the rows of a step offered again would come back with their old keys, and a new seed draws other keys: either
+  // starts the running reservoir again, so that it stays the sample of one stream of steps (reservoir_plan.h)
+  if (c->res_on && (seed != c->seed || step < c->step)) {
+    CK(c, cudaSetDevice(c->device));
+    CK(c, cudaStreamSynchronize(c->st.get()));
+    CK(c, live_reservoir_setup(&c->res, c->res_mem.get(), c->res.K, (uint32_t)c->N, c->D, c->coords.get(),
+                               c->logp.get(), c->sm_count, c->st.get()));
+    c->res_plan = ResSchedule(c->res.K, (uint64_t)c->N);
+  }
   c->seed = seed;
   c->step = step;
   return EB_OK;
@@ -1754,6 +1763,82 @@ int eb_trace_best(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, u
   return EB_OK;
 }
 
+int eb_reservoir_config(eb_ctx* c, uint64_t size, uint64_t every) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
+  if (size == 0) FAIL(c, EB_ERR_INVALID, "eb_reservoir_config: size must be >= 1");
+  if (size >= RES_SIZE_LIMIT)
+    FAIL(c, EB_ERR_NOMEM, "eb_reservoir_config: size %llu is not below 2^32, the entries the reservoir can address",
+         (unsigned long long)size);
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  if (every > 0 || !c->res_on) {  // every == 0 after a configuration keeps what was kept readable
+    LiveReservoir r;
+    cudaError_t s;
+    if (c->res_on && c->res.K == size) {  // the same size: empty the buffers in place
+      s = live_reservoir_setup(&r, c->res_mem.get(), size, (uint32_t)c->N, c->D, c->coords.get(), c->logp.get(),
+                               c->sm_count, c->st.get());
+    } else {
+      // entries are addressed with 32 bits; the buffers are checked against the free memory before anything changes
+      const uint64_t cap = res_cap(size, (uint64_t)c->N);  // size < 2^32: no wrap
+      size_t free_b = 0, total_b = 0;
+      CK(c, cudaMemGetInfo(&free_b, &total_b));
+      const size_t bytes = cap < RES_SIZE_LIMIT ? live_reservoir_bytes(size, (uint32_t)c->N, c->D) : SIZE_MAX;
+      if (bytes > free_b)
+        FAIL(c, EB_ERR_NOMEM, "eb_reservoir_config: %llu entries of %zu bytes, %zu bytes free",
+             (unsigned long long)cap, (size_t)c->D * sizeof(double) + 32, free_b);
+      DevPtr<void> mem;
+      CK_NOMEM(c, dev_alloc(mem, bytes), "eb_reservoir_config: allocating %zu bytes failed (%s)", bytes,
+               cudaGetErrorString(alloc_err));
+      s = live_reservoir_setup(&r, mem.get(), size, (uint32_t)c->N, c->D, c->coords.get(), c->logp.get(), c->sm_count,
+                               c->st.get());
+      if (s == cudaSuccess) c->res_mem = std::move(mem);
+    }
+    if (s != cudaSuccess) {
+      cudaGetLastError();
+      FAIL(c, EB_ERR_CUDA, "eb_reservoir_config: %s", cudaGetErrorString(s));
+    }
+    c->res = r;
+    c->res_plan = ResSchedule(size, (uint64_t)c->N);
+    c->res_on = true;
+  }
+  c->res_every = every;
+  return EB_OK;
+}
+
+int eb_reservoir_count(eb_ctx* c, uint64_t* offered, uint64_t* kept) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->res_on) FAIL(c, EB_ERR_STATE, "eb_reservoir_count: configure the reservoir with eb_reservoir_config first");
+  if (offered) *offered = c->res_plan.offered;
+  if (kept) *kept = c->res_plan.kept();
+  return EB_OK;
+}
+
+namespace {
+int reservoir_read(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, int64_t* walker, bool device_out) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->res_on) FAIL(c, EB_ERR_STATE, "eb_reservoir_read: configure the reservoir with eb_reservoir_config first");
+  CK(c, cudaSetDevice(c->device));
+  if (c->res_plan.compact_before_read()) {
+    uint64_t launches = 0;
+    CK(c, live_reservoir_compact(c->res, c->res_plan.bound, c->st.get(), launches));
+    c->res_plan.compacted();
+  }
+  CK(c, live_reservoir_read(c->res, c->res_plan.kept(), coords, log_prob, step, walker, device_out, c->st.get()));
+  return EB_OK;
+}
+}  // namespace
+
+int eb_reservoir_read(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, int64_t* walker) {
+  return reservoir_read(c, coords, log_prob, step, walker, false);
+}
+
+int eb_reservoir_read_to(eb_ctx* c, double* coords_dst, double* log_prob_dst, uint64_t* step, int64_t* walker) {
+  return reservoir_read(c, coords_dst, log_prob_dst, step, walker, true);
+}
+
 int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, int* flags) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -2051,6 +2136,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
     FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
   if (c->hist_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
   if (c->trace_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
+  if (c->res_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path

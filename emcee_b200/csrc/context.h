@@ -11,6 +11,7 @@
 #include "engine.cuh"
 #include "hist_bins.h"
 #include "owners.h"
+#include "reservoir_plan.h"
 #include "trace_sum.h"
 
 using namespace eb;
@@ -140,6 +141,13 @@ struct eb_ctx {
   DevPtr<double> trace_rows;        // [trace_cap, 2 D + 4], device
   uint64_t trace_cap = 0;
   std::vector<uint64_t> trace_steps;  // the step counter of each recorded row
+
+  // running reservoir (eb_reservoir_read): K of the rows of every `res_every`-th step, in device memory
+  uint64_t res_every = 0;
+  bool res_on = false;  // configured: res holds its buffers
+  LiveReservoir res;
+  DevPtr<void> res_mem;  // res's buffers
+  ResSchedule res_plan;  // rows offered, and the bound of the live entries that decides the compactions
 
   // WalkMove / GaussianMove scratch (moves_extra.cu)
   DevPtr<double> qbuf;       // [N, D] proposals

@@ -365,6 +365,41 @@ cudaError_t live_trace_launch(const LiveTrace& t, double* row, uint64_t step, cu
 // the best sample so far to the host (coords nullable); synchronises
 cudaError_t live_trace_best(const LiveTrace& t, TraceBest* best, double* coords, cudaStream_t st);
 
+// ---- running reservoir of recorded rows (reservoir.cu, eb_reservoir_config / eb_reservoir_read) ------------------
+struct ResCtl;  // the device's live count, tau, full flag and radix-select state
+// a reservoir of K rows inside `mem` (live_reservoir_bytes of it); cap = res_cap(K, N) entries (reservoir_plan.h)
+struct LiveReservoir {
+  uint32_t N = 0;
+  int D = 0;
+  uint64_t K = 0, cap = 0;
+  int sm_count = 0;
+  const double* coords = nullptr;
+  const double* logp = nullptr;
+  double* x = nullptr;                // [cap, D]
+  double* lp = nullptr;               // [cap]
+  unsigned long long* key = nullptr;  // [cap]
+  unsigned long long* step = nullptr;  // [cap]
+  uint32_t* walker = nullptr;         // [cap]
+  uint32_t* group = nullptr;          // [cap] the boundary group of a compaction, or the order of a read
+  uint32_t* holes = nullptr;          // [K] entries below K that a compaction drops
+  uint32_t* movers = nullptr;         // [K] entries from K on that it keeps
+  ResCtl* ctl = nullptr;
+};
+// bytes of a reservoir of K rows; cap must be below 2^32
+size_t live_reservoir_bytes(uint64_t K, uint32_t N, int D);
+// lays the pointers out, empties the reservoir and synchronises
+cudaError_t live_reservoir_setup(LiveReservoir* r, void* mem, uint64_t K, uint32_t N, int D, const double* coords,
+                                 const double* logp, int sm_count, cudaStream_t st);
+// offers the current state's N rows, recorded as `step`: one kernel on `st`; the caller has made room for N entries
+cudaError_t live_reservoir_record(const LiveReservoir& r, uint64_t seed, uint64_t step, cudaStream_t st,
+                                  uint64_t& launches);
+// keeps the K first of at most `bound` live entries: kernels only, on `st` (no-ops while no more than K are live)
+cudaError_t live_reservoir_compact(const LiveReservoir& r, uint64_t bound, cudaStream_t st, uint64_t& launches);
+// the `kept` entries of a compacted reservoir in the order (key, step, walker): coords[kept, D] and lp[kept] to the
+// host, or (device_out) to device memory; step and walker to the host.  Any output may be null; synchronises
+cudaError_t live_reservoir_read(const LiveReservoir& r, uint64_t kept, double* coords, double* lp, uint64_t* step,
+                                int64_t* walker, bool device_out, cudaStream_t st);
+
 inline int lanes_per_walker(int D) {
   int g = 4;
   while (g < 32 && g * 4 < D) g <<= 1;

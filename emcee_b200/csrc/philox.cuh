@@ -28,7 +28,8 @@ enum : uint32_t {
   TAG_ACCEPT = 5,   // Metropolis uniform of active rank i (red_blue.py:100)
   TAG_NORMAL = 6,   // bulk standard normals of row i: block k = normals 2k, 2k+1 (walk.py:36, gaussian.py:97)
   TAG_SUBSET = 7,   // round keys of the helper-subset permutation of active rank i (walk.py:34)
-  TAG_GRAPH = 9     // draws of a captured proposal's row i: block k = draws 2k, 2k+1 (eb_move_set_proposal_graphs)
+  TAG_GRAPH = 9,    // draws of a captured proposal's row i: block k = draws 2k, 2k+1 (eb_move_set_proposal_graphs)
+  TAG_RESERVOIR = 10  // the key of recorded row (step, walker i) of the running reservoir (eb_reservoir_config)
 };
 
 constexpr int FEISTEL_ROUNDS = 8;
@@ -106,6 +107,13 @@ EB_HD void graph_draw_pair(const u32x4& w, int normal, double& d0, double& d1) {
   }
   d0 = u53(w.x, w.y);
   d1 = u53(w.z, w.w);
+}
+
+// the reservoir key of walker w's row recorded at step counter `step`: (w1 << 32) | w0 of block (step, 0, TAG_RESERVOIR,
+// w); a separate purpose, so that recording rows changes no other draw
+EB_HD uint64_t reservoir_key(uint64_t seed, uint64_t step, uint32_t walker) {
+  const u32x4 w = draw_words(seed, step, 0, TAG_RESERVOIR, walker);
+  return ((uint64_t)w.y << 32) | (uint64_t)w.x;
 }
 
 // integer on [0,n): high 64 bits of (hi:lo) * n

@@ -1106,13 +1106,25 @@ int accumulate_trace(eb_ctx* c, uint64_t& launches) {
   return EB_OK;
 }
 
-enum : unsigned { STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4 };
+// offer the CURRENT state's rows to the reservoir, behind a compaction when the rows could overflow its buffer
+// (kernels only, enqueued on the stream)
+int accumulate_reservoir(eb_ctx* c, uint64_t& launches) {
+  if (c->res_plan.compact_before_record()) {
+    CK(c, live_reservoir_compact(c->res, c->res_plan.bound, c->st.get(), launches));
+    c->res_plan.compacted();
+  }
+  CK(c, live_reservoir_record(c->res, c->seed, c->step, c->st.get(), launches));
+  c->res_plan.recorded();
+  return EB_OK;
+}
+
+enum : unsigned { STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4, STAT_RESERVOIR = 8 };
 
 // the running statistics that record the state once the step counter reaches n: each its every `*_every`-th step
 unsigned stats_due(const eb_ctx* c, uint64_t n) {
   const auto at = [n](uint64_t every) { return every > 0 && n % every == 0; };
   return (at(c->moments_every) ? STAT_MOMENTS : 0u) | (at(c->hist_every) ? STAT_HIST : 0u) |
-         (at(c->trace_every) ? STAT_TRACE : 0u);
+         (at(c->trace_every) ? STAT_TRACE : 0u) | (at(c->res_every) ? STAT_RESERVOIR : 0u);
 }
 
 // the accumulations `due` (stats_due) of the CURRENT state, enqueued on the stream
@@ -1121,6 +1133,7 @@ int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches) {
   if (due & STAT_MOMENTS) rc = accumulate_moments(c, launches);
   if (!rc && (due & STAT_HIST)) rc = accumulate_histograms(c, launches);
   if (!rc && (due & STAT_TRACE)) rc = accumulate_trace(c, launches);
+  if (!rc && (due & STAT_RESERVOIR)) rc = accumulate_reservoir(c, launches);
   return rc;
 }
 

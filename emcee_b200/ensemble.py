@@ -38,6 +38,8 @@ _NO_SHARDED_HISTOGRAMS = "running histograms are counted on one GPU; they cannot
 _NO_HISTOGRAMS = "running histograms are not enabled: call enable_histograms(range, ...) first"
 _NO_SHARDED_TRACE = "the running trace is recorded on one GPU; it cannot be combined with a sharded ensemble"
 _NO_TRACE = "the running trace is not enabled: call enable_trace() first"
+_NO_SHARDED_RESERVOIR = "the running reservoir is kept on one GPU; it cannot be combined with a sharded ensemble"
+_NO_RESERVOIR = "the running reservoir is not enabled: call enable_reservoir(size) first"
 _NO_SHARDED_CUDA_ARRAYS = (
     "CUDA arrays in and out are copied on one GPU; a sharded ensemble takes and returns host arrays"
 )
@@ -53,6 +55,8 @@ _NOT_INDEPENDENT = (
 
 #: what :meth:`EnsembleSampler.trace` returns: one entry per recorded step
 Trace = namedtuple("Trace", ["step", "mean", "var", "log_prob_mean", "log_prob_max", "accepted"])
+#: what :meth:`EnsembleSampler.reservoir` returns: one entry per kept row
+Reservoir = namedtuple("Reservoir", ["coords", "log_prob", "step", "walker"])
 
 
 def _seed_from_numpy():
@@ -177,6 +181,7 @@ class EnsembleSampler(object):
         self._rdv = None  # multi-GPU: the host rendezvous this sampler is attached to (``attach``)
         self._hist = None  # running histograms: the configuration of enable_histograms (edges, pairs)
         self._trace_every = None  # running trace: the cadence its rows were recorded with (enable_trace)
+        self._reservoir_every = None  # running reservoir: the cadence its rows were recorded with (enable_reservoir)
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
@@ -281,6 +286,7 @@ class EnsembleSampler(object):
         d["_rdv"] = None  # a communicator does not survive pickling: re-attach after loading
         d["_hist"] = None  # the running histograms live in the engine's memory: enable them again after loading
         d["_trace_every"] = None  # and so do the rows of the running trace
+        d["_reservoir_every"] = None  # and the rows of the running reservoir
         d["pool"] = None
         return d
 
@@ -317,6 +323,8 @@ class EnsembleSampler(object):
             raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
         if getattr(self, "_trace_every", None) is not None:
             raise NotImplementedError(_NO_SHARDED_TRACE)
+        if getattr(self, "_reservoir_every", None) is not None:
+            raise NotImplementedError(_NO_SHARDED_RESERVOIR)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
@@ -467,6 +475,51 @@ class EnsembleSampler(object):
 
         mean = self.trace(discard).mean
         return self._trace_every * autocorr.integrated_time(mean[:, None, :], **kwargs)
+
+    def enable_reservoir(self, size, every=1):
+        """Keep a uniform random sample, without replacement, of ``size`` of the ``(step, walker)`` rows of every
+        ``every``-th step (the cadence of :meth:`enable_trace`) in GPU memory of a fixed size, for runs that store
+        nothing: what ``get_chain(flat=True, thin=every)`` of a stored run offers, for percentiles, expectations, corner
+        plots or downstream draws.  Each row gets a 64-bit key from the draw specification (tag 10, which no other draw
+        uses, so the chain does not change) and the ``size`` rows with the smallest ``(key, step, walker)`` are kept: a
+        pure function of the seed and the visited states, whatever the calls the run was cut into.  A row costs
+        ``8 * ndim + 32`` bytes and the buffer holds ``size + max(size, nwalkers)`` of them (``MemoryError`` when the
+        GPU has no room, or for ``size >= 2**32``, with nothing changed).  Setting ``random_state`` to another seed or
+        to an earlier step (as ``run_mcmc`` from an earlier state does) empties the reservoir and keeps it enabled:
+        the rows of a step offered again would come back with their old keys.
+
+        Every call with ``every > 0`` drops what was kept; ``every=0`` records nothing more and leaves the contents
+        readable.  The initial state is never recorded and blobs are not kept.  The contents are not pickled, and a
+        sharded ensemble is refused."""
+        if self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_RESERVOIR)
+        size = operator.index(size)
+        if size < 1:
+            raise ValueError("size must be >= 1, got {0}".format(size))
+        every = operator.index(every)
+        if every < 0:
+            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._engine.reservoir_config(size, every)
+        if every > 0 or getattr(self, "_reservoir_every", None) is None:
+            self._reservoir_every = every
+
+    def _reservoir_on(self):
+        if getattr(self, "_reservoir_every", None) is None:
+            raise RuntimeError(_NO_RESERVOIR)
+
+    def reservoir(self, cuda=False):
+        """The rows kept since :meth:`enable_reservoir`, as a :data:`Reservoir` of ``k = min(size,
+        reservoir_count())`` rows sorted by ``(key, step, walker)``: ``coords[k, ndim]``, ``log_prob[k]``,
+        ``step[k]`` (uint64, the step counter the row was recorded at) and ``walker[k]`` (int64).  Any prefix of
+        length ``j`` is a uniform sample of size ``j``, the reservoir of the same run with ``size=j``.
+        ``cuda=True`` returns coords and log_prob as :class:`~emcee_b200.DeviceArray` s."""
+        self._reservoir_on()
+        return Reservoir(*self._engine.reservoir_read(cuda=bool(cuda)))
+
+    def reservoir_count(self):
+        """Rows offered to the reservoir since :meth:`enable_reservoir`: ``nwalkers`` times the recorded steps."""
+        self._reservoir_on()
+        return self._engine.reservoir_count()[0]
 
     # ------------------------------------------------------------- the driver
     def _schedule(self):

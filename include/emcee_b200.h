@@ -344,7 +344,9 @@ int eb_compute_log_prob_blobs(eb_ctx* ctx, const double* coords, size_t m, doubl
 /* ---- random state (ensemble.py:216-238) --------------------------------- */
 /* The engine's "random_state" is (seed, step): every draw is a pure function
  * of (seed, step, split, active rank, purpose) -- see DESIGN.md "Draw
- * specification". */
+ * specification".  A new seed, or a step counter below the current one,
+ * empties the running reservoir (eb_reservoir_config): the rows of a step
+ * offered again would come back with their old keys. */
 int eb_set_rng(eb_ctx* ctx, uint64_t seed, uint64_t step);
 int eb_get_rng(const eb_ctx* ctx, uint64_t* seed, uint64_t* step);
 
@@ -585,6 +587,41 @@ int eb_trace_read(eb_ctx* ctx, uint64_t first, uint64_t count, uint64_t* step, d
  * the lowest walker.  Any output may be NULL; EB_ERR_STATE while no step has
  * been recorded. */
 int eb_trace_best(eb_ctx* ctx, double* coords, double* log_prob, uint64_t* step, uint64_t* walker);
+/* Running reservoir for store=False runs: a uniform sample without
+ * replacement of `size` (K) of the (step, walker) rows recorded after every
+ * step whose counter is a multiple of `every` (the cadence of
+ * eb_histograms_config), in device memory of a fixed size however long the
+ * run is.  Every recorded row gets the key (w1 << 32) | w0 of draw block
+ * (seed, step, split 0, tag 10, index = walker) of the draw specification, and
+ * the reservoir keeps the K rows first in the order (key, step, walker): a
+ * pure function of the seed and the recorded states, independent of how the
+ * steps were cut into calls; no other draw changes.  Rows pass a filter kernel
+ * behind the step on the engine's stream (key below the K-th kept key) into a
+ * buffer of K + max(K, nwalkers) entries of 8 ndim + 32 bytes, which a radix
+ * select on the device cuts back to K before a record that could overflow it
+ * and before every read (csrc/reservoir_plan.h); nothing is copied to the host
+ * or synchronised per recorded step.  The buffers are allocated here,
+ * checked against the free memory first (EB_ERR_NOMEM, with nothing
+ * changed); so is size >= 2^32, past the entries the reservoir addresses.
+ * size >= 1 (EB_ERR_INVALID).  every > 0 drops what was kept;
+ * every == 0 records nothing more and leaves the contents (and their size)
+ * readable.  eb_set_rng with a new seed, or a step counter moved back, empties
+ * the reservoir and keeps its configuration.  Blobs are not kept.  Sharded engines are refused with
+ * EB_ERR_UNSUPPORTED, both ways round (eb_comm_init). */
+int eb_reservoir_config(eb_ctx* ctx, uint64_t size, uint64_t every);
+/* rows offered since the last eb_reservoir_config with every > 0 (nwalkers
+ * times the recorded steps) and rows kept, min(size, offered); either output
+ * may be NULL.  EB_ERR_STATE before any configuration (as the reads). */
+int eb_reservoir_count(eb_ctx* ctx, uint64_t* offered, uint64_t* kept);
+/* the kept rows (eb_reservoir_count) in the order (key, step, walker), so that
+ * any prefix of length k is the reservoir of the same run with size k:
+ * coords[kept * ndim], log_prob[kept], step[kept] (the step counter the row
+ * was recorded at) and walker[kept], all host memory; any output may be NULL. */
+int eb_reservoir_read(eb_ctx* ctx, double* coords, double* log_prob, uint64_t* step, int64_t* walker);
+/* eb_reservoir_read with coords_dst[kept * ndim] and log_prob_dst[kept] in
+ * device memory (gathered on the device; any 8-byte aligned pointers); step
+ * and walker stay host memory. */
+int eb_reservoir_read_to(eb_ctx* ctx, double* coords_dst, double* log_prob_dst, uint64_t* step, int64_t* walker);
 /* walkers_independent (ensemble.py:653-663) on the device: gram[ndim*ndim] =
  * C^T C of the centred, column-normalised coords[rows, ndim] (:656-661), whose
  * extreme eigenvalues give cond(C)^2.  *flags: bit 0 = non-finite coordinate
