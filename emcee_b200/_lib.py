@@ -190,6 +190,9 @@ _SIGNATURES = {
     "eb_reservoir_read": (C.c_int, [C.c_void_p, _dp, _dp, C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]),
     "eb_reservoir_read_to": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64),
                                        C.POINTER(C.c_int64)]),
+    "eb_running_acf_config": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64]),
+    "eb_running_acf_count": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
+    "eb_running_acf_read": (C.c_int, [C.c_void_p, _dp]),
     "eb_walkers_gram": (C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp, C.POINTER(C.c_int)]),
     "eb_autocorr": (C.c_int, [C.c_void_p, _dp, C.c_size_t, C.c_size_t, C.c_size_t, _dp]),
     "eb_last_step_timing": (C.c_int, [C.c_void_p, _dp, C.POINTER(C.c_uint64)]),
@@ -1200,6 +1203,24 @@ class Engine(object):
             coords, lp = np.zeros((k, self.ndim), dtype=np.float64), np.zeros(k, dtype=np.float64)
             self._check(lib().eb_reservoir_read(self._h, _as_dp(coords), _as_dp(lp), sp, wp))
         return coords, lp, step, walker
+
+    def running_acf_config(self, max_lag, every):
+        """Lag sums up to ``max_lag`` of every ``every``-th step (``eb_running_acf_config``).  Values past uint64
+        reach the library as its largest value instead of wrapping: lags it cannot hold, a cadence no run reaches."""
+        top = 2**64 - 1
+        self._check(lib().eb_running_acf_config(self._h, min(int(max_lag), top), min(int(every), top)))
+
+    def running_acf_count(self):
+        """Steps recorded into the running autocorrelation (``eb_running_acf_count``)."""
+        n = C.c_uint64()
+        self._check(lib().eb_running_acf_count(self._h, C.byref(n)))
+        return int(n.value)
+
+    def running_acf_read(self, max_lag):
+        """``rho[min(n, max_lag + 1), ndim]`` of the recorded steps (``eb_running_acf_read``)."""
+        rho = np.zeros((min(self.running_acf_count(), int(max_lag) + 1), self.ndim), dtype=np.float64)
+        self._check(lib().eb_running_acf_read(self._h, _as_dp(rho)))
+        return rho
 
     def walkers_gram(self, coords):
         """``(gram[D, D], flags)`` of ``eb_walkers_gram`` for ``coords[rows, D]``."""

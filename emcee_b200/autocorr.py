@@ -66,16 +66,36 @@ def integrated_time(x, c=5, tol=50, quiet=False, has_walkers=True, engine=None):
     return integrated_time_from_acf(rho, c=c, tol=tol, quiet=quiet)
 
 
-def integrated_time_from_acf(rho, c=5, tol=50, quiet=False):
+def integrated_time_from_acf(rho, c=5, tol=50, quiet=False, n_t=None, thin=1):
     """Sokal's automatic window on the walker-averaged autocorrelation function
     ``rho[n_step, n_param]`` (``autocorr.py:107-123``): ``tau[n_param]``, with the
-    :class:`AutocorrError` / warning of :func:`integrated_time`."""
-    n_t, n_d = rho.shape
+    :class:`AutocorrError` / warning of :func:`integrated_time`.
+
+    ``n_t``: the length of the series when ``rho`` holds only its lags ``0 ..
+    max_lag`` (``max_lag = rho.shape[0] - 1 < n_t - 1``, the running
+    autocorrelation of ``EnsembleSampler.enable_autocorr``).  A window that
+    closes within those lags is the one the whole function gives.  A parameter
+    whose window lies beyond them raises :class:`AutocorrError` with ``tau =
+    thin * taus[max_lag]`` and a message naming ``max_lag``; with ``quiet`` the
+    message is logged as a warning and ``taus[max_lag]`` is the estimate.  The
+    length check then uses ``n_t``."""
+    L, n_d = rho.shape
+    n_t = L if n_t is None else int(n_t)
     taus = 2.0 * np.cumsum(rho, axis=0) - 1.0
-    lags = np.arange(n_t)[:, None]
+    lags = np.arange(L)[:, None]
     inside = lags < c * taus  # Sokal: smallest M with M >= c * tau(M)
-    window = np.where(np.any(inside, axis=0), np.argmin(inside, axis=0), n_t - 1)
+    window = np.where(np.any(inside, axis=0), np.argmin(inside, axis=0), L - 1)
+    beyond = np.all(inside, axis=0) if n_t > L else np.zeros(n_d, dtype=bool)  # no lag held closes the window
+    window[beyond] = L - 1
     tau_est = taus[window, np.arange(n_d)]
+    if np.any(beyond):
+        msg = (
+            "The autocorrelation window of {0} parameter(s) lies beyond max_lag = {1}, the largest lag recorded. "
+            "Enable the running autocorrelation with a larger max_lag.\ntau: {2}"
+        ).format(np.sum(beyond), L - 1, thin * tau_est)
+        if not quiet:
+            raise AutocorrError(thin * tau_est, msg)
+        logger.warning(msg)
     flag = tol * tau_est > n_t
     if np.any(flag):
         msg = (

@@ -1839,6 +1839,62 @@ int eb_reservoir_read_to(eb_ctx* c, double* coords_dst, double* log_prob_dst, ui
   return reservoir_read(c, coords_dst, log_prob_dst, step, walker, true);
 }
 
+int eb_running_acf_config(eb_ctx* c, uint64_t max_lag, uint64_t every) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running autocorrelation is not sharded across GPUs");
+  if (max_lag == 0) FAIL(c, EB_ERR_INVALID, "eb_running_acf_config: max_lag must be >= 1");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  if (every > 0 || !c->racf_on) {  // every == 0 after a configuration keeps what was recorded readable
+    LiveRacf r;
+    cudaError_t s;
+    if (c->racf_on && c->racf.max_lag == max_lag) {  // the same lags: zero the sums in place
+      s = live_racf_setup(&r, c->racf_mem.get(), (uint32_t)c->N, c->D, max_lag, c->coords.get(), c->st.get());
+    } else {
+      // checked against the free memory before anything changes; the old sums stay until the new ones exist
+      size_t free_b = 0, total_b = 0;
+      CK(c, cudaMemGetInfo(&free_b, &total_b));
+      const size_t bytes = live_racf_bytes((uint32_t)c->N, c->D, max_lag);
+      if (bytes > free_b)
+        FAIL(c, EB_ERR_NOMEM, "eb_running_acf_config: max_lag %llu needs %zu bytes, %zu bytes free",
+             (unsigned long long)max_lag, bytes, free_b);
+      DevPtr<void> mem;
+      CK_NOMEM(c, dev_alloc(mem, bytes), "eb_running_acf_config: allocating %zu bytes failed (%s)", bytes,
+               cudaGetErrorString(alloc_err));
+      s = live_racf_setup(&r, mem.get(), (uint32_t)c->N, c->D, max_lag, c->coords.get(), c->st.get());
+      if (s == cudaSuccess) c->racf_mem = std::move(mem);
+    }
+    if (s != cudaSuccess) {
+      cudaGetLastError();
+      FAIL(c, EB_ERR_CUDA, "eb_running_acf_config: %s", cudaGetErrorString(s));
+    }
+    c->racf = r;
+    c->racf_n = 0;
+    c->racf_on = true;
+  }
+  c->racf_every = every;
+  return EB_OK;
+}
+
+int eb_running_acf_count(eb_ctx* c, uint64_t* n) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->racf_on)
+    FAIL(c, EB_ERR_STATE, "eb_running_acf_count: configure the autocorrelation with eb_running_acf_config first");
+  if (n) *n = c->racf_n;
+  return EB_OK;
+}
+
+int eb_running_acf_read(eb_ctx* c, double* rho) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->racf_on)
+    FAIL(c, EB_ERR_STATE, "eb_running_acf_read: configure the autocorrelation with eb_running_acf_config first");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, live_racf_read(c->racf, c->racf_n, rho, c->st.get()));
+  return EB_OK;
+}
+
 int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, int* flags) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -2137,6 +2193,8 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
   if (c->hist_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
   if (c->trace_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
   if (c->res_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
+  if (c->racf_on && nranks > 1)
+    FAIL(c, EB_ERR_UNSUPPORTED, "the running autocorrelation is not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path

@@ -12,6 +12,7 @@
 #include "hist_bins.h"
 #include "owners.h"
 #include "reservoir_plan.h"
+#include "running_acf.h"
 #include "trace_sum.h"
 
 using namespace eb;
@@ -148,6 +149,13 @@ struct eb_ctx {
   LiveReservoir res;
   DevPtr<void> res_mem;  // res's buffers
   ResSchedule res_plan;  // rows offered, and the bound of the live entries that decides the compactions
+
+  // running autocorrelation function (eb_running_acf_read): lag sums of every series of every `racf_every`-th step
+  uint64_t racf_every = 0;
+  bool racf_on = false;  // configured: racf holds its buffers
+  uint64_t racf_n = 0;   // steps recorded since the last configuration with every > 0
+  LiveRacf racf;
+  DevPtr<void> racf_mem;  // racf's buffers
 
   // WalkMove / GaussianMove scratch (moves_extra.cu)
   DevPtr<double> qbuf;       // [N, D] proposals

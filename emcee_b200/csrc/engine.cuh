@@ -365,6 +365,33 @@ cudaError_t live_trace_launch(const LiveTrace& t, double* row, uint64_t step, cu
 // the best sample so far to the host (coords nullable); synchronises
 cudaError_t live_trace_best(const LiveTrace& t, TraceBest* best, double* coords, cudaStream_t st);
 
+// ---- running autocorrelation function (running_acf.cu, eb_running_acf_config / eb_running_acf_read) -------------
+// the sums of N D series over lags 0 .. max_lag inside one allocation of live_racf_bytes (running_acf.h)
+struct LiveRacf {
+  uint32_t N = 0;
+  int D = 0;
+  uint64_t max_lag = 0;
+  const double* coords = nullptr;
+  double* x0 = nullptr;       // [N D] first recorded value of every series
+  double* ring = nullptr;     // [max_lag + RACF_B, N D] the last recorded values, shifted by x0
+  double* head = nullptr;     // [max_lag, N D] the first recorded values, shifted
+  double* s_hi = nullptr;     // [max_lag + 1, N D] lag sums of the folded blocks (double-double)
+  double* s_lo = nullptr;
+  double* y_hi = nullptr;     // [N D] sum of the folded blocks' values (double-double)
+  double* y_lo = nullptr;
+  double* partial = nullptr;  // [walker chunks, max_lag + 1, D] of a read
+  double* rho = nullptr;      // [max_lag + 1, D] of a read
+};
+// bytes of the sums of an N x D ensemble up to max_lag (SIZE_MAX when a size_t cannot hold them)
+size_t live_racf_bytes(uint32_t N, int D, uint64_t max_lag);
+// lays the pointers out, zeroes the sums and synchronises
+cudaError_t live_racf_setup(LiveRacf* r, void* mem, uint32_t N, int D, uint64_t max_lag, const double* coords,
+                            cudaStream_t st);
+// records the current state as recorded step n (0-based), and folds the block it completes: kernels only, on `st`
+cudaError_t live_racf_record(const LiveRacf& r, uint64_t n, cudaStream_t st, uint64_t& launches);
+// rho[min(n, max_lag + 1), D] (host) after n recorded steps; nothing the later reads use changes; synchronises
+cudaError_t live_racf_read(const LiveRacf& r, uint64_t n, double* rho, cudaStream_t st);
+
 // ---- running reservoir of recorded rows (reservoir.cu, eb_reservoir_config / eb_reservoir_read) ------------------
 struct ResCtl;  // the device's live count, tau, full flag and radix-select state
 // a reservoir of K rows inside `mem` (live_reservoir_bytes of it); cap = res_cap(K, N) entries (reservoir_plan.h)

@@ -1118,13 +1118,22 @@ int accumulate_reservoir(eb_ctx* c, uint64_t& launches) {
   return EB_OK;
 }
 
-enum : unsigned { STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4, STAT_RESERVOIR = 8 };
+// write the CURRENT state into the autocorrelation ring, and fold the block of lag sums it completes (kernels only,
+// enqueued on the stream)
+int accumulate_running_acf(eb_ctx* c, uint64_t& launches) {
+  CK(c, live_racf_record(c->racf, c->racf_n, c->st.get(), launches));
+  c->racf_n += 1;
+  return EB_OK;
+}
+
+enum : unsigned { STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4, STAT_RESERVOIR = 8, STAT_AUTOCORR = 16 };
 
 // the running statistics that record the state once the step counter reaches n: each its every `*_every`-th step
 unsigned stats_due(const eb_ctx* c, uint64_t n) {
   const auto at = [n](uint64_t every) { return every > 0 && n % every == 0; };
   return (at(c->moments_every) ? STAT_MOMENTS : 0u) | (at(c->hist_every) ? STAT_HIST : 0u) |
-         (at(c->trace_every) ? STAT_TRACE : 0u) | (at(c->res_every) ? STAT_RESERVOIR : 0u);
+         (at(c->trace_every) ? STAT_TRACE : 0u) | (at(c->res_every) ? STAT_RESERVOIR : 0u) |
+         (at(c->racf_every) ? STAT_AUTOCORR : 0u);
 }
 
 // the accumulations `due` (stats_due) of the CURRENT state, enqueued on the stream
@@ -1134,6 +1143,7 @@ int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches) {
   if (!rc && (due & STAT_HIST)) rc = accumulate_histograms(c, launches);
   if (!rc && (due & STAT_TRACE)) rc = accumulate_trace(c, launches);
   if (!rc && (due & STAT_RESERVOIR)) rc = accumulate_reservoir(c, launches);
+  if (!rc && (due & STAT_AUTOCORR)) rc = accumulate_running_acf(c, launches);
   return rc;
 }
 

@@ -40,6 +40,10 @@ _NO_SHARDED_TRACE = "the running trace is recorded on one GPU; it cannot be comb
 _NO_TRACE = "the running trace is not enabled: call enable_trace() first"
 _NO_SHARDED_RESERVOIR = "the running reservoir is kept on one GPU; it cannot be combined with a sharded ensemble"
 _NO_RESERVOIR = "the running reservoir is not enabled: call enable_reservoir(size) first"
+_NO_SHARDED_AUTOCORR = (
+    "the running autocorrelation is summed on one GPU; it cannot be combined with a sharded ensemble"
+)
+_NO_AUTOCORR = "the running autocorrelation is not enabled: call enable_autocorr(max_lag) first"
 _NO_SHARDED_CUDA_ARRAYS = (
     "CUDA arrays in and out are copied on one GPU; a sharded ensemble takes and returns host arrays"
 )
@@ -182,6 +186,7 @@ class EnsembleSampler(object):
         self._hist = None  # running histograms: the configuration of enable_histograms (edges, pairs)
         self._trace_every = None  # running trace: the cadence its rows were recorded with (enable_trace)
         self._reservoir_every = None  # running reservoir: the cadence its rows were recorded with (enable_reservoir)
+        self._autocorr = None  # running autocorrelation: (max_lag, every) its sums were recorded with (enable_autocorr)
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
@@ -287,6 +292,7 @@ class EnsembleSampler(object):
         d["_hist"] = None  # the running histograms live in the engine's memory: enable them again after loading
         d["_trace_every"] = None  # and so do the rows of the running trace
         d["_reservoir_every"] = None  # and the rows of the running reservoir
+        d["_autocorr"] = None  # and the lag sums of the running autocorrelation
         d["pool"] = None
         return d
 
@@ -325,6 +331,8 @@ class EnsembleSampler(object):
             raise NotImplementedError(_NO_SHARDED_TRACE)
         if getattr(self, "_reservoir_every", None) is not None:
             raise NotImplementedError(_NO_SHARDED_RESERVOIR)
+        if getattr(self, "_autocorr", None) is not None:
+            raise NotImplementedError(_NO_SHARDED_AUTOCORR)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
@@ -520,6 +528,66 @@ class EnsembleSampler(object):
         """Rows offered to the reservoir since :meth:`enable_reservoir`: ``nwalkers`` times the recorded steps."""
         self._reservoir_on()
         return self._engine.reservoir_count()[0]
+
+    def enable_autocorr(self, max_lag, every=1):
+        """Estimate the autocorrelation time while sampling, for runs that store nothing: keep, on the GPU, the lag
+        sums up to ``max_lag`` of every (walker, parameter) series of the states recorded after every ``every``-th
+        step (the cadence of :meth:`enable_trace`; the initial state is never recorded).  They give the
+        walker-averaged autocorrelation function (:meth:`autocorr_function`) and the reference estimator's
+        :meth:`autocorr_time`, equal up to rounding to what a stored chain gives, in memory that does not grow with
+        the run: about ``8 * nwalkers * ndim * (4 * max_lag + 64)`` bytes, allocated here (``MemoryError`` when the
+        GPU has no room, with nothing changed).  Sokal's window reads the function up to about ``5 * tau``, so
+        ``max_lag`` a few times larger than that is enough.
+
+        Every call with ``every > 0`` drops what was recorded; ``every=0`` records nothing more and leaves the results
+        readable.  The sums cannot forget steps, so there is no ``discard``: to leave burn-in out, enable after it.
+        The sums are not pickled, and a sharded ensemble is refused."""
+        if self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_AUTOCORR)
+        max_lag = operator.index(max_lag)
+        if max_lag < 1:
+            raise ValueError("max_lag must be >= 1, got {0}".format(max_lag))
+        every = operator.index(every)
+        if every < 0:
+            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._engine.running_acf_config(max_lag, every)
+        if every > 0 or getattr(self, "_autocorr", None) is None:  # every=0 keeps the lags and cadence recorded
+            self._autocorr = (max_lag, every)
+
+    def _autocorr_on(self):
+        if getattr(self, "_autocorr", None) is None:
+            raise RuntimeError(_NO_AUTOCORR)
+        return self._autocorr
+
+    def autocorr_count(self):
+        """Steps recorded since :meth:`enable_autocorr`."""
+        self._autocorr_on()
+        return self._engine.running_acf_count()
+
+    def autocorr_function(self):
+        """``rho[min(n, max_lag + 1), ndim]`` of the ``n`` recorded steps: what
+        ``np.mean(autocorr._acf(x), axis=1)[:max_lag + 1]`` gives for the recorded states ``x[n, nwalkers, ndim]``
+        (the reference's walker-averaged ``function_1d``), up to rounding.  A walker whose series is constant makes
+        its parameter NaN, as numpy's ``0 / 0`` does.  Use :meth:`enable_autocorr` after burn-in to leave it out."""
+        max_lag, _ = self._autocorr_on()
+        return self._engine.running_acf_read(max_lag)
+
+    def autocorr_time(self, c=5, tol=50, quiet=False):
+        """Integrated autocorrelation time, in steps, of each parameter: what ``get_autocorr_time(thin=every, c=c,
+        tol=tol, quiet=quiet)`` gives for a run that stored exactly the recorded steps, with its
+        :class:`~emcee_b200.autocorr.AutocorrError` / warning for a series shorter than ``tol`` times the estimate.
+        That holds when each parameter's window closes within ``max_lag`` or all lags are held (``n - 1 <=
+        max_lag``); a window beyond ``max_lag`` raises :class:`~emcee_b200.autocorr.AutocorrError` with ``tau =
+        every * taus[max_lag]`` (with ``quiet``: a warning, and that estimate).  There is no ``discard``: enable
+        after burn-in."""
+        from . import autocorr
+
+        max_lag, every = self._autocorr_on()
+        n = self.autocorr_count()
+        if n == 0:
+            raise RuntimeError("no step has been recorded since enable_autocorr")
+        rho = self._engine.running_acf_read(max_lag)
+        return every * autocorr.integrated_time_from_acf(rho, c=c, tol=tol, quiet=quiet, n_t=n, thin=every)
 
     # ------------------------------------------------------------- the driver
     def _schedule(self):

@@ -622,6 +622,32 @@ int eb_reservoir_read(eb_ctx* ctx, double* coords, double* log_prob, uint64_t* s
  * device memory (gathered on the device; any 8-byte aligned pointers); step
  * and walker stay host memory. */
 int eb_reservoir_read_to(eb_ctx* ctx, double* coords_dst, double* log_prob_dst, uint64_t* step, int64_t* walker);
+/* Running autocorrelation function for store=False runs: the walker-averaged
+ * normalised autocorrelation function of every parameter at lags 0 ..
+ * max_lag (autocorr.py:49-104 of the reference's estimator) of the states
+ * recorded after every step whose counter is a multiple of `every` (the
+ * cadence of eb_trace_config), in device memory of a fixed size however long
+ * the run is: about 8 nwalkers ndim (4 max_lag + 64) bytes.  Each (walker,
+ * parameter) series is shifted by its first recorded value; every recorded
+ * step writes the state into a ring, and every 64 recorded steps one kernel
+ * adds the block's lag products into double-double lag sums
+ * (csrc/running_acf.h), so the result is a pure function of the recorded
+ * states, independent of how the steps were cut into calls.  The buffers are
+ * allocated here, checked against the free memory first (EB_ERR_NOMEM, with
+ * nothing changed).  max_lag >= 1 (EB_ERR_INVALID).  every > 0 drops what
+ * was recorded; every == 0 records nothing more and leaves the result
+ * readable.  Sharded engines are refused with EB_ERR_UNSUPPORTED, both ways
+ * round (eb_comm_init). */
+int eb_running_acf_config(eb_ctx* ctx, uint64_t max_lag, uint64_t every);
+/* steps recorded since the last eb_running_acf_config with every > 0.
+ * EB_ERR_STATE before any configuration (as the read). */
+int eb_running_acf_count(eb_ctx* ctx, uint64_t* n);
+/* rho[min(n, max_lag + 1) * ndim] (host memory): rho[tau, d] is the mean over
+ * the walkers of c_w(tau) / c_w(0), c_w the autocovariance of walker w's
+ * parameter d about its mean over the n recorded steps (NaN for a walker
+ * whose series is constant).  Values of an unfinished block are folded into
+ * copies of the sums, so a read changes nothing a later read returns. */
+int eb_running_acf_read(eb_ctx* ctx, double* rho);
 /* walkers_independent (ensemble.py:653-663) on the device: gram[ndim*ndim] =
  * C^T C of the centred, column-normalised coords[rows, ndim] (:656-661), whose
  * extreme eigenvalues give cond(C)^2.  *flags: bit 0 = non-finite coordinate
