@@ -193,6 +193,10 @@ _SIGNATURES = {
     "eb_running_acf_config": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64]),
     "eb_running_acf_count": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "eb_running_acf_read": (C.c_int, [C.c_void_p, _dp]),
+    "eb_window_config": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64]),
+    "eb_window_count": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_window_steps": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_window_chain": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "eb_walkers_gram": (C.c_int, [C.c_void_p, _dp, C.c_size_t, _dp, C.POINTER(C.c_int)]),
     "eb_autocorr": (C.c_int, [C.c_void_p, _dp, C.c_size_t, C.c_size_t, C.c_size_t, _dp]),
     "eb_last_step_timing": (C.c_int, [C.c_void_p, _dp, C.POINTER(C.c_uint64)]),
@@ -941,6 +945,19 @@ class Chain(object):
         return hist
 
 
+class RingChain(Chain):
+    """A :class:`Chain` reader over an engine's running window (``eb_window_chain``): the ring belongs to the engine,
+    which this object keeps alive; :meth:`close` releases nothing."""
+
+    def __init__(self, engine, handle):
+        self._engine = engine
+        self._h = handle
+        self.nwalkers, self.ndim, self.device = engine.nwalkers, engine.ndim, engine.device
+
+    def close(self):
+        pass
+
+
 class Engine(object):
     """Thin owner of one ``eb_ctx``.  Maps error codes onto the exception types
     the reference raises for the same conditions (``ensemble.py:314-323,
@@ -1221,6 +1238,32 @@ class Engine(object):
         rho = np.zeros((min(self.running_acf_count(), int(max_lag) + 1), self.ndim), dtype=np.float64)
         self._check(lib().eb_running_acf_read(self._h, _as_dp(rho)))
         return rho
+
+    def window_config(self, size, every):
+        """Keep the last ``size`` states of every ``every``-th step (``eb_window_config``).  Values past uint64 reach
+        the library as its largest value instead of wrapping: a size it cannot allocate, a cadence no run reaches."""
+        top = 2**64 - 1
+        self._check(lib().eb_window_config(self._h, min(int(size), top), min(int(every), top)))
+
+    def window_count(self):
+        """``(recorded, filled)`` of the running window (``eb_window_count``)."""
+        recorded, filled = C.c_uint64(), C.c_uint64()
+        self._check(lib().eb_window_count(self._h, C.byref(recorded), C.byref(filled)))
+        return int(recorded.value), int(filled.value)
+
+    def window_steps(self):
+        """``(steps[filled], seeds[filled])`` (uint64) of the window's slots, oldest first (``eb_window_steps``)."""
+        n = self.window_count()[1]
+        steps, seeds = np.zeros(n, dtype=np.uint64), np.zeros(n, dtype=np.uint64)
+        self._check(lib().eb_window_steps(self._h, steps.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                          seeds.ctypes.data_as(C.POINTER(C.c_uint64))))
+        return steps, seeds
+
+    def window_chain(self):
+        """A :class:`RingChain` over the window's ring (``eb_window_chain``), current as of this call."""
+        h = C.c_void_p()
+        self._check(lib().eb_window_chain(self._h, C.byref(h)))
+        return RingChain(self, h)
 
     def walkers_gram(self, coords):
         """``(gram[D, D], flags)`` of ``eb_walkers_gram`` for ``coords[rows, D]``."""

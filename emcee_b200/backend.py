@@ -3,6 +3,8 @@
 get_chain / get_log_prob / get_last_sample / shape / iteration / accepted /
 random_state``.  ``Backend`` keeps the chain in host memory, with the reference's
 blob storage; ``DeviceBackend`` keeps it in the GPU's, without blobs.
+``ChainWindow`` reads a sampler's running window, the last steps it recorded,
+with ``DeviceBackend``'s readers.
 
 The engine's ``eb_step_store_blobs`` writes stored steps straight into the
 ``chain`` / ``log_prob`` / ``blobs`` arrays of this class (pinned double-buffered
@@ -16,7 +18,7 @@ import numpy as np
 
 from .state import State
 
-__all__ = ["Backend", "DeviceBackend", "slice_plan"]
+__all__ = ["Backend", "ChainWindow", "DeviceBackend", "slice_plan"]
 
 
 class Backend(object):
@@ -515,3 +517,94 @@ class DeviceBackend(object):
             self.random_state = d["random_state"]
         if d["closed"]:
             self.close()
+
+
+_WINDOW_READ_ONLY = "a ChainWindow is a read-only view of the sampler's running window; {0} is refused"
+
+
+class ChainWindow(DeviceBackend):
+    """The last ``size`` steps a sampler recorded (``EnsembleSampler.enable_window``), read like a
+    :class:`DeviceBackend` that stored them: every reader and analysis of ``DeviceBackend`` (``get_chain``,
+    ``get_log_prob``, ``get_value``, ``get_last_sample``, ``cuda=True``, ``get_autocorr_time``, ``get_percentile``,
+    ``get_moments``, ``get_histogram``, ``get_histogram2d``), with ``discard`` / ``thin`` taken over the window's own
+    slots, oldest first.  Each call reads the ring as it is then, in GPU memory (``eb_window_chain``).
+
+    ``iteration`` is the number of slots filled, ``recorded`` the steps recorded since ``enable_window``, ``steps``
+    the step counter of each slot.  ``accepted`` counts each walker's accepted proposals at the steps in the window,
+    and ``get_autocorr_time`` is in sampler steps (``every * thin * tau``).  The view writes nothing: ``reset``,
+    ``grow``, ``save_step`` and ``close`` raise ``TypeError``, and it cannot be pickled."""
+
+    def __init__(self, sampler):
+        self._sampler = sampler
+        self.dtype = np.float64
+        self.device = sampler._device
+        self.nwalkers, self.ndim = sampler.nwalkers, sampler.ndim
+        self.initialized = True
+        self._closed = False
+
+    @property
+    def _engine(self):
+        return self._sampler._engine
+
+    @property
+    def _ch(self):
+        return self._engine.window_chain()
+
+    _chain = _ch
+
+    @property
+    def every(self):
+        """The cadence the window's steps were recorded with."""
+        return self._sampler._window[1]
+
+    @property
+    def iteration(self):
+        """Slots filled: ``min(recorded, size)``."""
+        return self._engine.window_count()[1]
+
+    @property
+    def recorded(self):
+        """Steps recorded since ``enable_window``."""
+        return self._engine.window_count()[0]
+
+    @property
+    def steps(self):
+        """``uint64[iteration]``: the sampler's step counter after each slot's step, oldest first."""
+        return self._engine.window_steps()[0]
+
+    @property
+    def random_state(self):
+        """``("philox4x32-10", seed, step)`` after the newest slot's step (None when the window is empty): with that
+        slot's state it resumes the run exactly."""
+        from .rng import STATE_TAG
+
+        steps, seeds = self._engine.window_steps()
+        if len(steps) == 0:
+            return None
+        return (STATE_TAG, int(seeds[-1]), int(steps[-1]))
+
+    @property
+    def acceptance_fraction(self):
+        """``accepted / iteration``."""
+        return self.accepted / float(self.iteration)
+
+    def get_autocorr_time(self, discard=0, thin=1, **kwargs):
+        """``DeviceBackend.get_autocorr_time`` of the window, in sampler steps: ``every * thin * tau``, what
+        ``get_autocorr_time`` of a run that stored every step gives for the same states."""
+        return self.every * super().get_autocorr_time(discard=discard, thin=thin, **kwargs)
+
+    def reset(self, nwalkers, ndim):
+        raise TypeError(_WINDOW_READ_ONLY.format("reset"))
+
+    def grow(self, ngrow, blobs):
+        raise TypeError(_WINDOW_READ_ONLY.format("grow"))
+
+    def save_step(self, state, accepted):
+        raise TypeError(_WINDOW_READ_ONLY.format("save_step"))
+
+    def close(self):
+        raise TypeError(_WINDOW_READ_ONLY.format("close"))
+
+    def __getstate__(self):
+        raise TypeError("a ChainWindow reads the sampler's GPU memory and cannot be pickled; pickle "
+                        "get_chain() / get_log_prob() instead")

@@ -1144,7 +1144,7 @@ cudaError_t copy_rows(void* dst, size_t dpitch, const void* src, size_t spitch, 
 }
 
 int chain_check_slice(eb_chain* ch, const char* who, uint64_t first, uint64_t stride, uint64_t count) {
-  if (!for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+  if (!for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
                           [](size_t, uint64_t, uint64_t, uint64_t) {}))
     FAIL(ch, EB_ERR_INVALID, "%s: slots %llu + k * %llu, k < %llu, out of range (capacity %llu slots, stride >= 1)",
          who, (unsigned long long)first, (unsigned long long)stride, (unsigned long long)count,
@@ -1203,7 +1203,7 @@ std::vector<const double*> chain_slot_table(eb_chain* ch, bool coords, uint64_t 
                                             uint64_t count) {
   std::vector<const double*> t;
   t.reserve(count);
-  for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+  for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
                      [&](size_t s, uint64_t off, uint64_t, uint64_t n) {
                        for (uint64_t j = 0; j < n; ++j)
                          t.push_back(coords ? ch->segs[s].x.get() + (off + j * stride) * ch->xs
@@ -1245,6 +1245,28 @@ int moments_config(eb_ctx* c, uint64_t every) {
   return EB_OK;
 }
 
+// an empty chain of nwalkers x ndim on `device`: its stream and its [N] accept buffers (eb_chain_create, and the ring
+// of eb_window_config); synchronises
+cudaError_t chain_init(eb_chain* ch, int device, int64_t nwalkers, int ndim) {
+  ch->device = device;
+  ch->N = nwalkers;
+  ch->D = ndim;
+  ch->xs = ((size_t)nwalkers * (size_t)ndim + 1) & ~(size_t)1;
+  ch->ls = ((size_t)nwalkers + 1) & ~(size_t)1;
+  cudaError_t e = cudaSetDevice(device);
+  int v = 0;
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device);
+  ch->sm_count = v;
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&v, cudaDevAttrMaxPitch, device);
+  ch->max_pitch = (size_t)v;
+  if (e == cudaSuccess) e = stream_create(ch->st, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = dev_alloc(ch->accepted, (size_t)nwalkers * sizeof(double));
+  if (e == cudaSuccess) e = dev_alloc(ch->mask, (size_t)nwalkers);
+  if (e == cudaSuccess) e = cudaMemsetAsync(ch->accepted.get(), 0, (size_t)nwalkers * sizeof(double), ch->st.get());
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ch->st.get());
+  return e;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1258,28 +1280,14 @@ int eb_chain_create(int device, int64_t nwalkers, int64_t ndim, eb_chain** out) 
   const int rc = check_create_args("eb_chain_create", device, nwalkers, ndim);
   if (rc) return rc;
   std::unique_ptr<eb_chain> ch(new eb_chain());
-  ch->device = device;
-  ch->N = nwalkers;
-  ch->D = (int)ndim;
-  ch->xs = ((size_t)nwalkers * (size_t)ndim + 1) & ~(size_t)1;
-  ch->ls = ((size_t)nwalkers + 1) & ~(size_t)1;
-  CREATE_CK(cudaSetDevice(device));
-  int v = 0;
-  CREATE_CK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device));
-  ch->sm_count = v;
-  CREATE_CK(cudaDeviceGetAttribute(&v, cudaDevAttrMaxPitch, device));
-  ch->max_pitch = (size_t)v;
-  CREATE_CK(stream_create(ch->st, cudaStreamNonBlocking));
-  CREATE_CK(dev_alloc(ch->accepted, (size_t)nwalkers * sizeof(double)));
-  CREATE_CK(dev_alloc(ch->mask, (size_t)nwalkers));
-  CREATE_CK(cudaMemsetAsync(ch->accepted.get(), 0, (size_t)nwalkers * sizeof(double), ch->st.get()));
-  CREATE_CK(cudaStreamSynchronize(ch->st.get()));
+  CREATE_CK(chain_init(ch.get(), device, nwalkers, (int)ndim));
   *out = ch.release();
   return EB_OK;
 }
 
 int eb_chain_destroy(eb_chain* ch) {
   if (!ch) return EB_OK;
+  if (ch->ring) FAIL(ch, EB_ERR_INVALID, "eb_chain_destroy: a running window's ring belongs to its engine");
   cudaSetDevice(ch->device);
   cudaStreamSynchronize(ch->st.get());
   delete ch;  // the owners release the segments and buffers, then the stream
@@ -1289,6 +1297,7 @@ int eb_chain_destroy(eb_chain* ch) {
 
 int eb_chain_grow(eb_chain* ch, uint64_t nslots) {
   if (!ch) return EB_ERR_INVALID;
+  if (ch->ring) FAIL(ch, EB_ERR_INVALID, "eb_chain_grow: a running window's ring is sized by eb_window_config");
   const uint64_t have = ch->start.back();
   if (nslots <= have) return EB_OK;
   CK(ch, cudaSetDevice(ch->device));
@@ -1318,13 +1327,15 @@ int eb_chain_capacity(const eb_chain* ch, uint64_t* nslots, uint64_t* bytes) {
   if (!ch) return EB_ERR_INVALID;
   if (nslots) *nslots = ch->start.back();
   if (bytes)
-    *bytes = ch->start.back() * (ch->xs + ch->ls) * sizeof(double) + (uint64_t)ch->N * (sizeof(double) + 1);
+    *bytes = ch->start.back() * (ch->xs + ch->ls) * sizeof(double) + (uint64_t)ch->N * (sizeof(double) + 1) +
+             (ch->ring ? ch->start.back() * (uint64_t)ch->N : 0);
   return EB_OK;
 }
 
 int eb_chain_write(eb_chain* ch, uint64_t slot, const double* coords, const double* log_prob,
                    const uint8_t* accepted) {
   if (!ch) return EB_ERR_INVALID;
+  if (ch->ring) FAIL(ch, EB_ERR_INVALID, "eb_chain_write: a running window's ring is written by the steps only");
   if (!coords || !log_prob) FAIL(ch, EB_ERR_INVALID, "eb_chain_write: null buffer");
   int rc = chain_check_slice(ch, "eb_chain_write", slot, 1, 1);
   if (rc) return rc;
@@ -1351,7 +1362,7 @@ static int chain_read(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t co
                       cudaMemcpyKind kind) {
   const size_t N = (size_t)ch->N, nx = N * ch->D;
   cudaError_t e = cudaSuccess;
-  for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+  for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
                      [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
                        if (coords && e == cudaSuccess)
                          e = copy_rows(coords + k0 * nx, nx * sizeof(double), ch->segs[s].x.get() + off * ch->xs,
@@ -1390,6 +1401,8 @@ int eb_chain_read_to(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t cou
 int eb_chain_accepted(eb_chain* ch, double* accepted) {
   if (!ch || !accepted) return EB_ERR_INVALID;
   CK(ch, cudaSetDevice(ch->device));
+  if (ch->ring)  // the accepted proposals of the steps still in the window
+    CK(ch, launch_mask_sum(ch->slot_mask.get(), ch->filled, ch->N, ch->accepted.get(), ch->st.get()));
   CK(ch, cudaMemcpyAsync(accepted, ch->accepted.get(), (size_t)ch->N * sizeof(double), cudaMemcpyDeviceToHost,
                          ch->st.get()));
   CK(ch, cudaStreamSynchronize(ch->st.get()));
@@ -1408,7 +1421,7 @@ int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t co
   return acf_slabs(ch, "eb_chain_autocorr", ch->st.get(), (size_t)count, nw, nd, acf,
                    [&](double* xin, size_t w0, size_t wn) {
                      cudaError_t e = cudaSuccess;
-                     for_each_chain_run(ch->start.data(), ch->segs.size(), first, stride, count,
+                     for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
                                         [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
                                           if (e == cudaSuccess)
                                             e = copy_rows(xin + k0 * wn * nd, wn * nd * sizeof(double),
@@ -1895,6 +1908,79 @@ int eb_running_acf_read(eb_ctx* c, double* rho) {
   return EB_OK;
 }
 
+int eb_window_config(eb_ctx* c, uint64_t size, uint64_t every) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running window is not sharded across GPUs");
+  if (size == 0) FAIL(c, EB_ERR_INVALID, "eb_window_config: size must be >= 1");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st.get()));
+  if (every > 0 || !c->win) {  // every == 0 after a configuration keeps what was recorded readable
+    if (!c->win || c->win->start.back() != size) {
+      // checked against the free memory before anything changes; the old ring stays until the new one exists
+      const size_t N = (size_t)c->N, xs = (N * (size_t)c->D + 1) & ~(size_t)1, ls = (N + 1) & ~(size_t)1;
+      const size_t per_slot = (xs + ls) * sizeof(double) + N;
+      size_t free_b = 0, total_b = 0;
+      CK(c, cudaMemGetInfo(&free_b, &total_b));
+      if (size > (free_b - std::min(free_b, N * (sizeof(double) + 1))) / per_slot)
+        FAIL(c, EB_ERR_NOMEM, "eb_window_config: %llu slots need %.0f bytes, %zu bytes free",
+             (unsigned long long)size, (double)size * (double)per_slot + (double)N * (sizeof(double) + 1), free_b);
+      std::unique_ptr<eb_chain> ring(new eb_chain());
+      cudaError_t e = chain_init(ring.get(), c->device, c->N, c->D);
+      if (e == cudaSuccess) {
+        ChainSeg seg;
+        e = dev_alloc(seg.x, (size_t)size * xs * sizeof(double));
+        if (e == cudaSuccess) e = dev_alloc(seg.lp, (size_t)size * ls * sizeof(double));
+        if (e == cudaSuccess) e = dev_alloc(ring->slot_mask, (size_t)size * N);
+        ring->segs.push_back(std::move(seg));
+        ring->start.push_back(size);
+      }
+      CK_NOMEM(c, e, "eb_window_config: %llu slots of %zu bytes: allocation failed (%s)", (unsigned long long)size,
+               per_slot, cudaGetErrorString(alloc_err));
+      std::vector<uint64_t> steps((size_t)size), seeds((size_t)size);
+      ring->ring = true;
+      c->win = std::move(ring);
+      c->win_steps.swap(steps);
+      c->win_seeds.swap(seeds);
+    }
+    c->win->origin = 0;
+    c->win->filled = 0;
+    c->win_n = 0;
+  }
+  c->win_every = every;
+  return EB_OK;
+}
+
+int eb_window_count(eb_ctx* c, uint64_t* recorded, uint64_t* filled) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->win) FAIL(c, EB_ERR_STATE, "eb_window_count: configure the window with eb_window_config first");
+  if (recorded) *recorded = c->win_n;
+  if (filled) *filled = c->win->filled;
+  return EB_OK;
+}
+
+int eb_window_steps(eb_ctx* c, uint64_t* steps, uint64_t* seeds) {
+  if (!c) return EB_ERR_INVALID;
+  if (!c->win) FAIL(c, EB_ERR_STATE, "eb_window_steps: configure the window with eb_window_config first");
+  const uint64_t size = c->win->start.back();
+  for (uint64_t k = 0; k < c->win->filled; ++k) {
+    const size_t slot = (size_t)((c->win->origin + k) % size);
+    if (steps) steps[k] = c->win_steps[slot];
+    if (seeds) seeds[k] = c->win_seeds[slot];
+  }
+  return EB_OK;
+}
+
+int eb_window_chain(eb_ctx* c, eb_chain** ring) {
+  if (!c || !ring) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (!c->win) FAIL(c, EB_ERR_STATE, "eb_window_chain: configure the window with eb_window_config first");
+  CK(c, cudaSetDevice(c->device));
+  CK(c, cudaStreamSynchronize(c->st.get()));  // the ring's reads run on its own stream, behind the steps' stores
+  *ring = c->win.get();
+  return EB_OK;
+}
+
 int eb_walkers_gram(eb_ctx* c, const double* coords, size_t rows, double* gram, int* flags) {
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
@@ -2195,6 +2281,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
   if (c->res_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
   if (c->racf_on && nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "the running autocorrelation is not sharded across GPUs");
+  if (c->win && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running window is not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path

@@ -4,6 +4,7 @@
 
 #include <stdio.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -39,6 +40,11 @@ struct eb_chain {
   std::vector<uint64_t> start{0};  // segment s holds slots [start[s], start[s + 1])
   DevPtr<double> accepted;         // [N] float64 (backend.py:31)
   DevPtr<uint8_t> mask;            // [N] eb_chain_write's accept mask
+  // a running window's ring (eb_window_chain): one segment owned by an engine, read from logical slot 0 at physical
+  // slot `origin` (chain_map.h); eb_chain_accepted sums the accept masks of its `filled` slots
+  bool ring = false;
+  uint64_t origin = 0, filled = 0;
+  DevPtr<uint8_t> slot_mask;  // ring: [capacity, N] the accept mask of the step each slot holds
   std::string err;
 };
 
@@ -156,6 +162,13 @@ struct eb_ctx {
   uint64_t racf_n = 0;   // steps recorded since the last configuration with every > 0
   LiveRacf racf;
   DevPtr<void> racf_mem;  // racf's buffers
+
+  // running window (eb_window_config): the last `capacity` of the states of every `win_every`-th step, in a ring
+  uint64_t win_every = 0;
+  uint64_t win_n = 0;               // steps recorded since the last configuration with every > 0
+  std::unique_ptr<eb_chain> win;    // the ring (ring == true), or null before any configuration
+  std::vector<uint64_t> win_steps;  // [capacity] the step counter and the Philox key of each physical slot's step
+  std::vector<uint64_t> win_seeds;
 
   // WalkMove / GaussianMove scratch (moves_extra.cu)
   DevPtr<double> qbuf;       // [N, D] proposals

@@ -272,10 +272,13 @@ cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, c
 cudaError_t launch_acf_scale(double* f, size_t n, double scale, cudaStream_t st);
 
 // ---- device chain storage (chain.cu) ----------------------------------------------------------
-// one stored step: cx[nx] = x[nx], clp[nl] = lp[nl], accepted[N] += acc[N] (acc nullable; nx = nl = 0: only the
-// accept counts).  x, lp, cx, clp 16-byte aligned.
+// one stored step: cx[nx] = x[nx], clp[nl] = lp[nl], accepted[N] += acc[N] and cmask[N] = acc[N] (acc, accepted
+// and cmask nullable; nx = nl = 0: only the accept counts).  x, lp, cx, clp 16-byte aligned.
 cudaError_t launch_chain_store(const double* x, const double* lp, const uint8_t* acc, double* cx, double* clp,
-                               double* accepted, size_t nx, size_t nl, int64_t N, int sm_count, cudaStream_t st);
+                               double* accepted, size_t nx, size_t nl, int64_t N, int sm_count, cudaStream_t st,
+                               uint8_t* cmask = nullptr);
+// sums[N] (device) = the per-walker sums of the accept masks mask[nslots, N], in slot order
+cudaError_t launch_mask_sum(const uint8_t* mask, uint64_t nslots, int64_t N, double* sums, cudaStream_t st);
 
 // ---- exact order statistics of a stored slice (select.cu, eb_chain_select) ----------------------------------
 constexpr size_t SELECT_PAIR_BATCH = 16384;          // (parameter, rank) pairs planned at once

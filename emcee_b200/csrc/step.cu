@@ -1126,14 +1126,33 @@ int accumulate_running_acf(eb_ctx* c, uint64_t& launches) {
   return EB_OK;
 }
 
-enum : unsigned { STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4, STAT_RESERVOIR = 8, STAT_AUTOCORR = 16 };
+// copy the CURRENT state and the step's accept mask into the window's ring, at physical slot win_n mod size (a kernel
+// enqueued on the stream); once the ring is full the oldest slot moves on with every record
+int accumulate_window(eb_ctx* c, uint64_t& launches) {
+  eb_chain* w = c->win.get();
+  const uint64_t size = w->start.back(), slot = c->win_n % size;
+  CK(c, launch_chain_store(c->coords.get(), c->logp.get(), c->accepted.get(), w->segs[0].x.get() + slot * w->xs,
+                           w->segs[0].lp.get() + slot * w->ls, nullptr, (size_t)c->N * c->D, (size_t)c->N, c->N,
+                           c->sm_count, c->st.get(), w->slot_mask.get() + slot * (uint64_t)c->N));
+  ++launches;
+  c->win_steps[(size_t)slot] = c->step;
+  c->win_seeds[(size_t)slot] = c->seed;
+  c->win_n += 1;
+  w->filled = std::min(c->win_n, size);
+  w->origin = c->win_n >= size ? c->win_n % size : 0;
+  return EB_OK;
+}
+
+enum : unsigned {
+  STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4, STAT_RESERVOIR = 8, STAT_AUTOCORR = 16, STAT_WINDOW = 32
+};
 
 // the running statistics that record the state once the step counter reaches n: each its every `*_every`-th step
 unsigned stats_due(const eb_ctx* c, uint64_t n) {
   const auto at = [n](uint64_t every) { return every > 0 && n % every == 0; };
   return (at(c->moments_every) ? STAT_MOMENTS : 0u) | (at(c->hist_every) ? STAT_HIST : 0u) |
          (at(c->trace_every) ? STAT_TRACE : 0u) | (at(c->res_every) ? STAT_RESERVOIR : 0u) |
-         (at(c->racf_every) ? STAT_AUTOCORR : 0u);
+         (at(c->racf_every) ? STAT_AUTOCORR : 0u) | (at(c->win_every) ? STAT_WINDOW : 0u);
 }
 
 // the accumulations `due` (stats_due) of the CURRENT state, enqueued on the stream
@@ -1144,6 +1163,7 @@ int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches) {
   if (!rc && (due & STAT_TRACE)) rc = accumulate_trace(c, launches);
   if (!rc && (due & STAT_RESERVOIR)) rc = accumulate_reservoir(c, launches);
   if (!rc && (due & STAT_AUTOCORR)) rc = accumulate_running_acf(c, launches);
+  if (!rc && (due & STAT_WINDOW)) rc = accumulate_window(c, launches);
   return rc;
 }
 
@@ -1272,6 +1292,7 @@ int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
   NOT_IN_CALLBACK(c);
   if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
   if (!ch) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: null chain");
+  if (ch->ring) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: a running window's ring is written by its engine only");
   if (ch->device != c->device || ch->N != c->N || ch->D != c->D)
     FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: the chain is [%lld, %d] on device %d, the engine [%lld, %d] on device %d",
          (long long)ch->N, ch->D, ch->device, (long long)c->N, c->D, c->device);

@@ -18,7 +18,7 @@ from collections.abc import Iterable
 import numpy as np
 
 from . import _lib
-from .backend import Backend, DeviceBackend
+from .backend import Backend, ChainWindow, DeviceBackend
 from .model import Model
 from .models import CallbackFunction, CudaGraphFunction, DeviceModel, graph_row_counts
 from .moves import StretchMove
@@ -44,6 +44,8 @@ _NO_SHARDED_AUTOCORR = (
     "the running autocorrelation is summed on one GPU; it cannot be combined with a sharded ensemble"
 )
 _NO_AUTOCORR = "the running autocorrelation is not enabled: call enable_autocorr(max_lag) first"
+_NO_SHARDED_WINDOW = "the running window is kept on one GPU; it cannot be combined with a sharded ensemble"
+_NO_WINDOW = "the running window is not enabled: call enable_window(size) first"
 _NO_SHARDED_CUDA_ARRAYS = (
     "CUDA arrays in and out are copied on one GPU; a sharded ensemble takes and returns host arrays"
 )
@@ -187,6 +189,7 @@ class EnsembleSampler(object):
         self._trace_every = None  # running trace: the cadence its rows were recorded with (enable_trace)
         self._reservoir_every = None  # running reservoir: the cadence its rows were recorded with (enable_reservoir)
         self._autocorr = None  # running autocorrelation: (max_lag, every) its sums were recorded with (enable_autocorr)
+        self._window = None  # running window: (size, every) its steps were recorded with (enable_window)
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
@@ -293,6 +296,7 @@ class EnsembleSampler(object):
         d["_trace_every"] = None  # and so do the rows of the running trace
         d["_reservoir_every"] = None  # and the rows of the running reservoir
         d["_autocorr"] = None  # and the lag sums of the running autocorrelation
+        d["_window"] = None  # and the steps of the running window
         d["pool"] = None
         return d
 
@@ -333,6 +337,8 @@ class EnsembleSampler(object):
             raise NotImplementedError(_NO_SHARDED_RESERVOIR)
         if getattr(self, "_autocorr", None) is not None:
             raise NotImplementedError(_NO_SHARDED_AUTOCORR)
+        if getattr(self, "_window", None) is not None:
+            raise NotImplementedError(_NO_SHARDED_WINDOW)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
@@ -588,6 +594,35 @@ class EnsembleSampler(object):
             raise RuntimeError("no step has been recorded since enable_autocorr")
         rho = self._engine.running_acf_read(max_lag)
         return every * autocorr.integrated_time_from_acf(rho, c=c, tol=tol, quiet=quiet, n_t=n, thin=every)
+
+    def enable_window(self, size, every=1):
+        """Keep the last ``size`` of the states recorded after every ``every``-th step (the cadence of
+        :meth:`enable_trace`; the initial state is never recorded) in GPU memory, for runs that store nothing:
+        :meth:`window` reads them as an ordered chain, the steps ``get_chain(thin=every)[-size:]`` of a run that
+        stored every step returns, so the converged tail of an open-ended run can be thinned and analysed like a
+        stored chain.  The ring takes ``size * nwalkers * (ndim + 1) * 8`` bytes of states and ``size * nwalkers``
+        bytes of accept masks, allocated here (``MemoryError`` when the GPU has no room, with nothing changed).
+
+        Every call with ``every > 0`` drops what was recorded; ``every=0`` records nothing more and leaves the
+        contents readable.  Blobs are not kept.  The contents are not pickled, and a sharded ensemble is refused."""
+        if self._rdv is not None:
+            raise NotImplementedError(_NO_SHARDED_WINDOW)
+        size = operator.index(size)
+        if size < 1:
+            raise ValueError("size must be >= 1, got {0}".format(size))
+        every = operator.index(every)
+        if every < 0:
+            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._engine.window_config(size, every)
+        if every > 0 or getattr(self, "_window", None) is None:  # every=0 keeps the size and cadence recorded
+            self._window = (size, every)
+
+    def window(self):
+        """The running window (:meth:`enable_window`) as a :class:`~emcee_b200.backend.ChainWindow`: a read-only
+        view with ``DeviceBackend``'s readers and analyses that reads the live ring at each call."""
+        if getattr(self, "_window", None) is None:
+            raise RuntimeError(_NO_WINDOW)
+        return ChainWindow(self)
 
     # ------------------------------------------------------------- the driver
     def _schedule(self):

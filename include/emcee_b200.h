@@ -648,6 +648,40 @@ int eb_running_acf_count(eb_ctx* ctx, uint64_t* n);
  * whose series is constant).  Values of an unfinished block are folded into
  * copies of the sums, so a read changes nothing a later read returns. */
 int eb_running_acf_read(eb_ctx* ctx, double* rho);
+/* Running window for store=False runs: the states after the last `size`
+ * steps whose counter is a multiple of `every` (the cadence of
+ * eb_trace_config), kept in device memory as a ring chain that every
+ * eb_chain_* reader takes: size * nwalkers * (ndim + 1) * 8 bytes of states
+ * and size * nwalkers bytes of accept masks.  A recorded step copies the
+ * coords, log-probabilities and the step's accept mask into physical slot
+ * (recorded mod size) with one kernel behind the step; once the ring is full,
+ * logical slot 0 (the oldest step) is physical slot (recorded mod size).  The
+ * ring is allocated here, checked against the free memory first (EB_ERR_NOMEM,
+ * with nothing changed); size >= 1 (EB_ERR_INVALID).  every > 0 drops what
+ * was recorded; every == 0 records nothing more and leaves the contents
+ * readable.  Sharded engines are refused with EB_ERR_UNSUPPORTED, both ways
+ * round (eb_comm_init). */
+int eb_window_config(eb_ctx* ctx, uint64_t size, uint64_t every);
+/* steps recorded since the last eb_window_config with every > 0, and the slots
+ * they fill: min(recorded, size).  EB_ERR_STATE before any configuration (as
+ * the other eb_window_* calls). */
+int eb_window_count(eb_ctx* ctx, uint64_t* recorded, uint64_t* filled);
+/* for each filled slot in logical order (oldest first): steps[filled] the step
+ * counter after the recorded step, seeds[filled] the Philox key it ran with
+ * (either nullable); (seed, step) is the random state that resumes the run
+ * from that slot's state. */
+int eb_window_steps(eb_ctx* ctx, uint64_t* steps, uint64_t* seeds);
+/* *ring = the window's ring, a borrowed eb_chain of `size` slots whose slot k
+ * is the k-th oldest filled slot.  eb_chain_read, _read_to, _autocorr,
+ * _select, _moments, _histogram and _histogram2d take it with slices of the
+ * filled slots; eb_chain_accepted gives the per-walker sums of the accept
+ * masks of the filled slots (summed on the device); eb_chain_capacity counts
+ * the masks too.  eb_chain_grow, eb_chain_write, eb_chain_destroy and
+ * eb_step_store_chain refuse it (EB_ERR_INVALID).  The handle is valid until
+ * the next eb_window_config or the engine's destruction.  This call
+ * synchronises the engine's stream: reads through the handle see every step
+ * recorded before it. */
+int eb_window_chain(eb_ctx* ctx, eb_chain** ring);
 /* walkers_independent (ensemble.py:653-663) on the device: gram[ndim*ndim] =
  * C^T C of the centred, column-normalised coords[rows, ndim] (:656-661), whose
  * extreme eigenvalues give cond(C)^2.  *flags: bit 0 = non-finite coordinate
