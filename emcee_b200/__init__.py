@@ -8,8 +8,9 @@ __version__ = "0.1.0"
 from . import autocorr, models, moves
 from ._lib import DeviceArray
 from .backend import Backend, DeviceBackend
+from .batch import BatchSampler
 from .ensemble import EnsembleSampler, walkers_independent
 from .model import Model
 from .state import State
 
-__all__ = ["EnsembleSampler", "walkers_independent", "State", "Model", "Backend", "DeviceBackend", "DeviceArray", "moves", "models", "autocorr", "__version__"]
+__all__ = ["EnsembleSampler", "BatchSampler", "walkers_independent", "State", "Model", "Backend", "DeviceBackend", "DeviceArray", "moves", "models", "autocorr", "__version__"]

@@ -112,6 +112,10 @@ _SIGNATURES = {
     "eb_abi_version": (C.c_int, []),
     "eb_device_count": (C.c_int, []),
     "eb_create": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_uint64, C.POINTER(C.c_void_p)]),
+    "eb_create_batch": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_uint64),
+                                  C.POINTER(C.c_void_p)]),
+    "eb_batch_rng_get": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "eb_batch_rng_set": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_uint64]),
     "eb_destroy": (C.c_int, [C.c_void_p]),
     "eb_last_error": (C.c_char_p, [C.c_void_p]),
     "eb_model_set": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_size_t]),
@@ -801,6 +805,92 @@ def make_trampoline(h, evaluate, where, failure, blobs=None):
             return 1
         finally:
             rows._release()
+
+    return LOGPROB_FN(host if where == EB_CALLBACK_HOST else device)
+
+
+class BatchRows(DeviceRows):
+    """The ``[nbatch, m, ndim]`` rows a device-mode batch callback receives (:class:`DeviceRows` otherwise)."""
+
+    __slots__ = ()
+
+    def __init__(self, ptr, nbatch, m, ndim, stream):
+        super().__init__(ptr, nbatch * m, ndim, stream)
+        self._cai["shape"] = (int(nbatch), int(m), int(ndim))
+
+
+def _batch_shape_error(shape, K, m, ndim):
+    return NotImplementedError(
+        "a batched log-probability function receives x[nbatch, m, ndim] = [%d, %d, %d] and must return lp[nbatch, m] "
+        "= (%d, %d) float64 values; it returned shape %s" % (K, m, ndim, K, m, tuple(shape)))
+
+
+def _batch_host_values(out, K, m, ndim):
+    """A batched function's host result ``lp[K, m]`` as a float64 ``[K m]`` array, or the shape / dtype error."""
+    a = np.asarray(out)
+    if a.shape != (K, m):
+        raise _batch_shape_error(a.shape, K, m, ndim)
+    if a.dtype != np.float64:
+        raise TypeError("the log-probability function must return float64 values, got %s" % a.dtype)
+    return np.ascontiguousarray(a).reshape(K * m)
+
+
+def _batch_result(h, lp, out, K, m, ndim):
+    """Flatten a device-mode batched function's ``lp[K, m]`` -- a numpy array or a CUDA-array-interface object whose
+    rows follow each other at one stride -- into the engine's ``lp[K m]`` (``eb_callback_result``)."""
+    cai = getattr(out, "__cuda_array_interface__", None)
+    if cai is None:
+        a = _batch_host_values(out, K, m, ndim)
+        ptr, stride, stream = a.ctypes.data, 8, 0
+    else:
+        shape = tuple(cai["shape"])
+        if shape != (K, m):
+            raise _batch_shape_error(shape, K, m, ndim)
+        if np.dtype(cai["typestr"]) != np.float64:
+            raise TypeError("the log-probability function must return float64 values, got %s" % cai["typestr"])
+        if cai.get("mask") is not None:
+            raise ValueError("masked CUDA arrays are not supported as log-probabilities")
+        strides = cai.get("strides")
+        stride = 8
+        if strides is not None:
+            s0, s1 = int(strides[0]), int(strides[1])
+            stride = s1 if m > 1 else s0
+            if K > 1 and m > 1 and s0 != m * s1:
+                raise ValueError("the log-probabilities lp[nbatch, m] must be one strided run of nbatch * m values "
+                                 "(strides %s)" % (tuple(strides),))
+        stream = (cai["stream"] or 0) if "stream" in cai else EB_STREAM_UNKNOWN
+        ptr = cai["data"][0]
+    rc = lib().eb_callback_result(h, lp, C.c_void_p(ptr), int(stride), int(K * m), int(stream))
+    if rc != EB_OK:
+        _raise(rc, lib().eb_last_error(h).decode())
+
+
+def make_batch_trampoline(h, fn, where, failure, nbatch):
+    """The C callback of a batch engine: the engine's ``[nbatch m, ndim]`` rows go to ``fn`` as ``x[nbatch, m,
+    ndim]`` (host mode: a fresh ndarray; device mode: :class:`BatchRows`), and its ``lp[nbatch, m]`` comes back
+    flattened.  Exceptions as :func:`make_trampoline`."""
+
+    def host(user, x, rows, ndim, lp, stream):
+        try:
+            m = rows // nbatch
+            out = fn(np.ctypeslib.as_array(x, shape=(rows, ndim)).copy().reshape(nbatch, m, ndim))
+            np.ctypeslib.as_array(lp, shape=(rows,))[:] = _batch_host_values(out, nbatch, m, ndim)
+            return 0
+        except BaseException as e:  # noqa: B902
+            failure[0] = e
+            return 1
+
+    def device(user, x, rows, ndim, lp, stream):
+        m = rows // nbatch
+        block = BatchRows(C.cast(x, C.c_void_p).value, nbatch, m, ndim, stream)
+        try:
+            _batch_result(h, lp, fn(block), nbatch, m, ndim)
+            return 0
+        except BaseException as e:  # noqa: B902
+            failure[0] = e
+            return 1
+        finally:
+            block._release()
 
     return LOGPROB_FN(host if where == EB_CALLBACK_HOST else device)
 
@@ -1513,3 +1603,46 @@ class Engine(object):
 
     def comm_import(self, blobs):
         self._check(lib().eb_comm_import(self._h, blobs))
+
+
+class BatchEngine(Engine):
+    """Thin owner of a batch ``eb_ctx`` (``eb_create_batch``): ``nbatch`` ensembles of ``ens_walkers`` walkers
+    stacked as its ``nwalkers = nbatch * ens_walkers`` rows, so every row-wise method of :class:`Engine` takes and
+    returns the stacked rows."""
+
+    def __init__(self, nbatch, nwalkers, ndim, seeds, device=0):
+        self._h = C.c_void_p()
+        self._cb = None
+        self._cb_failure = [None]
+        self._blob_sink = None
+        self._blob_layout = None
+        self._props = {}
+        self.nbatch, self.ens_walkers = int(nbatch), int(nwalkers)
+        self.nwalkers, self.ndim, self.device = self.nbatch * self.ens_walkers, int(ndim), int(device)
+        seeds = np.ascontiguousarray(seeds, dtype=np.uint64)
+        rc = lib().eb_create_batch(self.device, self.nbatch, self.ens_walkers, self.ndim,
+                                   seeds.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(self._h))
+        if rc != EB_OK:
+            msg = lib().eb_last_error(None).decode()
+            self._h = C.c_void_p()
+            _raise(rc, msg)
+
+    def set_callback(self, fn, where):
+        """Make ``fn(x[nbatch, m, ndim]) -> lp[nbatch, m]`` the model, called once per half-step for every
+        ensemble; ``where`` as :meth:`Engine.set_callback`."""
+        mode = {"host": EB_CALLBACK_HOST, "device": EB_CALLBACK_DEVICE}[where]
+        cb = make_batch_trampoline(self._h, fn, mode, self._cb_failure, self.nbatch)
+        self._check(lib().eb_model_set_callback(self._h, cb, None, mode))
+        self._cb = cb
+
+    def get_rng(self):
+        """``(seeds[nbatch] uint64, step)``."""
+        seeds, step = np.zeros(self.nbatch, dtype=np.uint64), C.c_uint64()
+        self._check(lib().eb_batch_rng_get(self._h, seeds.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(step)))
+        return seeds, int(step.value)
+
+    def set_rng(self, seeds, step):
+        seeds = np.ascontiguousarray(seeds, dtype=np.uint64)
+        if seeds.shape != (self.nbatch,):
+            raise ValueError("expected %d seeds, got shape %s" % (self.nbatch, seeds.shape))
+        self._check(lib().eb_batch_rng_set(self._h, seeds.ctypes.data_as(C.POINTER(C.c_uint64)), int(step)))

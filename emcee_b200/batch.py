@@ -1,0 +1,305 @@
+"""``BatchSampler``: many independent ensembles advanced together, one launch per half-step for all of them.
+
+The common emcee workload is many small fits -- one per object, dataset or start point, each a few dozen walkers
+in a handful of dimensions.  Run one ``EnsembleSampler`` after another, each pays the launch latency of every
+half-step (and a user function its Python round trip) around very little work.  A ``BatchSampler`` holds ``nbatch``
+ensembles stacked as the rows of one engine (``eb_create_batch``) and runs each half-step of all of them as one
+kernel, and each call of a user function for all of them at once.
+
+Every draw is a pure function of ``(seed, step, split, index, tag)``, and set sizes depend on ``nwalkers`` and the
+split count only, so ensemble ``k`` with key ``seeds[k]`` produces exactly the chain of ``EnsembleSampler(nwalkers,
+ndim, log_prob_fn, moves=moves, seed=seeds[k])`` started from the same state, whatever else shares the launch."""
+
+import logging
+import operator
+
+import numpy as np
+
+from . import _lib
+from .backend import Backend
+from .ensemble import _NOT_INDEPENDENT, _seed_from_numpy
+from .models import CallbackFunction, CudaGraphFunction, DeviceModel, HostFunction
+from .moves import DEMove, DESnookerMove, StretchMove
+from .state import State
+
+__all__ = ["BatchSampler"]
+
+logger = logging.getLogger(__name__)
+
+_MOVES = (StretchMove, DEMove, DESnookerMove)
+_ONE_MOVE = (
+    "a BatchSampler runs exactly one StretchMove, DEMove or DESnookerMove for every ensemble; a schedule of several "
+    "moves would need a move, and with it a split count, per ensemble and step"
+)
+_MODELS = (
+    "a BatchSampler takes a registered device model (optionally models.Bounded), models.CudaArrayFunction(fn) or "
+    "models.HostFunction(fn, vectorize=True), where fn maps x[nbatch, m, ndim] to lp[nbatch, m]"
+)
+
+
+def _batch_seeds(seeds, K):
+    """``seeds[K]`` (uint64) from ``None`` (derived from numpy's global state without consuming it, as
+    ``EnsembleSampler`` does), one integer ``s`` (``s, s + 1, ..., s + K - 1``) or a sequence of ``K`` integers."""
+    if seeds is None:
+        seeds = _seed_from_numpy()
+    if np.ndim(seeds) == 0:
+        s = operator.index(seeds)
+        return np.array([(s + k) & (2**64 - 1) for k in range(K)], dtype=np.uint64)
+    seeds = [operator.index(s) & (2**64 - 1) for s in seeds]
+    if len(seeds) != K:
+        raise ValueError("seeds must hold one integer per ensemble: expected %d, got %d" % (K, len(seeds)))
+    return np.array(seeds, dtype=np.uint64)
+
+
+def _walkers_independent(coords):
+    """The reference's ``walkers_independent`` (``ensemble.py:653-663``) of every ensemble of ``coords[K, N, D]`` in
+    one batched pass: ``bool[K]``."""
+    finite = np.all(np.isfinite(coords), axis=(1, 2))
+    with np.errstate(all="ignore"):
+        centred = coords - np.mean(coords, axis=1)[:, None, :]
+        span = np.amax(np.abs(centred), axis=1)
+        ok = finite & np.all(span != 0, axis=1)
+        centred = centred / np.where(span == 0, 1.0, span)[:, None, :]
+        centred = centred / np.sqrt(np.sum(centred**2, axis=1))[:, None, :]
+    if not np.any(ok):
+        return ok
+    cond = np.full(len(coords), np.inf)
+    cond[ok] = np.linalg.cond(centred[ok])
+    return ok & (cond <= 1e8)
+
+
+class BatchSampler(object):
+    """``nbatch`` independent ensembles of ``nwalkers x ndim``, each the twin of ``EnsembleSampler(nwalkers, ndim,
+    log_prob_fn, moves=moves, seed=seeds[k])``, advanced together on one H100.
+
+    ``log_prob_fn`` is a registered device model (its parameters shared by every ensemble), or a user function
+    ``fn(x[nbatch, m, ndim]) -> lp[nbatch, m]`` wrapped in ``models.CudaArrayFunction`` or
+    ``models.HostFunction(fn, vectorize=True)``: it is called once per half-step with the proposals of every
+    ensemble, so per-ensemble data broadcasts along the leading axis (``data[nbatch, T]``).  ``moves`` is one
+    ``StretchMove``, ``DEMove`` or ``DESnookerMove`` (default ``StretchMove()``), with any of its parameters.
+
+    ``seeds`` is a sequence of ``nbatch`` integers, or one integer ``s`` for ``s, s + 1, ..., s + nbatch - 1``;
+    ``None`` derives ``s`` from numpy's global state.  States are ``State(coords[nbatch, nwalkers, ndim],
+    log_prob[nbatch, nwalkers])``, chains ``[n, nbatch, nwalkers, ndim]``; the reference's errors apply per ensemble
+    with ``EnsembleSampler``'s types and messages."""
+
+    def __init__(self, nbatch, nwalkers, ndim, log_prob_fn, moves=None, *, seeds=None, device=0):
+        self.nbatch, self.nwalkers, self.ndim = operator.index(nbatch), operator.index(nwalkers), operator.index(ndim)
+        if self.nbatch < 1:
+            raise ValueError("nbatch must be >= 1, got {0}".format(self.nbatch))
+        if self.nbatch * self.nwalkers > 2**31 - 1:
+            raise ValueError("a batch holds at most 2**31 - 1 walkers in all (int32 split tables); got {0} x {1}".format(
+                self.nbatch, self.nwalkers))
+        if isinstance(log_prob_fn, CudaGraphFunction):
+            raise NotImplementedError("CudaGraphFunction is not batched; " + _MODELS)
+        if isinstance(log_prob_fn, CallbackFunction):
+            if log_prob_fn.blobs_dtype is not None:
+                raise NotImplementedError("blobs_dtype is not batched; " + _MODELS)
+            if isinstance(log_prob_fn, HostFunction) and not log_prob_fn.vectorize:
+                raise NotImplementedError("HostFunction(vectorize=False) is not batched; " + _MODELS)
+        elif not isinstance(log_prob_fn, DeviceModel):
+            raise TypeError(_MODELS)
+        if moves is None:
+            moves = StretchMove()
+        elif isinstance(moves, (list, tuple)):
+            if len(moves) != 1:
+                raise NotImplementedError(_ONE_MOVE)
+            moves = moves[0][0] if isinstance(moves[0], (list, tuple)) else moves[0]
+        if type(moves) not in _MOVES:
+            raise NotImplementedError(_ONE_MOVE + "; got {0!r}".format(moves))
+        self.move = moves
+        self.log_prob_fn = log_prob_fn
+        seeds = _batch_seeds(seeds, self.nbatch)
+        self._engine = _lib.BatchEngine(self.nbatch, self.nwalkers, self.ndim, seeds, device=device)
+        m = log_prob_fn
+        if isinstance(m, CallbackFunction):
+            self._engine.set_callback(m._call, m.where)
+        else:
+            self._engine.set_model(m.kind, m.device_params(self.ndim))
+            box = m.bounds(self.ndim)
+            if box is not None:
+                self._engine.set_bounds(*box)
+        self.backend = Backend()
+        self._previous_state = None
+        self.reset()
+
+    # ------------------------------------------------------------------ state
+    @property
+    def random_state(self):
+        """``("philox4x32-10", seeds[nbatch] uint64, step)``: one step counter for every ensemble."""
+        seeds, step = self._engine.get_rng()
+        return ("philox4x32-10", seeds, step)
+
+    @random_state.setter
+    def random_state(self, state):
+        # as EnsembleSampler: try, and stay as we are if it is garbage
+        try:
+            name, seeds, step = state
+            if name == "philox4x32-10":
+                self._engine.set_rng(seeds, operator.index(step))
+        except Exception:
+            pass
+
+    @property
+    def iteration(self):
+        return self.backend.iteration
+
+    def reset(self):
+        self.backend.reset(self.nbatch * self.nwalkers, self.ndim)
+
+    def _state(self, coords, log_prob):
+        K, N, D = self.nbatch, self.nwalkers, self.ndim
+        return State(coords.reshape(K, N, D), log_prob=log_prob.reshape(K, N), random_state=self.random_state)
+
+    # ------------------------------------------------------------- the driver
+    def _stored_before_failure(self, step0, thin_by, k0):
+        b = self.backend
+        _, step = self._engine.get_rng()
+        stored = (step - step0) // thin_by
+        b.iteration = k0 + stored
+        if stored:
+            b.random_state = (self.random_state[0], self.random_state[1], step0 + stored * thin_by)
+
+    def sample(self, initial_state, iterations=1, tune=False, skip_initial_state_check=False, thin_by=1, store=True):
+        """Advance every ensemble as a generator (``EnsembleSampler.sample``): yields the live ``State`` of
+        ``coords[nbatch, nwalkers, ndim]`` every ``thin_by`` steps.  ``initial_state`` is a ``State`` or a bare
+        ``[nbatch, nwalkers, ndim]`` array."""
+        return self._sample(initial_state, iterations, skip_initial_state_check, thin_by, store, bulk=False)
+
+    def _sample(self, initial_state, iterations, skip_initial_state_check, thin_by, store, bulk):
+        K, N, D = self.nbatch, self.nwalkers, self.ndim
+        if iterations is None and store:
+            raise ValueError("'store' must be False when 'iterations' is None")
+        thin_by = int(thin_by)
+        if thin_by <= 0:
+            raise ValueError("Invalid thinning argument")
+        if N < 2 * D and not self.move.live_dangerously:  # red_blue.py:64-70
+            raise RuntimeError(
+                "It is unadvisable to use a red-blue move with fewer walkers than twice the number of dimensions.")
+        state = State(initial_state)
+        coords = np.asarray(state.coords, dtype=np.float64)
+        if coords.shape != (K, N, D):
+            raise ValueError("incompatible input dimensions {0}".format(coords.shape))
+        if not skip_initial_state_check:
+            bad = np.flatnonzero(~_walkers_independent(coords))
+            if len(bad):
+                raise ValueError(_NOT_INDEPENDENT + " (ensemble {0})".format(int(bad[0])))
+        self.random_state = state.random_state
+        lp = None
+        if state.log_prob is not None:
+            lp = np.asarray(state.log_prob, dtype=np.float64)
+            if lp.shape != (K, N):
+                raise ValueError("incompatible input dimensions")
+            lp = lp.reshape(K * N)
+        eng = self._engine
+        eng.set_state(coords.reshape(K * N, D), lp)
+        if store:
+            self.backend.grow(iterations, None)
+        sched = [(self.move.descriptor(), 1.0)]
+        return self._steps(sched, iterations, thin_by, store, bulk)
+
+    def _steps(self, sched, iterations, thin_by, store, bulk):
+        eng, b = self._engine, self.backend
+        if bulk:
+            total = iterations * thin_by
+            if total > 0:
+                if store:
+                    k0, k1 = b.iteration, b.iteration + iterations
+                    step0 = eng.get_rng()[1]
+                    try:
+                        eng.step_store(sched, total, thin_by, b.chain[k0:k1], b.log_prob[k0:k1], b.accepted)
+                    except BaseException:
+                        self._stored_before_failure(step0, thin_by, k0)
+                        raise
+                    b.iteration = k1
+                    b.random_state = self.random_state
+                else:
+                    eng.step(sched, total, want_accepted=False)
+            yield self._state(*eng.get_state())
+            return
+        counter = iter(int, 1) if iterations is None else range(iterations)
+        for _ in counter:
+            if store:
+                k = b.iteration
+                eng.step_store(sched, thin_by, thin_by, b.chain[k : k + 1], b.log_prob[k : k + 1], b.accepted)
+                b.iteration = k + 1
+                b.random_state = self.random_state
+            else:
+                eng.step(sched, thin_by, want_accepted=False)
+            yield self._state(*eng.get_state())
+
+    def run_mcmc(self, initial_state, nsteps, thin_by=1, store=True, skip_initial_state_check=False):
+        """Advance every ensemble ``nsteps`` iterations in one call and return the last ``State``
+        (``EnsembleSampler.run_mcmc``); ``initial_state=None`` continues the run."""
+        if initial_state is None:
+            if self._previous_state is None:
+                raise ValueError("Cannot have `initial_state=None` if run_mcmc has never been called.")
+            initial_state = self._previous_state
+        results = None
+        for results in self._sample(initial_state, nsteps, skip_initial_state_check, thin_by, store, bulk=True):
+            pass
+        if nsteps > 0:
+            self._previous_state = results
+        return results if nsteps > 0 else None
+
+    def compute_log_prob(self, coords):
+        """``lp[nbatch, m]`` of ``coords[nbatch, m, ndim]``: the model's kernel, or one call of the function."""
+        coords = np.asarray(coords, dtype=np.float64)
+        if coords.ndim != 3 or coords.shape[0] != self.nbatch or coords.shape[2] != self.ndim:
+            raise ValueError("incompatible input dimensions {0}; expected [{1}, m, {2}]".format(
+                coords.shape, self.nbatch, self.ndim))
+        K, m, D = coords.shape
+        return self._engine.compute_log_prob(coords.reshape(K * m, D)).reshape(K, m)
+
+    # ---------------------------------------------------------------- results
+    def get_last_sample(self):
+        """The last stored step as a ``State`` of ``coords[nbatch, nwalkers, ndim]``."""
+        s = self.backend.get_last_sample()
+        K, N, D = self.nbatch, self.nwalkers, self.ndim
+        return State(s.coords.reshape(K, N, D), log_prob=s.log_prob.reshape(K, N), random_state=s.random_state)
+
+    @property
+    def acceptance_fraction(self):
+        """``[nbatch, nwalkers]``."""
+        return (self.backend.accepted / float(self.backend.iteration)).reshape(self.nbatch, self.nwalkers)
+
+    def get_value(self, name, flat=False, thin=1, discard=0):
+        """``[n, nbatch, nwalkers, ...]``, or with ``flat`` one flat sample per ensemble, ``[nbatch, n * nwalkers,
+        ...]``: row ``k`` is what ``get_value(name, flat=True, ...)`` of ensemble ``k``'s twin returns."""
+        v = self.backend.get_value(name, thin=thin, discard=discard)
+        v = v.reshape((v.shape[0], self.nbatch, self.nwalkers) + v.shape[2:])
+        if flat:
+            v = np.swapaxes(v, 0, 1).reshape((self.nbatch, v.shape[0] * self.nwalkers) + v.shape[3:])
+        return v
+
+    def get_chain(self, **kwargs):
+        return self.get_value("chain", **kwargs)
+
+    def get_log_prob(self, **kwargs):
+        return self.get_value("log_prob", **kwargs)
+
+    def get_autocorr_time(self, discard=0, thin=1, c=5, tol=50, quiet=False):
+        """``tau[nbatch, ndim]``: row ``k`` is ``thin * autocorr.integrated_time(get_chain(discard=discard,
+        thin=thin)[:, k], c=c, tol=tol, quiet=quiet)``.  When the chain of any ensemble is shorter than ``tol``
+        times its estimate, one :class:`~emcee_b200.autocorr.AutocorrError` (with ``quiet``: one warning) names
+        those ensembles, and its ``tau`` holds every row's estimate."""
+        from . import autocorr
+
+        x = self.get_chain(discard=discard, thin=thin)
+        taus = np.empty((self.nbatch, self.ndim))
+        failed, first = [], None
+        for k in range(self.nbatch):
+            try:
+                taus[k] = autocorr.integrated_time(x[:, k], c=c, tol=tol, quiet=False)
+            except autocorr.AutocorrError as e:
+                taus[k] = e.tau
+                failed.append(k)
+                first = first or str(e)
+        taus *= thin
+        if failed:
+            msg = "The autocorrelation estimate of ensemble(s) {0} is unreliable. First of them:\n{1}".format(
+                failed, first)
+            if not quiet:
+                raise autocorr.AutocorrError(taus, msg)
+            logger.warning(msg)
+        return taus

@@ -168,6 +168,68 @@ int eb_create(int device, int64_t nwalkers, int64_t ndim, uint64_t seed, eb_ctx*
   return EB_OK;
 }
 
+int eb_create_batch(int device, int64_t nbatch, int64_t nwalkers, int64_t ndim, const uint64_t* seeds,
+                    eb_ctx** out) {
+  if (!out) return EB_ERR_INVALID;
+  *out = nullptr;
+  if (!seeds || nbatch < 1 || nwalkers < 2 || nbatch > (int64_t)0x7fffffff / nwalkers) {
+    g_create_err = "eb_create_batch: need nbatch >= 1, nwalkers >= 2, seeds, and nbatch * nwalkers < 2^31 (the int32 "
+                   "split tables)";
+    return EB_ERR_INVALID;
+  }
+  const int64_t rows = nbatch * nwalkers;
+  int rc = check_create_args("eb_create_batch", device, rows, ndim);
+  if (rc) return rc;
+  // what eb_create allocates for the rows (state, counters, split tables up to 64 MiB), against the free memory
+  CREATE_CK(cudaSetDevice(device));
+  size_t free_b = 0, total_b = 0;
+  CREATE_CK(cudaMemGetInfo(&free_b, &total_b));
+  const double need = (double)rows * ((double)ndim * 8.0 + 8.0 + 1.0 + 8.0 + 4.0) + (double)(64u << 20);
+  if (need > (double)free_b) {
+    char b[256];
+    snprintf(b, sizeof(b), "eb_create_batch: %lld ensembles of %lld x %lld need about %.0f bytes, %zu bytes free",
+             (long long)nbatch, (long long)nwalkers, (long long)ndim, need, free_b);
+    g_create_err = b;
+    return EB_ERR_NOMEM;
+  }
+  eb_ctx* c = nullptr;
+  rc = eb_create(device, rows, ndim, 0, &c);
+  if (rc) return rc;
+  std::unique_ptr<eb_ctx> owner(c);
+  c->nbatch = nbatch;
+  c->bn = nwalkers;
+  c->seeds.assign(seeds, seeds + nbatch);
+  c->allow_dmma = false;  // a batch runs batch_half_step_kernel, and the initial log-probabilities the generic kernel
+  c->allow_tma = 0;
+  CREATE_CK(dev_alloc(c->seeds_dev, (size_t)nbatch * sizeof(uint64_t)));
+  CREATE_CK(cudaMemcpy(c->seeds_dev.get(), seeds, (size_t)nbatch * sizeof(uint64_t), cudaMemcpyHostToDevice));
+  *out = owner.release();
+  return EB_OK;
+}
+
+int eb_batch_rng_get(const eb_ctx* c, uint64_t* seeds, uint64_t* step) {
+  if (!c || c->nbatch == 0) return c ? EB_ERR_UNSUPPORTED : EB_ERR_INVALID;
+  if (seeds) std::copy(c->seeds.begin(), c->seeds.end(), seeds);
+  if (step) *step = c->step;
+  return EB_OK;
+}
+
+int eb_batch_rng_set(eb_ctx* c, const uint64_t* seeds, uint64_t step) {
+  if (!c) return EB_ERR_INVALID;
+  NOT_IN_CALLBACK(c);
+  if (c->nbatch == 0) FAIL(c, EB_ERR_UNSUPPORTED, "eb_batch_rng_set: not a batch context (eb_set_rng)");
+  if (!seeds) FAIL(c, EB_ERR_INVALID, "eb_batch_rng_set: null seeds");
+  if (!std::equal(c->seeds.begin(), c->seeds.end(), seeds)) {
+    CK(c, cudaSetDevice(c->device));
+    CK(c, cudaStreamSynchronize(c->st.get()));  // the split-table launches still read seeds_dev
+    CK(c, cudaMemcpy(c->seeds_dev.get(), seeds, (size_t)c->nbatch * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    c->seeds.assign(seeds, seeds + c->nbatch);
+    c->tbl_n = 0;  // the cached split tables were built under the old keys
+  }
+  c->step = step;
+  return EB_OK;
+}
+
 int eb_destroy(eb_ctx* c) {
   if (!c) return EB_OK;
   NOT_IN_CALLBACK(c);
@@ -381,6 +443,7 @@ extern "C" {
 int eb_callback_blobs(eb_ctx* c, const void* src, int64_t record_bytes, int64_t stride_bytes, int64_t m,
                       uint64_t src_stream) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_callback_blobs");
   if (!c->in_callback) FAIL(c, EB_ERR_STATE, "eb_callback_blobs: only from inside a log-probability callback");
   if (c->cb_blob_rows >= 0) FAIL(c, EB_ERR_INVALID, "eb_callback_blobs: this call's blobs were already delivered");
   if (m != c->cb_m)
@@ -465,6 +528,7 @@ static int ensure_graph_err(eb_ctx* c) {
 
 int eb_model_set_graphs(eb_ctx* c, const eb_graph* graphs, size_t n) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_model_set_graphs");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "log-probability graphs are not sharded across GPUs");
   if (!graphs || n == 0) FAIL(c, EB_ERR_INVALID, "eb_model_set_graphs: no graphs");
@@ -520,6 +584,7 @@ int eb_model_set_graphs(eb_ctx* c, const eb_graph* graphs, size_t n) {
 
 int eb_move_set_proposal(eb_ctx* c, int32_t slot, eb_proposal_fn fn, void* user, int where) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_move_set_proposal");
   NOT_IN_CALLBACK(c);
   if (slot < 0 || slot >= EB_MAX_PROPOSAL_SLOTS)
     FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal: slot must be in [0, %d) (got %d)", EB_MAX_PROPOSAL_SLOTS, slot);
@@ -550,6 +615,7 @@ static int check_graph_rows(eb_ctx* c, size_t k, const char* what, const void* p
 int eb_move_set_proposal_graphs(eb_ctx* c, int32_t slot, int draw_kind, int64_t ndraws, const eb_proposal_graph* graphs,
                                 size_t n) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_move_set_proposal_graphs");
   NOT_IN_CALLBACK(c);
   if (slot < 0 || slot >= EB_MAX_PROPOSAL_SLOTS)
     FAIL(c, EB_ERR_INVALID, "eb_move_set_proposal_graphs: slot must be in [0, %d) (got %d)", EB_MAX_PROPOSAL_SLOTS,
@@ -826,6 +892,7 @@ int eb_compute_log_prob(eb_ctx* c, const double* coords, size_t m, double* out) 
 int eb_compute_log_prob_from(eb_ctx* c, const void* coords, int64_t row_stride_bytes, int64_t m, double* out_dst,
                              uint64_t src_stream) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_compute_log_prob_from");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "eb_compute_log_prob_from: sharded ensembles take coordinates from host memory");
@@ -851,6 +918,7 @@ int eb_compute_log_prob_from(eb_ctx* c, const void* coords, int64_t row_stride_b
 int eb_compute_log_prob_blobs(eb_ctx* c, const double* coords, size_t m, double* out, void** blobs_out,
                               size_t* record_bytes) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_compute_log_prob_blobs");
   NOT_IN_CALLBACK(c);
   if (!blobs_out || !record_bytes) FAIL(c, EB_ERR_INVALID, "eb_compute_log_prob_blobs: null output");
   *blobs_out = nullptr;
@@ -983,6 +1051,7 @@ int eb_get_state(eb_ctx* c, double* coords, double* log_prob) {
 int eb_set_state_from(eb_ctx* c, const void* coords, int64_t coords_row_stride_bytes, const void* log_prob,
                       int64_t lp_stride_bytes, uint64_t src_stream) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_set_state_from");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "eb_set_state_from: sharded ensembles take their state from host memory (eb_set_state)");
@@ -1022,6 +1091,7 @@ int eb_set_state_from(eb_ctx* c, const void* coords, int64_t coords_row_stride_b
 
 int eb_get_state_to(eb_ctx* c, double* coords_dst, double* log_prob_dst) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_get_state_to");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "eb_get_state_to: sharded ensembles return their state in host memory (eb_get_state)");
@@ -1041,6 +1111,7 @@ int eb_get_state_to(eb_ctx* c, double* coords_dst, double* log_prob_dst) {
 
 int eb_set_state_blobs(eb_ctx* c, const void* blobs, size_t record_bytes) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_set_state_blobs");
   NOT_IN_CALLBACK(c);
   if (!c->have_state) FAIL(c, EB_ERR_STATE, "eb_set_state_blobs: no state set");
   if ((blobs == nullptr) != (record_bytes == 0))
@@ -1104,6 +1175,7 @@ int eb_get_state_rows(eb_ctx* c, int64_t row0, int64_t nrows, double* coords, do
 
 int eb_set_rng(eb_ctx* c, uint64_t seed, uint64_t step) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_set_rng");
   NOT_IN_CALLBACK(c);
   // the rows of a step offered again would come back with their old keys, and a new seed draws other keys: either
   // starts the running reservoir again, so that it stays the sample of one stream of steps (reservoir_plan.h)
@@ -1638,6 +1710,7 @@ int eb_histograms_config(eb_ctx* c, uint64_t every, uint32_t bins, const double*
                          int log_prob, const uint32_t* params2d, size_t nparams2d, uint32_t bins2d,
                          const double* edges2d) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_histograms_config");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
   if (bins == 0 || !outer || !edges) FAIL(c, EB_ERR_INVALID, "eb_histograms_config: bins == 0 or null buffer");
@@ -1707,6 +1780,7 @@ int eb_histograms(eb_ctx* c, uint64_t* hist, uint64_t* hist2d, uint64_t* count) 
 
 int eb_trace_config(eb_ctx* c, uint64_t every) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_trace_config");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
   CK(c, cudaSetDevice(c->device));
@@ -1778,6 +1852,7 @@ int eb_trace_best(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, u
 
 int eb_reservoir_config(eb_ctx* c, uint64_t size, uint64_t every) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_reservoir_config");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
   if (size == 0) FAIL(c, EB_ERR_INVALID, "eb_reservoir_config: size must be >= 1");
@@ -1854,6 +1929,7 @@ int eb_reservoir_read_to(eb_ctx* c, double* coords_dst, double* log_prob_dst, ui
 
 int eb_running_acf_config(eb_ctx* c, uint64_t max_lag, uint64_t every) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_running_acf_config");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running autocorrelation is not sharded across GPUs");
   if (max_lag == 0) FAIL(c, EB_ERR_INVALID, "eb_running_acf_config: max_lag must be >= 1");
@@ -1910,6 +1986,7 @@ int eb_running_acf_read(eb_ctx* c, double* rho) {
 
 int eb_window_config(eb_ctx* c, uint64_t size, uint64_t every) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_window_config");
   NOT_IN_CALLBACK(c);
   if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running window is not sharded across GPUs");
   if (size == 0) FAIL(c, EB_ERR_INVALID, "eb_window_config: size must be >= 1");
@@ -2063,6 +2140,7 @@ const char* eb_last_kernel_variant(const eb_ctx* c) { return c ? c->last_variant
 
 int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
   if (!c || !name) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_set_option");
   NOT_IN_CALLBACK(c);
   if (!strcmp(name, "debug_taps")) {
     CK(c, cudaSetDevice(c->device));
@@ -2138,6 +2216,7 @@ int eb_set_option(eb_ctx* c, const char* name, int64_t value) {
 
 int eb_debug_timeline(eb_ctx* c, int64_t* out, size_t capacity, size_t* written) {
   if (!c || !out) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_debug_timeline");
   NOT_IN_CALLBACK(c);
   if (!c->timeline) FAIL(c, EB_ERR_STATE, "eb_debug_timeline: enable with eb_set_option(\"dmma_timeline\", 1)");
   CK(c, cudaSetDevice(c->device));
@@ -2151,6 +2230,7 @@ int eb_debug_timeline(eb_ctx* c, int64_t* out, size_t capacity, size_t* written)
 int eb_debug_taps(eb_ctx* c, int64_t* partners, double* scalar, double* u_accept, int64_t* active,
                   int64_t* nactive) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_debug_taps");
   NOT_IN_CALLBACK(c);
   if (!c->debug || !c->tap_scalar) FAIL(c, EB_ERR_STATE, "eb_debug_taps: enable with eb_set_option(\"debug_taps\", 1)");
   CK(c, cudaSetDevice(c->device));
@@ -2273,6 +2353,7 @@ int eb_comm_id(char id[EB_COMM_ID_BYTES]) { return comm_unique_id(id) ? EB_ERR_C
 
 int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nranks, int mode) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_comm_init");
   NOT_IN_CALLBACK(c);
   if (c->have_model && c->model.kind == MODEL_EXTERNAL && nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
@@ -2293,6 +2374,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
 
 int eb_comm_export(eb_ctx* c, char blob[EB_IPC_BLOB_BYTES]) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_comm_export");
   NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   if (comm_export(c->comm, blob)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
@@ -2301,6 +2383,7 @@ int eb_comm_export(eb_ctx* c, char blob[EB_IPC_BLOB_BYTES]) {
 
 int eb_comm_probe(eb_ctx* c, int peer, int what, double* gbs) {
   if (!c || !gbs) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_comm_probe");
   NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   if (comm_probe(c->comm, peer, what, c->D, c->st.get(), gbs)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
@@ -2309,6 +2392,7 @@ int eb_comm_probe(eb_ctx* c, int peer, int what, double* gbs) {
 
 int eb_comm_import(eb_ctx* c, const char* blobs) {
   if (!c) return EB_ERR_INVALID;
+  NOT_BATCH(c, "eb_comm_import");
   NOT_IN_CALLBACK(c);
   CK(c, cudaSetDevice(c->device));
   if (comm_import(c->comm, blobs)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());

@@ -54,7 +54,13 @@ struct eb_ctx {
   int64_t N = 0;
   int D = 0;
   uint64_t seed = 0, step = 0;
+  // a batch context (eb_create_batch): nbatch independent ensembles of bn walkers stacked as the N = nbatch * bn
+  // rows of the live state, ensemble k in rows [k bn, (k + 1) bn), each drawing under its own key seeds[k] (the
+  // step counter is shared); 0 for a single ensemble
+  int64_t nbatch = 0, bn = 0;
+  std::vector<uint64_t> seeds;
   StreamPtr st;  // declared first among the owners: destroyed after the events and the memory
+  DevPtr<uint64_t> seeds_dev;  // [nbatch]
   EventPtr ev0, ev1;
 
   DevPtr<double> coords;  // [N, D], then the peer-memory barrier flags (exported to the peers, comm.h)
@@ -280,6 +286,12 @@ enum { CB_STEP = 0, CB_SET_STATE = 1, CB_COMPUTE = 2 };
                                       : "engine is inside a user proposal";       \
       return EB_ERR_STATE;                                                        \
     }                                                                             \
+  } while (0)
+
+// an entry point without a meaning for a batch context (eb_create_batch)
+#define NOT_BATCH(ctx, who)                                                                               \
+  do {                                                                                                    \
+    if ((ctx)->nbatch > 0) FAIL(ctx, EB_ERR_UNSUPPORTED, "%s is not available on a batch context", who); \
   } while (0)
 
 #define FAIL(ctx, code, ...)                      \

@@ -104,7 +104,38 @@ struct ExternalBufs {
   const double* lp;  // accept: [a_count] log-probabilities of the proposals
 };
 
+// one half-step of every ensemble of a batch context (batch.cu): K ensembles of n walkers stacked as K n rows.  Set
+// sizes depend on n and the split count only, so every ensemble has the same active set [a_start, a_start + a_count)
+// of its own segment of the split table, and the half-step covers K a_count active ranks.
+struct BatchArgs {
+  double* coords;  // [K n, D]
+  double* logp;    // [K n]
+  uint8_t* accepted;
+  unsigned long long* nacc;
+  int* status;
+  const int32_t* order;   // [K, n] this step's split tables: ensemble k's walker ids (0 .. n - 1) at k n
+  const uint64_t* seeds;  // [K] the Philox key of each ensemble
+  int64_t n;
+  int64_t K;
+  int D;
+  int split;
+  int a_start, a_count;
+  int c_start[3], c_count[3];  // snooker: the three complement sets
+  uint64_t step;
+  double p0, p1;  // as HalfStepArgs
+  ModelDev model;
+  const double* qbuf;  // accept phase of MODEL_EXTERNAL: [K a_count, D] the proposals the propose phase staged
+};
+
 // ---- kernel launchers (implemented in the .cu files) ----------------------
+// batch.cu: the split tables of nsteps_chunk steps of a batch, [nsteps_chunk, K, n]; block (k, s) runs
+// split_table_kernel's permutation of ensemble k under seeds[k] at step step0 + s
+cudaError_t launch_batch_split_tables(int32_t* order, const StepInfo* info_dev, int nsteps_chunk, int64_t n, int64_t K,
+                                      const uint64_t* seeds, uint64_t step0, cudaStream_t st);
+// batch.cu: half_step_generic_kernel's per-walker body for the K a_count active ranks of a batch half-step.  A
+// registered model runs move_kind STRETCH / DE / SNOOKER fused; MODEL_EXTERNAL runs them as the propose phase (row
+// k a_count + i of ext.q, ext.f) and MOVE_PRECOMPUTED as the accept phase (a.qbuf, ext.f, ext.lp)
+cudaError_t launch_batch_half_step(int move_kind, const BatchArgs& a, const ExternalBufs& ext, cudaStream_t st);
 // ranges (nullable): [nsteps_chunk, MAX_SPLITS] int2 = active ranks of each set owned by walkers [w_lo, w_hi)
 cudaError_t launch_split_tables(int32_t* order, const StepInfo* info_dev, int nsteps_chunk, int64_t N,
                                 uint64_t seed, uint64_t step0, int64_t w_lo, int64_t w_hi, int2* ranges,

@@ -84,6 +84,16 @@ int check_proposal_graphs(eb_ctx* c, const eb_move& m) {
 
 int build_schedule(eb_ctx* c, const eb_move* moves, size_t nmoves, Schedule& s) {
   if (!moves || nmoves == 0) FAIL(c, EB_ERR_INVALID, "eb_step: empty move schedule");
+  if (c->nbatch > 0) {
+    // one red-blue move for every ensemble: a schedule would pick a move, and with it a split count, per ensemble
+    const eb_move& m = moves[0];
+    if (nmoves != 1 || (m.kind != EB_MOVE_STRETCH && m.kind != EB_MOVE_DE && m.kind != EB_MOVE_SNOOKER))
+      FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: a batch runs exactly one StretchMove, DEMove or DESnookerMove");
+    if (m.nsplits < 2 || m.nsplits > MAX_SPLITS || m.nsplits > c->bn)
+      FAIL(c, EB_ERR_UNSUPPORTED, "eb_step: nsplits must be in [2, min(%d, nwalkers)] (got %d)", MAX_SPLITS, m.nsplits);
+    if (m.kind == EB_MOVE_DE && c->bn - (c->bn + m.nsplits - 1) / m.nsplits < 2)
+      FAIL(c, EB_ERR_INVALID, "eb_step: DEMove needs at least 2 complement walkers");
+  }
   s.moves.assign(moves, moves + nmoves);
   double tot = 0.0;
   s.gform.assign(nmoves, 0);
@@ -310,7 +320,7 @@ bool dmma_eligible(const eb_ctx* c, const eb_move& mv) {
 }
 
 int check_walker_count(eb_ctx* c, const eb_move& mv) {
-  if (c->N < 2 * (int64_t)c->D && !mv.live_dangerously)  // red_blue.py:64-70
+  if ((c->nbatch > 0 ? c->bn : c->N) < 2 * (int64_t)c->D && !mv.live_dangerously)  // red_blue.py:64-70
     FAIL(c, EB_ERR_FEW_WALKERS,
          "It is unadvisable to use a red-blue move with fewer walkers than twice the number of dimensions.");
   return EB_OK;
@@ -394,6 +404,60 @@ int launch_step_generic(eb_ctx* c, const eb_move& mv, uint64_t step, size_t tbl,
     if (comm_after_split(c->comm, c->st.get(), c->status_dev.get(), launches))
       FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
   }
+  return EB_OK;
+}
+
+// the P half-steps of one step of every ensemble of a batch context: one launch each, or under a log-probability
+// function the propose launch, the function on the [K, a_count] block, and the accept launch
+int launch_step_batch(eb_ctx* c, const eb_move& mv, uint64_t step, size_t tbl, uint64_t& launches) {
+  int rc = check_walker_count(c, mv);
+  if (rc) return rc;
+  int start[MAX_SPLITS + 1];
+  split_starts(c->bn, mv.nsplits, start);
+  const HalfStepArgs m = move_args(c, mv);
+  const bool external = c->model.kind == MODEL_EXTERNAL;
+  const ExternalBufs ext{c->qbuf.get(), c->ext_f.get(), c->ext_lp.get()};
+  for (int split = 0; split < mv.nsplits; ++split) {
+    BatchArgs a{};
+    a.coords = c->coords.get();
+    a.logp = c->logp.get();
+    a.accepted = c->accepted.get();
+    a.nacc = c->nacc.get();
+    a.status = c->status_dev.get();
+    a.order = c->order.get() + tbl * (size_t)c->N;
+    a.seeds = c->seeds_dev.get();
+    a.n = c->bn;
+    a.K = c->nbatch;
+    a.D = c->D;
+    a.split = split;
+    a.a_start = start[split];
+    a.a_count = start[split + 1] - start[split];
+    int k = 0;
+    for (int j = 0; j < mv.nsplits && k < 3; ++j) {
+      if (j == split) continue;
+      a.c_start[k] = start[j];
+      a.c_count[k] = start[j + 1] - start[j];
+      ++k;
+    }
+    a.step = step;
+    a.p0 = m.p0;
+    a.p1 = m.p1;
+    a.model = c->model;
+    a.qbuf = c->qbuf.get();
+    CK(c, launch_batch_half_step(mv.kind, a, ext, c->st.get()));
+    ++launches;
+    if (!external) continue;
+    c->cb_phase = CB_STEP;
+    c->cb_split = split;
+    rc = run_callback(c, c->qbuf.get(), c->nbatch * a.a_count, c->ext_lp.get(), false);
+    if (rc) return rc;
+    CK(c, launch_batch_half_step(MOVE_PRECOMPUTED, a, ext, c->st.get()));
+    ++launches;
+  }
+  if (external)
+    note_callback(c);
+  else
+    note_kernel(c, "batch", "batch G=%d K=%lld", lanes_per_walker(c->D), (long long)c->nbatch);
   return EB_OK;
 }
 
@@ -847,6 +911,12 @@ int upload_chunk(eb_ctx* c, const Chunk& ch, uint64_t& launches) {
     CK(c, cudaMemcpyAsync(c->info_dev.get(), c->info_host.get(), ch.build * sizeof(StepInfo), cudaMemcpyHostToDevice,
                           c->st.get()));
     const Comm& cm = c->comm;
+    if (c->nbatch > 0) {
+      CK(c, launch_batch_split_tables(c->order.get(), c->info_dev.get(), (int)ch.build, c->bn, c->nbatch,
+                                      c->seeds_dev.get(), c->step, c->st.get()));
+      ++launches;
+      return EB_OK;
+    }
     CK(c, launch_split_tables(c->order.get(), c->info_dev.get(), (int)ch.build, c->N, c->seed, c->step,
                               cm.rows_per_rank * cm.rank, cm.rows_per_rank * (cm.rank + 1),
                               cm.nranks > 1 ? cm.ranges : nullptr, c->st.get()));
@@ -994,7 +1064,8 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
             rc = launch_step_user_mh(c, mv, c->step, launches);
             break;
           default:
-            rc = launch_step_generic(c, mv, c->step, tbl, launches);
+            rc = c->nbatch > 0 ? launch_step_batch(c, mv, c->step, tbl, launches)
+                               : launch_step_generic(c, mv, c->step, tbl, launches);
         }
         if (rc) return rc;
       }
@@ -1291,6 +1362,7 @@ int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
   if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
+  NOT_BATCH(c, "eb_step_store_chain");
   if (!ch) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: null chain");
   if (ch->ring) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: a running window's ring is written by its engine only");
   if (ch->device != c->device || ch->N != c->N || ch->D != c->D)

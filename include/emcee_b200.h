@@ -116,6 +116,21 @@ int eb_device_count(void);
  * engine for an [nwalkers, ndim] float64 ensemble on CUDA device `device`, its
  * Philox key = seed, step counter = 0. */
 int eb_create(int device, int64_t nwalkers, int64_t ndim, uint64_t seed, eb_ctx** out);
+/* a batch context: nbatch independent [nwalkers, ndim] ensembles stacked as the nbatch * nwalkers rows of one
+ * engine, ensemble k in rows [k nwalkers, (k + 1) nwalkers), with Philox key seeds[k] (host, read during the call)
+ * and one step counter.  Ensemble k of a batch advances exactly as an eb_create engine of key seeds[k] running the
+ * generic kernel.  Every call that takes or returns rows (eb_set_state, eb_get_state, eb_compute_log_prob,
+ * eb_step, eb_step_store, eb_get_naccepted, ...) sees the nbatch * nwalkers rows; a callback model is called once
+ * per half-step with the [nbatch, m] block of all ensembles' proposals, ensemble-major (m = the split's size).
+ * The schedule is one EB_MOVE_STRETCH / EB_MOVE_DE / EB_MOVE_SNOOKER entry (EB_ERR_UNSUPPORTED otherwise).  Calls
+ * without a meaning for a batch return EB_ERR_UNSUPPORTED: device chains, running statistics, options and debug
+ * taps, user proposals, graphs, blobs, CUDA-array state and results, eb_set_rng and communicators.
+ * EB_ERR_INVALID for nbatch * nwalkers >= 2^31; EB_ERR_NOMEM when the rows do not fit in free device memory. */
+int eb_create_batch(int device, int64_t nbatch, int64_t nwalkers, int64_t ndim, const uint64_t* seeds, eb_ctx** out);
+/* the Philox keys seeds[nbatch] and the step counter of a batch context (either output may be NULL); setting them
+ * resumes the batch there.  EB_ERR_UNSUPPORTED on a single-ensemble context. */
+int eb_batch_rng_get(const eb_ctx* ctx, uint64_t* seeds, uint64_t* step);
+int eb_batch_rng_set(eb_ctx* ctx, const uint64_t* seeds, uint64_t step);
 int eb_destroy(eb_ctx* ctx);
 /* message of the last failing call on ctx (ctx == NULL: last eb_create failure
  * of this thread).  Pointer valid until the next call on the same ctx. */
