@@ -227,6 +227,16 @@ _SIGNATURES = {
     "eb_get_state_to": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "eb_compute_log_prob_from": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_uint64]),
     "eb_chain_read_to": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "eb_chain_read_segments_to": (
+        C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "eb_chain_autocorr_segments": (C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_uint64, _dp]),
+    "eb_chain_select_segments": (
+        C.c_int,
+        [C.c_void_p, C.c_int64, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64), C.c_size_t, _dp,
+         C.POINTER(C.c_uint8), C.POINTER(C.c_uint32)],
+    ),
+    "eb_chain_moments_segments": (
+        C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_uint64, _dp, _dp, C.POINTER(C.c_uint64)]),
 }
 
 _lib = None
@@ -971,41 +981,68 @@ class Chain(object):
             None if x is None else C.c_void_p(x._ptr), None if lp is None else C.c_void_p(lp._ptr)))
         return x, lp
 
+    def read_segments_to(self, nseg, first, stride, count, coords=True, log_prob=True):
+        """:meth:`read_to` in the per-segment layout (``eb_chain_read_segments_to``): the walkers are ``nseg``
+        segments of ``nw = nwalkers / nseg``, and the result is ``(coords[nseg, count * nw, ndim] or None,
+        log_prob[nseg, count * nw] or None)`` as :class:`DeviceArray` s."""
+        nseg = int(nseg)
+        nw = self.nwalkers // nseg
+        x = DeviceArray((nseg, count * nw, self.ndim), self.device) if coords else None
+        lp = DeviceArray((nseg, count * nw), self.device) if log_prob else None
+        self._check(lib().eb_chain_read_segments_to(
+            self._h, nseg, int(first), int(stride), int(count),
+            None if x is None else C.c_void_p(x._ptr), None if lp is None else C.c_void_p(lp._ptr)))
+        return x, lp
+
     def accepted(self):
         out = np.empty(self.nwalkers)
         self._check(lib().eb_chain_accepted(self._h, _as_dp(out)))
         return out
 
-    def autocorr_function(self, first, stride, count):
+    def autocorr_function(self, first, stride, count, nseg=1):
         """Walker-averaged normalised autocorrelation function ``[count, ndim]`` of the stored slice
-        (``eb_chain_autocorr``; the same numbers as :meth:`Engine.autocorr_function` of its host copy)."""
-        out = np.empty((self.ndim, int(count)), dtype=np.float64)
-        self._check(lib().eb_chain_autocorr(self._h, int(first), int(stride), int(count), _as_dp(out)))
-        return np.ascontiguousarray(out.T)
+        (``eb_chain_autocorr``; the same numbers as :meth:`Engine.autocorr_function` of its host copy).  With
+        ``nseg > 1``, one per segment of ``nwalkers / nseg`` walkers: ``[nseg, count, ndim]``, row ``k`` equal to
+        the function of segment ``k`` stored alone (``eb_chain_autocorr_segments``)."""
+        nseg = int(nseg)
+        out = np.empty((nseg, self.ndim, int(count)), dtype=np.float64)
+        self._check(lib().eb_chain_autocorr_segments(self._h, nseg, int(first), int(stride), int(count),
+                                                     _as_dp(out)))
+        out = np.ascontiguousarray(np.swapaxes(out, 1, 2))
+        return out[0] if nseg == 1 else out
 
-
-    def select(self, what, first, stride, count, ranks):
+    def select(self, what, first, stride, count, ranks, nseg=1):
         """``(values[len(ranks), D], has_nan[D], passes)``: the exact order statistics at 0-based ``ranks`` of
         each parameter's ``count * nwalkers`` values in the stored slice (``eb_chain_select``); ``what`` is
-        ``"chain"`` (D = ndim) or ``"log_prob"`` (D = 1)."""
+        ``"chain"`` (D = ndim) or ``"log_prob"`` (D = 1).  With ``nseg > 1``, those of each segment of
+        ``nw = nwalkers / nseg`` walkers (``count * nw`` values): ``(values[nseg, len(ranks), D],
+        has_nan[nseg, D], passes)`` (``eb_chain_select_segments``)."""
+        nseg = int(nseg)
         ranks = np.ascontiguousarray(ranks, dtype=np.uint64)
         D = self.ndim if what == "chain" else 1
-        out = np.empty((ranks.size, D))
-        has_nan = np.zeros(D, dtype=np.uint8)
+        out = np.empty((nseg, ranks.size, D))
+        has_nan = np.zeros((nseg, D), dtype=np.uint8)
         passes = C.c_uint32()
-        self._check(lib().eb_chain_select(
-            self._h, EB_CHAIN_COORDS if what == "chain" else EB_CHAIN_LOG_PROB, int(first), int(stride), int(count),
-            ranks.ctypes.data_as(C.POINTER(C.c_uint64)), ranks.size, _as_dp(out),
+        self._check(lib().eb_chain_select_segments(
+            self._h, nseg, EB_CHAIN_COORDS if what == "chain" else EB_CHAIN_LOG_PROB, int(first), int(stride),
+            int(count), ranks.ctypes.data_as(C.POINTER(C.c_uint64)), ranks.size, _as_dp(out),
             has_nan.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(passes)))
+        if nseg == 1:
+            return out[0], has_nan[0].astype(bool), int(passes.value)
         return out, has_nan.astype(bool), int(passes.value)
 
-    def moments(self, first, stride, count):
-        """``(mean[ndim], cov[ndim, ndim], n)`` of the stored slice (``eb_chain_moments``)."""
-        mean = np.empty(self.ndim)
-        cov = np.empty((self.ndim, self.ndim))
+    def moments(self, first, stride, count, nseg=1):
+        """``(mean[ndim], cov[ndim, ndim], n)`` of the stored slice (``eb_chain_moments``).  With ``nseg > 1``,
+        those of each segment of ``nwalkers / nseg`` walkers: ``(mean[nseg, ndim], cov[nseg, ndim, ndim], n)``
+        with ``n`` the samples of one segment (``eb_chain_moments_segments``)."""
+        nseg = int(nseg)
+        shape = () if nseg == 1 else (nseg,)
+        mean = np.empty(shape + (self.ndim,))
+        cov = np.empty(shape + (self.ndim, self.ndim))
         n = C.c_uint64()
-        self._check(lib().eb_chain_moments(self._h, int(first), int(stride), int(count), _as_dp(mean), _as_dp(cov),
-                                           C.byref(n)))
+        fn = lib().eb_chain_moments if nseg == 1 else lib().eb_chain_moments_segments
+        args = () if nseg == 1 else (nseg,)
+        self._check(fn(self._h, *args, int(first), int(stride), int(count), _as_dp(mean), _as_dp(cov), C.byref(n)))
         return mean, cov, int(n.value)
 
     def histogram(self, what, first, stride, count, bins, outer, edges):

@@ -16,7 +16,7 @@ import operator
 import numpy as np
 
 from . import _lib
-from .backend import Backend
+from .backend import Backend, DeviceBackend, _check_summary_name, slice_plan
 from .ensemble import _NOT_INDEPENDENT, _seed_from_numpy
 from .models import CallbackFunction, CudaGraphFunction, DeviceModel, HostFunction
 from .moves import DEMove, DESnookerMove, StretchMove
@@ -81,9 +81,16 @@ class BatchSampler(object):
     ``seeds`` is a sequence of ``nbatch`` integers, or one integer ``s`` for ``s, s + 1, ..., s + nbatch - 1``;
     ``None`` derives ``s`` from numpy's global state.  States are ``State(coords[nbatch, nwalkers, ndim],
     log_prob[nbatch, nwalkers])``, chains ``[n, nbatch, nwalkers, ndim]``; the reference's errors apply per ensemble
-    with ``EnsembleSampler``'s types and messages."""
+    with ``EnsembleSampler``'s types and messages.
 
-    def __init__(self, nbatch, nwalkers, ndim, log_prob_fn, moves=None, *, seeds=None, device=0):
+    ``backend`` stores the chain: ``None`` for a host :class:`~emcee_b200.backends.Backend`, or a
+    :class:`~emcee_b200.DeviceBackend` on the sampler's device, which keeps it in GPU memory (a stored step is one
+    copy inside HBM) and summarises every ensemble there: :meth:`get_percentile`, :meth:`get_moments` and
+    :meth:`get_autocorr_time` read the chain where it is.  The backend holds the ensembles stacked, ``nbatch *
+    nwalkers`` walkers; an initialised one of that shape with stored steps continues its run (``random_state`` and
+    ``run_mcmc(None, ...)`` resume from its last sample)."""
+
+    def __init__(self, nbatch, nwalkers, ndim, log_prob_fn, moves=None, *, seeds=None, device=0, backend=None):
         self.nbatch, self.nwalkers, self.ndim = operator.index(nbatch), operator.index(nwalkers), operator.index(ndim)
         if self.nbatch < 1:
             raise ValueError("nbatch must be >= 1, got {0}".format(self.nbatch))
@@ -119,9 +126,21 @@ class BatchSampler(object):
             box = m.bounds(self.ndim)
             if box is not None:
                 self._engine.set_bounds(*box)
-        self.backend = Backend()
+        self.backend = Backend() if backend is None else backend
         self._previous_state = None
-        self.reset()
+        if isinstance(self.backend, DeviceBackend) and self.backend.device != device:
+            raise ValueError("the backend keeps its chain on device {0}, the sampler runs on device {1}".format(
+                self.backend.device, device))
+        if not self.backend.initialized:
+            self.reset()
+        else:
+            shape = (self.nbatch * self.nwalkers, self.ndim)
+            if self.backend.shape != shape:
+                raise ValueError("the shape of the backend ({0}) is incompatible with the shape of the batch ({1}: "
+                                 "nbatch * nwalkers walkers)".format(self.backend.shape, shape))
+            self.random_state = self.backend.random_state
+            if self.backend.iteration > 0:
+                self._previous_state = self.get_last_sample()
 
     # ------------------------------------------------------------------ state
     @property
@@ -200,6 +219,7 @@ class BatchSampler(object):
 
     def _steps(self, sched, iterations, thin_by, store, bulk):
         eng, b = self._engine, self.backend
+        device_store = isinstance(b, DeviceBackend)
         if bulk:
             total = iterations * thin_by
             if total > 0:
@@ -207,7 +227,10 @@ class BatchSampler(object):
                     k0, k1 = b.iteration, b.iteration + iterations
                     step0 = eng.get_rng()[1]
                     try:
-                        eng.step_store(sched, total, thin_by, b.chain[k0:k1], b.log_prob[k0:k1], b.accepted)
+                        if device_store:
+                            eng.step_store_chain(sched, total, thin_by, b._ch, k0)
+                        else:
+                            eng.step_store(sched, total, thin_by, b.chain[k0:k1], b.log_prob[k0:k1], b.accepted)
                     except BaseException:
                         self._stored_before_failure(step0, thin_by, k0)
                         raise
@@ -221,7 +244,10 @@ class BatchSampler(object):
         for _ in counter:
             if store:
                 k = b.iteration
-                eng.step_store(sched, thin_by, thin_by, b.chain[k : k + 1], b.log_prob[k : k + 1], b.accepted)
+                if device_store:
+                    eng.step_store_chain(sched, thin_by, thin_by, b._ch, k)
+                else:
+                    eng.step_store(sched, thin_by, thin_by, b.chain[k : k + 1], b.log_prob[k : k + 1], b.accepted)
                 b.iteration = k + 1
                 b.random_state = self.random_state
             else:
@@ -263,13 +289,30 @@ class BatchSampler(object):
         """``[nbatch, nwalkers]``."""
         return (self.backend.accepted / float(self.backend.iteration)).reshape(self.nbatch, self.nwalkers)
 
-    def get_value(self, name, flat=False, thin=1, discard=0):
+    def get_value(self, name, flat=False, thin=1, discard=0, cuda=False):
         """``[n, nbatch, nwalkers, ...]``, or with ``flat`` one flat sample per ensemble, ``[nbatch, n * nwalkers,
-        ...]``: row ``k`` is what ``get_value(name, flat=True, ...)`` of ensemble ``k``'s twin returns."""
+        ...]``: row ``k`` is what ``get_value(name, flat=True, ...)`` of ensemble ``k``'s twin returns.  ``cuda=True``
+        (a :class:`~emcee_b200.DeviceBackend` only): the same values as a :class:`~emcee_b200.DeviceArray`, copied
+        inside the GPU's memory."""
+        K, N = self.nbatch, self.nwalkers
+        if cuda:
+            b = self.backend
+            if not isinstance(b, DeviceBackend):
+                raise TypeError("cuda=True reads a DeviceBackend; this batch stores into {0}".format(type(b).__name__))
+            ch, (first, stride, count) = b._plan(discard, thin)
+            if name not in ("chain", "log_prob"):
+                raise AttributeError(name)
+            want_chain = name == "chain"
+            if flat:
+                x, lp = ch.read_segments_to(K, first, stride, count, coords=want_chain, log_prob=not want_chain)
+                return x if want_chain else lp
+            shape = (count, K, N) + ((self.ndim,) if want_chain else ())
+            x, lp = ch.read_to(first, stride, count, shape if want_chain else None, None if want_chain else shape)
+            return x if want_chain else lp
         v = self.backend.get_value(name, thin=thin, discard=discard)
-        v = v.reshape((v.shape[0], self.nbatch, self.nwalkers) + v.shape[2:])
+        v = v.reshape((v.shape[0], K, N) + v.shape[2:])
         if flat:
-            v = np.swapaxes(v, 0, 1).reshape((self.nbatch, v.shape[0] * self.nwalkers) + v.shape[3:])
+            v = np.swapaxes(v, 0, 1).reshape((K, v.shape[0] * N) + v.shape[3:])
         return v
 
     def get_chain(self, **kwargs):
@@ -278,27 +321,79 @@ class BatchSampler(object):
     def get_log_prob(self, **kwargs):
         return self.get_value("log_prob", **kwargs)
 
+    def get_percentile(self, q, discard=0, thin=1, name="chain"):
+        """``[nbatch] + np.percentile(flat_k, q, axis=0).shape``: row ``k`` is ``np.percentile(get_value(name,
+        flat=True, discard=discard, thin=thin)[k], q, axis=0)``, equal with ``==``.  With a ``DeviceBackend`` the
+        exact order statistics of every ensemble are selected on the GPU in the same passes
+        (``eb_chain_select_segments``) and numpy's interpolation runs on the host; a bad ``q`` raises numpy's
+        exception before any device work, an empty slice numpy's error for one."""
+        from .summary import percentile_finish, percentile_ranks
+
+        _check_summary_name(name)
+        b, K = self.backend, self.nbatch
+        if not isinstance(b, DeviceBackend):
+            flat = self.get_value(name, flat=True, discard=discard, thin=thin)
+            return np.array([np.percentile(flat[k], q, axis=0) for k in range(K)])
+        ch, (first, stride, count) = b._plan(discard, thin)
+        plan = percentile_ranks(q, count * self.nwalkers)
+        shape = (0, self.ndim) if name == "chain" else (0,)
+        if count == 0:  # numpy's own result, or error, for an empty slice
+            return np.array([np.percentile(np.empty(shape), q, axis=0) for _ in range(K)])
+        if plan.ranks.size == 0:
+            return np.array([percentile_finish(plan, np.empty(shape)) for _ in range(K)])
+        stats, has_nan, _ = ch.select(name, first, stride, count, plan.ranks, nseg=K)
+        stats = stats.reshape((K, plan.ranks.size) + (() if name == "log_prob" else (self.ndim,)))
+        has_nan = has_nan.reshape((K,) + (() if name == "log_prob" else (self.ndim,)))
+        return np.array([percentile_finish(plan, stats[k], has_nan[k]) for k in range(K)])
+
+    def get_moments(self, discard=0, thin=1):
+        """``(mean[nbatch, ndim], cov[nbatch, ndim, ndim], n)``: row ``k`` is ``np.mean(axis=0)`` /
+        ``np.cov(rowvar=False)`` of ``get_chain(flat=True, discard=discard, thin=thin)[k]``, ``n`` the samples of one
+        ensemble; NaN for an empty slice.  With a ``DeviceBackend`` the sums of every ensemble are formed on the GPU
+        in one pass (``eb_chain_moments_segments``); ``ndim`` up to 1024."""
+        b, K, D = self.backend, self.nbatch, self.ndim
+        if isinstance(b, DeviceBackend):
+            ch, (first, stride, count) = b._plan(discard, thin)
+            mean, cov, n = ch.moments(first, stride, count, nseg=K)
+            return mean.reshape(K, D), cov.reshape(K, D, D), n
+        flat = self.get_chain(flat=True, discard=discard, thin=thin)
+        n = flat.shape[1]
+        if n == 0:
+            return np.full((K, D), np.nan), np.full((K, D, D), np.nan), 0
+        mean = np.array([np.mean(flat[k], axis=0) for k in range(K)])
+        cov = np.array([np.cov(flat[k], rowvar=False).reshape(D, D) for k in range(K)])
+        return mean, cov, n
+
     def get_autocorr_time(self, discard=0, thin=1, c=5, tol=50, quiet=False):
         """``tau[nbatch, ndim]``: row ``k`` is ``thin * autocorr.integrated_time(get_chain(discard=discard,
         thin=thin)[:, k], c=c, tol=tol, quiet=quiet)``.  When the chain of any ensemble is shorter than ``tol``
         times its estimate, one :class:`~emcee_b200.autocorr.AutocorrError` (with ``quiet``: one warning) names
-        those ensembles, and its ``tau`` holds every row's estimate."""
+        those ensembles, and its ``tau`` holds every row's estimate.  With a ``DeviceBackend`` the autocorrelation
+        functions of every ensemble come from one call on the GPU, where the chain is
+        (``eb_chain_autocorr_segments``), each bit-identical to that ensemble's own ``DeviceBackend``'s."""
         from . import autocorr
 
-        x = self.get_chain(discard=discard, thin=thin)
-        taus = np.empty((self.nbatch, self.ndim))
-        failed, first = [], None
-        for k in range(self.nbatch):
+        K = self.nbatch
+        if isinstance(self.backend, DeviceBackend):
+            ch, (first, stride, count) = self.backend._plan(discard, thin)
+            rho = ch.autocorr_function(first, stride, count, nseg=K).reshape(K, count, self.ndim)
+            estimate = lambda k: autocorr.integrated_time_from_acf(rho[k], c=c, tol=tol, quiet=False)
+        else:
+            x = self.get_chain(discard=discard, thin=thin)
+            estimate = lambda k: autocorr.integrated_time(x[:, k], c=c, tol=tol, quiet=False)
+        taus = np.empty((K, self.ndim))
+        failed, first_msg = [], None
+        for k in range(K):
             try:
-                taus[k] = autocorr.integrated_time(x[:, k], c=c, tol=tol, quiet=False)
+                taus[k] = estimate(k)
             except autocorr.AutocorrError as e:
                 taus[k] = e.tau
                 failed.append(k)
-                first = first or str(e)
+                first_msg = first_msg or str(e)
         taus *= thin
         if failed:
             msg = "The autocorrelation estimate of ensemble(s) {0} is unreliable. First of them:\n{1}".format(
-                failed, first)
+                failed, first_msg)
             if not quiet:
                 raise autocorr.AutocorrError(taus, msg)
             logger.warning(msg)

@@ -26,6 +26,23 @@ inline size_t acf_slab_walkers(size_t n_t, size_t nw, size_t nd) {
   return wb < 1 ? 1 : (wb > nw ? nw : wb);
 }
 
+// Walkers per slab of a chain of nseg segments (ensembles) of seg_w = nw / nseg walkers each: whole segments, as many
+// as ~ACF_SLAB_BYTES of scratch holds, when one segment fits; otherwise the slab acf_slab_walkers gives one segment
+// alone, so that a segment is split exactly as the chain of that ensemble alone would be.  nseg = 1: acf_slab_walkers.
+inline size_t acf_segment_slab_walkers(size_t n_t, size_t nw, size_t nd, size_t nseg) {
+  const size_t seg_w = nw / nseg;
+  const size_t one = acf_slab_walkers(n_t, seg_w, nd);
+  if (one < seg_w) return one;
+  return acf_slab_walkers(n_t, nw, nd) / seg_w * seg_w;
+}
+
+// Walkers of the slab starting at walker w0 (slabs of wb walkers from acf_segment_slab_walkers): a slab of whole
+// segments stops at the chain's end, a slab inside one segment at that segment's end.
+inline size_t acf_slab_next(size_t w0, size_t nw, size_t seg_w, size_t wb) {
+  const size_t end = wb >= seg_w ? nw : (w0 / seg_w + 1) * seg_w;
+  return wb < end - w0 ? wb : end - w0;
+}
+
 // Grids of the kernels launch_acf_slab runs over a slab of S = wb * nd series of n_t samples.  Every grid is 1-D,
 // on x (limit 2^31 - 1), so the series and parameter counts are bounded by memory, not by grid y's 65 535.
 struct AcfGrid {
@@ -37,10 +54,12 @@ struct AcfGrid {
   uint64_t load_blocks;         //   ... times ceil(S / 32) along the series: CTA k = series tile * load_tiles_t + t tile
   uint64_t global_blocks;       // fft_global_stage_kernel: S * M / 2 butterflies, 256 per CTA
   uint64_t lag_tiles;           // acf_accumulate_kernel: ceil(n_t / 256) tiles of 256 lags ...
-  uint64_t accumulate_blocks;   //   ... times nd: CTA k = parameter * lag_tiles + lag tile
+  uint64_t accumulate_blocks;   //   ... times nd times the segments the slab holds: CTA k = (segment * nd + parameter)
+                                //   * lag_tiles + lag tile
 };
 
-inline AcfGrid acf_grid(uint64_t n_t, uint64_t wb, uint64_t nd, int M) {
+// nks: the segments the slab's walkers belong to (1 for a single ensemble)
+inline AcfGrid acf_grid(uint64_t n_t, uint64_t wb, uint64_t nd, int M, uint64_t nks = 1) {
   const uint64_t S = wb * nd, m = (uint64_t)M;
   AcfGrid g;
   g.B = M < ACF_BLOCK ? M : ACF_BLOCK;
@@ -51,7 +70,7 @@ inline AcfGrid acf_grid(uint64_t n_t, uint64_t wb, uint64_t nd, int M) {
   g.load_blocks = g.load_tiles_t * ((S + 31) / 32);
   g.global_blocks = (S * (m / 2) + 255) / 256;
   g.lag_tiles = (n_t + 255) / 256;
-  g.accumulate_blocks = g.lag_tiles * nd;
+  g.accumulate_blocks = g.lag_tiles * nd * nks;
   return g;
 }
 

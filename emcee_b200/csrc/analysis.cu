@@ -11,6 +11,8 @@
 //   autocorr.function_1d / integrated_time ... autocorr.py:21-46, 49-123
 #include <math.h>
 
+#include <algorithm>
+
 #include "engine.cuh"
 
 namespace eb {
@@ -290,24 +292,85 @@ __global__ void __launch_bounds__(512) fft_local_kernel(double2* __restrict__ z,
   for (int i = threadIdx.x; i < B; i += blockDim.x) base[i] = sz[i];
 }
 
-// f[d][lag] += sum over the slab's walkers (ascending) of acf[(w, d)][lag] / acf[(w, d)][0]   (autocorr.py:45,105);
-// CTA k = d * lag_tiles + lag tile
+// f[k][d][lag] += sum over the slab's walkers of segment k (ascending) of acf[(w, d)][lag] / acf[(w, d)][0]
+// (autocorr.py:45,105).  The slab holds walkers [w0, w0 + wb) of a chain of segments of seg_w walkers; CTA
+// c = (j * nd + d) * lag_tiles + lag tile serves the slab's j-th segment, k = w0 / seg_w + j.
 __global__ void acf_accumulate_kernel(const double2* __restrict__ z, int wb, int nd, int n_t, int M,
-                                      unsigned lag_tiles, double* __restrict__ f) {
-  const int d = (int)(blockIdx.x / lag_tiles);
-  const int lag = (int)(blockIdx.x - (unsigned)d * lag_tiles) * blockDim.x + threadIdx.x;
+                                      unsigned lag_tiles, int64_t seg_w, int64_t w0, double* __restrict__ f) {
+  const unsigned sd = blockIdx.x / lag_tiles;
+  const int d = (int)(sd % (unsigned)nd);
+  const int64_t k = w0 / seg_w + (int64_t)(sd / (unsigned)nd);
+  const int lag = (int)(blockIdx.x - sd * lag_tiles) * blockDim.x + threadIdx.x;
   if (lag >= n_t) return;
+  const int lo = (int)(max(k * seg_w, w0) - w0), hi = (int)(min((k + 1) * seg_w, w0 + (int64_t)wb) - w0);
   double acc = 0.0;
-  for (int w = 0; w < wb; ++w) {
+  for (int w = lo; w < hi; ++w) {
     const double2* x = z + (size_t)(w * nd + d) * M;
     acc += x[lag].x / x[0].x;
   }
-  f[(size_t)d * n_t + lag] += acc;
+  f[((size_t)k * nd + d) * n_t + lag] += acc;
 }
 
 __global__ void acf_scale_kernel(double* __restrict__ f, size_t n, double scale) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) f[i] *= scale;
+}
+
+// ===========================================================================
+// segmented moments of a stored slice: nseg ensembles of N walkers stacked in every stored step
+// ===========================================================================
+// The batch regime: many segments of a few dozen walkers in a few dimensions, where one 8 x 8 DMMA block per
+// (step, segment) would be mostly padding and launches.  One thread per (segment k, i, j) of the D x D sums, a
+// chunk of stored steps per grid row y; every sum runs in (step, walker) order, so the result does not depend on
+// the schedule.  Element (k, w, d) of stored step s is slots[s][(k * N + w) * D + d].
+
+// shift[k][d] = the mean over walkers (ascending) of stored step 0's segment k
+__global__ void moments_seg_shift_kernel(const double* const* __restrict__ slots, int64_t nseg, int64_t N, int D,
+                                         double* __restrict__ shift) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= nseg * D) return;
+  const int64_t k = e / D;
+  const int d = (int)(e - k * D);
+  const double* x = slots[0] + (size_t)k * N * D + d;
+  double acc = 0.0;
+  for (int64_t w = 0; w < N; ++w) acc += x[(size_t)w * D];
+  shift[e] = acc / (double)N;
+}
+
+// partial[y][k][D + D*D]: [sum(x - shift) | (x - shift)^T (x - shift)] of segment k over stored steps
+// [y * cs, min(count, (y + 1) * cs)); thread (k, i, j) forms S2[i][j], and S1[i] when j == i
+__global__ void __launch_bounds__(256)
+    moments_seg_partial_kernel(const double* const* __restrict__ slots, uint64_t count, uint64_t cs, int64_t nseg,
+                               int64_t N, int D, const double* __restrict__ shift, double* __restrict__ partial) {
+  const int64_t DD = (int64_t)D * D;
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= nseg * DD) return;
+  const int64_t k = e / DD;
+  const int i = (int)((e - k * DD) / D), j = (int)(e - k * DD - (int64_t)i * D);
+  const double si = shift[k * D + i], sj = shift[k * D + j];
+  const uint64_t s0 = (uint64_t)blockIdx.y * cs, s1 = min(count, s0 + cs);
+  double a1 = 0.0, a2 = 0.0;
+  for (uint64_t s = s0; s < s1; ++s) {
+    const double* x = slots[s] + (size_t)k * N * D;
+    for (int64_t w = 0; w < N; ++w) {
+      const double xi = x[(size_t)w * D + i] - si, xj = x[(size_t)w * D + j] - sj;
+      a1 += xi;
+      a2 = fma(xi, xj, a2);
+    }
+  }
+  double* out = partial + ((size_t)blockIdx.y * nseg + k) * (size_t)(D + DD);
+  if (i == j) out[i] = a1;
+  out[D + (int64_t)i * D + j] = a2;
+}
+
+// acc[k][D + D*D] = sum over the chunks (ascending) of partial[y][k][...]
+__global__ void moments_seg_reduce_kernel(const double* __restrict__ partial, uint64_t nchunks, size_t n,
+                                          double* __restrict__ acc) {
+  const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  double s = 0.0;
+  for (uint64_t y = 0; y < nchunks; ++y) s += partial[y * n + e];
+  acc[e] = s;
 }
 
 }  // namespace
@@ -368,12 +431,14 @@ cudaError_t launch_acf_twiddles(double2* tw, int M, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-// One slab: xin[n_t][S = wb * nd] (device) -> f[nd][n_t] += sum over the slab's walkers of the normalised
-// autocorrelation functions.  z: S * M complex scratch, mean: S doubles.
+// One slab, walkers [w0, w0 + wb) of a chain of segments of seg_w walkers: xin[n_t][S = wb * nd] (device) ->
+// f[k][nd][n_t] += sum over the slab's walkers of segment k of the normalised autocorrelation functions.
+// z: S * M complex scratch, mean: S doubles.
 cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, const double2* tw, double2* z,
-                            double* mean, double* f, cudaStream_t st) {
+                            double* mean, double* f, int64_t seg_w, int64_t w0, cudaStream_t st) {
   const int S = wb * nd;
-  const AcfGrid g = acf_grid(n_t, wb, nd, M);
+  const int64_t nks = (w0 + wb - 1) / seg_w - w0 / seg_w + 1;
+  const AcfGrid g = acf_grid(n_t, wb, nd, M, (uint64_t)nks);
   const int B = g.B;
   acf_mean_kernel<<<(unsigned)g.mean_blocks, 128, 0, st>>>(xin, n_t, S, mean);
   acf_load_kernel<<<(unsigned)g.load_blocks, 256, 0, st>>>(xin, mean, n_t, S, M, (unsigned)g.load_tiles_t, z);
@@ -385,7 +450,37 @@ cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, c
   fft_local_kernel<<<(unsigned)g.local_blocks, g.local_threads, smem, st>>>(z, tw, M, B);
   for (int h = B; h <= M / 2; h <<= 1)
     fft_global_stage_kernel<<<(unsigned)g.global_blocks, 256, 0, st>>>(z, tw, S, M, h, 1);
-  acf_accumulate_kernel<<<(unsigned)g.accumulate_blocks, 256, 0, st>>>(z, wb, nd, n_t, M, (unsigned)g.lag_tiles, f);
+  acf_accumulate_kernel<<<(unsigned)g.accumulate_blocks, 256, 0, st>>>(z, wb, nd, n_t, M, (unsigned)g.lag_tiles, seg_w,
+                                                                      w0, f);
+  return cudaGetLastError();
+}
+
+// chunks of stored steps the segmented moments split a slice into: about 2^19 threads in all, at most one chunk per
+// stored step, at most 65 535 (grid y) and at most 256 MiB of partial sums.  A pure function of the shape, so repeated calls are bit-identical.
+uint64_t moments_seg_chunks(uint64_t count, int64_t nseg, int D) {
+  const uint64_t per = (uint64_t)nseg * ((uint64_t)D + (uint64_t)D * D);
+  uint64_t c = (((uint64_t)1 << 19) + per - 1) / per;
+  c = std::min<uint64_t>(std::min<uint64_t>(c, 65535), ((uint64_t)1 << 25) / per);
+  return std::max<uint64_t>(1, std::min<uint64_t>(c, count));
+}
+
+// shift[nseg][D], partial[nchunks][nseg][D + D*D] and acc[nseg][D + D*D] of a slice of `count` stored steps (slots:
+// device table of count pointers)
+cudaError_t launch_moments_segments(const double* const* slots, uint64_t count, int64_t nseg, int64_t N, int D,
+                                    uint64_t nchunks, double* shift, double* partial, double* acc, cudaStream_t st) {
+  const int64_t ne = nseg * D;
+  moments_seg_shift_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>(slots, nseg, N, D, shift);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const uint64_t cs = (count + nchunks - 1) / nchunks;
+  const uint64_t ny = (count + cs - 1) / cs;
+  const int64_t nt = nseg * D * D;
+  moments_seg_partial_kernel<<<dim3((unsigned)((nt + 255) / 256), (unsigned)ny), 256, 0, st>>>(slots, count, cs, nseg,
+                                                                                             N, D, shift, partial);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const size_t n = (size_t)nseg * ((size_t)D + (size_t)D * D);
+  moments_seg_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(partial, ny, n, acc);
   return cudaGetLastError();
 }
 

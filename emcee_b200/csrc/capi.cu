@@ -1224,31 +1224,52 @@ int chain_check_slice(eb_chain* ch, const char* who, uint64_t first, uint64_t st
   return EB_OK;
 }
 
-// the device part of autocorr.integrated_time over walker slabs of ~1 GiB: fill(xin, w0, wn) enqueues
-// chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd] for every t on stream st
+// nseg segments (ensembles) of equal size: nseg >= 1 divides the chain's walkers
+int chain_check_segments(eb_chain* ch, const char* who, int64_t nseg) {
+  if (nseg < 1 || ch->N % nseg != 0)
+    FAIL(ch, EB_ERR_INVALID, "%s: nseg = %lld must be >= 1 and divide nwalkers = %lld", who, (long long)nseg,
+         (long long)ch->N);
+  return EB_OK;
+}
+
+// the device part of autocorr.integrated_time over walker slabs of ~1 GiB, for each of nseg segments (ensembles) of
+// nw / nseg walkers: acf[nseg][nd][n_t].  fill(xin, w0, wn) enqueues chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd]
+// for every t on stream st.  A slab holds whole segments, or a part of one segment split as that segment alone
+// would be (acf_grid.h), and each segment's walkers are summed in ascending order from zero, so segment k's result
+// is bit-identical to the call on segment k alone.  The scratch is one allocation, checked against the free memory.
 template <class Obj, class Fill>
-int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, size_t nd, double* acf, Fill&& fill) {
+int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, size_t nd, size_t nseg, double* acf,
+              Fill&& fill) {
   if (n_t > ((size_t)1 << 26) || nw * nd > ((size_t)1 << 31))
     FAIL(c, EB_ERR_UNSUPPORTED, "%s: chain too long (n_step <= 2^26)", who);
   const int M = acf_fft_length(n_t);
-  const size_t wb = acf_slab_walkers(n_t, nw, nd);  // slab of walkers sized to ~1 GiB of scratch
-  const size_t S = wb * nd;
-  DevPtr<double> xin, mean, f;
-  DevPtr<double2> z, tw;
-  CK(c, dev_alloc(xin, n_t * S * sizeof(double)));
-  CK(c, dev_alloc(mean, S * sizeof(double)));
-  CK(c, dev_alloc(f, nd * n_t * sizeof(double)));
-  CK(c, dev_alloc(z, S * (size_t)M * sizeof(double2)));
-  CK(c, dev_alloc(tw, (size_t)std::max(1, M / 2) * sizeof(double2)));
-  CK(c, cudaMemsetAsync(f.get(), 0, nd * n_t * sizeof(double), st));
-  CK(c, launch_acf_twiddles(tw.get(), M, st));
-  for (size_t w0 = 0; w0 < nw; w0 += wb) {
-    const size_t wn = std::min(wb, nw - w0);
-    CK(c, fill(xin.get(), w0, wn));
-    CK(c, launch_acf_slab(xin.get(), (int)n_t, (int)wn, (int)nd, M, tw.get(), z.get(), mean.get(), f.get(), st));
+  const size_t seg_w = nw / nseg;
+  const size_t wb = acf_segment_slab_walkers(n_t, nw, nd, nseg);  // slab of walkers sized to ~1 GiB of scratch
+  const size_t S = wb * nd, nf = nseg * nd * n_t;
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t b_xin = al(n_t * S * sizeof(double)), b_mean = al(S * sizeof(double)), b_f = al(nf * sizeof(double));
+  const size_t b_z = al(S * (size_t)M * sizeof(double2)), b_tw = al((size_t)std::max(1, M / 2) * sizeof(double2));
+  const size_t bytes = b_xin + b_mean + b_f + b_z + b_tw;
+  size_t free_b = 0, total_b = 0;
+  CK(c, cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > free_b) FAIL(c, EB_ERR_NOMEM, "%s: %zu bytes of scratch, %zu bytes free", who, bytes, free_b);
+  DevPtr<char> scratch;
+  CK_NOMEM(c, dev_alloc(scratch, bytes), "%s: allocating %zu bytes of scratch failed (%s)", who, bytes,
+           cudaGetErrorString(alloc_err));
+  double* xin = reinterpret_cast<double*>(scratch.get());
+  double* mean = reinterpret_cast<double*>(scratch.get() + b_xin);
+  double* f = reinterpret_cast<double*>(scratch.get() + b_xin + b_mean);
+  double2* z = reinterpret_cast<double2*>(scratch.get() + b_xin + b_mean + b_f);
+  double2* tw = reinterpret_cast<double2*>(scratch.get() + b_xin + b_mean + b_f + b_z);
+  CK(c, cudaMemsetAsync(f, 0, nf * sizeof(double), st));
+  CK(c, launch_acf_twiddles(tw, M, st));
+  for (size_t w0 = 0, wn = 0; w0 < nw; w0 += wn) {
+    wn = acf_slab_next(w0, nw, seg_w, wb);
+    CK(c, fill(xin, w0, wn));
+    CK(c, launch_acf_slab(xin, (int)n_t, (int)wn, (int)nd, M, tw, z, mean, f, (int64_t)seg_w, (int64_t)w0, st));
   }
-  CK(c, launch_acf_scale(f.get(), nd * n_t, 1.0 / (double)nw, st));  // autocorr.py:106  f /= n_w
-  CK(c, cudaMemcpyAsync(acf, f.get(), nd * n_t * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(c, launch_acf_scale(f, nf, 1.0 / (double)seg_w, st));  // autocorr.py:106  f /= n_w
+  CK(c, cudaMemcpyAsync(acf, f, nf * sizeof(double), cudaMemcpyDeviceToHost, st));
   CK(c, cudaStreamSynchronize(st));
   return EB_OK;
 }
@@ -1470,6 +1491,44 @@ int eb_chain_read_to(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t cou
   return chain_read(ch, first, stride, count, coords_dst, log_prob_dst, cudaMemcpyDefault);
 }
 
+int eb_chain_read_segments_to(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                              double* coords_dst, double* log_prob_dst) {
+  if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_segments(ch, "eb_chain_read_segments_to", nseg);
+  if (!rc) rc = chain_check_slice(ch, "eb_chain_read_segments_to", first, stride, count);
+  if (rc || count == 0) return rc;
+  CK(ch, cudaSetDevice(ch->device));
+  if (coords_dst) rc = check_device_ptr(ch, ch->device, coords_dst, "eb_chain_read_segments_to", "coords_dst");
+  if (!rc && log_prob_dst)
+    rc = check_device_ptr(ch, ch->device, log_prob_dst, "eb_chain_read_segments_to", "log_prob_dst");
+  if (rc) return rc;
+  // segment k of stored step t goes to row block t of dst[k]: per run of n slots, one 2D copy per segment (n rows
+  // of the run's slots) or per slot (nseg rows of the slot's segments), whichever is fewer
+  const size_t K = (size_t)nseg, sn = (size_t)ch->N / K;
+  cudaError_t e = cudaSuccess;
+  auto part = [&](double* dst, const double* src, size_t w, size_t pitch, uint64_t k0, uint64_t n) {
+    // w doubles of a segment; src: the run's first slot, slots pitch doubles apart
+    if (n <= K) {
+      for (uint64_t j = 0; j < n && e == cudaSuccess; ++j)
+        e = copy_rows(dst + (k0 + j) * w, count * w * sizeof(double), src + j * pitch, w * sizeof(double),
+                      w * sizeof(double), K, cudaMemcpyDefault, ch->max_pitch, ch->st.get());
+    } else {
+      for (size_t k = 0; k < K && e == cudaSuccess; ++k)
+        e = copy_rows(dst + (k * count + k0) * w, w * sizeof(double), src + k * w, pitch * sizeof(double),
+                      w * sizeof(double), n, cudaMemcpyDefault, ch->max_pitch, ch->st.get());
+    }
+  };
+  for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
+                     [&](size_t s, uint64_t off, uint64_t k0, uint64_t n) {
+                       if (coords_dst)
+                         part(coords_dst, ch->segs[s].x.get() + off * ch->xs, sn * ch->D, stride * ch->xs, k0, n);
+                       if (log_prob_dst) part(log_prob_dst, ch->segs[s].lp.get() + off * ch->ls, sn, stride * ch->ls, k0, n);
+                     });
+  CK(ch, e);
+  CK(ch, cudaStreamSynchronize(ch->st.get()));
+  return EB_OK;
+}
+
 int eb_chain_accepted(eb_chain* ch, double* accepted) {
   if (!ch || !accepted) return EB_ERR_INVALID;
   CK(ch, cudaSetDevice(ch->device));
@@ -1482,15 +1541,22 @@ int eb_chain_accepted(eb_chain* ch, double* accepted) {
 }
 
 int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* acf) {
+  return eb_chain_autocorr_segments(ch, 1, first, stride, count, acf);
+}
+
+int eb_chain_autocorr_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                               double* acf) {
   if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_segments(ch, "eb_chain_autocorr", nseg);
+  if (rc) return rc;
   if (!acf || count == 0) FAIL(ch, EB_ERR_INVALID, "eb_chain_autocorr: empty chain or null buffer");
-  int rc = chain_check_slice(ch, "eb_chain_autocorr", first, stride, count);
+  rc = chain_check_slice(ch, "eb_chain_autocorr", first, stride, count);
   if (rc) return rc;
   CK(ch, cudaSetDevice(ch->device));
   const size_t nw = (size_t)ch->N, nd = (size_t)ch->D;
   // the slab is filled from the stored slots in place (one strided copy per run of steps inside a segment), so
   // the FFT kernels see the numbers eb_autocorr gets from the host copy of the same slice
-  return acf_slabs(ch, "eb_chain_autocorr", ch->st.get(), (size_t)count, nw, nd, acf,
+  return acf_slabs(ch, "eb_chain_autocorr", ch->st.get(), (size_t)count, nw, nd, (size_t)nseg, acf,
                    [&](double* xin, size_t w0, size_t wn) {
                      cudaError_t e = cudaSuccess;
                      for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
@@ -1507,15 +1573,23 @@ int eb_chain_autocorr(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t co
 
 int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uint64_t count, const uint64_t* ranks,
                     size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes) {
+  return eb_chain_select_segments(ch, 1, what, first, stride, count, ranks, nranks, out, has_nan, passes);
+}
+
+int eb_chain_select_segments(eb_chain* ch, int64_t nseg, int what, uint64_t first, uint64_t stride, uint64_t count,
+                             const uint64_t* ranks, size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes) {
   if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_segments(ch, "eb_chain_select", nseg);
+  if (rc) return rc;
   if (what != EB_CHAIN_COORDS && what != EB_CHAIN_LOG_PROB)
     FAIL(ch, EB_ERR_INVALID, "eb_chain_select: what must be EB_CHAIN_COORDS or EB_CHAIN_LOG_PROB");
   if (count == 0 || nranks == 0 || !ranks || !out || !has_nan)
     FAIL(ch, EB_ERR_INVALID, "eb_chain_select: empty slice, no rank or null buffer");
-  int rc = chain_check_slice(ch, "eb_chain_select", first, stride, count);
+  rc = chain_check_slice(ch, "eb_chain_select", first, stride, count);
   if (rc) return rc;
-  const uint64_t n = count * (uint64_t)ch->N;
-  if (n / (uint64_t)ch->N != count) FAIL(ch, EB_ERR_INVALID, "eb_chain_select: slice of more than 2^64 values");
+  const uint64_t sn = (uint64_t)ch->N / (uint64_t)nseg;  // rows of a segment in one stored step
+  const uint64_t n = count * sn;
+  if (n / sn != count) FAIL(ch, EB_ERR_INVALID, "eb_chain_select: slice of more than 2^64 values");
   for (size_t r = 0; r < nranks; ++r)
     if (ranks[r] >= n)
       FAIL(ch, EB_ERR_INVALID, "eb_chain_select: rank %llu of a slice of %llu values per parameter",
@@ -1523,14 +1597,16 @@ int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uin
   CK(ch, cudaSetDevice(ch->device));
   const bool coords = what == EB_CHAIN_COORDS;
   const int D = coords ? ch->D : 1;
+  const size_t ncol = (size_t)nseg * D;
+  if (ncol > 0x7fffffff) FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_select: more than 2^31 - 1 columns");
   uint32_t np = 0;
   const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
-  const SelectScratch z = select_scratch(count, D, (size_t)D * nranks);
+  const SelectScratch z = select_scratch(count, (int)ncol, ncol * nranks);
   DevPtr<void> scratch;
   rc = chain_scratch(ch, "eb_chain_select", z.bytes, scratch);
   if (rc) return rc;
-  const cudaError_t e = select_run(slots.data(), count, (uint32_t)ch->N, D, ranks, nranks, out, has_nan, &np, z,
-                                   scratch.get(), ch->sm_count, ch->st.get());
+  const cudaError_t e = select_run(slots.data(), count, (uint32_t)nseg, (uint32_t)sn, D, ranks, nranks, out, has_nan,
+                                   &np, z, scratch.get(), ch->sm_count, ch->st.get());
   cudaStreamSynchronize(ch->st.get());
   CK(ch, e);
   if (passes) *passes = np;
@@ -1571,6 +1647,50 @@ int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t cou
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   CK(ch, e);
   finish_moments(h.data() + D, h.data(), count * (uint64_t)ch->N, D, mean, cov);
+  return EB_OK;
+}
+
+int eb_chain_moments_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                              double* mean, double* cov, uint64_t* n) {
+  if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_segments(ch, "eb_chain_moments_segments", nseg);
+  if (rc) return rc;
+  if (ch->D > 1024) FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_moments_segments is limited to ndim <= 1024");
+  rc = chain_check_slice(ch, "eb_chain_moments_segments", first, stride, count);
+  if (rc) return rc;
+  const size_t D = (size_t)ch->D, na = D + D * D, K = (size_t)nseg;
+  const int64_t sn = ch->N / nseg;
+  if (n) *n = count * (uint64_t)sn;
+  if (count == 0) {
+    for (size_t k = 0; k < K; ++k)
+      finish_moments(nullptr, nullptr, 0, D, mean ? mean + k * D : nullptr, cov ? cov + k * D * D : nullptr);
+    return EB_OK;
+  }
+  CK(ch, cudaSetDevice(ch->device));
+  // [slot table | shift[K, D] | sums[K, D + D*D] | chunk partials[nchunks, K, D + D*D]]
+  const uint64_t nchunks = moments_seg_chunks(count, nseg, ch->D);
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t b_tab = al(count * sizeof(double*)), b_head = al((K * D + K * na) * sizeof(double));
+  const size_t bytes = b_tab + b_head + nchunks * K * na * sizeof(double);
+  DevPtr<void> scratch;
+  rc = chain_scratch(ch, "eb_chain_moments_segments", bytes, scratch);
+  if (rc) return rc;
+  char* base = static_cast<char*>(scratch.get());
+  const double** tab = reinterpret_cast<const double**>(base);
+  double* shift = reinterpret_cast<double*>(base + b_tab);
+  double* acc = shift + K * D;
+  double* partial = reinterpret_cast<double*>(base + b_tab + b_head);
+  const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
+  cudaStream_t st = ch->st.get();
+  std::vector<double> h(K * D + K * na);
+  cudaError_t e = cudaMemcpyAsync(tab, slots.data(), count * sizeof(double*), cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = launch_moments_segments(tab, count, nseg, sn, ch->D, nchunks, shift, partial, acc, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), shift, h.size() * sizeof(double), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  CK(ch, e);
+  for (size_t k = 0; k < K; ++k)
+    finish_moments(h.data() + K * D + k * na, h.data() + k * D, count * (uint64_t)sn, D,
+                   mean ? mean + k * D : nullptr, cov ? cov + k * D * D : nullptr);
   return EB_OK;
 }
 
@@ -2120,7 +2240,7 @@ int eb_autocorr(eb_ctx* c, const double* chain, size_t n_t, size_t nw, size_t nd
   NOT_IN_CALLBACK(c);
   if (!chain || !acf || n_t == 0 || nw == 0 || nd == 0) FAIL(c, EB_ERR_INVALID, "eb_autocorr: empty chain or null buffer");
   CK(c, cudaSetDevice(c->device));
-  return acf_slabs(c, "eb_autocorr", c->st.get(), n_t, nw, nd, acf, [&](double* xin, size_t w0, size_t wn) {
+  return acf_slabs(c, "eb_autocorr", c->st.get(), n_t, nw, nd, 1, acf, [&](double* xin, size_t w0, size_t wn) {
     // chain[t][w0 .. w0 + wn)[:] -> xin[t][wn * nd]: one strided copy (rows of the slab are contiguous in a step)
     return cudaMemcpy2DAsync(xin, wn * nd * sizeof(double), chain + w0 * nd, nw * nd * sizeof(double),
                              wn * nd * sizeof(double), n_t, cudaMemcpyHostToDevice, c->st.get());

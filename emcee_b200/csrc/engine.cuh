@@ -295,11 +295,19 @@ cudaError_t launch_moments(const double* X, int64_t nrows, int D, const double* 
                            int sm_count, cudaStream_t st, const int32_t* rowidx = nullptr, int skip_start = 0,
                            int skip_count = 0);
 
+// segmented moments of a stored slice (eb_chain_moments_segments): nseg segments of N walkers per stored step,
+// slots a device table of count step bases; shift[nseg, D], acc[nseg, D + D*D] (sums about shift) and
+// partial[nchunks, nseg, D + D*D] of scratch, nchunks = moments_seg_chunks(count, nseg, D)
+uint64_t moments_seg_chunks(uint64_t count, int64_t nseg, int D);
+cudaError_t launch_moments_segments(const double* const* slots, uint64_t count, int64_t nseg, int64_t N, int D,
+                                    uint64_t nchunks, double* shift, double* partial, double* acc, cudaStream_t st);
+
 // walker-averaged normalised autocorrelation function (autocorr.py:21-46,101-107), slab by slab (geometry:
 // acf_grid.h)
 cudaError_t launch_acf_twiddles(double2* tw, int M, cudaStream_t st);
+// the slab is walkers [w0, w0 + wb) of a chain of segments of seg_w walkers; f[segment][nd][n_t]
 cudaError_t launch_acf_slab(const double* xin, int n_t, int wb, int nd, int M, const double2* tw, double2* z,
-                            double* mean, double* f, cudaStream_t st);
+                            double* mean, double* f, int64_t seg_w, int64_t w0, cudaStream_t st);
 cudaError_t launch_acf_scale(double* f, size_t n, double scale, cudaStream_t st);
 
 // ---- device chain storage (chain.cu) ----------------------------------------------------------
@@ -320,11 +328,12 @@ struct SelectScratch {
   size_t bytes = 0;     // device scratch select_run needs
 };
 SelectScratch select_scratch(uint64_t count, int D, size_t npairs);
-// slots[count] (host array of device pointers): each stored step's [N, D] block.  out[nranks, D] and has_nan[D]
-// on the host; *passes = full reads of the slice.  scratch: z.bytes of device memory.
-cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint64_t* ranks,
-                       size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes, const SelectScratch& z,
-                       void* scratch, int sm_count, cudaStream_t st);
+// slots[count] (host array of device pointers): each stored step's [nseg, N, D] block, nseg segments of N rows.
+// out[nseg, nranks, D] and has_nan[nseg, D] on the host; *passes = full reads of the slice.  scratch: z.bytes of
+// device memory, z = select_scratch(count, nseg * D, nseg * D * nranks).
+cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t nseg, uint32_t N, int D,
+                       const uint64_t* ranks, size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes,
+                       const SelectScratch& z, void* scratch, int sm_count, cudaStream_t st);
 
 // ---- histograms of a stored slice (histogram.cu, eb_chain_histogram / eb_chain_histogram2d) ----------------------
 // can count * N rows be split over grid y with fewer than 2^32 counted by one CTA?

@@ -4,7 +4,9 @@
 //
 // Every pass reads the whole slice once, in place (a table of slot base pointers, one per stored step), with one
 // launch of select_pass_kernel: CTA x is a column block of at most SEL_WMAX parameters (SelTask), CTA y a range of
-// the slice's rows (stored step, walker).  A value's key is matched to its parameter's live group; a histogram
+// the slice's rows (stored step, walker).  A slot of nseg segments (eb_chain_select_segments) of N rows is read as
+// nseg * D columns of N rows: column c = k * D + d is parameter d of segment k, at offset k * N * D of the slot, so
+// one plan selects for every segment in the same passes.  A value's key is matched to its parameter's live group; a histogram
 // group counts the key's next digit in shared memory (flushed to 64-bit global counts at the end), a compaction
 // group copies the key into its slice of the candidate buffer.  select_sort_kernel then sorts each compacted group
 // (at most SEL_CAP keys, bitonic in shared memory) and gathers the ranks it answers.  The host refines the groups
@@ -23,7 +25,7 @@ constexpr int SEL_THREADS = 256;
 constexpr int SORT_THREADS = 512;
 
 __global__ void __launch_bounds__(SEL_THREADS)
-    select_pass_kernel(const double* const* __restrict__ slots, uint32_t N, int D, uint64_t nrows,
+    select_pass_kernel(const double* const* __restrict__ slots, uint32_t N, int D, uint64_t seg_stride, uint64_t nrows,
                        uint64_t rows_per_cta, const SelTask* __restrict__ tasks, const uint32_t* __restrict__ colrange,
                        const SelGroup* __restrict__ groups, int bits, unsigned long long* __restrict__ hist,
                        unsigned long long* __restrict__ cand, unsigned int* __restrict__ cand_cnt,
@@ -36,7 +38,9 @@ __global__ void __launch_bounds__(SEL_THREADS)
   const int c = tid % W, ro = tid / W;
   const bool col_ok = ro < per;
   const uint32_t glo = colrange[t.cr + 2 * c], ghi = colrange[t.cr + 2 * c + 1];
-  const int d = (int)t.d0 + c;
+  const int col = (int)t.d0 + c;  // k * D + d
+  const int kseg = col / D, d = col - kseg * D;
+  const size_t cbase = (size_t)kseg * seg_stride + (size_t)d;  // the column's offset in a slot
   for (int i = tid; i < SEL_HMAX * SEL_BINS; i += SEL_THREADS) sh[i] = 0;
   if (tid < W)
     for (uint32_t g = glo; g < ghi; ++g)
@@ -51,8 +55,8 @@ __global__ void __launch_bounds__(SEL_THREADS)
   for (uint64_t base = r0; base < r1; base += (uint64_t)per) {
     int hs = -1;  // shared histogram bin of this thread's value
     if (col_ok && R < r1) {
-      const double v = slots[s][(size_t)w * D + d];
-      if (nanflag && isnan(v)) nanflag[d] = 1;
+      const double v = slots[s][(size_t)w * D + cbase];
+      if (nanflag && isnan(v)) nanflag[col] = 1;
       const uint64_t key = order_key_bits((uint64_t)__double_as_longlong(v));
       const int g = find_group(groups, glo, ghi, key, bits);
       if (g >= 0) {
@@ -139,12 +143,15 @@ SelectScratch select_scratch(uint64_t count, int D, size_t npairs) {
   return z;
 }
 
-// See eb_chain_select.  slots[count]: base of each stored step's [N, D] block (device pointers, rows D apart);
-// ranks[nranks] < count * N.  out[nranks, D], has_nan[D] on the host; *passes counts full reads of the slice.
-cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint64_t* ranks,
-                       size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes, const SelectScratch& z,
-                       void* scratch, int sm_count, cudaStream_t st) {
+// See eb_chain_select_segments.  slots[count]: base of each stored step's [nseg, N, D] block (device pointers, rows
+// D apart); ranks[nranks] < count * N.  out[nseg, nranks, D], has_nan[nseg, D] on the host; *passes counts full
+// reads of the slice.  The planning runs over the nseg * D columns (select.cu's header).
+cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t nseg, uint32_t N, int Dp,
+                       const uint64_t* ranks, size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes,
+                       const SelectScratch& z, void* scratch, int sm_count, cudaStream_t st) {
   const uint64_t n = count * (uint64_t)N;
+  const int D = (int)nseg * Dp;  // columns
+  const uint64_t seg_stride = (uint64_t)N * (uint64_t)Dp;
   const size_t B = z.batch, T = B + (size_t)D;
   char* p = static_cast<char*>(scratch);
   auto take = [&](size_t bytes) {
@@ -173,7 +180,7 @@ cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, i
   SE(cudaMemsetAsync(d_nan, 0, (size_t)D, st));
   std::vector<uint8_t> nan((size_t)D, 0), dropped((size_t)D, 0);
   *passes = 0;
-  // (parameter, rank) pairs in (parameter, rank) order; pair i answers out[r * D + d]
+  // (column, rank) pairs in (column, rank) order; pair i of column d = k * Dp + p answers out[k][r][p]
   std::vector<uint32_t> order(nranks);
   for (size_t r = 0; r < nranks; ++r) order[r] = (uint32_t)r;
   std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return ranks[a] < ranks[b]; });
@@ -194,7 +201,7 @@ cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, i
       if (nan[d]) continue;  // a NaN seen by an earlier batch
       bd.push_back(d);
       bk.push_back(ranks[r]);
-      bo.push_back((size_t)r * D + d);
+      bo.push_back(((size_t)(d / Dp) * nranks + r) * Dp + d % Dp);
     }
     plan.init(bd.data(), bk.data(), bd.size(), n);
     while (plan.live()) {
@@ -214,7 +221,7 @@ cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t N, i
       const uint64_t rows_per = (n + ys - 1) / ys;
       ys = (n + rows_per - 1) / rows_per;
       select_pass_kernel<<<dim3((unsigned)nt, (unsigned)ys), SEL_THREADS, 0, st>>>(
-          d_slots, N, D, n, rows_per, d_tasks, d_colrange, d_groups, plan.bits, d_hist, d_cand, d_cnt, d_nan);
+          d_slots, N, Dp, seg_stride, n, rows_per, d_tasks, d_colrange, d_groups, plan.bits, d_hist, d_cand, d_cnt, d_nan);
       SE(cudaGetLastError());
       ++*passes;
       const std::vector<uint64_t> pidx = plan.picks();

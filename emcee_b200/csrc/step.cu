@@ -1362,7 +1362,6 @@ int eb_step_store_chain(eb_ctx* c, const eb_move* moves, size_t nmoves, uint64_t
   if (!c) return EB_ERR_INVALID;
   NOT_IN_CALLBACK(c);
   if (thin_by == 0) FAIL(c, EB_ERR_INVALID, "Invalid thinning argument");  // ensemble.py:380-381
-  NOT_BATCH(c, "eb_step_store_chain");
   if (!ch) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: null chain");
   if (ch->ring) FAIL(c, EB_ERR_INVALID, "eb_step_store_chain: a running window's ring is written by its engine only");
   if (ch->device != c->device || ch->N != c->N || ch->D != c->D)

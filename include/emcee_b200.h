@@ -417,7 +417,8 @@ int eb_chain_capacity(const eb_chain* ch, uint64_t* nslots, uint64_t* bytes);
  * (nsteps / thin_by of them) and its accept mask is added to the chain's
  * accepted, each by one kernel behind the step on the engine's stream; the call
  * synchronises once, at its end.  The chain must match the engine's shape and
- * device; sharded engines are refused (EB_ERR_UNSUPPORTED). */
+ * device (for a batch context, nbatch * nwalkers rows: ensemble k is segment k
+ * of the chain); sharded engines are refused (EB_ERR_UNSUPPORTED). */
 int eb_step_store_chain(eb_ctx* ctx, const eb_move* moves, size_t nmoves, uint64_t nsteps,
                         uint64_t thin_by, eb_chain* ch, uint64_t slot0);
 /* Backend.save_step (backend.py:214-231): host coords[nwalkers*ndim] /
@@ -457,6 +458,30 @@ int eb_chain_select(eb_chain* ch, int what, uint64_t first, uint64_t stride, uin
  * against the free memory first: EB_ERR_NOMEM. */
 int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, double* mean, double* cov,
                      uint64_t* n);
+/* Segmented analyses: the chain's nwalkers are nseg segments (ensembles, the
+ * rows of a batch context, eb_create_batch) of nw = nwalkers / nseg walkers,
+ * segment k being walkers [k * nw, (k + 1) * nw) of every stored step.  nseg >= 1
+ * must divide nwalkers (EB_ERR_INVALID otherwise); nseg = 1 is the whole chain.
+ *
+ * eb_chain_autocorr of each segment: acf[nseg, ndim, count], row k bit-identical
+ * to eb_chain_autocorr of segment k stored alone. */
+int eb_chain_autocorr_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                               double* acf);
+/* eb_chain_select of each segment: out[nseg, nranks, D] and has_nan[nseg, D],
+ * ranks < count * nw; every segment's parameters are refined in the same passes
+ * (nseg * D columns), so *passes does not grow with nseg. */
+int eb_chain_select_segments(eb_chain* ch, int64_t nseg, int what, uint64_t first, uint64_t stride, uint64_t count,
+                             const uint64_t* ranks, size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes);
+/* eb_chain_moments of each segment: mean[nseg, ndim], cov[nseg, ndim, ndim] and
+ * *n = count * nw, the sums of segment k about the column mean of its first
+ * stored step, in (step, walker) order with a fixed chunking of the steps (three
+ * launches for the whole slice).  ndim <= 1024; scratch checked: EB_ERR_NOMEM. */
+int eb_chain_moments_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                              double* mean, double* cov, uint64_t* n);
+/* eb_chain_read_to in the per-segment layout: coords_dst[nseg, count * nw, ndim]
+ * and log_prob_dst[nseg, count * nw] (either may be NULL), device to device. */
+int eb_chain_read_segments_to(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                              double* coords_dst, double* log_prob_dst);
 /* np.histogram of each parameter (what = EB_CHAIN_COORDS: ndim of them;
  * EB_CHAIN_LOG_PROB: one) of the stored slice first + k * stride, k < count, read
  * where it is stored, with numpy's edges given by the caller: outer[D * 3] holds
