@@ -1177,15 +1177,7 @@ int eb_set_rng(eb_ctx* c, uint64_t seed, uint64_t step) {
   if (!c) return EB_ERR_INVALID;
   NOT_BATCH(c, "eb_set_rng");
   NOT_IN_CALLBACK(c);
-  // the rows of a step offered again would come back with their old keys, and a new seed draws other keys: either
-  // starts the running reservoir again, so that it stays the sample of one stream of steps (reservoir_plan.h)
-  if (c->res_on && (seed != c->seed || step < c->step)) {
-    CK(c, cudaSetDevice(c->device));
-    CK(c, cudaStreamSynchronize(c->st.get()));
-    CK(c, live_reservoir_setup(&c->res, c->res_mem.get(), c->res.K, (uint32_t)c->N, c->D, c->coords.get(),
-                               c->logp.get(), c->sm_count, c->st.get()));
-    c->res_plan = ResSchedule(c->res.K, (uint64_t)c->N);
-  }
+  if (const int rc = running_set_rng(c, seed, step)) return rc;
   c->seed = seed;
   c->step = step;
   return EB_OK;
@@ -1249,13 +1241,9 @@ int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, s
   auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
   const size_t b_xin = al(n_t * S * sizeof(double)), b_mean = al(S * sizeof(double)), b_f = al(nf * sizeof(double));
   const size_t b_z = al(S * (size_t)M * sizeof(double2)), b_tw = al((size_t)std::max(1, M / 2) * sizeof(double2));
-  const size_t bytes = b_xin + b_mean + b_f + b_z + b_tw;
-  size_t free_b = 0, total_b = 0;
-  CK(c, cudaMemGetInfo(&free_b, &total_b));
-  if (bytes > free_b) FAIL(c, EB_ERR_NOMEM, "%s: %zu bytes of scratch, %zu bytes free", who, bytes, free_b);
   DevPtr<char> scratch;
-  CK_NOMEM(c, dev_alloc(scratch, bytes), "%s: allocating %zu bytes of scratch failed (%s)", who, bytes,
-           cudaGetErrorString(alloc_err));
+  const int rc = dev_alloc_checked(c, who, "scratch", b_xin + b_mean + b_f + b_z + b_tw, scratch);
+  if (rc) return rc;
   double* xin = reinterpret_cast<double*>(scratch.get());
   double* mean = reinterpret_cast<double*>(scratch.get() + b_xin);
   double* f = reinterpret_cast<double*>(scratch.get() + b_xin + b_mean);
@@ -1274,8 +1262,23 @@ int acf_slabs(Obj* c, const char* who, cudaStream_t st, size_t n_t, size_t nw, s
   return EB_OK;
 }
 
-// mean[D], cov[D * D] of m samples from the sums acc = [S1 | S2] about `shift` (eb_moments, eb_chain_moments):
-// mean = shift + S1 / m, cov = (S2 - S1 S1^T / m) / (m - 1)   (np.cov(flatchain, rowvar=False)); NaN when m == 0
+// the base of each stored step of the slice: coords ([N, D] blocks) or log_prob ([N] rows)
+std::vector<const double*> chain_slot_table(eb_chain* ch, bool coords, uint64_t first, uint64_t stride,
+                                            uint64_t count) {
+  std::vector<const double*> t;
+  t.reserve(count);
+  for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
+                     [&](size_t s, uint64_t off, uint64_t, uint64_t n) {
+                       for (uint64_t j = 0; j < n; ++j)
+                         t.push_back(coords ? ch->segs[s].x.get() + (off + j * stride) * ch->xs
+                                            : ch->segs[s].lp.get() + (off + j * stride) * ch->ls);
+                     });
+  return t;
+}
+
+}  // namespace
+
+// finish_moments and chain_init: context.h
 void finish_moments(const double* acc, const double* shift, uint64_t count, size_t D, double* mean, double* cov) {
   if (count == 0) {
     if (mean) std::fill(mean, mean + D, NAN);
@@ -1291,55 +1294,6 @@ void finish_moments(const double* acc, const double* shift, uint64_t count, size
         cov[r * D + k] = (acc[D + r * D + k] - acc[r] * acc[k] / m) / (m - 1.0);
 }
 
-// the base of each stored step of the slice: coords ([N, D] blocks) or log_prob ([N] rows)
-std::vector<const double*> chain_slot_table(eb_chain* ch, bool coords, uint64_t first, uint64_t stride,
-                                            uint64_t count) {
-  std::vector<const double*> t;
-  t.reserve(count);
-  for_each_chain_run(ch->start.data(), ch->segs.size(), ch->origin, first, stride, count,
-                     [&](size_t s, uint64_t off, uint64_t, uint64_t n) {
-                       for (uint64_t j = 0; j < n; ++j)
-                         t.push_back(coords ? ch->segs[s].x.get() + (off + j * stride) * ch->xs
-                                            : ch->segs[s].lp.get() + (off + j * stride) * ch->ls);
-                     });
-  return t;
-}
-
-// scratch of `bytes` on the chain's device, refused before the allocation when it cannot fit
-int chain_scratch(eb_chain* ch, const char* who, size_t bytes, DevPtr<void>& out) {
-  size_t free_b = 0, total_b = 0;
-  CK(ch, cudaMemGetInfo(&free_b, &total_b));
-  if (bytes > free_b)
-    FAIL(ch, EB_ERR_NOMEM, "%s: %zu bytes of scratch, %zu bytes free", who, bytes, free_b);
-  CK_NOMEM(ch, dev_alloc(out, bytes), "%s: allocating %zu bytes of scratch failed (%s)", who, bytes,
-           cudaGetErrorString(alloc_err));
-  return EB_OK;
-}
-
-// running chain moments (option "moments_every"): allocate and zero the accumulators
-int moments_config(eb_ctx* c, uint64_t every) {
-  CK(c, cudaSetDevice(c->device));
-  if (every > 0 && c->D > 1024) FAIL(c, EB_ERR_UNSUPPORTED, "chain moments are limited to ndim <= 1024");
-  const size_t n = (size_t)c->D + (size_t)c->D * c->D;
-  if (every > 0 && !c->mom_acc) {
-    DevPtr<double> acc, shift, partial;
-    CK(c, dev_alloc(acc, n * sizeof(double)));
-    CK(c, dev_alloc(shift, (size_t)c->D * sizeof(double)));
-    if (!c->mom_partial) CK(c, dev_alloc(partial, moments_partial_bytes(c->D, c->sm_count)));
-    c->mom_acc = std::move(acc);
-    c->mom_shift = std::move(shift);
-    if (partial) c->mom_partial = std::move(partial);
-  }
-  if (c->mom_acc) CK(c, cudaMemsetAsync(c->mom_acc.get(), 0, n * sizeof(double), c->st.get()));
-  c->mom_count = 0;
-  c->mom_have_shift = false;
-  c->moments_every = every;
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  return EB_OK;
-}
-
-// an empty chain of nwalkers x ndim on `device`: its stream and its [N] accept buffers (eb_chain_create, and the ring
-// of eb_window_config); synchronises
 cudaError_t chain_init(eb_chain* ch, int device, int64_t nwalkers, int ndim) {
   ch->device = device;
   ch->N = nwalkers;
@@ -1359,8 +1313,6 @@ cudaError_t chain_init(eb_chain* ch, int device, int64_t nwalkers, int ndim) {
   if (e == cudaSuccess) e = cudaStreamSynchronize(ch->st.get());
   return e;
 }
-
-}  // namespace
 
 extern "C" {
 
@@ -1603,7 +1555,7 @@ int eb_chain_select_segments(eb_chain* ch, int64_t nseg, int what, uint64_t firs
   const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
   const SelectScratch z = select_scratch(count, (int)ncol, ncol * nranks);
   DevPtr<void> scratch;
-  rc = chain_scratch(ch, "eb_chain_select", z.bytes, scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_select", "scratch", z.bytes, scratch);
   if (rc) return rc;
   const cudaError_t e = select_run(slots.data(), count, (uint32_t)nseg, (uint32_t)sn, D, ranks, nranks, out, has_nan,
                                    &np, z, scratch.get(), ch->sm_count, ch->st.get());
@@ -1629,7 +1581,7 @@ int eb_chain_moments(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t cou
   // [D shift | D + D*D sums | CTA partials of launch_moments]
   const size_t head = ((D + na) * sizeof(double) + 255) & ~(size_t)255;
   DevPtr<void> scratch;
-  rc = chain_scratch(ch, "eb_chain_moments", head + moments_partial_bytes(ch->D, ch->sm_count), scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_moments", "scratch", head + moments_partial_bytes(ch->D, ch->sm_count), scratch);
   if (rc) return rc;
   double* shift = static_cast<double*>(scratch.get());
   double* acc = shift + D;
@@ -1673,7 +1625,7 @@ int eb_chain_moments_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64
   const size_t b_tab = al(count * sizeof(double*)), b_head = al((K * D + K * na) * sizeof(double));
   const size_t bytes = b_tab + b_head + nchunks * K * na * sizeof(double);
   DevPtr<void> scratch;
-  rc = chain_scratch(ch, "eb_chain_moments_segments", bytes, scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_moments_segments", "scratch", bytes, scratch);
   if (rc) return rc;
   char* base = static_cast<char*>(scratch.get());
   const double** tab = reinterpret_cast<const double**>(base);
@@ -1718,7 +1670,7 @@ int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, 
   CK(ch, cudaSetDevice(ch->device));
   const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
   DevPtr<void> scratch;
-  rc = chain_scratch(ch, "eb_chain_histogram", hist1_scratch_bytes(count, D, (int)bins), scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_histogram", "scratch", hist1_scratch_bytes(count, D, (int)bins), scratch);
   if (rc) return rc;
   bool bad = false;
   const cudaError_t e = hist1_run(slots.data(), count, (uint32_t)ch->N, D, (int)bins, outer, edges, hist, &bad,
@@ -1762,7 +1714,8 @@ int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t
   CK(ch, cudaSetDevice(ch->device));
   const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
   DevPtr<void> scratch;
-  rc = chain_scratch(ch, "eb_chain_histogram2d", hist2_scratch_bytes(count, (int)nparams, (int)bins), scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_histogram2d", "scratch", hist2_scratch_bytes(count, (int)nparams, (int)bins),
+                         scratch);
   if (rc) return rc;
   const cudaError_t e = hist2_run(slots.data(), count, (uint32_t)ch->N, ch->D, params, (int)nparams, (int)bins, edges,
                                   hist, scratch.get(), ch->sm_count, ch->st.get());
@@ -1795,386 +1748,6 @@ int eb_reset_counters(eb_ctx* c) {
   CK(c, cudaSetDevice(c->device));
   CK(c, cudaMemsetAsync(c->nacc.get(), 0, (size_t)c->N * sizeof(unsigned long long), c->st.get()));
   CK(c, cudaStreamSynchronize(c->st.get()));
-  return EB_OK;
-}
-
-int eb_moments(eb_ctx* c, double* mean, double* cov, uint64_t* count, uint64_t* naccepted_total) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->mom_acc) FAIL(c, EB_ERR_STATE, "eb_moments: enable with eb_set_option(\"moments_every\", n) before stepping");
-  CK(c, cudaSetDevice(c->device));
-  const size_t D = (size_t)c->D, n = D + D * D;
-  std::vector<double> acc(n), shift(D);
-  CK(c, cudaMemcpyAsync(acc.data(), c->mom_acc.get(), n * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
-  CK(c, cudaMemcpyAsync(shift.data(), c->mom_shift.get(), D * sizeof(double), cudaMemcpyDeviceToHost, c->st.get()));
-  std::vector<unsigned long long> nacc;
-  int64_t r0, r1;
-  owned_rows(c, r0, r1);
-  if (naccepted_total) {
-    nacc.resize((size_t)(r1 - r0));
-    CK(c, cudaMemcpyAsync(nacc.data(), c->nacc.get() + r0, nacc.size() * sizeof(unsigned long long),
-                          cudaMemcpyDeviceToHost, c->st.get()));
-  }
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  if (count) *count = c->mom_count;
-  if (naccepted_total) {
-    unsigned long long tot = 0;
-    for (unsigned long long v : nacc) tot += v;
-    *naccepted_total = tot;
-  }
-  finish_moments(acc.data(), shift.data(), c->mom_count, D, mean, cov);
-  return EB_OK;
-}
-
-int eb_histograms_config(eb_ctx* c, uint64_t every, uint32_t bins, const double* outer, const double* edges,
-                         int log_prob, const uint32_t* params2d, size_t nparams2d, uint32_t bins2d,
-                         const double* edges2d) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_BATCH(c, "eb_histograms_config");
-  NOT_IN_CALLBACK(c);
-  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
-  if (bins == 0 || !outer || !edges) FAIL(c, EB_ERR_INVALID, "eb_histograms_config: bins == 0 or null buffer");
-  if (bins > (uint32_t)HIST_BINS_MAX)
-    FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are limited to bins <= %d on the device, got %u", HIST_BINS_MAX,
-         bins);
-  if (nparams2d > 0) {
-    if (!params2d || !edges2d || bins2d == 0)
-      FAIL(c, EB_ERR_INVALID, "eb_histograms_config: bins2d == 0 or null 2-D buffer");
-    if (bins2d > (uint32_t)HIST2_BINS_MAX)
-      FAIL(c, EB_ERR_UNSUPPORTED, "running 2-D histograms are limited to bins <= %d on the device, got %u",
-           HIST2_BINS_MAX, bins2d);
-    if (nparams2d < 2 || nparams2d > (size_t)c->D)
-      FAIL(c, EB_ERR_INVALID, "eb_histograms_config: need 2 <= nparams2d <= ndim = %d, got %zu", c->D, nparams2d);
-    std::vector<uint8_t> seen((size_t)c->D, 0);
-    for (size_t k = 0; k < nparams2d; ++k) {
-      if (params2d[k] >= (uint32_t)c->D || seen[params2d[k]])
-        FAIL(c, EB_ERR_INVALID, "eb_histograms_config: params2d must be distinct and < ndim = %d (params2d[%zu] = %u)",
-             c->D, k, params2d[k]);
-      seen[params2d[k]] = 1;
-    }
-  }
-  CK(c, cudaSetDevice(c->device));
-  // the old configuration goes first: its memory counts towards what the new one may take
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  c->hist_mem.reset();
-  c->hist = LiveHist{};
-  c->hist_on = false;
-  c->hist_every = 0;
-  c->hist_count = 0;
-  const int lp = log_prob ? 1 : 0, m = nparams2d > 0 ? (int)nparams2d : 0;
-  const size_t bytes = live_hist_bytes(c->D, (int)bins, lp, m, (int)bins2d);
-  size_t free_b = 0, total_b = 0;
-  CK(c, cudaMemGetInfo(&free_b, &total_b));
-  if (bytes > free_b)
-    FAIL(c, EB_ERR_NOMEM, "eb_histograms_config: %zu bytes of counts and tables, %zu bytes free", bytes, free_b);
-  DevPtr<void> mem;
-  CK_NOMEM(c, dev_alloc(mem, bytes), "eb_histograms_config: allocating %zu bytes failed (%s)", bytes,
-           cudaGetErrorString(alloc_err));
-  const cudaError_t s = live_hist_setup(&c->hist, mem.get(), (uint32_t)c->N, c->D, (int)bins, lp, outer, edges,
-                                        params2d, m, (int)bins2d, edges2d, c->coords.get(), c->logp.get(), c->sm_count,
-                                        c->st.get());
-  if (s != cudaSuccess) {
-    cudaGetLastError();
-    c->hist = LiveHist{};
-    FAIL(c, EB_ERR_CUDA, "eb_histograms_config: %s", cudaGetErrorString(s));
-  }
-  c->hist_mem = std::move(mem);
-  c->hist_on = true;
-  c->hist_every = every;
-  return EB_OK;
-}
-
-int eb_histograms(eb_ctx* c, uint64_t* hist, uint64_t* hist2d, uint64_t* count) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->hist_on) FAIL(c, EB_ERR_STATE, "eb_histograms: configure them with eb_histograms_config first");
-  CK(c, cudaSetDevice(c->device));
-  bool bad = false;
-  CK(c, live_hist_read(c->hist, hist, hist2d, &bad, c->st.get()));
-  if (count) *count = c->hist_count;
-  if (bad)
-    FAIL(c, EB_ERR_INVALID, "eb_histograms: a value's truncated bin index is above bins (np.histogram raises "
-         "IndexError there); the span does not fit the edges");
-  return EB_OK;
-}
-
-int eb_trace_config(eb_ctx* c, uint64_t every) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_BATCH(c, "eb_trace_config");
-  NOT_IN_CALLBACK(c);
-  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
-  CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  if (every > 0 || !c->trace_on) {  // every == 0 after a configuration keeps what was recorded readable
-    c->trace_rows.reset();
-    c->trace_cap = 0;
-    c->trace_steps.clear();
-    if (!c->trace_on) {
-      const size_t bytes = live_trace_fixed_bytes((uint32_t)c->N, c->D);
-      size_t free_b = 0, total_b = 0;
-      CK(c, cudaMemGetInfo(&free_b, &total_b));
-      if (bytes > free_b) FAIL(c, EB_ERR_NOMEM, "eb_trace_config: %zu bytes of partial sums, %zu bytes free", bytes, free_b);
-      CK_NOMEM(c, dev_alloc(c->trace_mem, bytes), "eb_trace_config: allocating %zu bytes failed (%s)", bytes,
-               cudaGetErrorString(alloc_err));
-    }
-    const cudaError_t s = live_trace_setup(&c->trace, c->trace_mem.get(), (uint32_t)c->N, c->D, c->coords.get(),
-                                           c->logp.get(), c->accepted.get(), c->st.get());
-    if (s != cudaSuccess) {
-      cudaGetLastError();
-      FAIL(c, EB_ERR_CUDA, "eb_trace_config: %s", cudaGetErrorString(s));
-    }
-    c->trace_on = true;
-  }
-  c->trace_every = every;
-  return EB_OK;
-}
-
-int eb_trace_count(eb_ctx* c, uint64_t* rows) {
-  if (!c || !rows) return EB_ERR_INVALID;
-  if (!c->trace_on) FAIL(c, EB_ERR_STATE, "eb_trace_count: configure the trace with eb_trace_config first");
-  *rows = c->trace_steps.size();
-  return EB_OK;
-}
-
-int eb_trace_read(eb_ctx* c, uint64_t first, uint64_t count, uint64_t* step, double* rows_out) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->trace_on) FAIL(c, EB_ERR_STATE, "eb_trace_read: configure the trace with eb_trace_config first");
-  const uint64_t have = c->trace_steps.size();
-  if (first > have || count > have - first)
-    FAIL(c, EB_ERR_INVALID, "eb_trace_read: rows %llu .. %llu + %llu of %llu recorded", (unsigned long long)first,
-         (unsigned long long)first, (unsigned long long)count, (unsigned long long)have);
-  if (count == 0) return EB_OK;
-  if (step) std::copy(c->trace_steps.begin() + first, c->trace_steps.begin() + first + count, step);
-  if (rows_out) {
-    const size_t W = 2 * (size_t)c->D + TRACE_EXTRA;
-    CK(c, cudaSetDevice(c->device));
-    CK(c, cudaMemcpyAsync(rows_out, c->trace_rows.get() + first * W, (size_t)count * W * sizeof(double),
-                          cudaMemcpyDeviceToHost, c->st.get()));
-    CK(c, cudaStreamSynchronize(c->st.get()));
-  }
-  return EB_OK;
-}
-
-int eb_trace_best(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, uint64_t* walker) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->trace_on) FAIL(c, EB_ERR_STATE, "eb_trace_best: configure the trace with eb_trace_config first");
-  if (c->trace_steps.empty()) FAIL(c, EB_ERR_STATE, "eb_trace_best: no step has been recorded yet");
-  CK(c, cudaSetDevice(c->device));
-  TraceBest b;
-  CK(c, live_trace_best(c->trace, &b, coords, c->st.get()));
-  if (log_prob) *log_prob = b.log_prob;
-  if (step) *step = b.step;
-  if (walker) *walker = b.walker;
-  return EB_OK;
-}
-
-int eb_reservoir_config(eb_ctx* c, uint64_t size, uint64_t every) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_BATCH(c, "eb_reservoir_config");
-  NOT_IN_CALLBACK(c);
-  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
-  if (size == 0) FAIL(c, EB_ERR_INVALID, "eb_reservoir_config: size must be >= 1");
-  if (size >= RES_SIZE_LIMIT)
-    FAIL(c, EB_ERR_NOMEM, "eb_reservoir_config: size %llu is not below 2^32, the entries the reservoir can address",
-         (unsigned long long)size);
-  CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  if (every > 0 || !c->res_on) {  // every == 0 after a configuration keeps what was kept readable
-    LiveReservoir r;
-    cudaError_t s;
-    if (c->res_on && c->res.K == size) {  // the same size: empty the buffers in place
-      s = live_reservoir_setup(&r, c->res_mem.get(), size, (uint32_t)c->N, c->D, c->coords.get(), c->logp.get(),
-                               c->sm_count, c->st.get());
-    } else {
-      // entries are addressed with 32 bits; the buffers are checked against the free memory before anything changes
-      const uint64_t cap = res_cap(size, (uint64_t)c->N);  // size < 2^32: no wrap
-      size_t free_b = 0, total_b = 0;
-      CK(c, cudaMemGetInfo(&free_b, &total_b));
-      const size_t bytes = cap < RES_SIZE_LIMIT ? live_reservoir_bytes(size, (uint32_t)c->N, c->D) : SIZE_MAX;
-      if (bytes > free_b)
-        FAIL(c, EB_ERR_NOMEM, "eb_reservoir_config: %llu entries of %zu bytes, %zu bytes free",
-             (unsigned long long)cap, (size_t)c->D * sizeof(double) + 32, free_b);
-      DevPtr<void> mem;
-      CK_NOMEM(c, dev_alloc(mem, bytes), "eb_reservoir_config: allocating %zu bytes failed (%s)", bytes,
-               cudaGetErrorString(alloc_err));
-      s = live_reservoir_setup(&r, mem.get(), size, (uint32_t)c->N, c->D, c->coords.get(), c->logp.get(), c->sm_count,
-                               c->st.get());
-      if (s == cudaSuccess) c->res_mem = std::move(mem);
-    }
-    if (s != cudaSuccess) {
-      cudaGetLastError();
-      FAIL(c, EB_ERR_CUDA, "eb_reservoir_config: %s", cudaGetErrorString(s));
-    }
-    c->res = r;
-    c->res_plan = ResSchedule(size, (uint64_t)c->N);
-    c->res_on = true;
-  }
-  c->res_every = every;
-  return EB_OK;
-}
-
-int eb_reservoir_count(eb_ctx* c, uint64_t* offered, uint64_t* kept) {
-  if (!c) return EB_ERR_INVALID;
-  if (!c->res_on) FAIL(c, EB_ERR_STATE, "eb_reservoir_count: configure the reservoir with eb_reservoir_config first");
-  if (offered) *offered = c->res_plan.offered;
-  if (kept) *kept = c->res_plan.kept();
-  return EB_OK;
-}
-
-namespace {
-int reservoir_read(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, int64_t* walker, bool device_out) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->res_on) FAIL(c, EB_ERR_STATE, "eb_reservoir_read: configure the reservoir with eb_reservoir_config first");
-  CK(c, cudaSetDevice(c->device));
-  if (c->res_plan.compact_before_read()) {
-    uint64_t launches = 0;
-    CK(c, live_reservoir_compact(c->res, c->res_plan.bound, c->st.get(), launches));
-    c->res_plan.compacted();
-  }
-  CK(c, live_reservoir_read(c->res, c->res_plan.kept(), coords, log_prob, step, walker, device_out, c->st.get()));
-  return EB_OK;
-}
-}  // namespace
-
-int eb_reservoir_read(eb_ctx* c, double* coords, double* log_prob, uint64_t* step, int64_t* walker) {
-  return reservoir_read(c, coords, log_prob, step, walker, false);
-}
-
-int eb_reservoir_read_to(eb_ctx* c, double* coords_dst, double* log_prob_dst, uint64_t* step, int64_t* walker) {
-  return reservoir_read(c, coords_dst, log_prob_dst, step, walker, true);
-}
-
-int eb_running_acf_config(eb_ctx* c, uint64_t max_lag, uint64_t every) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_BATCH(c, "eb_running_acf_config");
-  NOT_IN_CALLBACK(c);
-  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running autocorrelation is not sharded across GPUs");
-  if (max_lag == 0) FAIL(c, EB_ERR_INVALID, "eb_running_acf_config: max_lag must be >= 1");
-  CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  if (every > 0 || !c->racf_on) {  // every == 0 after a configuration keeps what was recorded readable
-    LiveRacf r;
-    cudaError_t s;
-    if (c->racf_on && c->racf.max_lag == max_lag) {  // the same lags: zero the sums in place
-      s = live_racf_setup(&r, c->racf_mem.get(), (uint32_t)c->N, c->D, max_lag, c->coords.get(), c->st.get());
-    } else {
-      // checked against the free memory before anything changes; the old sums stay until the new ones exist
-      size_t free_b = 0, total_b = 0;
-      CK(c, cudaMemGetInfo(&free_b, &total_b));
-      const size_t bytes = live_racf_bytes((uint32_t)c->N, c->D, max_lag);
-      if (bytes > free_b)
-        FAIL(c, EB_ERR_NOMEM, "eb_running_acf_config: max_lag %llu needs %zu bytes, %zu bytes free",
-             (unsigned long long)max_lag, bytes, free_b);
-      DevPtr<void> mem;
-      CK_NOMEM(c, dev_alloc(mem, bytes), "eb_running_acf_config: allocating %zu bytes failed (%s)", bytes,
-               cudaGetErrorString(alloc_err));
-      s = live_racf_setup(&r, mem.get(), (uint32_t)c->N, c->D, max_lag, c->coords.get(), c->st.get());
-      if (s == cudaSuccess) c->racf_mem = std::move(mem);
-    }
-    if (s != cudaSuccess) {
-      cudaGetLastError();
-      FAIL(c, EB_ERR_CUDA, "eb_running_acf_config: %s", cudaGetErrorString(s));
-    }
-    c->racf = r;
-    c->racf_n = 0;
-    c->racf_on = true;
-  }
-  c->racf_every = every;
-  return EB_OK;
-}
-
-int eb_running_acf_count(eb_ctx* c, uint64_t* n) {
-  if (!c) return EB_ERR_INVALID;
-  if (!c->racf_on)
-    FAIL(c, EB_ERR_STATE, "eb_running_acf_count: configure the autocorrelation with eb_running_acf_config first");
-  if (n) *n = c->racf_n;
-  return EB_OK;
-}
-
-int eb_running_acf_read(eb_ctx* c, double* rho) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->racf_on)
-    FAIL(c, EB_ERR_STATE, "eb_running_acf_read: configure the autocorrelation with eb_running_acf_config first");
-  CK(c, cudaSetDevice(c->device));
-  CK(c, live_racf_read(c->racf, c->racf_n, rho, c->st.get()));
-  return EB_OK;
-}
-
-int eb_window_config(eb_ctx* c, uint64_t size, uint64_t every) {
-  if (!c) return EB_ERR_INVALID;
-  NOT_BATCH(c, "eb_window_config");
-  NOT_IN_CALLBACK(c);
-  if (c->comm.nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running window is not sharded across GPUs");
-  if (size == 0) FAIL(c, EB_ERR_INVALID, "eb_window_config: size must be >= 1");
-  CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  if (every > 0 || !c->win) {  // every == 0 after a configuration keeps what was recorded readable
-    if (!c->win || c->win->start.back() != size) {
-      // checked against the free memory before anything changes; the old ring stays until the new one exists
-      const size_t N = (size_t)c->N, xs = (N * (size_t)c->D + 1) & ~(size_t)1, ls = (N + 1) & ~(size_t)1;
-      const size_t per_slot = (xs + ls) * sizeof(double) + N;
-      size_t free_b = 0, total_b = 0;
-      CK(c, cudaMemGetInfo(&free_b, &total_b));
-      if (size > (free_b - std::min(free_b, N * (sizeof(double) + 1))) / per_slot)
-        FAIL(c, EB_ERR_NOMEM, "eb_window_config: %llu slots need %.0f bytes, %zu bytes free",
-             (unsigned long long)size, (double)size * (double)per_slot + (double)N * (sizeof(double) + 1), free_b);
-      std::unique_ptr<eb_chain> ring(new eb_chain());
-      cudaError_t e = chain_init(ring.get(), c->device, c->N, c->D);
-      if (e == cudaSuccess) {
-        ChainSeg seg;
-        e = dev_alloc(seg.x, (size_t)size * xs * sizeof(double));
-        if (e == cudaSuccess) e = dev_alloc(seg.lp, (size_t)size * ls * sizeof(double));
-        if (e == cudaSuccess) e = dev_alloc(ring->slot_mask, (size_t)size * N);
-        ring->segs.push_back(std::move(seg));
-        ring->start.push_back(size);
-      }
-      CK_NOMEM(c, e, "eb_window_config: %llu slots of %zu bytes: allocation failed (%s)", (unsigned long long)size,
-               per_slot, cudaGetErrorString(alloc_err));
-      std::vector<uint64_t> steps((size_t)size), seeds((size_t)size);
-      ring->ring = true;
-      c->win = std::move(ring);
-      c->win_steps.swap(steps);
-      c->win_seeds.swap(seeds);
-    }
-    c->win->origin = 0;
-    c->win->filled = 0;
-    c->win_n = 0;
-  }
-  c->win_every = every;
-  return EB_OK;
-}
-
-int eb_window_count(eb_ctx* c, uint64_t* recorded, uint64_t* filled) {
-  if (!c) return EB_ERR_INVALID;
-  if (!c->win) FAIL(c, EB_ERR_STATE, "eb_window_count: configure the window with eb_window_config first");
-  if (recorded) *recorded = c->win_n;
-  if (filled) *filled = c->win->filled;
-  return EB_OK;
-}
-
-int eb_window_steps(eb_ctx* c, uint64_t* steps, uint64_t* seeds) {
-  if (!c) return EB_ERR_INVALID;
-  if (!c->win) FAIL(c, EB_ERR_STATE, "eb_window_steps: configure the window with eb_window_config first");
-  const uint64_t size = c->win->start.back();
-  for (uint64_t k = 0; k < c->win->filled; ++k) {
-    const size_t slot = (size_t)((c->win->origin + k) % size);
-    if (steps) steps[k] = c->win_steps[slot];
-    if (seeds) seeds[k] = c->win_seeds[slot];
-  }
-  return EB_OK;
-}
-
-int eb_window_chain(eb_ctx* c, eb_chain** ring) {
-  if (!c || !ring) return EB_ERR_INVALID;
-  NOT_IN_CALLBACK(c);
-  if (!c->win) FAIL(c, EB_ERR_STATE, "eb_window_chain: configure the window with eb_window_config first");
-  CK(c, cudaSetDevice(c->device));
-  CK(c, cudaStreamSynchronize(c->st.get()));  // the ring's reads run on its own stream, behind the steps' stores
-  *ring = c->win.get();
   return EB_OK;
 }
 
@@ -2477,12 +2050,7 @@ int eb_comm_init(eb_ctx* c, const char id[EB_COMM_ID_BYTES], int rank, int nrank
   NOT_IN_CALLBACK(c);
   if (c->have_model && c->model.kind == MODEL_EXTERNAL && nranks > 1)
     FAIL(c, EB_ERR_UNSUPPORTED, "log-probability callbacks are not sharded across GPUs");
-  if (c->hist_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "running histograms are not sharded across GPUs");
-  if (c->trace_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running trace is not sharded across GPUs");
-  if (c->res_on && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running reservoir is not sharded across GPUs");
-  if (c->racf_on && nranks > 1)
-    FAIL(c, EB_ERR_UNSUPPORTED, "the running autocorrelation is not sharded across GPUs");
-  if (c->win && nranks > 1) FAIL(c, EB_ERR_UNSUPPORTED, "the running window is not sharded across GPUs");
+  if (const int rc = running_check_sharding(c, nranks)) return rc;
   CK(c, cudaSetDevice(c->device));
   c->tbl_n = 0;  // the cached split tables carry the old ownership ranges
   c->have_state = false;  // ownership changes: the state must be set again through the sharded path

@@ -1,5 +1,5 @@
 // Private to the engine's C ABI: the engine and device-chain objects, the error macros, and the helpers that
-// the ABI (capi.cu) and the step driver (step.cu) share.
+// the ABI (capi.cu), the step driver (step.cu) and the running statistics (running.cu) share.
 #pragma once
 
 #include <stdio.h>
@@ -10,11 +10,8 @@
 
 #include "comm.h"
 #include "engine.cuh"
-#include "hist_bins.h"
 #include "owners.h"
-#include "reservoir_plan.h"
-#include "running_acf.h"
-#include "trace_sum.h"
+#include "running.h"
 
 using namespace eb;
 
@@ -130,51 +127,8 @@ struct eb_ctx {
   // on this rank until the next collective read (eb_get_state, eb_get_naccepted, ...) replicates them
   bool replicas_dirty = false;
 
-  // running chain moments (eb_moments): sum of (x - shift) and of its outer product over the owned
-  // rows of every `moments_every`-th step
-  uint64_t moments_every = 0;
-  DevPtr<double> mom_acc;      // [D + D*D] accumulators
-  DevPtr<double> mom_shift;    // [D]
-  DevPtr<double> mom_partial;  // per-CTA partials of one accumulation
-  unsigned long long mom_count = 0;
-  bool mom_have_shift = false;
-
-  // running histograms (eb_histograms): the owned rows of every `hist_every`-th step counted into hist.counts
-  uint64_t hist_every = 0;
-  bool hist_on = false;  // configured: hist holds tables and counts
-  LiveHist hist;
-  DevPtr<void> hist_mem;  // hist.mem
-  unsigned long long hist_count = 0;  // samples counted
-
-  // running trace (eb_trace_read): one row [2 D + 4] of ensemble statistics per `trace_every`-th step
-  uint64_t trace_every = 0;
-  bool trace_on = false;  // configured: trace holds its fixed part
-  LiveTrace trace;
-  DevPtr<void> trace_mem;           // trace.mem
-  DevPtr<double> trace_rows;        // [trace_cap, 2 D + 4], device
-  uint64_t trace_cap = 0;
-  std::vector<uint64_t> trace_steps;  // the step counter of each recorded row
-
-  // running reservoir (eb_reservoir_read): K of the rows of every `res_every`-th step, in device memory
-  uint64_t res_every = 0;
-  bool res_on = false;  // configured: res holds its buffers
-  LiveReservoir res;
-  DevPtr<void> res_mem;  // res's buffers
-  ResSchedule res_plan;  // rows offered, and the bound of the live entries that decides the compactions
-
-  // running autocorrelation function (eb_running_acf_read): lag sums of every series of every `racf_every`-th step
-  uint64_t racf_every = 0;
-  bool racf_on = false;  // configured: racf holds its buffers
-  uint64_t racf_n = 0;   // steps recorded since the last configuration with every > 0
-  LiveRacf racf;
-  DevPtr<void> racf_mem;  // racf's buffers
-
-  // running window (eb_window_config): the last `capacity` of the states of every `win_every`-th step, in a ring
-  uint64_t win_every = 0;
-  uint64_t win_n = 0;               // steps recorded since the last configuration with every > 0
-  std::unique_ptr<eb_chain> win;    // the ring (ring == true), or null before any configuration
-  std::vector<uint64_t> win_steps;  // [capacity] the step counter and the Philox key of each physical slot's step
-  std::vector<uint64_t> win_seeds;
+  RunningStats run;  // the running statistics (running.h)
+  DevPtr<double> mom_partial;  // per-CTA partials of one moment accumulation (launch_moments)
 
   // WalkMove / GaussianMove scratch (moves_extra.cu)
   DevPtr<double> qbuf;       // [N, D] proposals
@@ -322,6 +276,33 @@ enum { CB_STEP = 0, CB_SET_STATE = 1, CB_COMPUTE = 2 };
       FAIL(ctx, EB_ERR_NOMEM, __VA_ARGS__); \
     }                                       \
   } while (0)
+
+// `bytes` of device memory must fit in what is free, else the call fails with EB_ERR_NOMEM: "<who>: <n> bytes of
+// <what>, <free> bytes free".  Obj is an engine or a chain.
+template <class Obj>
+int check_free(Obj* c, const char* who, const char* what, size_t bytes) {
+  size_t free_b = 0, total_b = 0;
+  CK(c, cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > free_b) FAIL(c, EB_ERR_NOMEM, "%s: %zu bytes of %s, %zu bytes free", who, bytes, what, free_b);
+  return EB_OK;
+}
+
+// allocate `bytes` of device memory into `out`, refused by check_free before anything is allocated
+template <class Obj, class T>
+int dev_alloc_checked(Obj* c, const char* who, const char* what, size_t bytes, DevPtr<T>& out) {
+  const int rc = check_free(c, who, what, bytes);
+  if (rc) return rc;
+  CK_NOMEM(c, dev_alloc(out, bytes), "%s: allocating %zu bytes of %s failed (%s)", who, bytes, what,
+           cudaGetErrorString(alloc_err));
+  return EB_OK;
+}
+
+// an empty chain of nwalkers x ndim on `device`: its stream and its [N] accept buffers (eb_chain_create, and the ring
+// of eb_window_config); synchronises
+cudaError_t chain_init(eb_chain* ch, int device, int64_t nwalkers, int ndim);
+// mean[D], cov[D * D] of m samples from the sums acc = [S1 | S2] about `shift` (eb_moments, eb_chain_moments):
+// mean = shift + S1 / m, cov = (S2 - S1 S1^T / m) / (m - 1)   (np.cov(flatchain, rowvar=False)); NaN when m == 0
+void finish_moments(const double* acc, const double* shift, uint64_t count, size_t D, double* mean, double* cov);
 
 // a graph model (eb_model_set_graphs): its half-steps report errors through graph_err, read by fetch_status
 inline bool graph_mode(const eb_ctx* c) { return c->model.kind == MODEL_EXTERNAL && c->cb_where == EB_CALLBACK_GRAPH; }

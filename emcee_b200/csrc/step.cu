@@ -1,6 +1,6 @@
 // The host-side step driver of the C ABI: the move schedule, the half-step launches of every move kind, the
-// dense_dmma grouping, the per-step running statistics, and eb_step / eb_step_store / eb_step_store_blobs /
-// eb_step_store_chain.
+// dense_dmma grouping, the calls into the running statistics (running.cu), and eb_step / eb_step_store /
+// eb_step_store_blobs / eb_step_store_chain.
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -931,13 +931,6 @@ int upload_chunk(eb_ctx* c, const Chunk& ch, uint64_t& launches) {
   return EB_OK;
 }
 
-// run nsteps steps.  `after_step(k)` is called with the work of step k enqueued and may
-// enqueue copies on the stream; `sync_every` > 0 tells how often it actually does (every
-// sync_every-th step), so that steps in between can share one persistent launch.
-int reserve_trace(eb_ctx* c, uint64_t nsteps);                    // below
-unsigned stats_due(const eb_ctx* c, uint64_t n);                  // below
-int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches);  // below
-
 // graph mode (eb_model_set_graphs, eb_move_set_proposal_graphs): run_steps logs the steps it enqueues for
 // check_status while it runs
 struct GraphRun {
@@ -950,6 +943,9 @@ struct GraphRun {
   ~GraphRun() { c->graph_run = false; }
 };
 
+// run nsteps steps.  `after_step(k)` is called with the work of step k enqueued and may
+// enqueue copies on the stream; `sync_every` > 0 tells how often it actually does (every
+// sync_every-th step), so that steps in between can share one persistent launch.
 template <class F>
 int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every, F&& after_step) {
   uint64_t launches = 0;
@@ -964,10 +960,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
       c->ev_pool.push_back(std::move(e));
     }
   }
-  if (c->trace_every > 0) {
-    const int rc = reserve_trace(c, nsteps);
-    if (rc) return rc;
-  }
+  if (const int rc = running_prepare(c, nsteps)) return rc;
   c->dmma_nhalf_max = 0;
   CK(c, cudaEventRecord(c->ev0.get(), c->st.get()));
   if (comm_begin(c->comm, c->st.get(), c->status_dev.get(), launches)) FAIL(c, EB_ERR_COMM, "%s", c->comm.err.c_str());
@@ -999,7 +992,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         rc = fetch_status(c);
         if (rc) return rc;
       }
-      const unsigned due = stats_due(c, c->step + 1);
+      const bool due = running_due(c, c->step + 1);
       const bool stored = sync_every > 0 && (done + k + 1) % sync_every == 0;  // after_step enqueues copies
       if (perstep) {
         CK(c, cudaMemsetAsync(c->flush_buf.get(), (int)(k & 0xff), c->flush_bytes, c->st.get()));
@@ -1080,7 +1073,7 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
         }
       }
       if (due) {
-        rc = accumulate_due(c, due, launches);
+        rc = running_record(c, launches);
         if (rc) return rc;
         chain.live = false;
       }
@@ -1115,127 +1108,6 @@ int run_steps(eb_ctx* c, const Schedule& s, uint64_t nsteps, uint64_t sync_every
   }
   c->last_launches = launches;
   return check_status(c);
-}
-
-// ---- running statistics ------------------------------------------------------------------------
-// fold the rows this rank owns of the CURRENT state into the accumulators (enqueued on the stream)
-int accumulate_moments(eb_ctx* c, uint64_t& launches) {
-  int64_t r0, r1;
-  owned_rows(c, r0, r1);
-  const double* X = c->coords.get() + (size_t)r0 * c->D;
-  if (!c->mom_have_shift) {
-    // shift = the ensemble mean at the first accumulation: keeps the raw second moments well conditioned
-    CK(c, launch_colmean(X, r1 - r0, c->D, c->mom_shift.get(), nullptr, c->st.get()));
-    c->mom_have_shift = true;
-    ++launches;
-  }
-  CK(c, launch_moments(X, r1 - r0, c->D, c->mom_shift.get(), c->mom_partial.get(), c->mom_acc.get(), c->sm_count,
-                       c->st.get()));
-  launches += 2;
-  c->mom_count += (unsigned long long)(r1 - r0);
-  return EB_OK;
-}
-
-// count the CURRENT state into the running histograms (kernels only, enqueued on the stream)
-int accumulate_histograms(eb_ctx* c, uint64_t& launches) {
-  CK(c, live_hist_launch(c->hist, c->st.get(), launches));
-  c->hist_count += (unsigned long long)c->N;
-  return EB_OK;
-}
-
-// Room for the rows the next `nsteps` steps record, made before the first launch: the rows already recorded move
-// into a larger allocation (half as large again when that fits, so that a run of many short calls grows a few times).
-int reserve_trace(eb_ctx* c, uint64_t nsteps) {
-  const uint64_t add = (c->step + nsteps) / c->trace_every - c->step / c->trace_every;
-  const uint64_t have = c->trace_steps.size(), need = have + add;
-  if (need <= c->trace_cap) return EB_OK;
-  const size_t row = (2 * (size_t)c->D + TRACE_EXTRA) * sizeof(double);
-  size_t free_b = 0, total_b = 0;
-  CK(c, cudaMemGetInfo(&free_b, &total_b));
-  uint64_t cap = std::max(need, c->trace_cap + c->trace_cap / 2);
-  if (cap > free_b / row) cap = need;
-  if (cap > free_b / row)
-    FAIL(c, EB_ERR_NOMEM, "the trace needs room for %llu rows of %zu bytes, %zu bytes free", (unsigned long long)need,
-         row, free_b);
-  DevPtr<double> rows;
-  CK_NOMEM(c, dev_alloc(rows, (size_t)cap * row), "the trace: allocating %llu rows of %zu bytes failed (%s)",
-           (unsigned long long)cap, row, cudaGetErrorString(alloc_err));
-  if (have)
-    CK(c, cudaMemcpyAsync(rows.get(), c->trace_rows.get(), (size_t)have * row, cudaMemcpyDeviceToDevice, c->st.get()));
-  CK(c, cudaStreamSynchronize(c->st.get()));
-  c->trace_rows = std::move(rows);
-  c->trace_cap = cap;
-  c->trace_steps.reserve((size_t)cap);
-  return EB_OK;
-}
-
-// record the CURRENT state as one row of the trace (kernels only, enqueued on the stream)
-int accumulate_trace(eb_ctx* c, uint64_t& launches) {
-  double* row = c->trace_rows.get() + c->trace_steps.size() * (2 * (size_t)c->D + TRACE_EXTRA);
-  CK(c, live_trace_launch(c->trace, row, c->step, c->st.get(), launches));
-  c->trace_steps.push_back(c->step);
-  return EB_OK;
-}
-
-// offer the CURRENT state's rows to the reservoir, behind a compaction when the rows could overflow its buffer
-// (kernels only, enqueued on the stream)
-int accumulate_reservoir(eb_ctx* c, uint64_t& launches) {
-  if (c->res_plan.compact_before_record()) {
-    CK(c, live_reservoir_compact(c->res, c->res_plan.bound, c->st.get(), launches));
-    c->res_plan.compacted();
-  }
-  CK(c, live_reservoir_record(c->res, c->seed, c->step, c->st.get(), launches));
-  c->res_plan.recorded();
-  return EB_OK;
-}
-
-// write the CURRENT state into the autocorrelation ring, and fold the block of lag sums it completes (kernels only,
-// enqueued on the stream)
-int accumulate_running_acf(eb_ctx* c, uint64_t& launches) {
-  CK(c, live_racf_record(c->racf, c->racf_n, c->st.get(), launches));
-  c->racf_n += 1;
-  return EB_OK;
-}
-
-// copy the CURRENT state and the step's accept mask into the window's ring, at physical slot win_n mod size (a kernel
-// enqueued on the stream); once the ring is full the oldest slot moves on with every record
-int accumulate_window(eb_ctx* c, uint64_t& launches) {
-  eb_chain* w = c->win.get();
-  const uint64_t size = w->start.back(), slot = c->win_n % size;
-  CK(c, launch_chain_store(c->coords.get(), c->logp.get(), c->accepted.get(), w->segs[0].x.get() + slot * w->xs,
-                           w->segs[0].lp.get() + slot * w->ls, nullptr, (size_t)c->N * c->D, (size_t)c->N, c->N,
-                           c->sm_count, c->st.get(), w->slot_mask.get() + slot * (uint64_t)c->N));
-  ++launches;
-  c->win_steps[(size_t)slot] = c->step;
-  c->win_seeds[(size_t)slot] = c->seed;
-  c->win_n += 1;
-  w->filled = std::min(c->win_n, size);
-  w->origin = c->win_n >= size ? c->win_n % size : 0;
-  return EB_OK;
-}
-
-enum : unsigned {
-  STAT_MOMENTS = 1, STAT_HIST = 2, STAT_TRACE = 4, STAT_RESERVOIR = 8, STAT_AUTOCORR = 16, STAT_WINDOW = 32
-};
-
-// the running statistics that record the state once the step counter reaches n: each its every `*_every`-th step
-unsigned stats_due(const eb_ctx* c, uint64_t n) {
-  const auto at = [n](uint64_t every) { return every > 0 && n % every == 0; };
-  return (at(c->moments_every) ? STAT_MOMENTS : 0u) | (at(c->hist_every) ? STAT_HIST : 0u) |
-         (at(c->trace_every) ? STAT_TRACE : 0u) | (at(c->res_every) ? STAT_RESERVOIR : 0u) |
-         (at(c->racf_every) ? STAT_AUTOCORR : 0u) | (at(c->win_every) ? STAT_WINDOW : 0u);
-}
-
-// the accumulations `due` (stats_due) of the CURRENT state, enqueued on the stream
-int accumulate_due(eb_ctx* c, unsigned due, uint64_t& launches) {
-  int rc = EB_OK;
-  if (due & STAT_MOMENTS) rc = accumulate_moments(c, launches);
-  if (!rc && (due & STAT_HIST)) rc = accumulate_histograms(c, launches);
-  if (!rc && (due & STAT_TRACE)) rc = accumulate_trace(c, launches);
-  if (!rc && (due & STAT_RESERVOIR)) rc = accumulate_reservoir(c, launches);
-  if (!rc && (due & STAT_AUTOCORR)) rc = accumulate_running_acf(c, launches);
-  if (!rc && (due & STAT_WINDOW)) rc = accumulate_window(c, launches);
-  return rc;
 }
 
 int step_preflight(eb_ctx* c) {

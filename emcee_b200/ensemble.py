@@ -34,17 +34,22 @@ _NO_SHARDED_DEVICE_CHAIN = (
     "of the other ranks' rows before each stored step is built for host chains only; use Backend()"
 )
 _NO_DEVICE_CHAIN_BLOBS = "a DeviceBackend does not store blobs; use Backend() with a function that returns blobs"
-_NO_SHARDED_HISTOGRAMS = "running histograms are counted on one GPU; they cannot be combined with a sharded ensemble"
-_NO_HISTOGRAMS = "running histograms are not enabled: call enable_histograms(range, ...) first"
-_NO_SHARDED_TRACE = "the running trace is recorded on one GPU; it cannot be combined with a sharded ensemble"
-_NO_TRACE = "the running trace is not enabled: call enable_trace() first"
-_NO_SHARDED_RESERVOIR = "the running reservoir is kept on one GPU; it cannot be combined with a sharded ensemble"
-_NO_RESERVOIR = "the running reservoir is not enabled: call enable_reservoir(size) first"
-_NO_SHARDED_AUTOCORR = (
-    "the running autocorrelation is summed on one GPU; it cannot be combined with a sharded ensemble"
+#: the running statistics other than the moments: the sampler attribute that holds each one's configuration, and the
+#: refusal of a sharded ensemble.  The attribute is None until the statistic is enabled, and again after unpickling:
+#: what was recorded lives in the engine's memory.  It holds the histograms' configuration of enable_histograms (edges,
+#: pairs), the cadence the trace and the reservoir recorded their rows with, and the (max_lag, every) of the
+#: autocorrelation and the (size, every) of the window.
+_RUNNING = (
+    ("_hist", "running histograms are counted on one GPU; they cannot be combined with a sharded ensemble"),
+    ("_trace_every", "the running trace is recorded on one GPU; it cannot be combined with a sharded ensemble"),
+    ("_reservoir_every", "the running reservoir is kept on one GPU; it cannot be combined with a sharded ensemble"),
+    ("_autocorr", "the running autocorrelation is summed on one GPU; it cannot be combined with a sharded ensemble"),
+    ("_window", "the running window is kept on one GPU; it cannot be combined with a sharded ensemble"),
 )
+_NO_HISTOGRAMS = "running histograms are not enabled: call enable_histograms(range, ...) first"
+_NO_TRACE = "the running trace is not enabled: call enable_trace() first"
+_NO_RESERVOIR = "the running reservoir is not enabled: call enable_reservoir(size) first"
 _NO_AUTOCORR = "the running autocorrelation is not enabled: call enable_autocorr(max_lag) first"
-_NO_SHARDED_WINDOW = "the running window is kept on one GPU; it cannot be combined with a sharded ensemble"
 _NO_WINDOW = "the running window is not enabled: call enable_window(size) first"
 _NO_SHARDED_CUDA_ARRAYS = (
     "CUDA arrays in and out are copied on one GPU; a sharded ensemble takes and returns host arrays"
@@ -63,6 +68,14 @@ _NOT_INDEPENDENT = (
 Trace = namedtuple("Trace", ["step", "mean", "var", "log_prob_mean", "log_prob_max", "accepted"])
 #: what :meth:`EnsembleSampler.reservoir` returns: one entry per kept row
 Reservoir = namedtuple("Reservoir", ["coords", "log_prob", "step", "walker"])
+
+
+def _index_at_least(name, value, least):
+    """``operator.index(value)`` (``TypeError`` for what is not an integer), ``ValueError`` below ``least``."""
+    value = operator.index(value)
+    if value < least:
+        raise ValueError("{0} must be >= {1}, got {2}".format(name, least, value))
+    return value
 
 
 def _seed_from_numpy():
@@ -185,11 +198,8 @@ class EnsembleSampler(object):
             self._pinned = (_lib.pinned_empty((self.nwalkers, self.ndim)), _lib.pinned_empty((self.nwalkers,)))
         self._cuda_results = bool(cuda_results)
         self._rdv = None  # multi-GPU: the host rendezvous this sampler is attached to (``attach``)
-        self._hist = None  # running histograms: the configuration of enable_histograms (edges, pairs)
-        self._trace_every = None  # running trace: the cadence its rows were recorded with (enable_trace)
-        self._reservoir_every = None  # running reservoir: the cadence its rows were recorded with (enable_reservoir)
-        self._autocorr = None  # running autocorrelation: (max_lag, every) its sums were recorded with (enable_autocorr)
-        self._window = None  # running window: (size, every) its steps were recorded with (enable_window)
+        for attr, _ in _RUNNING:
+            setattr(self, attr, None)
         self._gather_results = True
 
         self.backend = Backend() if backend is None else backend
@@ -292,11 +302,8 @@ class EnsembleSampler(object):
         for k in ("_engine", "_random", "_pinned"):
             d.pop(k, None)
         d["_rdv"] = None  # a communicator does not survive pickling: re-attach after loading
-        d["_hist"] = None  # the running histograms live in the engine's memory: enable them again after loading
-        d["_trace_every"] = None  # and so do the rows of the running trace
-        d["_reservoir_every"] = None  # and the rows of the running reservoir
-        d["_autocorr"] = None  # and the lag sums of the running autocorrelation
-        d["_window"] = None  # and the steps of the running window
+        for attr, _ in _RUNNING:
+            d[attr] = None  # the running statistics live in the engine's memory: enable them again after loading
         d["pool"] = None
         return d
 
@@ -329,16 +336,9 @@ class EnsembleSampler(object):
             raise NotImplementedError(_NO_SHARDED_DEVICE_CHAIN)
         if getattr(self, "_cuda_results", False):
             raise NotImplementedError("cuda_results=True: " + _NO_SHARDED_CUDA_ARRAYS)
-        if getattr(self, "_hist", None) is not None:
-            raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
-        if getattr(self, "_trace_every", None) is not None:
-            raise NotImplementedError(_NO_SHARDED_TRACE)
-        if getattr(self, "_reservoir_every", None) is not None:
-            raise NotImplementedError(_NO_SHARDED_RESERVOIR)
-        if getattr(self, "_autocorr", None) is not None:
-            raise NotImplementedError(_NO_SHARDED_AUTOCORR)
-        if getattr(self, "_window", None) is not None:
-            raise NotImplementedError(_NO_SHARDED_WINDOW)
+        for attr, refusal in _RUNNING:
+            if getattr(self, attr, None) is not None:
+                raise NotImplementedError(refusal)
         if isinstance(self.log_prob_fn, CallbackFunction):
             raise NotImplementedError("a user log-probability function runs on one GPU; it cannot be sharded")
         if any(user_move_spec(m) is not None for m in self._moves):
@@ -354,6 +354,11 @@ class EnsembleSampler(object):
         """``slice`` of the walkers this process updates (all of them on one GPU)."""
         r0, n = self._engine.owned_rows()
         return slice(r0, r0 + n)
+
+    def _refuse_sharded(self, attr):
+        """Enabling the running statistic held in ``attr`` (``_RUNNING``) on a sharded ensemble raises."""
+        if self._rdv is not None:
+            raise NotImplementedError(dict(_RUNNING)[attr])
 
     def enable_moments(self, every=1):
         """Accumulate the chain mean / covariance on the device after every
@@ -388,11 +393,8 @@ class EnsembleSampler(object):
         The counts are not pickled, and a sharded ensemble is refused."""
         from .summary import running_histogram_plan
 
-        if self._rdv is not None:
-            raise NotImplementedError(_NO_SHARDED_HISTOGRAMS)
-        every = operator.index(every)
-        if every < 0:
-            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._refuse_sharded("_hist")
+        every = _index_at_least("every", every, 0)
         cfg = running_histogram_plan(self.ndim, range, bins, log_prob_range, params2d, bins2d)
         self._hist = None
         self._engine.histograms_config(every, cfg["bins"], cfg["outer"], cfg["edges"], cfg["log_prob"],
@@ -443,11 +445,8 @@ class EnsembleSampler(object):
         Every call with ``every > 0`` drops the rows and the best sample recorded so far; ``every=0`` records nothing
         more and leaves them readable.  The initial state is never recorded.  The rows are not pickled, and a
         sharded ensemble is refused."""
-        if self._rdv is not None:
-            raise NotImplementedError(_NO_SHARDED_TRACE)
-        every = operator.index(every)
-        if every < 0:
-            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._refuse_sharded("_trace_every")
+        every = _index_at_least("every", every, 0)
         self._engine.trace_config(every)
         if every > 0 or self._trace_every is None:
             self._trace_every = every
@@ -464,9 +463,7 @@ class EnsembleSampler(object):
         fixed order that depends on ``nwalkers`` alone, so the same steps give the same bytes however they were
         run."""
         self._trace_on()
-        discard = operator.index(discard)
-        if discard < 0:
-            raise ValueError("discard must be >= 0, got {0}".format(discard))
+        discard = _index_at_least("discard", discard, 0)
         step, rows = self._engine.trace_read(discard)
         D = self.ndim
         return Trace(step, rows[:, :D].copy(), rows[:, D:2 * D].copy(), rows[:, 2 * D].copy(),
@@ -505,14 +502,9 @@ class EnsembleSampler(object):
         Every call with ``every > 0`` drops what was kept; ``every=0`` records nothing more and leaves the contents
         readable.  The initial state is never recorded and blobs are not kept.  The contents are not pickled, and a
         sharded ensemble is refused."""
-        if self._rdv is not None:
-            raise NotImplementedError(_NO_SHARDED_RESERVOIR)
-        size = operator.index(size)
-        if size < 1:
-            raise ValueError("size must be >= 1, got {0}".format(size))
-        every = operator.index(every)
-        if every < 0:
-            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._refuse_sharded("_reservoir_every")
+        size = _index_at_least("size", size, 1)
+        every = _index_at_least("every", every, 0)
         self._engine.reservoir_config(size, every)
         if every > 0 or getattr(self, "_reservoir_every", None) is None:
             self._reservoir_every = every
@@ -548,14 +540,9 @@ class EnsembleSampler(object):
         Every call with ``every > 0`` drops what was recorded; ``every=0`` records nothing more and leaves the results
         readable.  The sums cannot forget steps, so there is no ``discard``: to leave burn-in out, enable after it.
         The sums are not pickled, and a sharded ensemble is refused."""
-        if self._rdv is not None:
-            raise NotImplementedError(_NO_SHARDED_AUTOCORR)
-        max_lag = operator.index(max_lag)
-        if max_lag < 1:
-            raise ValueError("max_lag must be >= 1, got {0}".format(max_lag))
-        every = operator.index(every)
-        if every < 0:
-            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._refuse_sharded("_autocorr")
+        max_lag = _index_at_least("max_lag", max_lag, 1)
+        every = _index_at_least("every", every, 0)
         self._engine.running_acf_config(max_lag, every)
         if every > 0 or getattr(self, "_autocorr", None) is None:  # every=0 keeps the lags and cadence recorded
             self._autocorr = (max_lag, every)
@@ -605,14 +592,9 @@ class EnsembleSampler(object):
 
         Every call with ``every > 0`` drops what was recorded; ``every=0`` records nothing more and leaves the
         contents readable.  Blobs are not kept.  The contents are not pickled, and a sharded ensemble is refused."""
-        if self._rdv is not None:
-            raise NotImplementedError(_NO_SHARDED_WINDOW)
-        size = operator.index(size)
-        if size < 1:
-            raise ValueError("size must be >= 1, got {0}".format(size))
-        every = operator.index(every)
-        if every < 0:
-            raise ValueError("every must be >= 0, got {0}".format(every))
+        self._refuse_sharded("_window")
+        size = _index_at_least("size", size, 1)
+        every = _index_at_least("every", every, 0)
         self._engine.window_config(size, every)
         if every > 0 or getattr(self, "_window", None) is None:  # every=0 keeps the size and cadence recorded
             self._window = (size, every)
