@@ -1613,7 +1613,7 @@ class Engine(object):
         buf = np.zeros(1 << 21, dtype=np.int64)
         n = C.c_size_t()
         self._check(lib().eb_debug_timeline(self._h, buf.ctypes.data_as(C.POINTER(C.c_int64)), buf.size, C.byref(n)))
-        return buf[: n.value].reshape(-1, 8, 8, 10)  # events 0..5 consumer, 6..8 producer (dense_dmma.cu)
+        return buf[: n.value].reshape(-1, 8, 8, 12)  # events 0..5, 9 consumer; 6..8, 10, 11 producer (dense_dmma.cu)
 
     # -- multi-GPU ---------------------------------------------------------------
     @staticmethod

@@ -238,6 +238,9 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   if (HAS_MEAN)
     for (int k = tid; k < D; k += DMMA_THREADS) sMu[k] = a.model.params[k];
   __syncthreads();
+  // TIMELINE stamps count cycles from here, where every warp of the CTA leaves the same barrier, so a producer's
+  // stamps and its consumer's compare directly
+  const long long t_base = TIMELINE ? clock64() : 0;
 
   // tile indices fit 32 bits: a half-step has at most 2^31 / 8 tiles (HalfDesc::a_count is an int32)
   const int tstride = (int)gridDim.x * DMMA_CONSUMERS;
@@ -258,9 +261,9 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   if (is_producer) {
     if constexpr (REBALANCE) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DMMA_PRODUCER_REGS));
     // ================= producer: draws, lookups, TMA row gather, proposal =================
-    // optional stamps of the LAST half-step, events 6..8 of the tile's record (cycles since this warp entered
-    // the kernel): 6 rows requested, 7 rows landed, 8 proposal published
-    const long long t_entry_p = clock64();
+    // optional stamps of the LAST half-step, events 6..8 of the tile's record (cycles since t_base): 6 rows
+    // requested, 7 rows landed, 8 proposal published; and, in the first tile's record, 10 griddepcontrol.wait
+    // returned (the predecessor kernel is complete), 11 partner rows requested (= 6 unless early own rows)
     long long* tlp = (TIMELINE && lane == 0)
                          ? a.timeline + ((size_t)blockIdx.x * DMMA_CONSUMERS + pair) * TL_TILES * TL_EVENTS : nullptr;
     const double dm1 = (double)a.D - 1.0;
@@ -325,8 +328,15 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
           const int32_t wr = partner ? p.wp : p.w;
           const double* base =
               (partner && a.peer_coords != nullptr) ? a.peer_coords[wr / a.rows_per_rank] : a.coords;
-          bulk_g2s(slot + (size_t)(partner ? 8 : 0) * RS + (size_t)row * RS, base + (size_t)wr * D,
-                   (unsigned)(D * sizeof(double)), barFull + pair);
+          double* dst = slot + (size_t)(partner ? 8 : 0) * RS + (size_t)row * RS;
+          // An active walker's own row is read once per half-step: the consumer writes an accepted row from its
+          // registers.  Partner rows are drawn with replacement and read again within the half-step, so the
+          // own rows' lines are the ones L2 should give up first.
+          if (partner)
+            bulk_g2s(dst, base + (size_t)wr * D, (unsigned)(D * sizeof(double)), barFull + pair);
+          else
+            bulk_g2s_hint(dst, base + (size_t)wr * D, (unsigned)(D * sizeof(double)), barFull + pair,
+                          l2_evict_first_policy());
         }
       };
       auto publish = [&](const Prep& p, int par) {
@@ -358,7 +368,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         cur = prep(tile0, true);
         if (lane == 0) mbar_arrive_expect_tx(barFull + pair, 16u * D * (unsigned)sizeof(double));
         __syncwarp();
-        if (tlp) tlp[6] = clock64() - t_entry_p;
+        if (tlp) tlp[6] = clock64() - t_base;
         request(cur, 0, 8);
       } else if (tile0 < ntiles) {
         cur = prep(tile0, false);  // (the old log-prob is state: it is read behind the barrier)
@@ -369,6 +379,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         // kernel wrote may be read from here on
         pdl_wait();
         pdl_launch_dependents();
+        if (tlp) tlp[10] = clock64() - t_base;
         // (a completed predecessor kernel needs no proxy fence: griddepcontrol.wait returns with its writes
         // performed; the fence costs ~1 us per launch).  Sharded: the peer barrier is NOT taken here -- tiles
         // whose partners are local start at once; issue() takes it before the first remote fetch, pair 0's
@@ -383,11 +394,15 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
           // (best effort: a bounded peek at the neighbour's barrier, never a dependency)
           if (a.dmma_stagger && pair >= DMMA_CONSUMERS / 2)
             mbar_wait_for(barFull + pair - DMMA_CONSUMERS / 2, 0, multi ? 40000 : 12000);
+          if (tlp) {
+            const long long t_req = clock64() - t_base;
+            tlp[11] = t_req;
+            if (!early) tlp[6] = t_req;
+          }
           if (early) {
             request(cur, 8, 16);
             publish(cur, (int)(k & 1u));
           } else {
-            if (tlp) tlp[6] = clock64() - t_entry_p;
             if (!issue(cur, (int)(k & 1u), true)) return;
           }
         }
@@ -419,7 +434,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         if (!mbar_wait_abortable(barFull + pair, k & 1u, sAbort)) return;
         long long* tlq = (tlp && h == nhalf - 1 && (tile - tile0) / tstride < TL_TILES && lane == 0)
                              ? tlp + ((tile - tile0) / tstride) * TL_EVENTS : nullptr;
-        if (tlq) tlq[7] = clock64() - t_entry_p;
+        if (tlq) tlq[7] = clock64() - t_base;
         if constexpr (BOUNDED) {
           // the same pass tests the prior's support: lane (g, t) checks its columns, the 4 lanes of row g AND
           bool in = true;
@@ -447,13 +462,13 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(barReady + pair);
-        if (tlq) tlq[8] = clock64() - t_entry_p;
+        if (tlq) tlq[8] = clock64() - t_base;
         // ---- as soon as the consumer has the proposal in registers, refill the slot
         if (tile + tstride < ntiles) {
           cur = nxt;
           if (!mbar_wait_abortable(barFree + pair, k & 1u, sAbort)) return;
           if (tlq && (tile - tile0) / tstride + 1 < TL_TILES)
-            tlq[TL_EVENTS + 6] = clock64() - t_entry_p;  // (stamp 6 of the NEXT tile: its rows are requested)
+            tlq[TL_EVENTS + 6] = clock64() - t_base;  // (stamp 6 of the NEXT tile: its rows are requested)
           if (!issue(cur, (int)((k + 1) & 1u), h > 0 && tile == tile0)) return;
           if (tile + 2 * tstride < ntiles) nxt = prep(tile + 2 * tstride, true);
         }
@@ -469,9 +484,8 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
     mbar_arrive_expect_tx(barL, bytes);
     bulk_g2s(sL, a.model.chol, bytes, barL);
   }
-  // optional per-tile timestamps of the LAST half-step (cycles since this warp entered the kernel):
-  // 1 wait start, 2 proposal ready, 3 proposal in registers, 4 DMMA block done, 5 tile done
-  const long long t_entry = clock64();
+  // optional per-tile timestamps of the LAST half-step (cycles since t_base): 1 wait start, 2 proposal ready,
+  // 3 proposal in registers, 4 DMMA block done, 5 tile done; and, in the first tile's record, 9 factor landed
   long long* tl = TIMELINE ? a.timeline + ((size_t)blockIdx.x * DMMA_CONSUMERS + pair) * TL_TILES * TL_EVENTS : nullptr;
   pdl_wait();  // nothing of this warp's global traffic may overtake the previous kernel
   pdl_launch_dependents();
@@ -479,6 +493,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   // siblings, so nobody is left waiting for a warp that left.
   // (the consumer's waits have no trap: with one, ptxas would not let this code use the raised register limit)
   bool alive = mbar_wait_abortable_notrap(barL, 0, sAbort, a.status, FLAG_WAIT_TIMEOUT);
+  if (TIMELINE && lane == 0) tl[9] = clock64() - t_base;
   for (int h = 0; h < nhalf; ++h) {
     const HalfDesc d = (h == 0) ? d0 : descs[h];
     const int2 rg = a.range ? a.range[(size_t)d.order_step * MAX_SPLITS + d.split] : make_int2(0, d.a_count);
@@ -490,13 +505,13 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       long long* tlk = (tl && h == nhalf - 1 && kk < TL_TILES && lane == 0) ? tl + kk * TL_EVENTS : nullptr;
       if (tlk) {
         tlk[0] = (long long)tile;
-        tlk[1] = clock64() - t_entry;
+        tlk[1] = clock64() - t_base;
       }
       if (!mbar_wait_abortable_notrap(barReady + pair, k & 1u, sAbort, a.status, FLAG_WAIT_TIMEOUT)) {
         alive = false;
         break;
       }
-      if (tlk) tlk[2] = clock64() - t_entry;
+      if (tlk) tlk[2] = clock64() - t_base;
       double q[2 * KB];
 #pragma unroll
       for (int j = 0; j < KB; ++j) {
@@ -506,7 +521,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(barFree + pair);  // the slot may be refilled while this tile computes
-      if (tlk) tlk[3] = clock64() - t_entry;
+      if (tlk) tlk[3] = clock64() - t_base;
 
       // ---- y = L^T (q - mu) on the tensor pipe; rs = sum_n y_n^2
       const double rs = tile_sumsq<KB, HAS_MEAN>(q, sL, sMu, lane, g, t);
@@ -516,7 +531,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       const int32_t w = m->w[g];
       const double factor = m->factor[g], log_u = m->log_u[g], lp_old = m->lp_old[g];
       const double lp_new = (BOUNDED && sInbox[(2 * pair + (k & 1u)) * 8 + g] == 0) ? -INFINITY : -0.5 * rs;
-      if (tlk) tlk[4] = clock64() - t_entry;
+      if (tlk) tlk[4] = clock64() - t_base;
 
       // ---- guards (ensemble.py:476-479, 550-551): a non-finite lp is the only way
       // a non-finite coordinate can show, so the element scan is off the fast path
@@ -560,7 +575,7 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
         }
         a.accepted[w] = acc ? 1 : 0;
       }
-      if (tlk) tlk[5] = clock64() - t_entry;
+      if (tlk) tlk[5] = clock64() - t_base;
     }
     if (h + 1 < nhalf) {
       // this CTA's updates of half-step h are out: tell the grid (consumer warps only, named barrier 1)

@@ -14,7 +14,9 @@ namespace eb {
 
 constexpr int MAX_SPLITS = 32;      // split_table_kernel uses one warp per set
 constexpr int TABLE_THREADS = 1024;
-constexpr int TL_TILES = 8, TL_EVENTS = 10;  // dense_dmma timeline buffer shape (6 consumer + 4 producer stamps)
+// dense_dmma timeline buffer shape: per tile record 0 tile id, 1..5 and 9 consumer stamps, 6..8, 10 and 11 producer
+// stamps (dense_dmma.cu)
+constexpr int TL_TILES = 8, TL_EVENTS = 12;
 
 // device status flags (OR-ed by kernels, read back after every call)
 enum : int {

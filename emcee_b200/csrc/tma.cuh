@@ -82,6 +82,21 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned by
                : "memory");
 }
 
+// the same copy with an L2 eviction priority (`policy` from l2_evict_first_policy)
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, unsigned bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+// L2 cache policy: the lines a copy brings in are the first to be evicted
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+
 // shared -> global bulk copy (TMA store); completion tracked by the thread's bulk async-group
 __device__ __forceinline__ void bulk_s2g(void* dst, const void* src, unsigned bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes)

@@ -760,8 +760,8 @@ int eb_last_step_timing(const eb_ctx* ctx, double* ms, uint64_t* launches);
 int eb_debug_taps(eb_ctx* ctx, int64_t* partners, double* scalar, double* u_accept,
                   int64_t* active, int64_t* nactive);
 /* per-tile cycle stamps of the dense_dmma consumers during the LAST half-step
- * launched (option "dmma_timeline"): [SM][8 consumers][8 tiles][10 events]
- * (0..5 consumer, 6..8 producer). */
+ * launched (option "dmma_timeline"): [SM][8 consumers][8 tiles][12 events]
+ * (0..5 and 9 consumer, 6..8, 10 and 11 producer). */
 int eb_debug_timeline(eb_ctx* ctx, int64_t* out, size_t capacity, size_t* written);
 /* engine options: "debug_taps" (0/1: record the draws of each half-step for
  * eb_debug_taps; forces the generic kernel), "dense_dmma" (0/1: allow the
