@@ -237,6 +237,16 @@ _SIGNATURES = {
     ),
     "eb_chain_moments_segments": (
         C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_uint64, _dp, _dp, C.POINTER(C.c_uint64)]),
+    "eb_chain_histogram_segments": (
+        C.c_int,
+        [C.c_void_p, C.c_int64, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, _dp, _dp,
+         C.POINTER(C.c_uint64)],
+    ),
+    "eb_chain_histogram2d_segments": (
+        C.c_int,
+        [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint32), C.c_size_t, C.c_uint32,
+         _dp, C.POINTER(C.c_uint64)],
+    ),
 }
 
 _lib = None
@@ -1045,30 +1055,36 @@ class Chain(object):
         self._check(fn(self._h, *args, int(first), int(stride), int(count), _as_dp(mean), _as_dp(cov), C.byref(n)))
         return mean, cov, int(n.value)
 
-    def histogram(self, what, first, stride, count, bins, outer, edges):
+    def histogram(self, what, first, stride, count, bins, outer, edges, nseg=1):
         """``hist[D, bins]`` (int64) of the stored slice with numpy's uniform-bin rule (``eb_chain_histogram``):
         ``outer[D, 3]`` holds each column's ``(first_edge, last_edge, norm_denom)``, ``edges[D, bins + 1]`` its
-        edges; ``what`` is ``"chain"`` (D = ndim) or ``"log_prob"`` (D = 1)."""
-        D = self.ndim if what == "chain" else 1
+        edges; ``what`` is ``"chain"`` (D = ndim) or ``"log_prob"`` (D = 1).  With ``nseg > 1``, those of each
+        segment of ``nwalkers / nseg`` walkers: ``outer[nseg * D, 3]`` and ``edges[nseg * D, bins + 1]`` in column
+        order ``k * D + d``, ``hist[nseg * D, bins]`` (``eb_chain_histogram_segments``)."""
+        nseg = int(nseg)
+        D = nseg * (self.ndim if what == "chain" else 1)
         bins = int(bins)
         outer = _f64(outer, (D, 3))
         edges = _f64(edges, (D, bins + 1))
         hist = np.empty((D, bins), dtype=np.uint64)
-        self._check(lib().eb_chain_histogram(
-            self._h, EB_CHAIN_COORDS if what == "chain" else EB_CHAIN_LOG_PROB, int(first), int(stride), int(count),
-            bins, _as_dp(outer), _as_dp(edges), hist.ctypes.data_as(C.POINTER(C.c_uint64))))
+        self._check(lib().eb_chain_histogram_segments(
+            self._h, nseg, EB_CHAIN_COORDS if what == "chain" else EB_CHAIN_LOG_PROB, int(first), int(stride),
+            int(count), bins, _as_dp(outer), _as_dp(edges), hist.ctypes.data_as(C.POINTER(C.c_uint64))))
         return hist.astype(np.int64)
 
-    def histogram2d(self, first, stride, count, params, bins, edges):
+    def histogram2d(self, first, stride, count, params, bins, edges, nseg=1):
         """``hist[npairs, bins, bins]`` (uint64) of every pair of ``itertools.combinations(params, 2)`` with
-        ``np.histogramdd``'s rule against ``edges[len(params), bins + 1]`` (``eb_chain_histogram2d``)."""
+        ``np.histogramdd``'s rule against ``edges[len(params), bins + 1]`` (``eb_chain_histogram2d``).  With
+        ``nseg > 1``, those of each segment of ``nwalkers / nseg`` walkers: ``edges[nseg * len(params), bins + 1]``
+        (segment-major), ``hist[nseg, npairs, bins, bins]`` (``eb_chain_histogram2d_segments``)."""
+        nseg = int(nseg)
         params = np.ascontiguousarray(params, dtype=np.uint32)
         m, bins = params.size, int(bins)
-        edges = _f64(edges, (m, bins + 1))
-        hist = np.empty((m * (m - 1) // 2, bins, bins), dtype=np.uint64)
-        self._check(lib().eb_chain_histogram2d(
-            self._h, int(first), int(stride), int(count), params.ctypes.data_as(C.POINTER(C.c_uint32)), m, bins,
-            _as_dp(edges), hist.ctypes.data_as(C.POINTER(C.c_uint64))))
+        edges = _f64(edges, (nseg * m, bins + 1))
+        hist = np.empty(((nseg,) if nseg > 1 else ()) + (m * (m - 1) // 2, bins, bins), dtype=np.uint64)
+        self._check(lib().eb_chain_histogram2d_segments(
+            self._h, nseg, int(first), int(stride), int(count), params.ctypes.data_as(C.POINTER(C.c_uint32)), m,
+            bins, _as_dp(edges), hist.ctypes.data_as(C.POINTER(C.c_uint64))))
         return hist
 
 

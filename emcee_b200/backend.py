@@ -426,9 +426,10 @@ class DeviceBackend(object):
 
     def _column_extremes(self, ch, name, first, stride, count, ranges):
         """``(lo, hi, has_nan)`` per column of the slice (ranks 0 and n - 1 of ``eb_chain_select``, one call for
-        every column), or None when every column has a given range"""
+        every column); NaN extremes, unread, when every column has a given range"""
+        D = self.ndim if name == "chain" else 1
         if all(r is not None for r in ranges):
-            return None
+            return np.full(D, np.nan), np.full(D, np.nan), np.zeros(D, dtype=bool)
         n = count * self.nwalkers
         stats, has_nan, _ = ch.select(name, first, stride, count, np.array([0, n - 1], dtype=np.uint64))
         return stats[0], stats[1], has_nan
@@ -450,12 +451,8 @@ class DeviceBackend(object):
             out = [np.histogram(np.empty(0), bins=n, range=r) for r in ranges]
             hist, edges = np.array([h for h, _ in out]), np.array([e for _, e in out], dtype=np.float64)
             return (hist[0], edges[0]) if name == "log_prob" else (hist, edges)
-        ext = self._column_extremes(ch, name, first, stride, count, ranges)
-        outer = np.empty((D, 3))
-        edges = np.empty((D, n + 1))
-        for d in builtins.range(D):
-            kw = {} if ext is None else dict(lo=ext[0][d], hi=ext[1][d], has_nan=ext[2][d])
-            outer[d], edges[d] = uniform_edges(n, ranges[d], **kw)
+        lo, hi, has_nan = self._column_extremes(ch, name, first, stride, count, ranges)
+        outer, edges = uniform_edges(n, ranges, lo, hi, has_nan)
         hist = ch.histogram(name, first, stride, count, n, outer, edges)
         if name == "log_prob":
             return hist[0], edges[0]
@@ -474,14 +471,13 @@ class DeviceBackend(object):
         ranges = _histogram_ranges(range, self.ndim)
         n = histogram_bins(bins, HIST2_BINS_MAX, two_d=True)
         pairs = list(itertools.combinations(params, 2))
+        col_ranges = [ranges[p] for p in params]
+        m = len(params)
         if count == 0:  # numpy's empty-input result, no device work
-            e = [searched_edges(n, ranges[p], 0.0, 1.0) for p in params]
-            return np.zeros((len(pairs), n, n)), np.array(e, dtype=np.float64), pairs
-        ext = self._column_extremes(ch, "chain", first, stride, count, [ranges[p] for p in params])
-        edges = np.empty((len(params), n + 1))
-        for k, p in enumerate(params):
-            kw = {} if ext is None else dict(lo=ext[0][p], hi=ext[1][p], has_nan=ext[2][p])
-            edges[k] = searched_edges(n, ranges[p], **kw)
+            e = searched_edges(n, col_ranges, np.zeros(m), np.ones(m), np.zeros(m, dtype=bool))
+            return np.zeros((len(pairs), n, n)), e, pairs
+        lo, hi, has_nan = self._column_extremes(ch, "chain", first, stride, count, col_ranges)
+        edges = searched_edges(n, col_ranges, lo[params], hi[params], has_nan[params])
         hist = ch.histogram2d(first, stride, count, params, n, edges)
         return hist.astype(np.float64), edges, pairs
 

@@ -10,13 +10,16 @@ Every draw is a pure function of ``(seed, step, split, index, tag)``, and set si
 split count only, so ensemble ``k`` with key ``seeds[k]`` produces exactly the chain of ``EnsembleSampler(nwalkers,
 ndim, log_prob_fn, moves=moves, seed=seeds[k])`` started from the same state, whatever else shares the launch."""
 
+import builtins
+import itertools
 import logging
 import operator
 
 import numpy as np
 
 from . import _lib
-from .backend import Backend, DeviceBackend, _check_summary_name, slice_plan
+from .backend import (Backend, DeviceBackend, _check_histogram_name, _check_summary_name, _histogram_params,
+                      slice_plan)
 from .ensemble import _NOT_INDEPENDENT, _seed_from_numpy
 from .models import CallbackFunction, CudaGraphFunction, DeviceModel, HostFunction
 from .moves import DEMove, DESnookerMove, StretchMove
@@ -85,10 +88,10 @@ class BatchSampler(object):
 
     ``backend`` stores the chain: ``None`` for a host :class:`~emcee_b200.backends.Backend`, or a
     :class:`~emcee_b200.DeviceBackend` on the sampler's device, which keeps it in GPU memory (a stored step is one
-    copy inside HBM) and summarises every ensemble there: :meth:`get_percentile`, :meth:`get_moments` and
-    :meth:`get_autocorr_time` read the chain where it is.  The backend holds the ensembles stacked, ``nbatch *
-    nwalkers`` walkers; an initialised one of that shape with stored steps continues its run (``random_state`` and
-    ``run_mcmc(None, ...)`` resume from its last sample)."""
+    copy inside HBM) and summarises every ensemble there: :meth:`get_percentile`, :meth:`get_moments`,
+    :meth:`get_autocorr_time`, :meth:`get_histogram` and :meth:`get_histogram2d` read the chain where it is.  The
+    backend holds the ensembles stacked, ``nbatch * nwalkers`` walkers; an initialised one of that shape with stored
+    steps continues its run (``random_state`` and ``run_mcmc(None, ...)`` resume from its last sample)."""
 
     def __init__(self, nbatch, nwalkers, ndim, log_prob_fn, moves=None, *, seeds=None, device=0, backend=None):
         self.nbatch, self.nwalkers, self.ndim = operator.index(nbatch), operator.index(nwalkers), operator.index(ndim)
@@ -398,3 +401,130 @@ class BatchSampler(object):
                 raise autocorr.AutocorrError(taus, msg)
             logger.warning(msg)
         return taus
+
+    def _histogram_ranges(self, range, D, log_prob):
+        """``range`` of :meth:`get_histogram` / :meth:`get_histogram2d` as ``(r, per)``: ``r(k, d)`` is the range
+        numpy gets for parameter ``d`` of ensemble ``k``, ``per`` the array ``[nbatch, D, 2]`` of the per-ensemble
+        form (else None).  ``range`` is None, ``D`` pairs or None (one pair for ``log_prob``) shared by every
+        ensemble, or an array ``[nbatch, D, 2]`` (``[nbatch, 2]``); ``ValueError`` for any other shape."""
+        K = self.nbatch
+        if range is None:
+            return (lambda k, d: None), None
+        try:
+            shape = np.shape(range)
+        except ValueError:  # a ragged sequence: pairs and Nones
+            shape = None
+        if shape == ((K, 2) if log_prob else (K, D, 2)):
+            per = np.asarray(range)
+            if log_prob:
+                return (lambda k, d: per[k]), per[:, None]
+            return (lambda k, d: per[k, d]), per
+        if log_prob:
+            if shape != (2,):
+                raise ValueError("range of log_prob must be one (lo, hi) pair or an array [nbatch, 2] = [{0}, 2], "
+                                 "got shape {1}".format(K, shape))
+            return (lambda k, d: range), None
+        shared = list(range)
+        if len(shared) != D or any(r is not None and np.shape(r) != (2,) for r in shared):
+            raise ValueError("range must be one (lo, hi) pair or None per parameter ({0} of them), or an array "
+                             "[nbatch, ndim, 2] = [{1}, {0}, 2]".format(D, K))
+        return (lambda k, d: shared[d]), None
+
+    def get_histogram(self, bins=10, range=None, discard=0, thin=1, name="chain"):
+        """``(hist[nbatch, ndim, bins] int64, edges[nbatch, ndim, bins + 1])``: row ``k`` is what
+        ``Backend.get_histogram`` returns for ensemble ``k``'s flat slice ``get_chain(flat=True, discard=discard,
+        thin=thin)[k]``; with ``name="log_prob"``, ``(hist[nbatch, bins], edges[nbatch, bins + 1])``.  ``range`` is
+        None (each ensemble's own extremes), one ``(lo, hi)`` pair or None per parameter (one pair for
+        ``log_prob``) shared by every ensemble, or an array ``[nbatch, ndim, 2]`` (``[nbatch, 2]``) with one range
+        per ensemble -- the shape ``get_percentile`` output reshapes into.
+
+        With a ``DeviceBackend`` every ensemble is counted on the GPU in one read of the slice
+        (``eb_chain_histogram_segments``), autodetected ranges come from one selection of every ensemble's
+        extremes, and numpy's edges are formed on the host for all columns at once; results, dtypes and exceptions
+        are the host route's (the first failing ensemble, then parameter, raises).  ``bins`` is an int of at most
+        4096 there, and a finite range wider than the largest double raises ``ValueError``, as
+        ``DeviceBackend.get_histogram``."""
+        from .summary import HIST_BINS_MAX, histogram_bins, uniform_edges
+
+        _check_histogram_name(name)
+        b, K = self.backend, self.nbatch
+        log_prob = name == "log_prob"
+        D = 1 if log_prob else self.ndim
+        r, per = self._histogram_ranges(range, D, log_prob)
+        if not isinstance(b, DeviceBackend):
+            flat = self.get_value(name, flat=True, discard=discard, thin=thin)
+            if log_prob:
+                out = [np.histogram(flat[k], bins=bins, range=r(k, 0)) for k in builtins.range(K)]
+                return np.array([h for h, _ in out]), np.array([e for _, e in out], dtype=np.float64)
+            out = [[np.histogram(flat[k][:, d], bins=bins, range=r(k, d)) for d in builtins.range(D)]
+                   for k in builtins.range(K)]
+            return (np.array([[h for h, _ in row] for row in out]),
+                    np.array([[e for _, e in row] for row in out], dtype=np.float64))
+        ch, (first, stride, count) = b._plan(discard, thin)
+        n = histogram_bins(bins, HIST_BINS_MAX)
+        ranges = [r(k, d) for k in builtins.range(K) for d in builtins.range(D)]  # column k * D + d
+        if count == 0:  # numpy's empty-input result (edges over [0, 1] without a range), no device work
+            out = [np.histogram(np.empty(0), bins=n, range=rr) for rr in ranges]
+            hist = np.array([h for h, _ in out]).reshape((K, D, n))
+            edges = np.array([e for _, e in out], dtype=np.float64).reshape((K, D, n + 1))
+        else:
+            lo, hi, has_nan = self._extremes(ch, name, first, stride, count, ranges)
+            outer, edges = uniform_edges(n, ranges if per is None else per.reshape(K * D, 2), lo, hi, has_nan)
+            hist = ch.histogram(name, first, stride, count, n, outer, edges, nseg=K).reshape((K, D, n))
+            edges = edges.reshape((K, D, n + 1))
+        return (hist[:, 0], edges[:, 0]) if log_prob else (hist, edges)
+
+    def get_histogram2d(self, params=None, bins=10, range=None, discard=0, thin=1):
+        """``(hist[nbatch, npairs, bins, bins] float64, edges[nbatch, len(params), bins + 1], pairs)``: row ``k`` is
+        what ``Backend.get_histogram2d`` returns for ensemble ``k``'s flat slice, and ``pairs`` is
+        ``list(itertools.combinations(params, 2))``.  ``range`` takes the forms of :meth:`get_histogram`, indexed
+        by parameter number.  With a ``DeviceBackend`` every (ensemble, pair) is counted on the GPU in one launch
+        (``eb_chain_histogram2d_segments``), as :meth:`get_histogram` does; ``bins`` is an int of at most 128, and
+        the counts of every ensemble are held in device memory at once (``nbatch * npairs * bins^2 * 8`` bytes;
+        ``MemoryError`` when they do not fit)."""
+        from .summary import HIST2_BINS_MAX, histogram_bins, searched_edges
+
+        b, K, D = self.backend, self.nbatch, self.ndim
+        params = _histogram_params(params, D)
+        r, per = self._histogram_ranges(range, D, False)
+        pairs = list(itertools.combinations(params, 2))
+        m = len(params)
+        if not isinstance(b, DeviceBackend):
+            flat = self.get_chain(flat=True, discard=discard, thin=thin)
+            hist, edges = [], []
+            for k in builtins.range(K):
+                hk, ek = [], {}
+                for i, j in pairs:
+                    h, ei, ej = np.histogram2d(flat[k][:, i], flat[k][:, j], bins=bins,
+                                               range=None if range is None else [r(k, i), r(k, j)])
+                    hk.append(h)
+                    ek.setdefault(i, ei)
+                    ek.setdefault(j, ej)
+                hist.append(hk)
+                edges.append([ek[p] for p in params])
+            return np.array(hist), np.array(edges, dtype=np.float64), pairs
+        ch, (first, stride, count) = b._plan(discard, thin)
+        n = histogram_bins(bins, HIST2_BINS_MAX, two_d=True)
+        ranges = [r(k, p) for k in builtins.range(K) for p in params]  # column k * m + position
+        if count == 0:  # numpy's empty-input result, no device work
+            e = searched_edges(n, ranges, np.zeros(K * m), np.ones(K * m), np.zeros(K * m, dtype=bool))
+            return np.zeros((K, len(pairs), n, n)), e.reshape((K, m, n + 1)), pairs
+        lo, hi, has_nan = self._extremes(ch, "chain", first, stride, count, ranges)
+        at = (np.arange(K)[:, None] * D + np.asarray(params)[None, :]).ravel()
+        edges = searched_edges(n, ranges if per is None else per[:, params].reshape(K * m, 2), lo[at], hi[at],
+                               has_nan[at])
+        hist = ch.histogram2d(first, stride, count, params, n, edges, nseg=K)
+        return hist.reshape((K, len(pairs), n, n)).astype(np.float64), edges.reshape((K, m, n + 1)), pairs
+
+    def _extremes(self, ch, name, first, stride, count, ranges):
+        """``(lo, hi, has_nan)`` of every column ``k * D + d`` (ranks 0 and n - 1 of every ensemble, one
+        ``eb_chain_select_segments`` call), or NaN, unread, when every range the call uses is given"""
+        K = self.nbatch
+        C = K * (self.ndim if name == "chain" else 1)
+        if all(rr is not None for rr in ranges):
+            return np.full(C, np.nan), np.full(C, np.nan), np.zeros(C, dtype=bool)
+        n = count * self.nwalkers
+        stats, has_nan, _ = ch.select(name, first, stride, count, np.array([0, n - 1], dtype=np.uint64), nseg=K)
+        stats = stats.reshape(K, 2, -1)
+        return stats[:, 0].ravel(), stats[:, 1].ravel(), has_nan.reshape(-1)
+

@@ -1648,33 +1648,43 @@ int eb_chain_moments_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64
 
 int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, uint64_t count, uint32_t bins,
                        const double* outer, const double* edges, uint64_t* hist) {
+  return eb_chain_histogram_segments(ch, 1, what, first, stride, count, bins, outer, edges, hist);
+}
+
+int eb_chain_histogram_segments(eb_chain* ch, int64_t nseg, int what, uint64_t first, uint64_t stride, uint64_t count,
+                                uint32_t bins, const double* outer, const double* edges, uint64_t* hist) {
   if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_segments(ch, "eb_chain_histogram", nseg);
+  if (rc) return rc;
   if (what != EB_CHAIN_COORDS && what != EB_CHAIN_LOG_PROB)
     FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram: what must be EB_CHAIN_COORDS or EB_CHAIN_LOG_PROB");
   if (bins == 0 || !outer || !edges || !hist) FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram: bins == 0 or null buffer");
   if (bins > (uint32_t)HIST_BINS_MAX)
     FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram is limited to bins <= %d on the device, got %u", HIST_BINS_MAX,
          bins);
-  int rc = chain_check_slice(ch, "eb_chain_histogram", first, stride, count);
+  rc = chain_check_slice(ch, "eb_chain_histogram", first, stride, count);
   if (rc) return rc;
   const bool coords = what == EB_CHAIN_COORDS;
   const int D = coords ? ch->D : 1;
+  const size_t ncol = (size_t)nseg * D;  // column k * D + d: parameter d of segment k
   if (count == 0) {
-    std::fill(hist, hist + (size_t)D * bins, (uint64_t)0);
+    std::fill(hist, hist + ncol * bins, (uint64_t)0);
     return EB_OK;
   }
-  const uint64_t n = count * (uint64_t)ch->N;
-  if (n / (uint64_t)ch->N != count || !hist_rows_fit(n))
+  const uint64_t sn = (uint64_t)ch->N / (uint64_t)nseg;  // rows of a segment in one stored step
+  const uint64_t n = count * sn;
+  if (n / sn != count || !hist_rows_fit(n))
     FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram: slice of %llu stored steps is too long",
          (unsigned long long)count);
+  if (ncol > 0x7fffffff) FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram: more than 2^31 - 1 columns");
   CK(ch, cudaSetDevice(ch->device));
   const std::vector<const double*> slots = chain_slot_table(ch, coords, first, stride, count);
   DevPtr<void> scratch;
-  rc = dev_alloc_checked(ch, "eb_chain_histogram", "scratch", hist1_scratch_bytes(count, D, (int)bins), scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_histogram", "scratch", hist1_scratch_bytes(count, ncol, (int)bins), scratch);
   if (rc) return rc;
   bool bad = false;
-  const cudaError_t e = hist1_run(slots.data(), count, (uint32_t)ch->N, D, (int)bins, outer, edges, hist, &bad,
-                                  scratch.get(), ch->sm_count, ch->st.get());
+  const cudaError_t e = hist1_run(slots.data(), count, (uint32_t)nseg, (uint32_t)ch->N, D, (int)bins, outer, edges,
+                                  hist, &bad, scratch.get(), ch->sm_count, ch->st.get());
   cudaStreamSynchronize(ch->st.get());
   CK(ch, e);
   if (bad)
@@ -1685,7 +1695,15 @@ int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, 
 
 int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, const uint32_t* params,
                          size_t nparams, uint32_t bins, const double* edges, uint64_t* hist) {
+  return eb_chain_histogram2d_segments(ch, 1, first, stride, count, params, nparams, bins, edges, hist);
+}
+
+int eb_chain_histogram2d_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                                  const uint32_t* params, size_t nparams, uint32_t bins, const double* edges,
+                                  uint64_t* hist) {
   if (!ch) return EB_ERR_INVALID;
+  int rc = chain_check_segments(ch, "eb_chain_histogram2d", nseg);
+  if (rc) return rc;
   if (bins == 0 || !params || !edges || !hist)
     FAIL(ch, EB_ERR_INVALID, "eb_chain_histogram2d: bins == 0 or null buffer");
   if (bins > (uint32_t)HIST2_BINS_MAX)
@@ -1700,25 +1718,32 @@ int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t
            ch->D, k, params[k]);
     seen[params[k]] = 1;
   }
-  int rc = chain_check_slice(ch, "eb_chain_histogram2d", first, stride, count);
+  rc = chain_check_slice(ch, "eb_chain_histogram2d", first, stride, count);
   if (rc) return rc;
-  const size_t out = nparams * (nparams - 1) / 2 * (size_t)bins * bins;
+  // nseg * npairs * bins^2 can pass 2^64 (2^31 segments, 2^27 pairs, 2^14 cells): refuse it in floating point first
+  const double outd = (double)nseg * (double)(nparams * (nparams - 1) / 2) * (double)bins * (double)bins;
+  if (outd > (double)((uint64_t)1 << 60))
+    FAIL(ch, EB_ERR_NOMEM, "eb_chain_histogram2d: %.0f counts of 8 bytes cannot be held", outd);
+  const uint64_t out = (uint64_t)nseg * (nparams * (nparams - 1) / 2) * bins * bins;
   if (count == 0) {
     std::fill(hist, hist + out, (uint64_t)0);
     return EB_OK;
   }
-  const uint64_t n = count * (uint64_t)ch->N;
-  if (n / (uint64_t)ch->N != count || !hist_rows_fit(n))
+  const uint64_t sn = (uint64_t)ch->N / (uint64_t)nseg;  // rows of a segment in one stored step
+  const uint64_t n = count * sn;
+  if (n / sn != count || !hist_rows_fit(n))
     FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram2d: slice of %llu stored steps is too long",
          (unsigned long long)count);
+  if (hist2_grid_x((uint32_t)nseg, (int)nparams, (int)bins) > 0x7fffffff)
+    FAIL(ch, EB_ERR_UNSUPPORTED, "eb_chain_histogram2d: more than 2^31 - 1 (segment, pair tile) blocks");
   CK(ch, cudaSetDevice(ch->device));
   const std::vector<const double*> slots = chain_slot_table(ch, true, first, stride, count);
   DevPtr<void> scratch;
-  rc = dev_alloc_checked(ch, "eb_chain_histogram2d", "scratch", hist2_scratch_bytes(count, (int)nparams, (int)bins),
-                         scratch);
+  rc = dev_alloc_checked(ch, "eb_chain_histogram2d", "scratch",
+                         hist2_scratch_bytes(count, (uint32_t)nseg, (int)nparams, (int)bins), scratch);
   if (rc) return rc;
-  const cudaError_t e = hist2_run(slots.data(), count, (uint32_t)ch->N, ch->D, params, (int)nparams, (int)bins, edges,
-                                  hist, scratch.get(), ch->sm_count, ch->st.get());
+  const cudaError_t e = hist2_run(slots.data(), count, (uint32_t)nseg, (uint32_t)ch->N, ch->D, params, (int)nparams,
+                                  (int)bins, edges, hist, scratch.get(), ch->sm_count, ch->st.get());
   cudaStreamSynchronize(ch->st.get());
   CK(ch, e);
   return EB_OK;

@@ -337,18 +337,23 @@ cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t nseg
                        const uint64_t* ranks, size_t nranks, double* out, uint8_t* has_nan, uint32_t* passes,
                        const SelectScratch& z, void* scratch, int sm_count, cudaStream_t st);
 
-// ---- histograms of a stored slice (histogram.cu, eb_chain_histogram / eb_chain_histogram2d) ----------------------
-// can count * N rows be split over grid y with fewer than 2^32 counted by one CTA?
+// ---- histograms of a stored slice (histogram.cu, eb_chain_histogram[2d]_segments) ---------------------------------
+// A slot holds nseg segments (ensembles) of N / nseg rows of D values each; nseg = 1 is the whole slot.
+// can count * (N / nseg) rows be split over grid y with fewer than 2^32 counted by one CTA?
 bool hist_rows_fit(uint64_t n);
-size_t hist1_scratch_bytes(uint64_t count, int D, int bins);
-// slots[count] (host array of device pointers); outer[D, 3] = (first, last, span), edges[D, bins + 1] and
-// hist[D, bins] on the host; *bad: some value's bin index fell outside the edges
-cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t N, int D, int bins, const double* outer,
-                      const double* edges, uint64_t* hist, bool* bad, void* scratch, int sm_count, cudaStream_t st);
-size_t hist2_scratch_bytes(uint64_t count, int m, int bins);
-// params[m] distinct columns; edges[m, bins + 1] and hist[m (m - 1) / 2, bins, bins] on the host
-cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint32_t* params, int m,
-                      int bins, const double* edges, uint64_t* hist, void* scratch, int sm_count, cudaStream_t st);
+size_t hist1_scratch_bytes(uint64_t count, size_t ncol, int bins);
+// slots[count] (host array of device pointers); outer[nseg * D, 3] = (first, last, span), edges[nseg * D, bins + 1]
+// and hist[nseg * D, bins] on the host, column k * D + d; *bad: some value's bin index fell outside the edges
+cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t nseg, uint32_t N, int D, int bins,
+                      const double* outer, const double* edges, uint64_t* hist, bool* bad, void* scratch, int sm_count,
+                      cudaStream_t st);
+// CTAs along grid x of the 2-D kernel: one copy of the pair tiles per segment
+uint64_t hist2_grid_x(uint32_t nseg, int m, int bins);
+size_t hist2_scratch_bytes(uint64_t count, uint32_t nseg, int m, int bins);
+// params[m] distinct columns; edges[nseg, m, bins + 1] and hist[nseg, m (m - 1) / 2, bins, bins] on the host
+cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t nseg, uint32_t N, int D,
+                      const uint32_t* params, int m, int bins, const double* edges, uint64_t* hist, void* scratch,
+                      int sm_count, cudaStream_t st);
 
 // ---- running histograms of the live state (histogram.cu, eb_histograms_config / eb_histograms) -------------------
 struct HistTile;

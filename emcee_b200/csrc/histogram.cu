@@ -4,9 +4,12 @@
 //
 // Both kernels read the slice once, in place, through a table of slot base pointers (one per stored step, as
 // select.cu does): CTA x is a column block (1-D) or a tile of parameter pairs (2-D), CTA y a range of the slice's
-// rows (stored step, walker).  Counts live in shared uint32 bins and are flushed, where non-zero, to 64-bit global
-// counts; a CTA counts fewer than 2^32 rows.  Counts are integers, so the result does not depend on the order in
-// which the atomics land.
+// rows (stored step, walker).  A slot of nseg segments (ensembles, eb_chain_histogram_segments) of n = N / nseg rows
+// is read as select.cu reads it: the 1-D kernel sees nseg * D columns of count * n rows, column c = k * D + d at
+// offset k * n * D + w * D + d of a slot (a column block may span segments), and the 2-D grid holds one copy of the
+// pair tiles per segment.  nseg = 1 is eb_chain_histogram itself.  Counts live in shared uint32 bins and are
+// flushed, where non-zero, to 64-bit global counts; a CTA counts fewer than 2^32 rows.  Counts are integers, so the
+// result does not depend on the order in which the atomics land.
 #include <algorithm>
 #include <vector>
 
@@ -29,13 +32,15 @@ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 // bytes of one column of the 1-D kernel's shared memory: its edges, (first, last, span) and uint32 bins
 size_t hist1_col_bytes(int bins) { return (size_t)(bins + 1 + 3) * sizeof(double) + (size_t)bins * sizeof(uint32_t); }
 
-// Column block x: parameters x * W .. x * W + w - 1.  outer[D, 3] = (first, last, span), edges[D, bins + 1].
+// Column block x: columns x * W .. x * W + w - 1 of ncol = nseg * D; a slot row holds D values and segment k starts
+// seg_stride = n * D values into the slot.  outer[ncol, 3] = (first, last, span), edges[ncol, bins + 1].
 __global__ void __launch_bounds__(HIST_THREADS)
-    hist1_kernel(const double* const* __restrict__ slots, uint32_t N, int D, uint64_t nrows, uint64_t rows_per_cta,
-                 int W, int bins, const double* __restrict__ outer, const double* __restrict__ edges,
-                 unsigned long long* __restrict__ hist, unsigned int* __restrict__ bad) {
+    hist1_kernel(const double* const* __restrict__ slots, uint32_t N, int D, uint64_t seg_stride, int ncol,
+                 uint64_t nrows, uint64_t rows_per_cta, int W, int bins, const double* __restrict__ outer,
+                 const double* __restrict__ edges, unsigned long long* __restrict__ hist,
+                 unsigned int* __restrict__ bad) {
   extern __shared__ __align__(16) unsigned char smem[];
-  const int d0 = (int)blockIdx.x * W, w = min(W, D - d0);
+  const int d0 = (int)blockIdx.x * W, w = min(W, ncol - d0);
   double* se = reinterpret_cast<double*>(smem);               // [w, bins + 1]
   double* so = se + (size_t)w * (bins + 1);                   // [w, 3]
   unsigned int* sh = reinterpret_cast<unsigned int*>(so + 3 * w);  // [w, bins]
@@ -49,6 +54,8 @@ __global__ void __launch_bounds__(HIST_THREADS)
   const bool col_ok = ro < per;
   const double first = so[3 * c], last = so[3 * c + 1], span = so[3 * c + 2];
   const double* e = se + (size_t)c * (bins + 1);
+  const int kseg = (d0 + c) / D;
+  const size_t cbase = (size_t)kseg * seg_stride + (size_t)(d0 + c - kseg * D);  // the column's offset in a slot
   const uint64_t r0 = (uint64_t)blockIdx.y * rows_per_cta;
   const uint64_t r1 = min(nrows, r0 + rows_per_cta);
   uint64_t R = r0 + (uint64_t)ro;
@@ -58,7 +65,7 @@ __global__ void __launch_bounds__(HIST_THREADS)
   for (uint64_t base = r0; base < r1; base += (uint64_t)per) {
     int hs = -1;  // shared bin of this thread's value
     if (col_ok && R < r1) {
-      const double v = slots[s][(size_t)wk * D + d0 + c];
+      const double v = slots[s][(size_t)wk * D + cbase];
       const int b = hist_bin_uniform(v, first, last, span, bins, e);
       if (b >= 0) hs = c * bins + b;
       else if (b == HIST_BAD) atomicOr(bad, 1u);
@@ -95,15 +102,21 @@ Hist2Geom hist2_geom(int m, int bins) {
   return g;
 }
 
-// Tile x: positions a0 .. a0 + na - 1 against b0 .. b0 + nb - 1 of params[m] (pairs i < j only).  edges[m, bins + 1]
-// in position order; hist[m (m - 1) / 2, bins, bins].  Each round stages HIST2_ROWS rows: every (row, position)
+// CTA x: tile x % ntiles of segment k = x / ntiles, positions a0 .. a0 + na - 1 against b0 .. b0 + nb - 1 of
+// params[m] (pairs i < j only).  Segment k's rows start seg_stride values into a slot; edges[nseg, m, bins + 1] in
+// position order; hist[nseg, m (m - 1) / 2, bins, bins].  Each round stages HIST2_ROWS rows: every (row, position)
 // value is binned once (idx, 0xff = outlier), then every (row, pair) adds one count.
 __global__ void __launch_bounds__(HIST2_THREADS)
-    hist2_kernel(const double* const* __restrict__ slots, uint32_t N, int D, uint64_t nrows, uint64_t rows_per_cta,
-                 const HistTile* __restrict__ tiles, const uint32_t* __restrict__ params, uint32_t m, int bins,
-                 const double* __restrict__ edges, unsigned long long* __restrict__ hist) {
+    hist2_kernel(const double* const* __restrict__ slots, uint32_t N, int D, uint64_t seg_stride, uint64_t nrows,
+                 uint64_t rows_per_cta, const HistTile* __restrict__ tiles, uint32_t ntiles,
+                 const uint32_t* __restrict__ params, uint32_t m, int bins, const double* __restrict__ edges,
+                 unsigned long long* __restrict__ hist) {
   extern __shared__ __align__(16) unsigned char smem[];
-  const HistTile t = tiles[blockIdx.x];
+  const uint32_t kseg = blockIdx.x / ntiles;
+  const HistTile t = tiles[blockIdx.x - kseg * ntiles];
+  edges += (size_t)kseg * m * (bins + 1);
+  hist += (uint64_t)kseg * ((uint64_t)m * (m - 1) / 2) * (uint64_t)bins * bins;
+  const size_t seg_off = (size_t)kseg * seg_stride;
   const int na = (int)t.na, nb = (int)t.nb, K = na + nb, P = na * nb, bb = bins * bins;
   const bool diag = t.a0 == t.b0;
   double* se = reinterpret_cast<double*>(smem);                                // [K, bins + 1]
@@ -129,7 +142,7 @@ __global__ void __launch_bounds__(HIST2_THREADS)
       const double* p = nullptr;
       if (R < r1) {
         const uint64_t s = R / N;
-        p = slots[s] + (size_t)(R - s * N) * D;
+        p = slots[s] + seg_off + (size_t)(R - s * N) * D;
       }
       rowp[tid] = p;
     }
@@ -189,15 +202,18 @@ void split_rows(uint64_t n, uint64_t nx, uint64_t ctas, uint64_t min_rows, uint6
 
 bool hist_rows_fit(uint64_t n) { return n <= 65535 * HIST_ROWS_PER_CTA_MAX; }
 
-size_t hist1_scratch_bytes(uint64_t count, int D, int bins) {
-  return align256(count * sizeof(double*)) + align256((size_t)D * 3 * sizeof(double)) +
-         align256((size_t)D * (bins + 1) * sizeof(double)) + align256((size_t)D * bins * sizeof(uint64_t)) +
+size_t hist1_scratch_bytes(uint64_t count, size_t ncol, int bins) {
+  return align256(count * sizeof(double*)) + align256(ncol * 3 * sizeof(double)) +
+         align256(ncol * (bins + 1) * sizeof(double)) + align256(ncol * bins * sizeof(uint64_t)) +
          align256(sizeof(uint32_t));
 }
 
-cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t N, int D, int bins, const double* outer,
-                      const double* edges, uint64_t* hist, bool* bad, void* scratch, int sm_count, cudaStream_t st) {
-  const uint64_t n = count * (uint64_t)N;
+cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t nseg, uint32_t N, int Dp, int bins,
+                      const double* outer, const double* edges, uint64_t* hist, bool* bad, void* scratch, int sm_count,
+                      cudaStream_t st) {
+  const uint32_t sn = N / nseg;  // rows of a segment in one stored step
+  const uint64_t n = count * (uint64_t)sn;
+  const size_t D = (size_t)nseg * Dp;  // columns
   char* p = static_cast<char*>(scratch);
   auto take = [&](size_t bytes) {
     char* q = p;
@@ -205,9 +221,9 @@ cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t N, in
     return q;
   };
   const double** d_slots = reinterpret_cast<const double**>(take(count * sizeof(double*)));
-  double* d_outer = reinterpret_cast<double*>(take((size_t)D * 3 * sizeof(double)));
-  double* d_edges = reinterpret_cast<double*>(take((size_t)D * (bins + 1) * sizeof(double)));
-  unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(take((size_t)D * bins * sizeof(uint64_t)));
+  double* d_outer = reinterpret_cast<double*>(take(D * 3 * sizeof(double)));
+  double* d_edges = reinterpret_cast<double*>(take(D * (bins + 1) * sizeof(double)));
+  unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(take(D * bins * sizeof(uint64_t)));
   unsigned int* d_bad = reinterpret_cast<unsigned int*>(take(sizeof(uint32_t)));
 #define HE(call)                      \
   do {                                \
@@ -215,44 +231,51 @@ cudaError_t hist1_run(const double* const* slots, uint64_t count, uint32_t N, in
     if (_e != cudaSuccess) return _e; \
   } while (0)
   HE(cudaMemcpyAsync(d_slots, slots, count * sizeof(double*), cudaMemcpyHostToDevice, st));
-  HE(cudaMemcpyAsync(d_outer, outer, (size_t)D * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-  HE(cudaMemcpyAsync(d_edges, edges, (size_t)D * (bins + 1) * sizeof(double), cudaMemcpyHostToDevice, st));
-  HE(cudaMemsetAsync(d_hist, 0, (size_t)D * bins * sizeof(uint64_t), st));
+  HE(cudaMemcpyAsync(d_outer, outer, D * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  HE(cudaMemcpyAsync(d_edges, edges, D * (bins + 1) * sizeof(double), cudaMemcpyHostToDevice, st));
+  HE(cudaMemsetAsync(d_hist, 0, D * bins * sizeof(uint64_t), st));
   HE(cudaMemsetAsync(d_bad, 0, sizeof(uint32_t), st));
   // the widest column block (at most 32 columns) whose shared memory fits HIST1_SMEM; one column always fits
   const size_t col = hist1_col_bytes(bins);
-  const int W = (int)std::max<size_t>(1, std::min<size_t>({(size_t)32, (size_t)D, HIST1_SMEM / col}));
+  const int W = (int)std::max<size_t>(1, std::min<size_t>({(size_t)32, D, HIST1_SMEM / col}));
   const size_t smem = (size_t)W * col;
   HE(cudaFuncSetAttribute(hist1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const uint64_t nx = ((uint64_t)D + W - 1) / W;
   uint64_t ys = 1, rows_per = n;
   split_rows(n, nx, (uint64_t)sm_count * 8, (uint64_t)(HIST_THREADS / W) * 16, &ys, &rows_per);
-  hist1_kernel<<<dim3((unsigned)nx, (unsigned)ys), HIST_THREADS, smem, st>>>(d_slots, N, D, n, rows_per, W, bins,
-                                                                            d_outer, d_edges, d_hist, d_bad);
+  hist1_kernel<<<dim3((unsigned)nx, (unsigned)ys), HIST_THREADS, smem, st>>>(
+      d_slots, sn, Dp, (uint64_t)sn * Dp, (int)D, n, rows_per, W, bins, d_outer, d_edges, d_hist, d_bad);
   HE(cudaGetLastError());
   uint32_t hb = 0;
-  HE(cudaMemcpyAsync(hist, d_hist, (size_t)D * bins * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  HE(cudaMemcpyAsync(hist, d_hist, D * bins * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   HE(cudaMemcpyAsync(&hb, d_bad, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   HE(cudaStreamSynchronize(st));
   *bad = hb != 0;
   return cudaSuccess;
 }
 
-size_t hist2_scratch_bytes(uint64_t count, int m, int bins) {
+uint64_t hist2_grid_x(uint32_t nseg, int m, int bins) {
+  return (uint64_t)nseg * hist2_ntiles(m, hist2_geom(m, bins).block);
+}
+
+size_t hist2_scratch_bytes(uint64_t count, uint32_t nseg, int m, int bins) {
   const Hist2Geom g = hist2_geom(m, bins);
   const size_t ntiles = (size_t)hist2_ntiles(m, g.block);  // the tile list itself is built once the scratch fits
   const size_t npairs = (size_t)m * (m - 1) / 2;
   return align256(count * sizeof(double*)) + align256(ntiles * sizeof(HistTile)) +
-         align256((size_t)m * sizeof(uint32_t)) + align256((size_t)m * (bins + 1) * sizeof(double)) +
-         align256(npairs * bins * bins * sizeof(uint64_t));
+         align256((size_t)m * sizeof(uint32_t)) + align256((size_t)nseg * m * (bins + 1) * sizeof(double)) +
+         align256((size_t)nseg * npairs * bins * bins * sizeof(uint64_t));
 }
 
-cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t N, int D, const uint32_t* params, int m,
-                      int bins, const double* edges, uint64_t* hist, void* scratch, int sm_count, cudaStream_t st) {
-  const uint64_t n = count * (uint64_t)N;
+cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t nseg, uint32_t N, int D,
+                      const uint32_t* params, int m, int bins, const double* edges, uint64_t* hist, void* scratch,
+                      int sm_count, cudaStream_t st) {
+  const uint32_t sn = N / nseg;  // rows of a segment in one stored step
+  const uint64_t n = count * (uint64_t)sn;
   const Hist2Geom g = hist2_geom(m, bins);
   const std::vector<HistTile> tiles = hist2_tiles(m, g.block);
-  const size_t npairs = (size_t)m * (m - 1) / 2, out = npairs * bins * bins;
+  const size_t npairs = (size_t)m * (m - 1) / 2, out = (size_t)nseg * npairs * bins * bins;
+  const size_t nedges = (size_t)nseg * m * (bins + 1);
   char* p = static_cast<char*>(scratch);
   auto take = [&](size_t bytes) {
     char* q = p;
@@ -262,19 +285,20 @@ cudaError_t hist2_run(const double* const* slots, uint64_t count, uint32_t N, in
   const double** d_slots = reinterpret_cast<const double**>(take(count * sizeof(double*)));
   HistTile* d_tiles = reinterpret_cast<HistTile*>(take(tiles.size() * sizeof(HistTile)));
   uint32_t* d_params = reinterpret_cast<uint32_t*>(take((size_t)m * sizeof(uint32_t)));
-  double* d_edges = reinterpret_cast<double*>(take((size_t)m * (bins + 1) * sizeof(double)));
+  double* d_edges = reinterpret_cast<double*>(take(nedges * sizeof(double)));
   unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(take(out * sizeof(uint64_t)));
   HE(cudaMemcpyAsync(d_slots, slots, count * sizeof(double*), cudaMemcpyHostToDevice, st));
   HE(cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(HistTile), cudaMemcpyHostToDevice, st));
   HE(cudaMemcpyAsync(d_params, params, (size_t)m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  HE(cudaMemcpyAsync(d_edges, edges, (size_t)m * (bins + 1) * sizeof(double), cudaMemcpyHostToDevice, st));
+  HE(cudaMemcpyAsync(d_edges, edges, nedges * sizeof(double), cudaMemcpyHostToDevice, st));
   HE(cudaMemsetAsync(d_hist, 0, out * sizeof(uint64_t), st));
   HE(cudaFuncSetAttribute(hist2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
+  const uint64_t nx = (uint64_t)nseg * tiles.size();  // at most 2^31 - 1 (the caller checks hist2_grid_x)
   uint64_t ys = 1, rows_per = n;
-  split_rows(n, tiles.size(), (uint64_t)sm_count * 2, (uint64_t)HIST2_ROWS * 4, &ys, &rows_per);
-  // grid x over the tiles in launches of at most 2^31 - 1 CTAs is never needed: m <= ndim <= 16384
-  hist2_kernel<<<dim3((unsigned)tiles.size(), (unsigned)ys), HIST2_THREADS, g.smem, st>>>(
-      d_slots, N, D, n, rows_per, d_tiles, d_params, (uint32_t)m, bins, d_edges, d_hist);
+  split_rows(n, nx, (uint64_t)sm_count * 2, (uint64_t)HIST2_ROWS * 4, &ys, &rows_per);
+  hist2_kernel<<<dim3((unsigned)nx, (unsigned)ys), HIST2_THREADS, g.smem, st>>>(
+      d_slots, sn, D, (uint64_t)sn * D, n, rows_per, d_tiles, (uint32_t)tiles.size(), d_params, (uint32_t)m, bins,
+      d_edges, d_hist);
   HE(cudaGetLastError());
   HE(cudaMemcpyAsync(hist, d_hist, out * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   HE(cudaStreamSynchronize(st));
@@ -383,12 +407,12 @@ cudaError_t live_hist_launch(const LiveHist& h, cudaStream_t st, uint64_t& launc
   // the attribute is set at every launch: eb_chain_histogram sets the same kernels' limits to its own sizes
   HE(cudaFuncSetAttribute(hist1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                           (int)std::max(h.smem1, h.lp ? h.smemlp : 0)));
-  hist1_kernel<<<h.grid1, HIST_THREADS, h.smem1, st>>>(h.slots, h.N, h.D, h.N, h.rows1, h.W1, h.bins, h.outer,
-                                                       h.edges, h.hist, h.bad);
+  hist1_kernel<<<h.grid1, HIST_THREADS, h.smem1, st>>>(h.slots, h.N, h.D, 0, h.D, h.N, h.rows1, h.W1, h.bins,
+                                                       h.outer, h.edges, h.hist, h.bad);
   HE(cudaGetLastError());
   ++launches;
   if (h.lp) {  // the log-probabilities: row D of the tables, one column of stride 1
-    hist1_kernel<<<h.gridlp, HIST_THREADS, h.smemlp, st>>>(h.slots + 1, h.N, 1, h.N, h.rowslp, h.Wlp, h.bins,
+    hist1_kernel<<<h.gridlp, HIST_THREADS, h.smemlp, st>>>(h.slots + 1, h.N, 1, 0, 1, h.N, h.rowslp, h.Wlp, h.bins,
                                                            h.outer + 3 * (size_t)h.D,
                                                            h.edges + (size_t)h.D * (h.bins + 1),
                                                            h.hist + (size_t)h.D * h.bins, h.bad);
@@ -397,8 +421,8 @@ cudaError_t live_hist_launch(const LiveHist& h, cudaStream_t st, uint64_t& launc
   }
   if (h.m >= 2) {
     HE(cudaFuncSetAttribute(hist2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h.smem2));
-    hist2_kernel<<<h.grid2, HIST2_THREADS, h.smem2, st>>>(h.slots, h.N, h.D, h.N, h.rows2, h.tiles, h.params,
-                                                          (uint32_t)h.m, h.bins2, h.edges2, h.hist2);
+    hist2_kernel<<<h.grid2, HIST2_THREADS, h.smem2, st>>>(h.slots, h.N, h.D, 0, h.N, h.rows2, h.tiles, h.ntiles,
+                                                          h.params, (uint32_t)h.m, h.bins2, h.edges2, h.hist2);
     HE(cudaGetLastError());
     ++launches;
   }

@@ -136,11 +136,7 @@ def _two_rows(lo, hi, has_nan):
     return np.array([np.nan, np.nan]) if has_nan else np.array([lo, hi], dtype=np.float64)
 
 
-def uniform_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
-    """``(outer[3], edges[bins + 1])`` of ``np.histogram(column, bins, rng)`` for a column with minimum ``lo`` and
-    maximum ``hi`` (used only when ``rng`` is None): ``outer`` is numpy's ``(first_edge, last_edge, norm_denom)``
-    of its uniform-bin fast path, as float64.  numpy's exceptions for a bad range; ``ValueError`` for an
-    overflowing one."""
+def _uniform_column(bins, rng, lo, hi, has_nan):
     a2 = _two_rows(lo, hi, has_nan)
     _check_overflow(a2, rng)
     edges = np.histogram_bin_edges(a2, bins, rng)
@@ -151,12 +147,7 @@ def uniform_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
     return np.array([first, last, span], dtype=np.float64), np.asarray(edges, dtype=np.float64)
 
 
-def searched_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
-    """``edges[bins + 1]`` of one axis of ``np.histogram2d`` / ``np.histogramdd`` for a column with minimum ``lo``
-    and maximum ``hi``: ``np.histogramdd`` of the column's ``[min; max]`` alone, which forms each axis's edges
-    independently of the others.  numpy's exceptions for a bad range; ``ValueError`` for an overflowing one.  A
-    finite range gives non-decreasing edges (``np.linspace`` rounds monotonically), so ``searchsorted`` is the count
-    of edges at or below a value."""
+def _searched_column(bins, rng, lo, hi, has_nan):
     a2 = _two_rows(lo, hi, has_nan)
     _check_overflow(a2, rng)
     with np.errstate(invalid="ignore"):
@@ -164,6 +155,155 @@ def searched_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
     if not np.all(np.isfinite(edges)):
         raise ValueError("histogram edges over [{0}, {1}] are not finite".format(edges[0], edges[-1]))
     return np.asarray(edges, dtype=np.float64)
+
+
+_EXACT_INT = 2**53  # a Python int range bound below this converts to float64 exactly, as numpy converts it
+
+
+def _range_dtype(r):
+    """the dtype numpy forms a given range ``r`` in (its ``linspace`` dtype): float64 for two Python or float64
+    numbers, float32 for two float32 scalars; None for anything else (formed one column at a time)"""
+    try:
+        lo, hi = r
+    except (TypeError, ValueError):
+        return None
+    kinds = set()
+    for v in (lo, hi):
+        if isinstance(v, float) or (type(v) is int and -_EXACT_INT <= v <= _EXACT_INT):
+            kinds.add(np.float64)  # np.float64 is a float
+        elif type(v) is np.float32:
+            kinds.add(np.float32)
+        else:
+            return None
+    return kinds.pop() if len(kinds) == 1 else None
+
+
+def _column_plan(rng, lo, hi, has_nan):
+    """The columns' ``(first, last)`` before numpy widens an empty range, by linspace dtype: ``groups`` maps float64
+    / float32 to ``(columns, first, last, given)``; ``single`` lists the columns whose range has another form.
+    ``rng`` is None, a sequence of one entry (None or a pair) per column, or a float array ``[C, 2]``."""
+    lo, hi = np.atleast_1d(np.asarray(lo, dtype=np.float64)), np.atleast_1d(np.asarray(hi, dtype=np.float64))
+    has_nan = np.atleast_1d(np.asarray(has_nan, dtype=bool))
+    C = max(lo.size, hi.size, has_nan.size)
+    lo, hi, has_nan = (np.broadcast_to(v, (C,)) for v in (lo, hi, has_nan))
+    if rng is None:
+        rng = [None] * C
+    if isinstance(rng, np.ndarray) and rng.ndim == 2 and rng.dtype.type in (np.float64, np.float32):
+        if len(rng) != C:
+            raise ValueError("{0} ranges for {1} columns".format(len(rng), C))
+        dt = rng.dtype.type
+        given = np.ones(C, dtype=bool)
+        groups = {dt: (np.arange(C), rng[:, 0].copy(), rng[:, 1].copy(), given)}
+        return C, lo, hi, has_nan, groups, np.zeros(0, dtype=np.intp)
+    if len(rng) != C:
+        raise ValueError("{0} ranges for {1} columns".format(len(rng), C))
+    code = np.empty(C, dtype=np.int8)  # 0 autodetected, 1 float64 given, 2 float32 given, 3 single
+    glo, ghi = np.empty(C), np.empty(C)
+    for c, r in enumerate(rng):
+        if r is None:
+            code[c] = 0
+            continue
+        dt = _range_dtype(r)
+        if dt is None:
+            code[c] = 3
+            continue
+        code[c] = 1 if dt is np.float64 else 2
+        glo[c], ghi[c] = r  # float32 bounds are exact in float64
+    auto = code == 0
+    with np.errstate(invalid="ignore"):
+        first = np.where(has_nan, np.nan, np.minimum(lo, hi))
+        last = np.where(has_nan, np.nan, np.maximum(lo, hi))
+    f64 = auto | (code == 1)
+    first[~auto], last[~auto] = glo[~auto], ghi[~auto]
+    groups = {}
+    cols = np.flatnonzero(f64)
+    if cols.size:
+        groups[np.float64] = (cols, first[cols], last[cols], ~auto[cols])
+    cols = np.flatnonzero(code == 2)
+    if cols.size:
+        groups[np.float32] = (cols, first[cols].astype(np.float32), last[cols].astype(np.float32),
+                              np.ones(cols.size, dtype=bool))
+    return C, lo, hi, has_nan, groups, np.flatnonzero(code == 3)
+
+
+def _linspace_rows(first, last, bins, dt):
+    """``np.linspace(first[c], last[c], bins + 1)`` of every row, computed in ``dt`` as numpy computes one (``y *
+    step + start``, the last element set to ``stop``), and the rows whose step is 0: numpy forms those with
+    another expression (``y / div * delta``) -- and an array call would switch every row to it -- so the caller
+    forms them one at a time."""
+    y = np.arange(0, bins + 1, dtype=dt)
+    with np.errstate(all="ignore"):  # an overflowing range is refused by the caller
+        delta = np.subtract(last, first, dtype=dt)
+        step = delta / bins
+        edges = y[None, :] * step[:, None] + first[:, None]
+    edges[:, -1] = last
+    return edges, delta, step == 0
+
+
+def _edge_columns(bins, rng, lo, hi, has_nan, uniform):
+    C, lo, hi, has_nan, groups, single = _column_plan(rng, lo, hi, has_nan)
+    outer = np.empty((C, 3)) if uniform else None
+    edges = np.empty((C, bins + 1))
+    suspect = np.zeros(C, dtype=bool)
+    suspect[single] = True
+    for dt, (cols, first, last, given) in groups.items():
+        with np.errstate(all="ignore"):
+            bad = ~(np.isfinite(first) & np.isfinite(last)) | (given & (first > last))
+            # _check_overflow: a finite range (the given one, or the column's [lo, hi]) whose float64 width is not
+            lo64 = np.where(given, first.astype(np.float64), lo[cols])
+            hi64 = np.where(given, last.astype(np.float64), hi[cols])
+            bad |= np.isfinite(lo64) & np.isfinite(hi64) & (lo64 < hi64) & ~np.isfinite(hi64 - lo64)
+            same = first == last  # _get_outer_edges widens an empty range by 0.5 each way, in the range's dtype
+            first = np.where(same, first - dt(0.5), first)
+            last = np.where(same, last + dt(0.5), last)
+        e, delta, step0 = _linspace_rows(first, last, bins, dt)
+        e = e.astype(np.float64)
+        bad |= step0 | ~np.all(np.isfinite(e), axis=1)
+        if uniform:
+            bad |= np.any(e[:, :-1] >= e[:, 1:], axis=1)  # numpy's "Too many bins for data range"
+            outer[cols] = np.stack([first, last, delta], axis=1)
+        edges[cols] = e
+        suspect[cols[bad]] = True
+    # every column that may fail, or that numpy forms another way, goes through numpy itself in column order: the
+    # first failing one raises what the per-column loop raises
+    for c in np.flatnonzero(suspect):
+        r = rng[c] if rng is not None else None
+        if isinstance(r, np.ndarray):
+            r = (r[0], r[1])
+        if uniform:
+            outer[c], edges[c] = _uniform_column(bins, r, lo[c], hi[c], has_nan[c])
+        else:
+            edges[c] = _searched_column(bins, r, lo[c], hi[c], has_nan[c])
+    return outer, edges
+
+
+def uniform_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
+    """``(outer[3], edges[bins + 1])`` of ``np.histogram(column, bins, rng)`` for a column with minimum ``lo`` and
+    maximum ``hi`` (used only when ``rng`` is None): ``outer`` is numpy's ``(first_edge, last_edge, norm_denom)``
+    of its uniform-bin fast path, as float64.  numpy's exceptions for a bad range; ``ValueError`` for an
+    overflowing one.
+
+    With arrays ``lo[C]``, ``hi[C]`` and ``has_nan[C]``, the same for ``C`` columns at once: ``rng`` is None, one
+    entry (None or a pair) per column or a float array ``[C, 2]``, and the result ``(outer[C, 3], edges[C, bins +
+    1])``, each row equal to the one-column call.  The columns are formed together in a few numpy calls; a column
+    that may raise, or that numpy forms another way (a step of 0, a range of another type), is formed by numpy
+    alone, in column order, so that the exception is the first failing column's."""
+    if np.ndim(lo) == 0 and np.ndim(hi) == 0 and np.ndim(has_nan) == 0:
+        outer, edges = _edge_columns(bins, [rng], lo, hi, has_nan, uniform=True)
+        return outer[0], edges[0]
+    return _edge_columns(bins, rng, lo, hi, has_nan, uniform=True)
+
+
+def searched_edges(bins, rng, lo=np.nan, hi=np.nan, has_nan=False):
+    """``edges[bins + 1]`` of one axis of ``np.histogram2d`` / ``np.histogramdd`` for a column with minimum ``lo``
+    and maximum ``hi``: ``np.histogramdd`` of the column's ``[min; max]`` alone, which forms each axis's edges
+    independently of the others.  numpy's exceptions for a bad range; ``ValueError`` for an overflowing one.  A
+    finite range gives non-decreasing edges (``np.linspace`` rounds monotonically), so ``searchsorted`` is the count
+    of edges at or below a value.  With arrays ``lo[C]``, ``hi[C]`` and ``has_nan[C]``: ``edges[C, bins + 1]`` of
+    ``C`` columns at once, as :func:`uniform_edges` forms them."""
+    if np.ndim(lo) == 0 and np.ndim(hi) == 0 and np.ndim(has_nan) == 0:
+        return _edge_columns(bins, [rng], lo, hi, has_nan, uniform=False)[1][0]
+    return _edge_columns(bins, rng, lo, hi, has_nan, uniform=False)[1]
 
 
 def running_histogram_plan(ndim, range, bins=10, log_prob_range=None, params2d=None, bins2d=10):
@@ -184,15 +324,13 @@ def running_histogram_plan(ndim, range, bins=10, log_prob_range=None, params2d=N
             len(ranges), ndim))
     n = histogram_bins(bins, HIST_BINS_MAX)
     rows = ranges + ([] if log_prob_range is None else [log_prob_range])
-    outer = np.empty((len(rows), 3))
-    edges = np.empty((len(rows), n + 1))
-    for d, r in enumerate(rows):
-        outer[d], edges[d] = uniform_edges(n, r)
+    outer, edges = uniform_edges(n, rows, np.full(len(rows), np.nan), np.full(len(rows), np.nan))
     cfg = dict(bins=n, outer=outer, edges=edges, log_prob=log_prob_range is not None, params2d=None, bins2d=0,
                edges2d=None, pairs=None)
     if params2d is not None:
         params2d = _histogram_params(params2d, ndim)
         n2 = histogram_bins(bins2d, HIST2_BINS_MAX, two_d=True)
-        edges2d = np.array([searched_edges(n2, ranges[p]) for p in params2d], dtype=np.float64)
+        edges2d = searched_edges(n2, [ranges[p] for p in params2d], np.full(len(params2d), np.nan),
+                                 np.full(len(params2d), np.nan))
         cfg.update(params2d=params2d, bins2d=n2, edges2d=edges2d, pairs=list(itertools.combinations(params2d, 2)))
     return cfg

@@ -506,6 +506,21 @@ int eb_chain_histogram(eb_chain* ch, int what, uint64_t first, uint64_t stride, 
  * device scratch at once, checked against the free memory first: EB_ERR_NOMEM. */
 int eb_chain_histogram2d(eb_chain* ch, uint64_t first, uint64_t stride, uint64_t count, const uint32_t* params,
                          size_t nparams, uint32_t bins, const double* edges, uint64_t* hist);
+/* eb_chain_histogram of each segment (nseg divides nwalkers; segment k is
+ * walkers k * nw .. (k + 1) * nw - 1, nw = nwalkers / nseg): column k * D + d
+ * is parameter d of segment k, with outer[nseg * D * 3], edges[nseg * D *
+ * (bins + 1)] and hist[nseg * D * bins] in that column order.  Every column is
+ * counted in the same read of the slice; eb_chain_histogram is nseg = 1. */
+int eb_chain_histogram_segments(eb_chain* ch, int64_t nseg, int what, uint64_t first, uint64_t stride, uint64_t count,
+                                uint32_t bins, const double* outer, const double* edges, uint64_t* hist);
+/* eb_chain_histogram2d of each segment: edges[nseg * nparams * (bins + 1)]
+ * holds segment k's edges of params[] at k * nparams * (bins + 1) and hist
+ * [nseg * npairs * bins^2] its pair counts at k * npairs * bins^2.  The counts of
+ * every segment are held in device scratch at once (EB_ERR_NOMEM when they do
+ * not fit); eb_chain_histogram2d is nseg = 1. */
+int eb_chain_histogram2d_segments(eb_chain* ch, int64_t nseg, uint64_t first, uint64_t stride, uint64_t count,
+                                  const uint32_t* params, size_t nparams, uint32_t bins, const double* edges,
+                                  uint64_t* hist);
 
 /* ---- device memory in and out (CUDA Array Interface) --------------------- */
 /* The device twins of the state, log-probability and chain transfers above, for callers that keep their arrays
