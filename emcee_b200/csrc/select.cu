@@ -198,10 +198,14 @@ cudaError_t select_run(const double* const* slots, uint64_t count, uint32_t nseg
     for (size_t i = p0; i < p1; ++i) {
       const uint32_t d = (uint32_t)(i / nranks);
       const uint32_t r = order[i % nranks];
-      if (nan[d]) continue;  // a NaN seen by an earlier batch
+      const size_t o = ((size_t)(d / Dp) * nranks + r) * Dp + d % Dp;
+      if (nan[d]) {  // a NaN seen by an earlier batch: the column's pairs in this batch are answered NaN too
+        out[o] = NAN;
+        continue;
+      }
       bd.push_back(d);
       bk.push_back(ranks[r]);
-      bo.push_back(((size_t)(d / Dp) * nranks + r) * Dp + d % Dp);
+      bo.push_back(o);
     }
     plan.init(bd.data(), bk.data(), bd.size(), n);
     while (plan.live()) {

@@ -7,7 +7,13 @@
 
 #include "../../emcee_b200/csrc/select_keys.h"
 
+namespace {
+int max_column_tasks = 0;  // the most CTA column blocks one parameter took in a pass of the last probe_select
+}
+
 extern "C" {
+
+int probe_select_max_column_tasks() { return max_column_tasks; }
 
 void probe_keys(const double* x, size_t n, uint64_t* keys, double* back) {
   for (size_t i = 0; i < n; ++i) {
@@ -38,12 +44,18 @@ int probe_select(const double* x, uint64_t rows, int D, const uint64_t* ranks, s
   std::vector<uint64_t> hist, cand;
   std::vector<uint32_t> cnt;
   bool first = true;
+  max_column_tasks = 0;
+  std::vector<int> col_tasks;
   while (plan.live()) {
     plan.layout(cand_budget);
     const size_t ng = plan.groups.size();
     hist.assign(ng * SEL_BINS, 0);
     cand.assign(plan.cand_used, 0);
     cnt.assign(ng, 0);
+    col_tasks.assign((size_t)D, 0);
+    for (const SelTask& t : plan.tasks)
+      for (uint32_t c = 0; c < t.w && t.d0 + c < (uint32_t)D; ++c)
+        max_column_tasks = std::max(max_column_tasks, ++col_tasks[t.d0 + c]);
     for (const SelTask& t : plan.tasks) {
       if (t.w == 0 || t.w > (uint32_t)SEL_WMAX) return -1;
       int slots = 0;

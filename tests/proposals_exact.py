@@ -5,6 +5,8 @@ chain moment sums (``test_gpu_proposals_exact.py`` holds the derivation of the b
 Arithmetic of the references: standard normals with ``mpmath`` at 45 digits; covariances exactly, from integer
 images of the coordinates; the thresholded Cholesky factor ``chol_psd`` with ``mpmath`` up to ``MP_MAX_D``
 columns and in ``np.longdouble`` above, whose own roundings (unit ``ULD``) are added to the bounds."""
+import math
+
 import mpmath
 import numpy as np
 from scipy.linalg import solve_triangular
@@ -294,6 +296,35 @@ def colmean_device_order(X):
     for y in range(8):
         s = s + part[y]
     return s / float(X.shape[0])
+
+
+def segment_moments_ratios(X, shift, mean_d, cov_d, depth):
+    """Largest |device - reference| / bound of the mean and of the covariance of the samples X[m, D] (float64)
+    against a two-pass long-double reference: the bound of ``test_gpu_chain_summary.test_moments_exact`` for sums
+    about ``shift`` that are at most ``depth`` operations deep (``eb_chain_moments_segments``: a chain of FMAs or
+    additions over a chunk's rows, then one addition per chunk)."""
+    m, D = X.shape
+    Y = X - shift
+    hi = np.array([math.fsum(X[:, c]) for c in range(D)])
+    lo = np.array([math.fsum(np.r_[X[:, c], -hi[c]]) for c in range(D)])
+    mean_ref = (hi.astype(np.longdouble) + lo.astype(np.longdouble)) / np.longdouble(m)
+    aY = np.abs(Y)
+    S1 = Y.sum(axis=0)
+    b_mean = (U + gamma(depth)) * aY.sum(axis=0) / m + 2 * U * np.abs(S1) / m + (U + ULD) * np.abs(mean_d)
+    e_mean = np.abs(mean_d.astype(np.longdouble) - mean_ref).astype(np.float64)
+    Xc = X.astype(np.longdouble) - mean_ref
+    ref = (Xc.T @ Xc) / np.longdouble(m - 1)
+    P = aY.T @ aY
+    aS1 = np.abs(S1)
+    dS1 = (U + gamma(depth)) * aY.sum(axis=0)
+    b_cov = ((2 * U + gamma(depth)) * P + (dS1[:, None] * aS1[None, :] + aS1[:, None] * dS1[None, :]) / m
+             + 2 * U * aS1[:, None] * aS1[None, :] / m) / (m - 1) + 2 * U * np.abs(ref.astype(np.float64))
+    b_cov += gamma(m + 2, ULD) * P / (m - 1)
+    e_cov = np.abs(cov_d.astype(np.longdouble) - ref).astype(np.float64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        r_mean = np.where(e_mean == 0, 0.0, e_mean / b_mean)
+        r_cov = np.where(e_cov == 0, 0.0, e_cov / b_cov)
+    return float(r_mean.max()), float(r_cov.max())
 
 
 def moments_depth(nrows, D, sm_count, ncalls):

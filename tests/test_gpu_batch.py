@@ -53,6 +53,19 @@ def _cases():
     return out
 
 
+# Large ensembles, each reaching a branch of batch.cu the rows of _cases() do not:
+#   N = 1 025, 2 048     batch_split_table_kernel runs a second chunk of TABLE_THREADS = 1 024 walkers
+#   D = 20, 60, 130      lanes_per_walker = 8, 16, 32
+#   D = 300, snooker x dense: 8 groups x 5 rows x 300 doubles = 96 000 bytes of shared memory, above the 48 KB default
+#   D = 700, snooker x dense: 224 000 bytes at 256 threads, so the launch halves to 128 threads (112 000 bytes)
+#   32 splits of 100 walkers, K = 3
+# (a red-blue move needs at least twice as many walkers as dimensions)
+LARGE_CASES = [("stretch", "gauss_iso", 2, 1025, 3, 2, True, 1), ("de", "ring", 2, 2048, 4, 3, True, 1),
+               ("stretch", "rosenbrock", 3, 48, 20, 2, True, 1), ("de_gamma0", "gauss_dense", 2, 128, 60, 2, False, 1),
+               ("stretch_a3", "ring", 2, 260, 130, 3, True, 2), ("snooker", "gauss_dense", 2, 600, 300, 4, True, 1),
+               ("snooker", "gauss_dense", 2, 1400, 700, 4, False, 1), ("de", "gauss_iso", 3, 100, 4, 32, True, 1)]
+
+
 def _p0(K, N, D, seed=11):
     return 0.7 * np.random.default_rng(seed).normal(size=(K, N, D))
 
@@ -77,7 +90,7 @@ def _assert_twin(b, k, t, last_b, last_t):
     assert np.array_equal(last_b.log_prob[k], last_t.log_prob)
 
 
-@pytest.mark.parametrize("mv,model,K,N,D,P,rand,thin_by", _cases())
+@pytest.mark.parametrize("mv,model,K,N,D,P,rand,thin_by", _cases() + LARGE_CASES)
 def test_twins_exact(mv, model, K, N, D, P, rand, thin_by):
     seeds = _seeds(K)
     p0 = _p0(K, N, D)

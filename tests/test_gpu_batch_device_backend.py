@@ -12,8 +12,6 @@
   ensemble's parameter; ``get_moments`` meets a long-double bound, agrees with the host route and repeats bit for bit.
 * Refusals: ``nseg`` that does not divide the walkers, and a ``grow`` that cannot fit.
 """
-import math
-
 import numpy as np
 import pytest
 
@@ -252,27 +250,12 @@ def test_moments_exact(K, N, D, start):
     scale = np.sqrt(np.einsum("kii->ki", np.abs(cov_h)))
     assert np.all(np.abs(mean_d - mean_h) <= 1e-10 * (np.abs(mean_h) + scale))
     assert np.all(np.abs(cov_d - cov_h) <= 1e-10 * (np.abs(cov_h) + scale[:, :, None] * scale[:, None, :]))
-    U, depth = PX.U, rows.shape[0] * N + rows.shape[0]
+    depth = rows.shape[0] * N + rows.shape[0]
     for k in range(K):
         X = rows[:, k].reshape(-1, D)
         shift = np.cumsum(rows[0, k], axis=0)[-1] / N  # the device's order: walkers ascending
-        Y = X - shift
-        hi = np.array([math.fsum(X[:, c]) for c in range(D)])
-        lo = np.array([math.fsum(np.r_[X[:, c], -hi[c]]) for c in range(D)])
-        mean_ref = (hi.astype(np.longdouble) + lo.astype(np.longdouble)) / np.longdouble(m)
-        aY = np.abs(Y)
-        S1 = Y.sum(axis=0)
-        b_mean = (U + PX.gamma(depth)) * aY.sum(axis=0) / m + 2 * U * np.abs(S1) / m + (U + PX.ULD) * np.abs(mean_d[k])
-        assert np.all(np.abs(mean_d[k].astype(np.longdouble) - mean_ref).astype(np.float64) <= b_mean)
-        Xc = X.astype(np.longdouble) - mean_ref
-        ref = (Xc.T @ Xc) / np.longdouble(m - 1)
-        P = aY.T @ aY
-        aS1 = np.abs(S1)
-        dS1 = (U + PX.gamma(depth)) * aY.sum(axis=0)
-        b_cov = ((2 * U + PX.gamma(depth)) * P + (dS1[:, None] * aS1[None, :] + aS1[:, None] * dS1[None, :]) / m
-                 + 2 * U * aS1[:, None] * aS1[None, :] / m) / (m - 1) + 2 * U * np.abs(ref.astype(np.float64))
-        b_cov += PX.gamma(m + 2, PX.ULD) * P / (m - 1)
-        assert np.all(np.abs(cov_d[k].astype(np.longdouble) - ref).astype(np.float64) <= b_cov)
+        r_mean, r_cov = PX.segment_moments_ratios(X, shift, mean_d[k], cov_d[k], depth)
+        assert r_mean <= 1.0 and r_cov <= 1.0, (k, r_mean, r_cov)
 
 
 def test_empty_slices_and_bad_q():
