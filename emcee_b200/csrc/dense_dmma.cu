@@ -351,6 +351,11 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
       // publish the meta record and launch the 16 row copies of one tile into the landing slot
       auto issue = [&](Prep& p, int par, bool load_lp) -> bool {
         if (__any_sync(0xffffffffu, p.remote) && !peers_ready()) return false;
+        // Every lane wrote its part of the previous tile's proposal over the partner rows through the generic
+        // proxy; the bulk copies below write the same slot through the async proxy.  Without this fence a
+        // proposal store may land after them and overwrite a row of this tile (seen at D = 120 with a mean and
+        // a box).  Here, behind the wait for the free slot, it is off the producer -> consumer path.
+        fence_async_smem();
         if (lane == 0) mbar_arrive_expect_tx(barFull + pair, 16u * D * (unsigned)sizeof(double));
         __syncwarp();
         request(p, 0, 16);
